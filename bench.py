@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- MoE-layer forward tokens/s on B200 (BASELINE.json metric), one fused persistent kernel per step.
+"""bench.py -- MoE-layer forward tokens/s on H100 (BASELINE.json metric), one fused persistent kernel per step.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config NAME] [--sweeps a,b,..]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -15,11 +16,13 @@ same JSON line (`"sweeps": [...]`).
 Prints ONE JSON line (rank 0).  `value` = N*S / (max over ranks of the device time per step), inputs resident in HBM;
 `e2e` = the same metric through the public host-buffer entry point (pinned host activations in, host output back, every
 step's copies inside the timed region; steps are pipelined three deep so the copies overlap the kernels).  `roofline`
-describes the dominant work (the two expert GEMMs on tcgen05) against the measured cuBLAS bf16 throughput of this pool
-(MEASURED_PEAKS.json: burst peak when the timed region is shorter than a second, else sustained; both fractions are
-printed); `parity_check` is one extra forward on seeded, scaled inputs after the timed loops, every rank's output and
+describes the dominant work (the two expert GEMMs on wgmma) against a bf16 peak (MEASURED_PEAKS.json when present:
+burst peak when the timed region is shorter than a second, else sustained; otherwise the H100 SXM data-sheet figure,
+which a card is not guaranteed to reach); `parity_check` is one extra forward on seeded, scaled inputs after the timed loops, every rank's output and
 top-k checked against the CPU oracle on a sample of its tokens (outside any timed region; a failure exits non-zero);
 `cpu_baseline` is a plain torch CPU forward of the same layer on the host cores (a reported baseline, not a target).
+`--dump-outputs DIR` writes what the timed path returned in its last timed step as float32 .npy files (see
+dump_outputs), so that two builds can be compared output for output on identical seeded inputs.
 `--impl reference` times that CPU implementation as the reference arm: the reference itself has no CPU path and cannot
 be built here (SURVEY.md section 8c), so the oracle port is the stated stand-in.
 """
@@ -84,8 +87,8 @@ def load_peaks():
         p = json.load(open(path))
         return {"bf16_burst": float(p["bf16_tflops"]), "bf16_sustained": float(p.get("bf16_tflops_sustained", p["bf16_tflops"])),
                 "hbm_gbs": float(p["hbm_gbs"]), "source": "measured (MEASURED_PEAKS.json)"}
-    # /opt/skills/guides/B200_PROFILING.md fallback figures
-    return {"bf16_burst": 1590.0, "bf16_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet: dense bf16 989 TFLOP/s, HBM3 3.35 TB/s (at up to 700 W; not a measured figure)
+    return {"bf16_burst": 989.0, "bf16_sustained": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (not measured)"}
 
 
 class ClockSampler:
@@ -357,7 +360,42 @@ def parity_check(env, ctx, cfg, xd, wgd, wed, n_tokens):
             "ok": bool(allr[:, 3].sum() == 0)}
 
 
-def run_config(env, name, steps, warmup, sampler, *, e2e=True, parity_tokens=0, out_in_slab=True):
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def _bf16_bits_to_f32(a):
+    import numpy as np
+
+    return (np.ascontiguousarray(a).view(np.uint16).astype(np.uint32) << 16).view(np.float32)
+
+
+def dump_outputs(dump_dir, ctx, cfg, out, rank, world):
+    """Write what the timed path returned in its last step as float32 .npy files in `dump_dir`: the output activations
+    `out` [S, H] and the routing tables `topk_idx` / `topk_weight` [S, k].  When all ranks' files would exceed
+    DUMP_LIMIT_BYTES, `out` holds a fixed seeded sample of rows, listed in `out_rows`.  At N > 1 every name gets a
+    `_rank<r>` suffix."""
+    import numpy as np
+
+    os.makedirs(dump_dir, exist_ok=True)
+    sfx = "" if world == 1 else f"_rank{rank}"
+    S, H, k = cfg.S, cfg.H, cfg.k
+    tables = {"topk_idx": ctx.read("topk_idx").reshape(S, k).astype(np.float32),
+              "topk_weight": _bf16_bits_to_f32(ctx.read("topk_w")).reshape(S, k)}
+    budget = DUMP_LIMIT_BYTES // world - sum(a.nbytes for a in tables.values()) - S * 8
+    rows = min(S, budget // (H * 4))
+    o = _bf16_bits_to_f32(out.reshape(S, H).view(torch.int16).cpu().numpy())
+    arrays = dict(tables)
+    if rows < S:
+        sample = np.sort(np.random.default_rng(0).choice(S, size=rows, replace=False))
+        arrays["out"] = np.ascontiguousarray(o[sample])
+        arrays["out_rows"] = sample.astype(np.float64)
+    else:
+        arrays["out"] = o
+    for name, a in arrays.items():
+        np.save(os.path.join(dump_dir, f"{name}{sfx}.npy"), a)
+
+
+def run_config(env, name, steps, warmup, sampler, *, e2e=True, parity_tokens=0, out_in_slab=True, dump_dir=None):
     """Measure one configuration; returns a dict with the device-resident and end-to-end numbers."""
     from flashmoe_b200.runtime import MoEContext
 
@@ -385,6 +423,8 @@ def run_config(env, name, steps, warmup, sampler, *, e2e=True, parity_tokens=0, 
     env.barrier()
     t_host1 = time.perf_counter()
     ctx.check()
+    if dump_dir is not None:
+        dump_outputs(dump_dir, ctx, cfg, out, rank, world)
     launches = ctx.launch_count - launches0
     ms = env.max_over_ranks(e0.elapsed_time(e1) / steps)
     windows = [(t_host0, t_host1)]
@@ -399,7 +439,7 @@ def run_config(env, name, steps, warmup, sampler, *, e2e=True, parity_tokens=0, 
         depth = 3
         x_pins = [x.clone().pin_memory() for _ in range(depth)]
         out_pins = [torch.empty_like(x).pin_memory() for _ in range(depth)]
-        e2e_steps = max(6, min(steps, 60))
+        e2e_steps = steps
 
         def run_e2e(n):
             tickets = []
@@ -449,14 +489,14 @@ def derived(res, world, peaks, steps):
     peak = peaks["bf16_burst"] if kind == "burst" else peaks["bf16_sustained"]
     hbm_alg = S * H * 2 * 2 + E * H * 2 + nlx * 2 * H * P * 2 + (rows_total / world) * (2 * H + 2 * P) * 2
     nvl_bytes = 2.0 * (rows_total / world) * (1.0 - 1.0 / world) * H * 2  # per GPU per direction: rows out + outputs back
-    nvl_floor_ms = nvl_bytes / 770e9 * 1e3   # measured peer-copy bandwidth of this pool (B200_PROFILING.md)
+    nvl_floor_ms = nvl_bytes / 450e9 * 1e3   # H100 SXM NVLink, data sheet: 900 GB/s total = 450 GB/s per direction
     flop_floor_ms = flops_rank / (peak * 1e12) * 1e3
     return {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
             "peak_kind": f"{kind} cuBLAS bf16 ({'timed region %.3f s' % timed_s}), {peaks['source']}",
             "frac_of_burst": achieved / peaks["bf16_burst"], "frac_of_sustained": achieved / peaks["bf16_sustained"],
             "algorithmic_flops_per_launch": flops_rank, "algorithmic_hbm_bytes_per_launch": hbm_alg,
             "hbm_frac_of_measured_copy": hbm_alg / (ms * 1e-3) / 1e9 / peaks["hbm_gbs"],
-            "nvlink_bytes_per_dir_per_gpu": nvl_bytes, "nvlink_floor_ms_at_770GBs": nvl_floor_ms,
+            "nvlink_bytes_per_dir_per_gpu": nvl_bytes, "nvlink_floor_ms_at_450GBs": nvl_floor_ms,
             "flop_floor_ms": flop_floor_ms, "frac_of_slower_floor": max(nvl_floor_ms, flop_floor_ms) / ms}
 
 
@@ -475,6 +515,8 @@ def main():
     ap.add_argument("--parity-tokens", type=int, default=int(os.environ.get("FM_BENCH_PARITY_TOKENS", "256")))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs as float32 .npy files into DIR")
     args = ap.parse_args()
     rank, world, local = env_int("RANK", 0), env_int("WORLD_SIZE", 1), env_int("LOCAL_RANK", 0)
     if world != args.gpus:
@@ -483,6 +525,8 @@ def main():
             return 2
         args.gpus = world
     if args.impl == "reference":
+        if args.dump_outputs is not None:   # that arm times a CPU forward of a token sample, not the GPU path's outputs
+            ap.error("--dump-outputs writes the outputs of the GPU path; it does not apply to --impl reference")
         return run_reference_arm(args, rank, world)
     if args.warmup < 3:
         args.warmup = 3
@@ -503,20 +547,11 @@ def main():
 
     name = args.config
     cfg = BASELINE_CONFIGS[name]
-    res = run_config(env, name, args.steps, args.warmup, sampler, e2e=not args.no_e2e, parity_tokens=args.parity_tokens)
+    res = run_config(env, name, args.steps, args.warmup, sampler, e2e=not args.no_e2e, parity_tokens=args.parity_tokens,
+                     dump_dir=args.dump_outputs)
     S, ms = cfg.S, res["ms"]
     roof = derived(res, world, peaks, args.steps)
-    # DRAM traffic per launch comes from a committed `ncu --set full` capture; it describes one configuration at one N only
-    roof["traffic"] = None
-    prof = os.path.join(ROOT, "profiles", "ncu_summary.json")
-    if os.path.exists(prof):
-        try:
-            pj = json.load(open(prof))
-            if pj.get("config", "B") == name and int(pj.get("n_gpus", 1)) == world:
-                roof["traffic"] = pj.get("dram_bytes_per_launch")
-                roof["traffic_source"] = pj.get("source")
-        except Exception:
-            pass
+    roof["traffic"] = None   # DRAM traffic is not measured (no hardware-counter profile in this run)
     cd = config_dict(name, cfg, world)
     line = {
         "metric": "moe_layer_fwd_tokens_per_s", "value": world * S / (ms * 1e-3), "unit": "tokens/s", "n_gpus": world,
@@ -524,7 +559,7 @@ def main():
         "vs_baseline": None, "dtype": "bf16", "data": "synthetic", "config": cd,
         "run": {"token_expert_pairs_executed": res["rows_total"], "output_buffer": res["out_buffer"],
                 "l2": "no explicit flush: the per-step working set (expert weights + activations/staging, >= 250 MB per "
-                      "rank for config B) exceeds the 126 MB L2"},
+                      "rank for config B) exceeds the 50 MB L2 of an H100"},
         "roofline": roof, "gpu_launches": res["launches"], "clocks": res["clocks"], "native_so_mapped": in_tree_native_libs(),
     }
     if "e2e_ms" in res:
@@ -558,7 +593,7 @@ def main():
                 entry = {"config": sname, "workload": CONFIG_DESCRIPTIONS[sname], "tokens_per_s": world * c.S / (r["ms"] * 1e-3),
                          "ms_per_step": r["ms"], "steps": args.sweep_steps, "tflops_per_gpu": rf["achieved"],
                          "frac_of_burst": rf["frac_of_burst"], "frac_of_sustained": rf["frac_of_sustained"],
-                         "nvlink_floor_ms_at_770GBs": rf["nvlink_floor_ms_at_770GBs"], "flop_floor_ms_burst": rf["algorithmic_flops_per_launch"] / (peaks["bf16_burst"] * 1e12) * 1e3,
+                         "nvlink_floor_ms_at_450GBs": rf["nvlink_floor_ms_at_450GBs"], "flop_floor_ms_burst": rf["algorithmic_flops_per_launch"] / (peaks["bf16_burst"] * 1e12) * 1e3,
                          "token_expert_pairs_executed": r["rows_total"], "clocks": r["clocks"]}
                 if "parity" in r:
                     entry["parity_check"] = r["parity"]

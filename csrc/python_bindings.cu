@@ -178,7 +178,7 @@ int get_num_local_experts() {
 }
 
 PYBIND11_MODULE(_C, m) {
-    m.doc() = "FlashMoE (B200): fused distributed MoE forward in a single sm_100a kernel";
+    m.doc() = "FlashMoE (H100): fused distributed MoE forward in a single sm_90a kernel";
     m.def("moe_forward", &moe_forward, "MoE forward pass. Tensors must match compiled config dimensions.",
           py::arg("input"), py::arg("gate_weights"), py::arg("expert_weights"));
     m.def("initialize", &initialize, "Create this process's context for the compiled configuration and map the peers");

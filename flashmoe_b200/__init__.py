@@ -1,4 +1,4 @@
-"""flashmoe_b200 -- Blackwell (sm_100a) native fused distributed-MoE forward, drop-in for the hot path of
+"""flashmoe_b200 -- Hopper (sm_90a) native fused distributed-MoE forward, drop-in for the hot path of
 osayamenja/FlashMoE (`flashmoe.run_moe`, `flashmoe.ops`, `flashmoe._C`).
 
     import flashmoe_b200 as flashmoe      # or `import flashmoe` (shim package re-exporting this one)

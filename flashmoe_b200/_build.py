@@ -1,9 +1,9 @@
-"""In-tree build of the native library: csrc/flashmoe_config.json -> -DFM_CFG_* -> nvcc (sm_100a) ->
+"""In-tree build of the native library: csrc/flashmoe_config.json -> -DFM_CFG_* -> nvcc (sm_90a) ->
 flashmoe_b200/libflashmoe_b200.so.
 
 Replaces the reference's setup.py / CMake JSON->macro plumbing (reference setup.py:227-292, csrc/CMakeLists.txt:114-237):
 no network downloads, reads the file the reference's CMake reads (csrc/flashmoe_config.json, not the dangling
-kleos_config.json), emits sm_100a only.  The .so is git-ignored but travels to the GPU box with the snapshot.
+kleos_config.json), emits sm_90a only.  The .so is a build product (git-ignored); build() writes it into the package.
 """
 from __future__ import annotations
 
@@ -37,7 +37,7 @@ def ext_path() -> Path:
 
 
 NVCC_FLAGS = [
-    "-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "--compiler-options", "-fPIC,-fvisibility=hidden", "-shared",
 ]
 
@@ -63,7 +63,7 @@ def _fingerprint(cfg: _config.MoEConfig) -> str:
 
 
 def build(config_path: Optional[os.PathLike] = None, force: bool = False, verbose: bool = False) -> Path:
-    """Compile the library for sm_100a with the given (default: csrc/flashmoe_config.json) config baked in."""
+    """Compile the library for sm_90a with the given (default: csrc/flashmoe_config.json) config baked in."""
     cfg = _config.load_config(config_path)
     cfg.check_hot_path()
     fp = _fingerprint(cfg)
@@ -105,7 +105,7 @@ def build_bindings(force: bool = False, verbose: bool = False) -> Path:
         return out
     if not LIB_PATH.exists():
         raise RuntimeError("build libflashmoe_b200.so first")
-    cmd = [find_nvcc(), "-std=c++17", "-O2", "-x", "cu", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    cmd = [find_nvcc(), "-std=c++17", "-O2", "-x", "cu", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
            "--compiler-options", "-fPIC,-fvisibility=hidden", "-shared",
            f"-I{pybind11.get_include()}", f"-I{sysconfig.get_paths()['include']}", f"-I{REPO_ROOT / 'include'}",
            "-o", str(out), str(BINDINGS_SRC), f"-L{PKG_DIR}", "-lflashmoe_b200",

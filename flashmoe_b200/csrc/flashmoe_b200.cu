@@ -1,4 +1,4 @@
-// flashmoe_b200.cu -- host runtime + C-ABI (include/flashmoe_b200.h) around the fused sm_100a kernel.
+// flashmoe_b200.cu -- host runtime + C-ABI (include/flashmoe_b200.h) around the fused sm_90a kernel.
 //
 // Replaces the used slice of the reference's host runtime: bootstrap.cuh:278-512 (symmetric heap + bookkeeping
 // allocation, peer pointer tables), moe.cuh:146-205 (launch) and python_bindings.cu:17-151 (argument checks) --
@@ -76,7 +76,7 @@ EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
-// 2-D row-major bf16 tensor [rows, cols], tile box [box_rows, 64 cols], 128-byte swizzle (matches the UMMA smem
+// 2-D row-major bf16 tensor [rows, cols], tile box [box_rows, 64 cols], 128-byte swizzle (matches the wgmma smem
 // descriptors built in fm_ptx.cuh), out-of-bounds elements read as zero.
 int make_tmap(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
     EncodeTiledFn fn = get_encode_fn();
@@ -103,11 +103,10 @@ struct fm_ctx {
     int grid = 0;
     int tpc = 0;
     int TN0 = 0, TN1 = 0, num_pkts = 0, num_blocks = 0, total_items = 0;
-    int bn0 = 256, bn1 = 256, claim_ahead_kb = 16;
+    int claim_ahead_kb = 16;
     int dbg_flags = 0;
     bool coop = true;    // cooperative launch attribute (validates co-residency of the persistent grid)
     int prefetch_kb = 0;
-    bool pair = false;   // cta_group::2: two CTAs (one cluster) per 256-row tile
     uint32_t epoch = 0;
     unsigned long long bar_count = 0;
     // in-kernel waits give up after this long (fm_set_timeout_ms): generous by default so that ordinary rank skew (a peer
@@ -145,11 +144,9 @@ struct fm_ctx {
     bool dense = false;   // E == 1: GEMM0 reads x in place, no router GEMV, no dispatch copy (reference fffn.cuh:31-167)
     float* aux = nullptr; // is_training: [2][2E+1] {gML, gMeC, loss} by epoch parity
     const void* cached_x = nullptr;
-    int* recv_tok = nullptr;            // [nLx, pEC] slot -> token of the local packets (TMA gather4 source rows)
+    int* recv_tok = nullptr;            // [nLx, pEC] slot -> token of the local packets (gather-mode source rows)
     unsigned int* tok_rows = nullptr;   // [2, nLx, TCM]
-    bool gather = false;
-    const void* cached_xg = nullptr;
-    CUtensorMap tm_xg;
+    int gather = 0;                     // FM_GATHER: 0 off, 1 early tiles only, 2 every local GEMM0 tile (tests)
     bool tc_gate = false;               // router logits on the tensor cores (E <= 256)
     const void* cached_gx = nullptr;
     const void* cached_gw = nullptr;
@@ -237,8 +234,8 @@ void set_peer_pointers(const fm_ctx* c, fm::FmParams& p) {
 
 int check_kernel_status(fm_ctx* c) {
     if (c->dbg_host != nullptr && c->dbg_host->code != 0) {
-        static const char* names[] = {"none", "smem-full mbarrier", "smem-empty mbarrier", "tmem-full mbarrier",
-                                      "tmem-empty mbarrier", "sched-full mbarrier", "sched-empty mbarrier",
+        static const char* names[] = {"none", "smem-full mbarrier", "smem-empty mbarrier", "(unused)",
+                                      "(unused)", "sched-full mbarrier", "sched-empty mbarrier",
                                       "grid barrier", "dispatch flag (packet never arrived)", "GEMM0 row-block counter",
                                       "return flag (expert output never arrived)",
                                       "dispatch row acknowledgement (rows of a packet never arrived)", "publisher mbarrier"};
@@ -277,21 +274,17 @@ int launch(fm_ctx* c, const void* x, const void* gate_w, const void* expert_w, c
     }
     if (c->tc_gate) {
         // router on tensor cores: x as [S, H] in 32-row boxes, Wg_eff = the [H, E] tensor read flat as [E, H]
-        // (python_bindings.cu:93-99, moe.cuh:107-109) in boxes of E_pad rows (a CTA pair stages half each); rows past E
-        // read as zero
+        // (python_bindings.cu:93-99, moe.cuh:107-109) in boxes of min(128, E rounded up to 64) rows; rows past E read as
+        // zero
         if (c->cached_gx != x) {
             if ((rc = make_tmap(&c->tm_gx, x, (uint64_t)d.S, d.H, 32))) return rc;
             c->cached_gx = x;
         }
         if (c->cached_gw != gate_w) {
-            const uint32_t e_pad = (uint32_t)((d.E + 15) / 16 * 16);
-            if ((rc = make_tmap(&c->tm_gw, gate_w, (uint64_t)d.E, d.H, c->pair ? e_pad / 2 : e_pad))) return rc;
+            const uint32_t e64 = (uint32_t)((d.E + 63) / 64 * 64);
+            if ((rc = make_tmap(&c->tm_gw, gate_w, (uint64_t)d.E, d.H, std::min(128u, e64)))) return rc;
             c->cached_gw = gate_w;
         }
-    }
-    if (c->gather && c->cached_xg != x) {   // x as [S, H] with a {64, 1} box: rows are picked one by one (TMA gather4)
-        if ((rc = make_tmap(&c->tm_xg, x, (uint64_t)d.S, d.H, 1))) return rc;
-        c->cached_xg = x;
     }
     if (!c->tm_static_ready) {
         if (!c->dense && (rc = make_tmap(&c->tm_a0, static_cast<char*>(c->symm) + c->off_recv_x, (uint64_t)c->num_pkts * d.pEC, d.H,
@@ -305,23 +298,20 @@ int launch(fm_ctx* c, const void* x, const void* gate_w, const void* expert_w, c
         // (python_bindings.cu:104-119).  One tensor map per GEMM over the whole tensor with a per-expert row stride
         // of 2*P (resp. 2*H) rows is not expressible in 2-D, so rows are addressed as [nLx*2*P, H] / [nLx*2*H, P]:
         // expert i's W_up starts at row i*2*P, its W_down at row (i*2+1)*H of the [.,P] view.
-        // in pair mode each CTA of the pair stages half of the B tile's rows
-        const uint32_t bdiv = c->pair ? 2u : 1u;
-        if ((rc = make_tmap(&c->tm_b0, expert_w, (uint64_t)nLx * 2 * d.P, d.H, (uint32_t)c->bn0 / bdiv))) return rc;
-        if ((rc = make_tmap(&c->tm_b1, expert_w, (uint64_t)nLx * 2 * d.H, d.P, (uint32_t)c->bn1 / bdiv))) return rc;
+        if ((rc = make_tmap(&c->tm_b0, expert_w, (uint64_t)nLx * 2 * d.P, d.H, fm::BLOCK_N))) return rc;
+        if ((rc = make_tmap(&c->tm_b1, expert_w, (uint64_t)nLx * 2 * d.H, d.P, fm::BLOCK_N))) return rc;
         c->cached_expert_w = expert_w;
     }
     fm::FmParams p;
     memset(&p, 0, sizeof(p));
     p.tm_a0 = c->tm_a0; p.tm_b0 = c->tm_b0; p.tm_a1 = c->tm_a1; p.tm_b1 = c->tm_b1;
-    if (c->gather) p.tm_xg = c->tm_xg;
     if (c->tc_gate) { p.tm_gx = c->tm_gx; p.tm_gw = c->tm_gw; }
     p.tc_gate = c->tc_gate ? 1 : 0;
     p.S = d.S; p.H = d.H; p.P = d.P; p.E = d.E; p.k = d.k; p.W = d.world; p.rank = d.rank; p.nLx = nLx;
     p.EC = d.EC; p.pEC = d.pEC; p.TCM = d.TCM; p.act = c->cfg.hidden_act;
     p.TN0 = c->TN0; p.TN1 = c->TN1; p.tpc = c->tpc; p.num_pkts = c->num_pkts; p.num_blocks = c->num_blocks;
     p.total_items = c->total_items;
-    p.bn[0] = c->bn0; p.bn[1] = c->bn1; p.claim_ahead_kb = c->claim_ahead_kb; p.dbg_flags = c->dbg_flags; p.prefetch_kb = c->prefetch_kb;
+    p.claim_ahead_kb = c->claim_ahead_kb; p.dbg_flags = c->dbg_flags; p.prefetch_kb = c->prefetch_kb;
     // the epoch and the grid-barrier target advance only when the launch has been accepted (see below): a failed launch
     // must not leave the host ahead of the device counter and of the peers
     const uint32_t epoch = c->epoch + ((phase_mask & 1u) ? 1u : 0u);
@@ -357,7 +347,7 @@ int launch(fm_ctx* c, const void* x, const void* gate_w, const void* expert_w, c
     if (d.world == 1) p.peer_out_acc[0] = p.out;
     p.aux = c->aux;
     p.dense = c->dense ? 1 : 0;
-    p.gather = c->gather ? 1 : 0;
+    p.gather = c->gather;
     p.recv_tok = c->recv_tok;
     p.tok_rows = c->tok_rows;
     p.dbg = c->dbg_dev;
@@ -368,24 +358,16 @@ int launch(fm_ctx* c, const void* x, const void* gate_w, const void* expert_w, c
     lc.blockDim = dim3(fm::NUM_THREADS);
     lc.dynamicSmemBytes = (size_t)fm::SMEM_BYTES;
     lc.stream = stream;
-    cudaLaunchAttribute attrs[2];
+    cudaLaunchAttribute attrs[1];
     int na = 0;
     if (c->coop) {
         attrs[na].id = cudaLaunchAttributeCooperative;   // all CTAs co-resident: in-kernel spin waits + grid barrier
         attrs[na].val.cooperative = 1;
         ++na;
     }
-    if (c->pair) {
-        attrs[na].id = cudaLaunchAttributeClusterDimension;
-        attrs[na].val.clusterDim.x = 2;
-        attrs[na].val.clusterDim.y = 1;
-        attrs[na].val.clusterDim.z = 1;
-        ++na;
-    }
     lc.attrs = attrs;
     lc.numAttrs = na;
-    if (c->pair) FM_CUDA(cudaLaunchKernelEx(&lc, fm::fm_moe_forward_kernel<true>, p));
-    else FM_CUDA(cudaLaunchKernelEx(&lc, fm::fm_moe_forward_kernel<false>, p));
+    FM_CUDA(cudaLaunchKernelEx(&lc, fm::fm_moe_forward_kernel, p));
     c->epoch = epoch;
     c->bar_count = bar_count;
     c->launches += 1;
@@ -398,7 +380,7 @@ int launch(fm_ctx* c, const void* x, const void* gate_w, const void* expert_w, c
 extern "C" {
 
 FM_API const char* fm_last_error(void) { return g_err.c_str(); }
-FM_API const char* fm_version(void) { return "flashmoe_b200 0.1.0 (sm_100a, tcgen05/TMEM/TMA)"; }
+FM_API const char* fm_version(void) { return "flashmoe_b200 0.1.0 (sm_90a, wgmma/TMA)"; }
 
 FM_API int fm_compiled_config(fm_config_t* out) {
     if (out == nullptr) return fail(FM_EINVAL, "null output");
@@ -439,8 +421,8 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
     FM_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     FM_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
-        return fail(FM_ECUDA, "device %d is sm_%d%d; this library contains sm_100a code only (tcgen05/TMEM/TMA)", device,
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(FM_ECUDA, "device %d is sm_%d%d; this library contains sm_90a code only (wgmma/TMA)", device,
                     prop.major, prop.minor);
     int coop = 0;
     FM_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
@@ -449,12 +431,10 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
     d.smem_bytes = fm::SMEM_BYTES;
     d.grid = prop.multiProcessorCount;
 
-    FM_CUDA(cudaFuncSetAttribute(reinterpret_cast<const void*>(&fm::fm_moe_forward_kernel<false>),
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, fm::SMEM_BYTES));
-    FM_CUDA(cudaFuncSetAttribute(reinterpret_cast<const void*>(&fm::fm_moe_forward_kernel<true>),
+    FM_CUDA(cudaFuncSetAttribute(reinterpret_cast<const void*>(&fm::fm_moe_forward_kernel),
                                  cudaFuncAttributeMaxDynamicSharedMemorySize, fm::SMEM_BYTES));
     int occ = 0;
-    FM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fm::fm_moe_forward_kernel<false>, fm::NUM_THREADS,
+    FM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fm::fm_moe_forward_kernel, fm::NUM_THREADS,
                                                           (size_t)fm::SMEM_BYTES));
     if (occ < 1) return fail(FM_ECUDA, "kernel does not fit on an SM (smem %d B)", fm::SMEM_BYTES);
 
@@ -462,31 +442,28 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
     ctx->cfg = c;
     ctx->d = d;
     ctx->device = device;
-    // tuning knobs (tile widths of the two GEMMs, scheduler look-ahead); environment overrides are for experiments
+    // tuning knobs (scheduler look-ahead, work order); environment overrides are for experiments
     auto env_int = [](const char* name, int dflt) {
         const char* v = getenv(name);
         return (v != nullptr && *v) ? atoi(v) : dflt;
     };
     ctx->grid = d.num_sms;  // one persistent CTA per SM; all co-resident (spin waits + grid barrier)
     {
-        const char* v = getenv("FM_PAIR");
-        ctx->pair = (v != nullptr && *v) ? atoi(v) != 0 : true;   // default: CTA pairs (measured +9 % on config B)
         // fused GEMM1 -> combine (REDG into the token's output row): only for k <= 2, where bf16 accumulation is
         // order-independent (0 + a exact, a + b commutative) and therefore bit-identical to the deterministic gather;
         // k > 2 keeps the gather so results do not depend on arrival order
         const char* f = getenv("FM_FUSED_COMBINE");
         ctx->fused = ((f != nullptr && *f) ? atoi(f) != 0 : true) && d.k <= 2;
         ctx->dense = d.E == 1 && world == 1 && env_int("FM_DENSE_E1", 1) != 0;
-        // router logits by tcgen05.mma instead of the CUDA-core GEMV (2*S*H*E flops: 4.3 GFLOP per rank at E = 128,
-        // d_model 2048, 8192 tokens -- ~0.2 ms on the CUDA cores); one accumulator holds <= 256 experts
-        // Default: from 17 experts up.  Measured on one B200: E = 128, d_model 2048, 56 tokens per CTA: router 29 us instead
-        // of 433 us; E = 8, d_model 1024, 28 tokens per CTA (config B): a wash (the GEMV is latency-, not flop-bound there).
+        // router logits by wgmma instead of the CUDA-core GEMV (2*S*H*E flops: 4.3 GFLOP per rank at E = 128,
+        // d_model 2048, 8192 tokens); up to 256 experts, 128 per pass over d_model.  Default: from 17 experts up (at a
+        // handful of experts the GEMV is latency-, not flop-bound).
         ctx->tc_gate = !ctx->dense && d.E <= 256 && env_int("FM_TC_GATE", d.E > 16 ? 1 : 0) != 0;
-        // TMA gather4 of local rows for tiles claimed before their copies landed: correct, but off by default -- measured on
-        // config B a gather tile takes 24 us instead of 6.6 (32 gather4 operations per k-block per CTA sustain only about
-        // one per 90 clocks), which costs far more than the ~5 us earlier start buys (160 vs 144 us per forward)
-        ctx->gather = !ctx->dense && env_int("FM_GATHER", 0) != 0;
-        if (ctx->pair && (ctx->grid & 1)) ctx->grid -= 1;  // CTA pairs need an even grid
+        // gather of local rows straight from x (by token index, in the producer warp) for tiles claimed before their row
+        // copies landed: correct, but off by default -- a gather tile loads its A operand through one warp's registers
+        // instead of the TMA engine, which costs more than the earlier start buys.  FM_GATHER=2 gathers every local
+        // GEMM0 tile (deterministic coverage of that path)
+        ctx->gather = ctx->dense ? 0 : std::min(2, std::max(0, env_int("FM_GATHER", 0)));
         ctx->d.grid = ctx->grid;
     }
     ctx->tpc = ceil_div(d.S, ctx->grid);
@@ -495,72 +472,31 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
         return fail(FM_EINVAL, "tokens-per-CTA * k = %d exceeds the router scratch (%d)", ctx->tpc * d.k, fm::G_SEL_MAX);
     }
     const int nLx = d.num_local_experts;
-    ctx->bn0 = env_int("FM_BN0", 256) == 128 ? 128 : 256;
-    ctx->bn1 = env_int("FM_BN1", 256) == 128 ? 128 : 256;
-    ctx->claim_ahead_kb = env_int("FM_CLAIM_AHEAD_KB", 16);   // measured on config B: 8 -> 144.5 us, 12 -> 142.3, 14 -> 140.6
+    ctx->claim_ahead_kb = env_int("FM_CLAIM_AHEAD_KB", 16);
     ctx->dbg_flags = env_int("FM_DBG_FLAGS", 0);
     // The persistent grid spins on flags, counters and one grid barrier, so every CTA must be resident: the launch is
     // cooperative (the driver then refuses to start it unless the whole grid fits, also next to other work on the GPU).
-    // One exception: Nsight Compute cannot replay a cooperative launch that also has cluster dimensions (the driver
-    // reports LaunchFailed), so under a CUDA injection profiler -- or with FM_COOP=0 -- the attribute is dropped and
-    // co-residency rests on the cudaOccupancyMaxActiveClusters check below plus exclusive use of the GPU.
-    const bool under_profiler = getenv("CUDA_INJECTION64_PATH") != nullptr || getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR") != nullptr ||
-                                getenv("NSIGHT_CUDA_DEBUGGER") != nullptr;
-    ctx->coop = env_int("FM_COOP", (ctx->pair && under_profiler) ? 0 : 1) != 0;
-    if (ctx->pair) {
-        cudaLaunchConfig_t oc = {};
-        oc.gridDim = dim3(ctx->grid);
-        oc.blockDim = dim3(fm::NUM_THREADS);
-        oc.dynamicSmemBytes = (size_t)fm::SMEM_BYTES;
-        cudaLaunchAttribute oa[1];
-        oa[0].id = cudaLaunchAttributeClusterDimension;
-        oa[0].val.clusterDim.x = 2; oa[0].val.clusterDim.y = 1; oa[0].val.clusterDim.z = 1;
-        oc.attrs = oa;
-        oc.numAttrs = 1;
-        int max_clusters = 0;
-        cudaError_t oe = cudaOccupancyMaxActiveClusters(&max_clusters, fm::fm_moe_forward_kernel<true>, &oc);
-        if (oe != cudaSuccess || max_clusters * 2 < ctx->grid) {
-            const int got = max_clusters;
-            delete ctx;
-            return fail(FM_ECUDA, "the persistent grid of %d CTA pairs cannot be co-resident (max active clusters %d, %s)",
-                        d.num_sms / 2, got, cudaGetErrorString(oe));
-        }
-    }
+    ctx->coop = env_int("FM_COOP", 1) != 0;
     ctx->prefetch_kb = env_int("FM_PREFETCH_KB", 0);
     if (ctx->prefetch_kb < 0) ctx->prefetch_kb = 0;
     if (ctx->claim_ahead_kb < 0) ctx->claim_ahead_kb = 0;
-    ctx->TN0 = ceil_div(d.P, ctx->bn0);
-    ctx->TN1 = ceil_div(d.H, ctx->bn1);
+    ctx->TN0 = ceil_div(d.P, fm::BLOCK_N);
+    ctx->TN1 = ceil_div(d.H, fm::BLOCK_N);
     ctx->num_pkts = world * nLx;
 
     // Work list.  Sources in the order own rank, rank+1, ... (local rows need no NVLink hop, so they are ready first).
-    // With CTA pairs a work item is a 256-row tile made of two 128-row halves that share the B operand (same local expert):
-    //   * world even: halves = the SAME row block of the packets of two different source ranks ("cross-source pairing":
-    //     no half is wasted when a packet has an odd number of row blocks -- with 128 experts on 8 GPUs every packet
-    //     has exactly one);
-    //   * otherwise:  halves = two consecutive row blocks of one packet.
-    // All GEMM0 blocks first, then the GEMM1 blocks (measured best on config B; FM_G1_LAG interleaves them with a lag).
-    // Cross-source pairing only pays when a packet has an ODD number of row blocks (otherwise pairing inside the packet
-    // wastes nothing and keeps the local packets -- whose rows are ready first -- free of any remote dependency).
-    const bool xpair = ctx->pair && world >= 2 && (world % 2) == 0 && (d.TCM % 2) == 1 && env_int("FM_XPAIR", 1) != 0;
-    struct Unit { int pkt, pkt2; bool local; };
+    // A work item is one 128 x 128 output tile of one packet.
+    struct Unit { int pkt; bool local; };
     std::vector<Unit> units;
-    if (xpair) {
-        for (int j = 0; j < world; j += 2)
-            for (int le = 0; le < nLx; ++le)
-                units.push_back({((rank + j) % world) * nLx + le, ((rank + j + 1) % world) * nLx + le, j == 0});
-    } else {
-        for (int j = 0; j < world; ++j)
-            for (int le = 0; le < nLx; ++le) units.push_back({((rank + j) % world) * nLx + le, -1, j == 0});
-    }
+    for (int j = 0; j < world; ++j)
+        for (int le = 0; le < nLx; ++le) units.push_back({((rank + j) % world) * nLx + le, j == 0});
     std::vector<fm::TileBlock> blocks;
     int start = 0;
     auto push = [&](int kind, const Unit& u) {
         fm::TileBlock b;
-        b.kind = kind; b.pkt = u.pkt; b.start = start; b.pkt2 = u.pkt2;
+        b.kind = kind; b.pkt = u.pkt; b.start = start; b.pad = 0;
         blocks.push_back(b);
-        const int row_items = (ctx->pair && u.pkt2 < 0) ? (d.TCM + 1) / 2 : d.TCM;
-        start += row_items * (kind == 0 ? ctx->TN0 : ctx->TN1);
+        start += d.TCM * (kind == 0 ? ctx->TN0 : ctx->TN1);
     };
     // GEMM0: local sources first (their rows are acknowledged first), then rank+1, rank+2, ...  GEMM1: REMOTE sources
     // first, local last -- the outputs of remote packets cross NVLink as reductions and their done flags have a link round
@@ -570,13 +506,13 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
     for (const Unit& u : units) if (!u.local) g1_units.push_back(u);
     for (const Unit& u : units) if (u.local) g1_units.push_back(u);
     // FM_G1_LAG: -1 (default) = the orders described here; n >= 1 = GEMM1 of a unit n units after its GEMM0.
-    //   one rank:    all GEMM0, then all GEMM1 (measured best on config B);
+    //   one rank:    all GEMM0, then all GEMM1;
     //   two ranks:   GEMM0 local, GEMM0 remote, GEMM1 remote, GEMM1 local (the remote rows land while the local packets
     //                run; the local adds, which nobody else waits for, come last);
     //   four+ ranks: GEMM0 local, GEMM1 local, then the remote units with GEMM1 one unit behind GEMM0 -- the local
-    //                packets are the only work available until the remote rows have crossed NVLink (~50 us at 8 GPUs),
-    //                and starting the remote units' GEMM1 early spreads the return traffic (reductions over NVLink at
-    //                ~350 GB/s per GPU, which would otherwise pile up behind the last tiles) over the whole phase.
+    //                packets are the only work available until the remote rows have crossed NVLink, and starting the
+    //                remote units' GEMM1 early spreads the return traffic (reductions over NVLink, which would otherwise
+    //                pile up behind the last tiles) over the whole phase.
     const int lag = env_int("FM_G1_LAG", -1);
     if (lag >= 1 && lag < (int)units.size()) {
         for (size_t i = 0; i < units.size(); ++i) {
@@ -589,8 +525,8 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
         for (const Unit& u : units) (u.local ? loc : rem).push_back(u);
         for (const Unit& u : loc) push(0, u);
         for (const Unit& u : loc) push(1, u);
-        // remote units grouped by source rank (nLx units per source, or per source pair): GEMM1 one source behind GEMM0
-        const size_t per_src = xpair ? (size_t)nLx : (size_t)nLx;
+        // remote units grouped by source rank (nLx units per source): GEMM1 one source behind GEMM0
+        const size_t per_src = (size_t)nLx;
         for (size_t g0 = 0; g0 < rem.size(); g0 += per_src) {
             for (size_t i = g0; i < std::min(g0 + per_src, rem.size()); ++i) push(0, rem[i]);
             if (g0 >= per_src)
@@ -604,7 +540,7 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
     ctx->num_blocks = (int)blocks.size();
     ctx->total_items = start;
     fm::TileBlock sentinel;
-    sentinel.kind = -1; sentinel.pkt = 0; sentinel.start = start; sentinel.pkt2 = -1;
+    sentinel.kind = -1; sentinel.pkt = 0; sentinel.start = start; sentinel.pad = 0;
     blocks.push_back(sentinel);
 
 #define FM_TRY(expr)          \

@@ -1,29 +1,28 @@
-// fm_kernel.cuh -- the fused persistent MoE-forward kernel for sm_100a.
+// fm_kernel.cuh -- the fused persistent MoE-forward kernel for sm_90a.
 //
 // One launch = one MoE layer forward on this rank (reference: flashmoe::moe::forward, csrc/include/flashmoe/moe/moe.cuh:77-144):
 //
-//   prologue  mbarriers + TMEM allocation for the later phases (off the critical path)
+//   prologue  mbarriers for the later phases (off the critical path)
 //   phase G   router    x.Wg^T -> online softmax -> top-k -> capacity slots         (reference moe/gate.cuh:473-720)
 //             grid barrier (the only one, like the reference's gate.cuh:761)
 //   phase D   dispatch  token rows -> owner rank's receive buffer over NVLink (TMA bulk copies) + one flag per expert
 //                                                                                    (reference os/packet.cuh:21-286)
-//   phase F   expert FFN  persistent tcgen05 tile loop over CTA pairs: GEMM0(+bias+act) -> h, GEMM1(+bias) -> for k <= 2
+//   phase F   expert FFN  persistent wgmma tile loop: GEMM0(+bias+act) -> h, GEMM1(+bias) -> for k <= 2
 //             scaled and ADDED straight into the token's output row on the source rank (REDG.BF16x8 over peer memory),
 //             otherwise stored to the source rank's return buffer + per-row-block flag
 //                                                                                    (reference os/processor/processor.cuh:340-468,
 //                                                                                    685-750; the OS CTA of os/os.cuh, scheduler.cuh,
 //                                                                                    subscriber.cuh is replaced by an atomic tile
-//                                                                                    claim + flag waits in one warp per CTA pair)
+//                                                                                    claim + flag waits in one warp per CTA)
 //   phase C   completion: wait for the experts' done flags (fused path) or gather-combine the k returned rows per token
 //                                                                                    (reference processor.cuh:27-205)
 //
-// CTA = 384 threads, one CTA per SM, all co-resident (74 clusters of 2; cooperative launch, and co-residency is checked on
-// the host with cudaOccupancyMaxActiveClusters).  After the grid barrier the warps specialise: warp 0 = TMA producer,
-// warp 1 = tcgen05.mma issuer (leader CTA of the pair), warp 3 = tile scheduler (leader CTA), warps 2 and 4-11 = dispatch,
-// then warps 4-11 = epilogue (TMEM -> registers -> bias/activation/combine scaling -> bf16 -> swizzled smem transpose ->
-// 16-byte global / peer stores or adds; two warps per TMEM lane quarter, each draining half of the tile's columns) and
-// warp 2 = publisher (the release fence + counter / flag traffic of every finished tile, off the epilogue warps' critical
-// path); warp 2 also owns the TMEM allocation.
+// CTA = 384 threads, one CTA per SM, all co-resident (cooperative launch).  After the grid barrier the warps specialise:
+// warp 0 = TMA producer, warp 3 = tile scheduler, warps 2 and 4-11 = dispatch, then warps 4-11 = two consumer warpgroups
+// (wgmma into register accumulators, warpgroup g owns rows [64g, 64g + 64) of the 128 x 128 tile, then the epilogue:
+// bias/activation/combine scaling -> bf16 -> swizzled smem transpose -> 16-byte global / peer stores or adds) and
+// warp 2 = publisher (the release fence + counter / flag traffic of every finished tile, off the consumer warps'
+// critical path).  Warp 1 has no role in phase F.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -36,58 +35,51 @@
 namespace fm {
 
 constexpr int BLOCK_M = 128;   // token rows per tile (= reference BLOCK_M)
-constexpr int BLOCK_N = 256;   // max output columns per tile (one tcgen05.mma N); per-GEMM width is p.bn[kind]
+constexpr int BLOCK_N = 128;   // output columns per tile: 64 fp32 accumulators per consumer thread
 constexpr int BLOCK_K = 64;    // 64 bf16 = 128 B = one swizzle row
-constexpr int UMMA_K = 16;
+constexpr int WGMMA_K = 16;
 constexpr int NSCHED = 4;
 constexpr int NUM_THREADS = 384;
 constexpr int NUM_WARPS = NUM_THREADS / 32;
-constexpr int EPI_WARP0 = 4;   // warps 4..11: warp % 4 selects the TMEM lane quarter, (warp - 4) / 4 the column half
+constexpr int EPI_WARP0 = 4;   // warps 4..11: warpgroup (warp - 4) / 4 owns tile rows [64g, 64g + 64), warp % 4 its 16-row slice
 constexpr int NUM_EPI_WARPS = 8;
-constexpr int TMEM_COLS = 512; // two 128x256 fp32 accumulators per CTA (double-buffered against the epilogue)
 constexpr int TRACE_SLOTS = 128; // per CTA: [0..6] phase stamps, [8..14] sub-phase stamps (13 = first tile of a remote packet
-                                 // ready, 14 = all done flags seen); per tile i < 16 of this CTA (pair):
+                                 // ready, 14 = all done flags seen); per tile i < 16 of this CTA:
                                  // [16+i] dependencies resolved (scheduler), [32+i] first k-block landed, [48+i] last MMA
-                                 // issued (MMA thread), [64+i] accumulator complete (epilogue sees tmem_full), [80+i]
-                                 // epilogue stores issued, [96+i] published, [112+i] claimed (scheduler)
+                                 // complete (consumers), [64+i] epilogue started, [80+i] epilogue stores issued,
+                                 // [96+i] published, [112+i] claimed (scheduler)
 
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;                  // 16 KiB
-constexpr int PIPE_BYTES = 196608;                                    // 4 x 48 KiB (solo) = 6 x 32 KiB (CTA pair)
-constexpr int MAX_STAGES = 6;
+constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;                  // 16 KiB
+constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+constexpr int STAGES = 6;
+constexpr int PIPE_BYTES = STAGES * STAGE_BYTES;                      // 192 KiB
 constexpr int EPI_ROW_BYTES = 128;                                    // 64 bf16; 16-byte pieces XOR-swizzled by (row & 7)
 constexpr int EPI_WARP_BYTES = 32 * EPI_ROW_BYTES;                    // 4 KiB per epilogue warp
 constexpr int OFF_EPI = PIPE_BYTES;                                   // 196608
 constexpr int OFF_BARS = OFF_EPI + NUM_EPI_WARPS * EPI_WARP_BYTES;    // 229376
-// barriers: full[6] empty[6] tmem_full[2] tmem_empty[2] sched_full[4] sched_empty[4] prod_take[4] xrows disp_done
-//           pub_full[2] pub_empty[2]
-constexpr int BAR_FULL = 0, BAR_EMPTY = MAX_STAGES, BAR_TMEM_FULL = 2 * MAX_STAGES, BAR_TMEM_EMPTY = BAR_TMEM_FULL + 2;
-constexpr int BAR_SCHED_FULL = BAR_TMEM_EMPTY + 2, BAR_SCHED_EMPTY = BAR_SCHED_FULL + NSCHED;
+// barriers: full[6] empty[6] sched_full[4] sched_empty[4] prod_take[4] xrows disp_done pub_full[2] pub_empty[2] wg remote
+//           gfull[8] gempty[8]
+constexpr int BAR_FULL = 0, BAR_EMPTY = STAGES;
+constexpr int BAR_SCHED_FULL = 2 * STAGES, BAR_SCHED_EMPTY = BAR_SCHED_FULL + NSCHED;
 constexpr int BAR_PROD_TAKE = BAR_SCHED_EMPTY + NSCHED;
 constexpr int BAR_XROWS = BAR_PROD_TAKE + NSCHED;                     // dispatch phase: bulk row load
 constexpr int BAR_DISP_DONE = BAR_XROWS + 1;                          // this CTA's dispatch no longer uses the stage area
-constexpr int BAR_PUB_FULL = BAR_DISP_DONE + 1;                       // epilogue warps -> publisher: tile's stores issued
-constexpr int BAR_PUB_EMPTY = BAR_PUB_FULL + 2;                       // publisher -> epilogue warps: slot consumed
+constexpr int BAR_PUB_FULL = BAR_DISP_DONE + 1;                       // consumer warps -> publisher: tile's stores issued
+constexpr int BAR_PUB_EMPTY = BAR_PUB_FULL + 2;                       // publisher -> consumer warps: slot consumed
 constexpr int BAR_WG = BAR_PUB_EMPTY + 2;                             // router: bulk-staged gate weights
 constexpr int BAR_REMOTE = BAR_WG + 1;                                // dispatch, warp 2: staged rows for other ranks
 constexpr int GATE_STAGES = 8;                                        // router GEMM on tensor cores: up to 8 smem stages
-constexpr int BAR_GFULL = BAR_REMOTE + 1;                             // full / empty per stage, accumulator complete
+constexpr int BAR_GFULL = BAR_REMOTE + 1;                             // full / empty per stage
 constexpr int BAR_GEMPTY = BAR_GFULL + GATE_STAGES;
-constexpr int BAR_GACC = BAR_GEMPTY + GATE_STAGES;
-constexpr int NUM_BARS = BAR_GACC + 2;                                // 54 (one spare keeps the ring 16-byte aligned)
+constexpr int NUM_BARS = BAR_GEMPTY + GATE_STAGES;                    // 48
 constexpr int OFF_RING = OFF_BARS + NUM_BARS * 8;                     // 16-byte aligned
-constexpr int OFF_TMEM_PTR = OFF_RING + NSCHED * 64;
-constexpr int OFF_MISC = OFF_TMEM_PTR + 16;
-constexpr int SMEM_USED = OFF_MISC + 64;
+constexpr int SMEM_USED = OFF_RING + NSCHED * 64;
 constexpr int SMEM_BYTES = SMEM_USED + 1024;                          // + slack for manual 1 KiB alignment
-static_assert(OFF_RING % 16 == 0, "ring entries are copied with 16-byte accesses");
+static_assert(OFF_RING % 16 == 0, "ring entries are 16-byte aligned");
 static_assert(SMEM_BYTES <= 232448, "227 KiB of dynamic shared memory per CTA");
-
-template <bool PAIR>
-struct PipeCfg {   // solo: one CTA per 128x256 tile; pair: two CTAs share one 256x256 tile (cta_group::2)
-    static constexpr int STAGES = PAIR ? 6 : 4;
-    static constexpr int B_ROWS_DIV = PAIR ? 2 : 1;                   // each CTA of a pair stages half of the B rows
-    static constexpr int STAGE_BYTES = PIPE_BYTES / STAGES;           // 32 KiB / 48 KiB
-};
+// named barriers (bar.sync ids): 2-7 dispatch / staging hand-over (see dispatch_phase), 8 the router's consumer warpgroups
+constexpr int NAMED_BAR_GATE_MMA = 8;
 
 // gate-phase aliases of the (not yet used) pipeline stage area
 constexpr int G_OFF_WG = 0;              // bf16 [EG][Hc]           <= 64 KiB
@@ -104,27 +96,23 @@ struct TileBlock {  // one contiguous run of work items: all tiles of one GEMM o
     int kind;       // 0 = GEMM0 (x.W_up^T), 1 = GEMM1 (h.W_down^T)
     int pkt;        // local packet index = src * nLx + le
     int start;      // first global item id of this block
-    int pkt2;       // CTA pairs: -1 = the pair's second 128-row half is the NEXT row block of `pkt`; >= 0 = it is the SAME
-                    // row block of packet pkt2 (same local expert, another source rank) -- see the host's work list
+    int pad;
 };
 
 struct FmParams {
     CUtensorMap tm_a0;  // recv_x  as [W*nLx*pEC, H]  box {64, 128}
-    CUtensorMap tm_b0;  // expert_weights as [nLx*2*P, H]  box {64, 256}  (W_up rows)
+    CUtensorMap tm_b0;  // expert_weights as [nLx*2*P, H]  box {64, 128}  (W_up rows)
     CUtensorMap tm_a1;  // hidden  as [W*nLx*pEC, P]  box {64, 128}
-    CUtensorMap tm_b1;  // expert_weights as [nLx*2*H, P]  box {64, 256}  (W_down rows)
-    CUtensorMap tm_xg;  // x as [S, H], box {64, 1}: TMA gather4 of token rows for local packets (no dispatch copy needed)
+    CUtensorMap tm_b1;  // expert_weights as [nLx*2*H, P]  box {64, 128}  (W_down rows)
     CUtensorMap tm_gx;  // router on tensor cores: x as [S, H], box {64, 32}
-    CUtensorMap tm_gw;  // router on tensor cores: Wg_eff [E, H], box {64, E_pad} (CTA pair: {64, E_pad / 2})
-    int tc_gate;        // 1 = logits by tcgen05.mma (E <= 256); 0 = register-blocked CUDA-core GEMV
+    CUtensorMap tm_gw;  // router on tensor cores: Wg_eff [E, H], box {64, min(128, E rounded up to 64)}
+    int tc_gate;        // 1 = logits by wgmma (E <= 256); 0 = register-blocked CUDA-core GEMV
     int S, H, P, E, k, W, rank, nLx, EC, pEC, TCM, act;
     int TN0, TN1, tpc, num_pkts, num_blocks, total_items;
-    int bn[2];          // tile width of GEMM0 / GEMM1 (128 or 256)
     int claim_ahead_kb; // the scheduler claims the next tile when this many k-blocks of the current one remain
     int prefetch_kb;    // L2 prefetch distance of the TMA producer in k-blocks (0 = off)
     int dbg_flags;      // experiments only (results are garbage for bits 0-3): bit0 = skip all TMA loads, bit1 = skip MMA
-                        // issue, bit2 = skip the A loads, bit3 = skip the B loads, bit4 = partner CTA's producer also
-                        // arrives on the leader's `full` barrier (the round-1 handshake), bit5 = ignore BAR_DISP_DONE
+                        // issue, bit2 = skip the A loads, bit3 = skip the B loads, bit5 = ignore BAR_DISP_DONE
     unsigned int epoch, phase_mask;
     unsigned long long bar_target, timeout_ns;
     const __nv_bfloat16 *x, *wg, *b_up, *b_down;
@@ -167,10 +155,10 @@ struct FmParams {
     // training mode (is_training = 1): [2][2E+1] f32 by epoch parity = {gML[E] mean gate probability per expert,
     // gMeC[E] mean routed fraction per expert, loss} (reference moe/gate.cuh:608-635,698-706,763-773); nullptr otherwise
     // local packets (source = this rank): token of every slot, acknowledged BEFORE the row copies, so a GEMM0 tile
-    // claimed early can gather its A rows straight from x (TMA gather4) instead of waiting for the copies to land
+    // claimed early can gather its A rows straight from x instead of waiting for the copies to land
     int* recv_tok;             // [nLx, pEC] (local packets only, indexed by local expert)
     unsigned int* tok_rows;    // [2, nLx, TCM] rows of block b whose token entry is written, by epoch parity
-    int gather;                // 0 = off
+    int gather;                // 0 = off, 1 = when a tile's rows have not landed yet, 2 = every local GEMM0 tile
     float* aux;
     int dense;          // E == 1: no router GEMV, no dispatch copy; GEMM0 reads x in place (reference moe/fffn.cuh:31-167)
     DebugRecord* dbg;
@@ -225,97 +213,103 @@ __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
 //   interleaving of the reference's BlockScan + atomicAdd(eC) order, gate.cuh:678-718).
 // ============================================================================================================
 // Router logits on the tensor cores (E <= 256): logits[t, e] = sum_h x[t,h] * Wg_eff[e,h] for one sub-chunk of <= 128 tokens
-// of this CTA as ONE tcgen05.mma accumulator: A = the tokens' x rows (TMA, 32-row boxes straight from x), B = Wg_eff padded
-// to a multiple of 16 experts (TMA; rows past E read as zero), D = [128 tokens x E_pad] fp32 in TMEM columns [0, E_pad).
-// A CTA pair runs it as cta_group::2 (M = 256: each CTA's own tokens; each CTA stages half of the Wg rows), because all
-// tcgen05 instructions of a kernel must use one cta_group; the two CTAs therefore walk the sub-chunks in lock-step.
-// Two smem stages in the router's weight scratch (one when E_pad > 128).  Afterwards warps 0-3 copy the accumulator to
-// the logits scratch (thread = token row), where the softmax / top-k code finds it exactly like after the GEMV.
+// of this CTA with wgmma: A = the tokens' x rows (TMA, 32-row boxes straight from x), B = Wg_eff in groups of
+// GB = min(128, E rounded up to 64) rows (TMA; rows past E read as zero).  Warp 0 loads; the two consumer warpgroups
+// (warps 4-11; warpgroup g = token rows [64g, 64g + 64), idle when the sub-chunk has none there) multiply into a GB-column
+// register accumulator and write the logits straight into the logits scratch, where the softmax / top-k code finds them
+// exactly like after the GEMV.  E > 128 takes one pass over H per group of 128 experts; the stages then stay clear of the
+// logits scratch, which the earlier pass has already filled.
 // The reference computes the same product with mma.sync tiles padded to 64 experts (gate.cuh:526-535); fp32 accumulation
 // order differs between the two (and from the oracle's), which is what the oracle's ambiguity flags are for.
-struct GateTcState { int gkb; uint32_t accphase; };
-template <bool PAIR>
-__device__ __forceinline__ void gate_logits_tc(const FmParams& p, uint8_t* smem, int t0, int s0, int n_sub, int rows_span,
-                                               int rows_cap, uint32_t crank, uint32_t tmem_base, float* logit_s, int ldl,
-                                               GateTcState& st) {
+struct GateTcState { int gkb; };
+__device__ __forceinline__ void gate_logits_tc(const FmParams& p, uint8_t* smem, int t0, int s0, int n_sub, int rows_cap,
+                                               float* logit_s, int ldl, GateTcState& st) {
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BARS);
     uint64_t* gfull = bars + BAR_GFULL;
     uint64_t* gempty = bars + BAR_GEMPTY;
-    uint64_t* gacc = bars + BAR_GACC;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int E = p.E, E_pad = (E + 15) & ~15;
-    const int b_rows = PAIR ? E_pad / 2 : E_pad;                 // Wg_eff rows this CTA stages
-    const int b_bytes = b_rows * BLOCK_K * 2;
+    const int E = p.E, E64 = (E + 63) & ~63;
+    const int GB = min(128, E64);                                // Wg_eff rows per pass (the tensor map's box height)
+    const int npass = (E64 + GB - 1) / GB;                      // 1, or 2 for 129 <= E <= 256
+    const int b_bytes = GB * BLOCK_K * 2;
     const int nk = p.H / BLOCK_K;
-    const int nb32 = (rows_span + 31) / 32;                      // 32-row boxes of x per k-block (same in both CTAs of a pair)
-    const int a_bytes = nb32 * 32 * BLOCK_K * 2;                 // x rows actually staged; the MMA reads 128 rows from the stage
-                                                                 // base -- rows beyond a_bytes are whatever follows (their
-                                                                 // accumulator rows are never read)
-    const uint32_t tx_cta = (uint32_t)(a_bytes + b_bytes);
-    // stages live in the router's weight + logits scratch (the logits are written only after the last MMA of the
-    // sub-chunk has completed); compact stride = what a FULL sub-chunk stages, so a 28-token chunk with 8 experts gets 8
-    // stages of 5 KB.  The layout (stride, stage count, offset of the Wg rows) is the same for every sub-chunk of the
-    // launch -- the stage / phase arithmetic runs across sub-chunks -- only the number of x boxes loaded follows rows_span
-    // (the last sub-chunk of a CTA is usually shorter).
-    const int a_cap = ((rows_cap + 31) / 32) * 32 * BLOCK_K * 2;
+    const int nb32 = (n_sub + 31) / 32;                          // 32-row boxes of x per k-block
+    const uint32_t tx = (uint32_t)(nb32 * 32 * BLOCK_K * 2 + b_bytes);
+    // Stages live in the router's weight + logits scratch; compact stride = what a FULL sub-chunk stages (x rows rounded
+    // up to a warpgroup's 64), so a 28-token chunk with 64 experts gets 5 stages of 24 KB.  The layout (stride, stage
+    // count, offset of the Wg rows) is the same for every sub-chunk of the launch -- the stage / phase arithmetic runs
+    // across sub-chunks -- only the number of x boxes loaded follows the sub-chunk's row count.
+    const int a_cap = ((rows_cap + 63) / 64) * 64 * BLOCK_K * 2;
     const int stage_bytes = (a_cap + b_bytes + 1023) & ~1023;
-    const int NS = max(1, min(GATE_STAGES, (G_WG_BYTES + G_LOGIT_BYTES - (A_STAGE_BYTES - a_cap)) / stage_bytes));
-    if (warp == 0 && lane == 0) {          // TMA issuer of this CTA
-        for (int kb = 0; kb < nk; ++kb) {
-            const int g = st.gkb + kb, s = g % NS;
-            const uint32_t ph = (uint32_t)(g / NS) & 1u;
-            mbar_wait(&gempty[s], ph ^ 1u, p.dbg, p.timeout_ns, FM_TRAP_MBAR_EMPTY, 910 + s);
-            uint8_t* sa = smem + G_OFF_WG + s * stage_bytes;
-            if (PAIR) {
-                if (crank == 0) mbar_arrive_expect_tx(&gfull[s], 2u * tx_cta);
-                const uint32_t leader_full = mapa_shared(smem_u32(&gfull[s]), 0);
-                for (int j = 0; j < nb32; ++j)
-                    tma_load_2d_pair(sa + j * 4096, &p.tm_gx, kb * BLOCK_K, t0 + s0 + j * 32, leader_full);
-                tma_load_2d_pair(sa + a_cap, &p.tm_gw, kb * BLOCK_K, (int)crank * b_rows, leader_full);
-            } else {
-                mbar_arrive_expect_tx(&gfull[s], tx_cta);
+    const int region = npass > 1 ? G_WG_BYTES : G_WG_BYTES + G_LOGIT_BYTES;
+    const int NS = max(1, min(GATE_STAGES, region / stage_bytes));
+    for (int pass = 0; pass < npass; ++pass) {
+        const int e0 = pass * GB;
+        if (warp == 0 && lane == 0) {          // TMA issuer
+            fence_proxy_async_smem();          // earlier generic accesses of the scratch (logits, softmax) -> TMA writes
+            for (int kb = 0; kb < nk; ++kb) {
+                const int g = st.gkb + kb, s = g % NS;
+                const uint32_t ph = (uint32_t)(g / NS) & 1u;
+                mbar_wait(&gempty[s], ph ^ 1u, p.dbg, p.timeout_ns, FM_TRAP_MBAR_EMPTY, 910 + s);
+                uint8_t* sa = smem + G_OFF_WG + s * stage_bytes;
+                mbar_arrive_expect_tx(&gfull[s], tx);
                 for (int j = 0; j < nb32; ++j) tma_load_2d(sa + j * 4096, &p.tm_gx, kb * BLOCK_K, t0 + s0 + j * 32, &gfull[s]);
-                tma_load_2d(sa + a_cap, &p.tm_gw, kb * BLOCK_K, 0, &gfull[s]);
+                tma_load_2d(sa + a_cap, &p.tm_gw, kb * BLOCK_K, e0, &gfull[s]);
             }
-        }
-    } else if (warp == 1 && lane == 0 && crank == 0) {   // MMA issuer (leader CTA)
-        const uint32_t idesc = umma_idesc_bf16_f32(PAIR ? 2 * BLOCK_M : BLOCK_M, (uint32_t)E_pad);
-        for (int kb = 0; kb < nk; ++kb) {
-            const int g = st.gkb + kb, s = g % NS;
-            const uint32_t ph = (uint32_t)(g / NS) & 1u;
-            mbar_wait(&gfull[s], ph, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 910 + s);
-            tcgen05_fence_after();
-            const uint32_t sa = smem_u32(smem + G_OFF_WG + s * stage_bytes);
-            const uint64_t da = umma_smem_desc_sw128(sa);
-            const uint64_t db = umma_smem_desc_sw128(sa + a_cap);
+        } else if (warp >= EPI_WARP0) {        // consumer warpgroups
+            const int wg = (warp - EPI_WARP0) >> 2;
+            const bool active = wg * 64 < n_sub;   // warpgroup-uniform
+            // one accumulator of 64 or 128 expert columns (the m64n64 fragment is the first half of the m64n128 one)
+            float acc[64];
 #pragma unroll
-            for (int kk = 0; kk < BLOCK_K / UMMA_K; ++kk) {
-                if (PAIR) umma_bf16_ss_pair(tmem_base, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc, (kb | kk) != 0 ? 1u : 0u);
-                else umma_bf16_ss(tmem_base, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc, (kb | kk) != 0 ? 1u : 0u);
-            }
-            if (PAIR) umma_commit_pair(&gempty[s]); else umma_commit(&gempty[s]);
-        }
-        if (PAIR) umma_commit_pair(gacc); else umma_commit(gacc);
-    }
-    st.gkb += nk;
-    // accumulator complete (in a pair the commit is multicast to both CTAs' barriers)
-    mbar_wait(gacc, st.accphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_TMEM_FULL, 911);
-    st.accphase ^= 1u;
-    tcgen05_fence_after();
-    if (warp < 4) {   // TMEM lanes [32w, 32w+32) = token rows; 16 columns (experts) per load
-        const int row = warp * 32 + lane;
-        for (int c0 = 0; c0 < E_pad; c0 += 16) {
-            uint32_t v[16];
-            tmem_ld_32x32b_x16(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-            tmem_ld_wait();
-            if (row < n_sub) {
+            for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+            for (int kb = 0; kb < nk; ++kb) {
+                const int g = st.gkb + kb, s = g % NS;
+                const uint32_t ph = (uint32_t)(g / NS) & 1u;
+                mbar_wait(&gfull[s], ph, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 910 + s);
+                if (active) {
+                    const uint32_t sa = smem_u32(smem + G_OFF_WG + s * stage_bytes);
+                    const uint64_t da = gmma_smem_desc_sw128(sa + wg * 64 * 128);
+                    const uint64_t db = gmma_smem_desc_sw128(sa + a_cap);
+                    wgmma_fence_regs(acc);   // the accumulator's register writes stay ahead of the fence
+                    wgmma_fence();
+                    if (GB > 64) {
 #pragma unroll
-                for (int i = 0; i < 16; ++i)
-                    if (c0 + i < E) logit_s[row * ldl + c0 + i] = __uint_as_float(v[i]);
+                        for (int kk = 0; kk < BLOCK_K / WGMMA_K; ++kk)
+                            wgmma_m64n128k16_bf16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2));
+                    } else {
+#pragma unroll
+                        for (int kk = 0; kk < BLOCK_K / WGMMA_K; ++kk)
+                            wgmma_m64n64k16_bf16(reinterpret_cast<float(&)[32]>(acc), da + (uint64_t)(kk * 2),
+                                                 db + (uint64_t)(kk * 2));
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_regs(acc);
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&gempty[s]);
+            }
+            // both warpgroups are done reading the stages (which may overlap the logits scratch)
+            asm volatile("bar.sync %0, 256;" ::"n"(NAMED_BAR_GATE_MMA) : "memory");
+            if (active) {
+                const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), cq = (lane & 3) * 2;
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    if (j * 8 >= GB) break;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = r0 + 8 * h, col = e0 + j * 8 + cq;
+                        if (row < n_sub) {
+                            if (col < E) logit_s[row * ldl + col] = acc[j * 4 + 2 * h];
+                            if (col + 1 < E) logit_s[row * ldl + col + 1] = acc[j * 4 + 2 * h + 1];
+                        }
+                    }
+                }
             }
         }
+        st.gkb += nk;
     }
-    tcgen05_fence_before();
 }
 
 // E == 1 (reference: the dense fffn kernel is selected instead of the MoE kernel, moe.cuh:174-177): every token goes to
@@ -340,8 +334,7 @@ __device__ __forceinline__ void gate_phase_dense(const FmParams& p, int t0, int 
     }
 }
 
-template <bool PAIR>
-__device__ __forceinline__ void gate_phase(const FmParams& p, uint8_t* smem, int t0, int n_tok, uint32_t crank) {
+__device__ __forceinline__ void gate_phase(const FmParams& p, uint8_t* smem, int t0, int n_tok) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int E = p.E, H = p.H, k = p.k;
     __nv_bfloat16* wg_s = reinterpret_cast<__nv_bfloat16*>(smem + G_OFF_WG);
@@ -361,32 +354,17 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, uint8_t* smem, int
     const int ldl = E + 1;                                  // padded logits row (bank spread for thread-per-row)
     int TS = G_LOGIT_BYTES / (ldl * 4);                     // tokens per sub-chunk
     const bool tc = p.tc_gate != 0;
-    if (tc) TS = min(TS, BLOCK_M);                          // one tcgen05 accumulator = 128 token rows
+    if (tc) TS = min(TS, BLOCK_M);                          // two wgmma warpgroups = 128 token rows
     else if (TS > n_tok) TS = n_tok;
-    // tensor-core logits: the two CTAs of a pair issue one cta_group::2 MMA per sub-chunk together, so both walk the same
-    // number of sub-chunks (tpc tokens) even if this CTA owns fewer tokens
-    const int span = tc ? p.tpc : n_tok;
     GateTcState tcs;
-    tcs.gkb = 0; tcs.accphase = 0u;
-    uint32_t tmem_base = 0;
-    if (tc) {
-        // TMEM was allocated in the prologue by warp 2; in a pair the partner's barriers and TMEM must exist before the
-        // first remote completion / multicast commit (the grid barrier, which used to order that, comes later)
-        tcgen05_fence_before();
-        if (PAIR) cluster_sync_all(); else __syncthreads();
-        tcgen05_fence_after();
-        tmem_base = *reinterpret_cast<volatile uint32_t*>(smem + OFF_TMEM_PTR);
-    }
+    tcs.gkb = 0;
+    if (tc) __syncthreads();   // the router's stage barriers (initialised in the prologue) are visible to every warp
 
-    for (int s0 = 0; s0 < span; s0 += TS) {
-        const int n_sub = max(0, min(TS, n_tok - s0));
+    for (int s0 = 0; s0 < n_tok; s0 += TS) {
+        const int n_sub = min(TS, n_tok - s0);
         if (tc) {
-            if (s0 > 0) {   // the accumulator columns and the logits scratch are reused: everybody is done with the previous ones
-                tcgen05_fence_before();
-                if (PAIR) cluster_sync_all(); else __syncthreads();
-                tcgen05_fence_after();
-            }
-            gate_logits_tc<PAIR>(p, smem, t0, s0, n_sub, min(TS, p.tpc - s0), min(TS, p.tpc), crank, tmem_base, logit_s, ldl, tcs);
+            if (s0 > 0) __syncthreads();   // the logits scratch is reused: everybody is done with the previous sub-chunk
+            gate_logits_tc(p, smem, t0, s0, n_sub, min(TS, p.tpc), logit_s, ldl, tcs);
         } else {
         for (int i = tid; i < n_sub * ldl; i += NUM_THREADS) logit_s[i] = 0.0f;
         for (int eg0 = 0; eg0 < E; eg0 += EG) {
@@ -833,7 +811,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
         }
     }
     // Local packets first get their token table (slot -> token) and an acknowledgement of it: a GEMM0 tile claimed before
-    // the row copies below have landed gathers its rows from x by these indices (ffn_producer, TMA gather4).
+    // the row copies below have landed gathers its rows from x by these indices (ffn_producer).
     const unsigned int par = p.epoch & 1u;
     if (p.gather) {
         const int first_local = p.rank * p.nLx;
@@ -1051,188 +1029,145 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
 }
 
 // ============================================================================================================
-// Phase F: expert FFN.  Work items (global order, claimed with one atomic counter by the pair's scheduler warp):
+// Phase F: expert FFN.  Work items (global order, claimed with one atomic counter by the scheduler warp):
 //   packets in the order (own rank first, then rank+1, ...); all GEMM0 blocks, then the GEMM1 blocks (host knob FM_G1_LAG
-//   interleaves them with a lag instead).  item -> (row-block pair m fastest, column tile n).  The item list is a static
+//   interleaves them with a lag instead).  item -> (row block m fastest, column tile n).  The item list is a static
 //   superset: row blocks beyond the packet's row count are skipped once the packet flag is known.  A GEMM1 tile waits for
-//   g0_done[pkt][m] == TN0 (both row blocks of the pair).
+//   g0_done[pkt][m] == TN0.
 // ============================================================================================================
-struct TileInfo {     // 64 bytes, written by the (leader's) scheduler warp, read by producer / MMA / epilogue / publisher warps.
-                      // Per-half fields are indexed by the CTA's rank in the pair (solo CTAs use index 0).
+struct TileInfo {     // written by the scheduler warp, read by the producer / consumer / publisher warps
     int kind;         // 0 GEMM0, 1 GEMM1, -1 stop
     int ntile;
-    int le;           // local expert (both halves share it: same B operand)
-    int b_row;        // TMA row coordinate of the B tile (rank 1 of a pair: + bn/2)
-    int gather[2];    // GEMM0, local packet: 1 = this half's A rows are gathered from x (its row copies had not landed yet)
-    int pkt[2];       // local packet index src * nLx + le of each half
-    int mblk[2];      // 128-row block of that packet
-    int rows[2];      // valid rows of that block (0 = this half is idle)
-    int src[2];       // source rank of the packet
-    int cnt[2];       // rows of the whole packet
+    int le;           // local expert
+    int b_row;        // TMA row coordinate of the B tile
+    int gather;       // GEMM0, local packet: 1 = the A rows are gathered from x (their row copies had not landed yet)
+    int pkt;          // local packet index src * nLx + le
+    int mblk;         // 128-row block of that packet
+    int rows;         // valid rows of that block
+    int src;          // source rank of the packet
+    int cnt;          // rows of the whole packet
+    int pad[2];
 };
-static_assert(sizeof(TileInfo) == 64, "TileInfo must be 4 x 16 bytes");
+static_assert(sizeof(TileInfo) <= 64, "a ring slot is 64 bytes");
 
-template <bool PAIR>
-__device__ __forceinline__ void wait_sched_full(const FmParams& p, uint64_t* bar, uint32_t parity, unsigned int info) {
-    if (PAIR) mbar_wait_cluster(bar, parity, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, info);  // data came over DSMEM
-    else mbar_wait(bar, parity, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, info);
-}
-// consumers of a ring slot release it on the LEADER's barrier (the scheduler lives there)
-template <bool PAIR>
-__device__ __forceinline__ void release_to_leader(uint64_t* bar, uint32_t crank) {
-    if (PAIR && crank != 0) mbar_arrive_cluster_plain(bar, 0);
-    else mbar_arrive(bar);
-}
-
-// warp 3 (leader CTA in pair mode): claims work items and resolves their dependencies AHEAD of the TMA producer, so the
-// atomic, the packet-flag and the h-row-block-counter round trips overlap the previous tile's loads (the job of the
-// reference's OS CTA: subscriber decode + scheduler doorbells, os/subscriber.cuh, os/scheduler.cuh -- here one warp, no queues).
-template <bool PAIR>
+// warp 3, lane 0: claims work items and resolves their dependencies AHEAD of the TMA producer, so the atomic, the
+// packet-flag and the h-row-block-counter round trips overlap the previous tile's loads (the job of the reference's OS
+// CTA: subscriber decode + scheduler doorbells, os/subscriber.cuh, os/scheduler.cuh -- here one thread, no queues).
 __device__ __forceinline__ void ffn_scheduler(const FmParams& p, uint8_t* smem, uint64_t* bars) {
     uint64_t* sched_full = bars + BAR_SCHED_FULL;
     uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
     uint64_t* prod_take = bars + BAR_PROD_TAKE;
     TileInfo* ring = reinterpret_cast<TileInfo*>(smem + OFF_RING);
-    const int lane = threadIdx.x & 31;
-    const int nh = PAIR ? 2 : 1;                            // 128-row halves per work item
     int q = 0, qphase = 0, cursor = 0, n = 0;
     bool seen_remote = false;   // trace only: first tile of a packet from another rank
     for (;;) {
-        if (lane == 0 && n >= 1) {  // bounded look-ahead: wait until the producer is close to finishing tile n-1
+        if (n >= 1) {  // bounded look-ahead: wait until the producer is close to finishing tile n-1
             const int pq = (q + NSCHED - 1) % NSCHED;
             mbar_wait(&prod_take[pq], ((n - 1) / NSCHED) & 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_EMPTY, 200 + pq);
         }
-        __syncwarp();
-        // The whole warp walks the claim loop in lock-step; lane h resolves the dependencies of half h of the item (the
-        // two halves' flag / counter round trips overlap), lane 0 assembles and publishes the descriptor.
-        int kind = -1, nt = 0, le = 0;
-        int h_pkt = 0, h_mb = 0, h_src = 0, h_rows = 0, h_cnt = 0, h_gather = 0;
+        TileInfo ti;
+        ti.kind = -1; ti.ntile = 0; ti.le = 0; ti.b_row = 0; ti.gather = 0; ti.pkt = 0; ti.mblk = 0; ti.rows = 0;
+        ti.src = 0; ti.cnt = 0; ti.pad[0] = ti.pad[1] = 0;
         for (;;) {
-            int id = 0;
-            if (lane == 0) id = (int)atomicAdd(p.claim, 1u);
-            id = __shfl_sync(0xffffffffu, id, 0);
+            const int id = (int)atomicAdd(p.claim, 1u);
             if (id >= p.total_items) break;
-            if (lane == 0 && n < 16) trace_stamp(p, 112 + n);   // claim time of tile n (ready time is slot 16+n)
+            if (n < 16) trace_stamp(p, 112 + n);   // claim time of tile n (ready time is slot 16+n)
             while (id >= p.blocks[cursor + 1].start) ++cursor;
             const TileBlock blk = p.blocks[cursor];
             const int local = id - blk.start;
-            // item -> (row block(s), column tile); row blocks fastest.  Within-packet pairing: halves = row blocks
-            // 2m, 2m+1 of one packet.  Cross-source pairing (pkt2 >= 0): halves = row block m of two packets.
-            const bool cross = PAIR && blk.pkt2 >= 0;
-            const int m_items = (PAIR && !cross) ? (p.TCM + 1) / 2 : p.TCM;
-            const int m = local % m_items;
-            nt = local / m_items;
-            le = blk.pkt % p.nLx;
-            const int h = lane;
-            h_pkt = (h == 1 && cross) ? blk.pkt2 : blk.pkt;
-            h_mb = cross ? m : (PAIR ? 2 * m + (h & 1) : m);
-            h_src = h_pkt / p.nLx;
-            h_rows = 0; h_cnt = 0; h_gather = 0;
-            if (h < nh && h_mb < p.TCM) {
-                const bool same_gpu = h_src == p.rank;   // flag and counters written from this GPU: gpu scope suffices
-                // wait for the packet (src, le): flag = {epoch, rows}  (reference subscriber.cuh:52-185)
-                unsigned long long f = ((unsigned long long)p.epoch << 32) | (unsigned int)p.S;   // dense: all S rows, in x
-                bool stale = false;
-                if (!p.dense) {
-                    SpinGuard g;
-                    for (;;) {
-                        f = same_gpu ? ld_acquire_gpu_u64(p.recv_flag + h_pkt) : ld_acquire_sys_u64(p.recv_flag + h_pkt);
-                        const int ahead = (int)((unsigned int)(f >> 32) - p.epoch);
-                        if (ahead == 0) break;
-                        // The source rank is already in a LATER forward: it only gets there after every real tile of
-                        // this packet has been returned to it, so whatever item of the static superset is left here
-                        // is an empty row block.
-                        if (ahead > 0) { stale = true; break; }
-                        g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_FLAG, h_pkt, (unsigned int)(f >> 32), p.epoch);
-                    }
-                }
-                if (!stale) {
-                    h_cnt = (int)(f & 0xffffffffull);
-                    if (h == 0 || cross) {   // once per packet and GEMM (its first item): bookkeeping that needs the count
-                        if (local == 0 && blk.kind == 0 && !p.dense) p.recv_cnt[h_pkt] = h_cnt;
-                        if (p.fused && local == 0 && blk.kind == 1 && h_cnt == 0)   // nothing to contribute: tell the source now
-                            st_release_sys_u64(p.peer_done_flag[h_src] + (size_t)(p.rank * p.nLx + le),
-                                               (unsigned long long)p.epoch << 32);
-                    }
-                    h_rows = max(0, min(BLOCK_M, h_cnt - h_mb * BLOCK_M));
-                }
-                if (h_rows > 0) {
-                    SpinGuard g;
-                    const unsigned int* rctr = p.recv_rows + ((size_t)(p.epoch & 1u) * p.num_pkts + h_pkt) * p.TCM + h_mb;
-                    if (blk.kind == 1) {  // GEMM1 needs the whole h row block (reference notifyNext, processor.cuh:490-615)
-                        const unsigned int* ctr = p.g0_done + (size_t)h_pkt * p.TCM + h_mb;
-                        while (ld_acquire_gpu_u32(ctr) < (unsigned int)p.TN0)
-                            g.tick(p.dbg, p.timeout_ns, FM_TRAP_G0_DONE, h_pkt, h_mb, 0);
-                        if (p.gather && p.fused && same_gpu && (p.phase_mask & 1u)) {
-                            // the block's GEMM0 tiles may all have run in gather mode, i.e. before its row copies and
-                            // routing records landed: the combine epilogue reads those records, so order behind their ack
-                            while (ld_acquire_gpu_u32(rctr) < (unsigned int)h_rows)
-                                g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_ROWS, h_pkt, h_mb, h_rows);
-                        }
-                    } else if ((p.phase_mask & 1u) && !p.dense) {  // GEMM0 needs the rows of this block to have landed (dispatch acks)
-                        // local packet: the token table of the block is acknowledged before its row copies -- if it is
-                        // complete while the rows are not, the producer gathers the rows from x itself (FM_GATHER=1)
-                        const unsigned int* tctr = (p.gather && same_gpu)
-                            ? p.tok_rows + ((size_t)(p.epoch & 1u) * p.nLx + le) * p.TCM + h_mb : nullptr;
-                        for (;;) {
-                            const unsigned int got = same_gpu ? ld_acquire_gpu_u32(rctr) : ld_acquire_sys_u32(rctr);
-                            if (got >= (unsigned int)h_rows) break;
-                            if (tctr != nullptr && ld_acquire_gpu_u32(tctr) >= (unsigned int)h_rows) { h_gather = 1; break; }
-                            g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_ROWS, h_pkt, h_mb, h_rows);
-                        }
-                    }
+            const int mb = local % p.TCM, nt = local / p.TCM;   // row blocks fastest
+            const int pkt = blk.pkt, le = pkt % p.nLx, src = pkt / p.nLx;
+            const bool same_gpu = src == p.rank;   // flag and counters written from this GPU: gpu scope suffices
+            // wait for the packet (src, le): flag = {epoch, rows}  (reference subscriber.cuh:52-185)
+            unsigned long long f = ((unsigned long long)p.epoch << 32) | (unsigned int)p.S;   // dense: all S rows, in x
+            bool stale = false;
+            if (!p.dense) {
+                SpinGuard g;
+                for (;;) {
+                    f = same_gpu ? ld_acquire_gpu_u64(p.recv_flag + pkt) : ld_acquire_sys_u64(p.recv_flag + pkt);
+                    const int ahead = (int)((unsigned int)(f >> 32) - p.epoch);
+                    if (ahead == 0) break;
+                    // The source rank is already in a LATER forward: it only gets there after every real tile of
+                    // this packet has been returned to it, so whatever item of the static superset is left here
+                    // is an empty row block.
+                    if (ahead > 0) { stale = true; break; }
+                    g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_FLAG, pkt, (unsigned int)(f >> 32), p.epoch);
                 }
             }
-            __syncwarp();
-            const bool any = __any_sync(0xffffffffu, h_rows > 0 && lane < nh);
-            if (!any) continue;   // every half is an empty row block of the static superset
-            kind = blk.kind;
+            if (stale) continue;
+            const int cnt = (int)(f & 0xffffffffull);
+            // once per packet and GEMM (its first item): bookkeeping that needs the count
+            if (local == 0 && blk.kind == 0 && !p.dense) p.recv_cnt[pkt] = cnt;
+            if (p.fused && local == 0 && blk.kind == 1 && cnt == 0)   // nothing to contribute: tell the source now
+                st_release_sys_u64(p.peer_done_flag[src] + (size_t)(p.rank * p.nLx + le), (unsigned long long)p.epoch << 32);
+            const int rows = max(0, min(BLOCK_M, cnt - mb * BLOCK_M));
+            if (rows == 0) continue;   // an empty row block of the static superset
+            int gather = 0;
+            SpinGuard g;
+            const unsigned int* rctr = p.recv_rows + ((size_t)(p.epoch & 1u) * p.num_pkts + pkt) * p.TCM + mb;
+            if (blk.kind == 1) {  // GEMM1 needs the whole h row block (reference notifyNext, processor.cuh:490-615)
+                const unsigned int* ctr = p.g0_done + (size_t)pkt * p.TCM + mb;
+                while (ld_acquire_gpu_u32(ctr) < (unsigned int)p.TN0) g.tick(p.dbg, p.timeout_ns, FM_TRAP_G0_DONE, pkt, mb, 0);
+                if (p.gather && p.fused && same_gpu && (p.phase_mask & 1u)) {
+                    // the block's GEMM0 tiles may all have run in gather mode, i.e. before its row copies and routing
+                    // records landed: the combine epilogue reads those records, so order behind their ack
+                    while (ld_acquire_gpu_u32(rctr) < (unsigned int)rows)
+                        g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_ROWS, pkt, mb, rows);
+                }
+            } else if ((p.phase_mask & 1u) && !p.dense) {  // GEMM0 needs the rows of this block to have landed (dispatch acks)
+                // local packet: the token table of the block is acknowledged before its row copies -- if it is complete
+                // while the rows are not, the producer gathers the rows from x itself (FM_GATHER=1); FM_GATHER=2 gathers
+                // every local GEMM0 tile, so the gather path runs whatever the timing
+                const unsigned int* tctr = (p.gather && same_gpu)
+                    ? p.tok_rows + ((size_t)(p.epoch & 1u) * p.nLx + le) * p.TCM + mb : nullptr;
+                for (;;) {
+                    if (p.gather != 2 || tctr == nullptr) {
+                        const unsigned int got = same_gpu ? ld_acquire_gpu_u32(rctr) : ld_acquire_sys_u32(rctr);
+                        if (got >= (unsigned int)rows) break;
+                    }
+                    if (tctr != nullptr && ld_acquire_gpu_u32(tctr) >= (unsigned int)rows) { gather = 1; break; }
+                    g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_ROWS, pkt, mb, rows);
+                }
+            }
+            ti.kind = blk.kind; ti.ntile = nt; ti.le = le; ti.gather = gather; ti.pkt = pkt; ti.mblk = mb; ti.rows = rows;
+            ti.src = src; ti.cnt = cnt;
+            // expert_weights [nLx,2,P,H]: W_up(le) starts at row le*2*P of the [.,H] view; W_down(le) (the [P,H]
+            // block flat-viewed as [H,P]) starts at row (le*2+1)*H of the [.,P] view.
+            ti.b_row = (blk.kind == 0 ? le * 2 * p.P : (le * 2 + 1) * p.H) + nt * BLOCK_N;
             break;
         }
-        // lane 0 collects both halves
-        TileInfo ti;
-        ti.kind = kind; ti.ntile = nt; ti.le = le;
-        // expert_weights [nLx,2,P,H]: W_up(le) starts at row le*2*P of the [.,H] view; W_down(le) (the [P,H]
-        // block flat-viewed as [H,P]) starts at row (le*2+1)*H of the [.,P] view.
-        ti.b_row = kind < 0 ? 0 : (kind == 0 ? le * 2 * p.P : (le * 2 + 1) * p.H) + nt * p.bn[kind];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            ti.pkt[h] = __shfl_sync(0xffffffffu, h_pkt, h);
-            ti.mblk[h] = __shfl_sync(0xffffffffu, h_mb, h);
-            ti.src[h] = __shfl_sync(0xffffffffu, h_src, h);
-            ti.rows[h] = (kind >= 0 && h < nh) ? __shfl_sync(0xffffffffu, h_rows, h) : 0;
-            ti.cnt[h] = __shfl_sync(0xffffffffu, h_cnt, h);
-            ti.gather[h] = (kind >= 0 && h < nh) ? __shfl_sync(0xffffffffu, h_gather, h) : 0;
+        if (ti.kind >= 0 && n < 16) trace_stamp(p, 16 + n);
+        if (ti.kind >= 0 && ti.src != p.rank && !seen_remote) {
+            seen_remote = true;
+            trace_stamp(p, 13);
         }
-        if (lane == 0) {
-            if (ti.kind >= 0 && n < 16) trace_stamp(p, 16 + n);
-            if (ti.kind >= 0 && (ti.src[0] != p.rank || (PAIR && ti.rows[1] > 0 && ti.src[1] != p.rank)) && !seen_remote) {
-                seen_remote = true;
-                trace_stamp(p, 13);
-            }
-            mbar_wait(&sched_empty[q], qphase ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_EMPTY, q);
-            ring[q] = ti;
-            if (PAIR) {  // mirror the descriptor into the peer CTA's ring over DSMEM, then signal both rings
-                const uint4* src4 = reinterpret_cast<const uint4*>(&ti);
-                const uint32_t remote = mapa_shared(smem_u32(&ring[q]), 1);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) st_shared_cluster_v4(remote + 16 * i, src4[i]);
-                mbar_arrive_cluster(&sched_full[q], 1);
-            }
-            mbar_arrive(&sched_full[q]);
-        }
+        mbar_wait(&sched_empty[q], qphase ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_EMPTY, q);
+        ring[q] = ti;
+        mbar_arrive(&sched_full[q]);
         if (++q == NSCHED) { q = 0; qphase ^= 1; }
         ++n;
-        if (kind < 0) break;
-        __syncwarp();
+        if (ti.kind < 0) break;
     }
 }
 
-// warp 0 of every CTA: TMA producer.  In pair mode each CTA loads its own A row block and its half of the B rows; all
-// completion bytes are credited to the leader's `full` barrier (the only one the MMA issuer waits on).
-template <bool PAIR>
-__device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem, uint64_t* bars, uint32_t crank) {
-    using PC = PipeCfg<PAIR>;
+// gather mode: the 128 A rows of k-block kb come straight from x by token index (lane l owns rows 4l .. 4l+3), stored
+// with the 128-byte swizzle the TMA would have applied (16-byte piece c of row r at piece c ^ (r & 7))
+__device__ __forceinline__ void gather_a_rows(const FmParams& p, uint8_t* sa, int kb, int lane, const int4& tok) {
+    const int toks[4] = {tok.x, tok.y, tok.z, tok.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int row = lane * 4 + i;
+        const __nv_bfloat16* src = p.x + (size_t)toks[i] * p.H + kb * BLOCK_K;
+        uint4 v[8];
+#pragma unroll
+        for (int c = 0; c < 8; ++c) v[c] = ld_global_nc_v4(src + c * 8);
+#pragma unroll
+        for (int c = 0; c < 8; ++c) *reinterpret_cast<uint4*>(sa + row * 128 + ((c ^ (row & 7)) << 4)) = v[c];
+    }
+}
+
+// warp 0: TMA producer
+__device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem, uint64_t* bars) {
     uint64_t* full = bars + BAR_FULL;
     uint64_t* empty = bars + BAR_EMPTY;
     uint64_t* sched_full = bars + BAR_SCHED_FULL;
@@ -1246,20 +1181,19 @@ __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem, u
         int kind = -1, gather = 0, g_base = 0, g_rows = 0;
         TileInfo ti;
         if (lane == 0) {
-            wait_sched_full<PAIR>(p, &sched_full[q], qphase, 300 + q);
+            mbar_wait(&sched_full[q], qphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, 300 + q);
             ti = ring[q];
-            release_to_leader<PAIR>(&sched_empty[q], crank);
+            mbar_arrive(&sched_empty[q]);
             kind = ti.kind;
-            const int hh0 = PAIR ? (int)crank : 0;
-            gather = ti.gather[hh0];
-            g_base = ti.le * p.pEC + ti.mblk[hh0] * BLOCK_M;   // this half's first slot in the local token table
-            g_rows = ti.rows[hh0];
+            gather = ti.gather;
+            g_base = ti.le * p.pEC + ti.mblk * BLOCK_M;   // the block's first slot in the local token table
+            g_rows = ti.rows;
         }
         kind = __shfl_sync(0xffffffffu, kind, 0);
         if (kind < 0) break;
         gather = __shfl_sync(0xffffffffu, gather, 0);
         // gather mode (GEMM0 tile of a local packet whose row copies have not landed): every lane owns four rows of the
-        // A tile and fetches them from x by token index, k-block by k-block (cp.async.bulk.tensor ... tile::gather4)
+        // A tile and fetches them from x by token index, k-block by k-block
         int4 tok = make_int4(0, 0, 0, 0);
         if (gather) {
             g_base = __shfl_sync(0xffffffffu, g_base, 0);
@@ -1280,122 +1214,47 @@ __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem, u
         nk = __shfl_sync(0xffffffffu, nk, 0);
         const CUtensorMap* ta = kind == 0 ? &p.tm_a0 : &p.tm_a1;
         const CUtensorMap* tb = kind == 0 ? &p.tm_b0 : &p.tm_b1;
-        const int b_rows = p.bn[kind] / PC::B_ROWS_DIV;
         const int take_at = min(nk - 1, max(0, nk - p.claim_ahead_kb));
         int a_row = 0, b_row = 0;
         if (lane == 0) {
-            const int hh = PAIR ? (int)crank : 0;
-            a_row = ti.pkt[hh] * p.pEC + ti.mblk[hh] * BLOCK_M;
-            b_row = ti.b_row + (PAIR ? (int)crank * b_rows : 0);
+            a_row = ti.pkt * p.pEC + ti.mblk * BLOCK_M;
+            b_row = ti.b_row;
             const int pf = p.prefetch_kb;
             if (pf > 0) {   // warm L2 for the k-blocks just beyond the smem pipeline
-                for (int kb = PC::STAGES; kb < min(nk, PC::STAGES + pf); ++kb) {
+                for (int kb = STAGES; kb < min(nk, STAGES + pf); ++kb) {
                     tma_prefetch_l2_2d(ta, kb * BLOCK_K, a_row);
                     tma_prefetch_l2_2d(tb, kb * BLOCK_K, b_row);
                 }
             }
         }
         for (int kb = 0; kb < nk; ++kb) {
-            uint8_t* sa = smem + stage * PC::STAGE_BYTES;
+            uint8_t* sa = smem + stage * STAGE_BYTES;
             const bool ld_a = (p.dbg_flags & 5) == 0, ld_b = (p.dbg_flags & 9) == 0;   // experiments only
             if (lane == 0) {
                 const int pf = p.prefetch_kb;
-                if (pf > 0 && kb + PC::STAGES + pf < nk) {
-                    tma_prefetch_l2_2d(ta, (kb + PC::STAGES + pf) * BLOCK_K, a_row);
-                    tma_prefetch_l2_2d(tb, (kb + PC::STAGES + pf) * BLOCK_K, b_row);
+                if (pf > 0 && kb + STAGES + pf < nk) {
+                    tma_prefetch_l2_2d(ta, (kb + STAGES + pf) * BLOCK_K, a_row);
+                    tma_prefetch_l2_2d(tb, (kb + STAGES + pf) * BLOCK_K, b_row);
                 }
-                if (kb == take_at && crank == 0) mbar_arrive(&prod_take[q]);  // lets the scheduler claim the next tile
+                if (kb == take_at) mbar_arrive(&prod_take[q]);  // lets the scheduler claim the next tile
                 mbar_wait(&empty[stage], phase ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_EMPTY, stage);
-                const uint32_t tx = (ld_a ? (uint32_t)A_STAGE_BYTES : 0u) + (ld_b ? (uint32_t)(b_rows * BLOCK_K * 2) : 0u);
-                if (PAIR) {
-                    // the leader's expect_tx covers both CTAs' bytes (every completion is credited to ITS barrier), so
-                    // the partner's producer needs no arrival of its own: it only has to wait for its `empty` slot
-                    if (crank == 0) {
-                        if (tx) mbar_arrive_expect_tx(&full[stage], 2u * tx); else mbar_arrive(&full[stage]);
-                    } else if (p.dbg_flags & 17) {   // (bit 0: without loads nothing else keeps the partner in lock-step)
-                        mbar_arrive_cluster_plain(&full[stage], 0);
-                    }
-                    const uint32_t leader_full = mapa_shared(smem_u32(&full[stage]), 0);
-                    if (ld_a && !gather) tma_load_2d_pair(sa, ta, kb * BLOCK_K, a_row, leader_full);
-                    if (ld_b) tma_load_2d_pair(sa + A_STAGE_BYTES, tb, kb * BLOCK_K, b_row, leader_full);
-                } else {
-                    if (tx) mbar_arrive_expect_tx(&full[stage], tx); else mbar_arrive(&full[stage]);
-                    if (ld_a && !gather) tma_load_2d(sa, ta, kb * BLOCK_K, a_row, &full[stage]);
-                    if (ld_b) tma_load_2d(sa + A_STAGE_BYTES, tb, kb * BLOCK_K, b_row, &full[stage]);
-                }
+            }
+            if (gather) {   // warp-uniform: the A rows are in shared memory before the stage's barrier can complete
+                __syncwarp();   // lane 0 has seen the stage empty
+                if (ld_a) gather_a_rows(p, sa, kb, lane, tok);
+                fence_proxy_async_smem();   // generic-proxy smem writes -> the consumers' wgmma (async proxy) reads
+                __syncwarp();
+            }
+            if (lane == 0) {
+                const uint32_t tx = (ld_a && !gather ? (uint32_t)A_STAGE_BYTES : 0u) + (ld_b ? (uint32_t)B_STAGE_BYTES : 0u);
+                if (tx) mbar_arrive_expect_tx(&full[stage], tx); else mbar_arrive(&full[stage]);
+                if (ld_a && !gather) tma_load_2d(sa, ta, kb * BLOCK_K, a_row, &full[stage]);
+                if (ld_b) tma_load_2d(sa + A_STAGE_BYTES, tb, kb * BLOCK_K, b_row, &full[stage]);
                 if (!stamped) { trace_stamp(p, 7); stamped = true; }   // first loads of the first tile issued
             }
-            if (gather) {   // warp-uniform
-                __syncwarp();   // lane 0 has seen the stage empty
-                if (ld_a) {
-                    if (PAIR) tma_gather4_pair(sa + lane * 512, &p.tm_xg, kb * BLOCK_K, tok.x, tok.y, tok.z, tok.w,
-                                               mapa_shared(smem_u32(&full[stage]), 0));
-                    else tma_gather4(sa + lane * 512, &p.tm_xg, kb * BLOCK_K, tok.x, tok.y, tok.z, tok.w, &full[stage]);
-                }
-            }
-            if (++stage == PC::STAGES) { stage = 0; phase ^= 1; }
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
         if (++q == NSCHED) { q = 0; qphase ^= 1; }
-        __syncwarp();
-    }
-}
-
-// warp 1 (leader CTA only in pair mode): the single thread that issues tcgen05.mma
-template <bool PAIR>
-__device__ __forceinline__ void ffn_mma(const FmParams& p, uint8_t* smem, uint64_t* bars, uint32_t tmem_base) {
-    using PC = PipeCfg<PAIR>;
-    uint64_t* full = bars + BAR_FULL;
-    uint64_t* empty = bars + BAR_EMPTY;
-    uint64_t* tmem_full = bars + BAR_TMEM_FULL;
-    uint64_t* tmem_empty = bars + BAR_TMEM_EMPTY;
-    uint64_t* sched_full = bars + BAR_SCHED_FULL;
-    uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
-    const TileInfo* ring = reinterpret_cast<const TileInfo*>(smem + OFF_RING);
-    const int lane = threadIdx.x & 31;
-    int stage = 0, phase = 0, q = 0, qphase = 0, as = 0, aphase = 0, nt = 0;
-    for (;;) {
-        int kind = -1, nk = 0, bn = BLOCK_N;
-        if (lane == 0) {
-            mbar_wait(&sched_full[q], qphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, q);
-            kind = ring[q].kind;
-            nk = kind < 0 ? 0 : (kind == 0 ? p.H : p.P) / BLOCK_K;
-            bn = kind < 0 ? BLOCK_N : p.bn[kind];
-            mbar_arrive(&sched_empty[q]);
-        }
-        kind = __shfl_sync(0xffffffffu, kind, 0);
-        if (++q == NSCHED) { q = 0; qphase ^= 1; }
-        if (kind < 0) break;
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc_bf16_f32(PAIR ? 2 * BLOCK_M : BLOCK_M, (uint32_t)bn);
-            mbar_wait(&tmem_empty[as], aphase ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_TMEM_EMPTY, as);
-            tcgen05_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)as * BLOCK_N;
-            for (int kb = 0; kb < nk; ++kb) {
-                mbar_wait(&full[stage], phase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, stage);
-                if (kb == 0 && nt < 16) trace_stamp(p, 32 + nt);
-                tcgen05_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * PC::STAGE_BYTES);
-                const uint64_t da = umma_smem_desc_sw128(sa);
-                const uint64_t db = umma_smem_desc_sw128(sa + A_STAGE_BYTES);
-#pragma unroll
-                for (int kk = 0; kk < BLOCK_K / UMMA_K; ++kk) {
-                    if (p.dbg_flags & 2) break;   // experiment: no MMA, commits only
-                    // +32 bytes per UMMA_K step inside the 128-byte swizzle row (address field is in 16-byte units)
-                    if (PAIR) umma_bf16_ss_pair(d_tmem, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc,
-                                                (kb | kk) != 0 ? 1u : 0u);
-                    else umma_bf16_ss(d_tmem, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2), idesc,
-                                      (kb | kk) != 0 ? 1u : 0u);
-                }
-                // smem slot reusable once these MMAs have read it (pair: signalled to both CTAs' producers)
-                if (PAIR) umma_commit_pair(&empty[stage]); else umma_commit(&empty[stage]);
-                if (++stage == PC::STAGES) { stage = 0; phase ^= 1; }
-            }
-            // accumulator complete -> epilogue warps (of both CTAs in pair mode)
-            if (PAIR) umma_commit_pair(&tmem_full[as]); else umma_commit(&tmem_full[as]);
-            if (nt < 16) trace_stamp(p, 48 + nt);
-        }
-        if (++as == 2) { as = 0; aphase ^= 1; }
-        ++nt;
         __syncwarp();
     }
 }
@@ -1407,74 +1266,58 @@ __device__ __noinline__ float gelu_erf(float v) {   // GELU, erf form (cutlass::
 enum : int { EPI_G0_RELU = 0, EPI_G0_GELU = 1, EPI_G1_STORE = 2, EPI_G1_FUSED_ADD = 3, EPI_G1_FUSED_COPY = 4 };
 
 struct DrainArgs {
-    uint8_t* stg;                  // this warp's 32 x 128 B transpose tile (16-byte pieces XOR-swizzled by row & 7)
-    uint32_t t_row;                // TMEM address of this warp's lane quarter, accumulator column 0
-    int c0, c1;                    // this warp's 64-column chunks [c0, c1) of the tile
-    int lane, quarter, my_rows, N, n0;
+    uint8_t* stg;                  // this warp's transpose tile: 16 rows of 128 B (16-byte pieces XOR-swizzled by row & 7)
+    int nchunks;                   // 64-column chunks of the tile that exist (1 or 2)
+    int lane, row0, my_rows, N, n0;
     const __nv_bfloat16* bias;     // [N] or nullptr
     __nv_bfloat16* out_rows;       // row 0 of the destination row block (h staging or return buffer)
     __nv_bfloat16* acc_base;       // fused GEMM1: the source rank's output accumulator
-    int my_tok;                    // fused GEMM1: token of accumulator row (quarter*32 + lane)
+    int my_tok;                    // fused GEMM1, lanes 0-15: token of tile row (row0 + lane)
     float my_pw, my_mcw;
-    uint64_t* release_bar;         // tmem_empty barrier of this accumulator
-    uint32_t crank;
-    bool stamp;
 };
 
-// TMEM -> registers (thread = accumulator row) -> bias / activation / combine scaling in fp32 -> bf16 (RNE) -> smem
-// transpose -> full-line 16-byte global stores (or REDG adds).  64 accumulator columns per step.
-template <int MODE, bool HAS_BIAS, bool PAIR>
-__device__ __forceinline__ void drain_accumulator(const FmParams& p, const DrainArgs& a) {
-    uint8_t* my_row = a.stg + a.lane * EPI_ROW_BYTES;
-    const int sw = a.lane & 7;
-    for (int c = a.c0; c < a.c1; ++c) {
-        uint32_t v[2][32];
-        tmem_ld_32x32b_x32(a.t_row + c * 64, v[0]);
-        tmem_ld_32x32b_x32(a.t_row + c * 64 + 32, v[1]);
-        tmem_ld_wait();
-        if (c == a.c1 - 1) {  // last TMEM read of this warp: hand its share of the accumulator back to the MMA issuer
-            tcgen05_fence_before();
-            __syncwarp();
-            if (a.lane == 0) release_to_leader<PAIR>(a.release_bar, a.crank);
-        }
+// registers (wgmma fragment: rows r0 = lane/4 and r0 + 8 of this warp's 16, column pairs 8j + 2*(lane%4)) -> bias /
+// activation / combine scaling in fp32 -> bf16 (RNE) -> smem transpose -> full-line 16-byte global stores (or REDG adds).
+// 64 accumulator columns per step.
+template <int MODE, bool HAS_BIAS>
+__device__ __forceinline__ void drain_accumulator(const FmParams& p, const DrainArgs& a, const float (&acc)[64]) {
+    const int lane = a.lane, r0 = lane >> 2, cq = (lane & 3) * 2;
+    float pw[2], mcw[2];
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
+    for (int h = 0; h < 2; ++h) {
+        pw[h] = __shfl_sync(0xffffffffu, a.my_pw, r0 + 8 * h);
+        mcw[h] = __shfl_sync(0xffffffffu, a.my_mcw, r0 + 8 * h);
+    }
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {   // 8 columns -> one 16-byte smem store
-                float f[8];
+    for (int c = 0; c < 2; ++c) {
+        if (c >= a.nchunks) break;
 #pragma unroll
-                for (int i = 0; i < 8; ++i) f[i] = __uint_as_float(v[half][g * 8 + i]);
-                if (HAS_BIAS) {
-                    float bv[8];
-                    unpack8(ld_global_nc_v4(a.bias + a.n0 + c * 64 + half * 32 + g * 8), bv);
+        for (int j = 0; j < 8; ++j) {   // 8 columns -> one 4-byte smem store per fragment row
+            float2 bv = make_float2(0.0f, 0.0f);
+            if (HAS_BIAS) bv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.bias + a.n0 + c * 64 + j * 8 + cq));
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) f[i] += bv[i];
-                }
-                if (MODE == EPI_G0_RELU) {
+            for (int h = 0; h < 2; ++h) {
+                float f[2] = {acc[c * 32 + j * 4 + 2 * h], acc[c * 32 + j * 4 + 2 * h + 1]};
+                if (HAS_BIAS) { f[0] += bv.x; f[1] += bv.y; }
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) f[i] = fmaxf(f[i], 0.0f);                 // ReLU (types.cuh:151-159)
-                } else if (MODE == EPI_G0_GELU) {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) f[i] = gelu_erf(f[i]);
-                } else if (MODE == EPI_G1_FUSED_ADD) {
+                for (int i = 0; i < 2; ++i) {
+                    if (MODE == EPI_G0_RELU) f[i] = fmaxf(f[i], 0.0f);                 // ReLU (types.cuh:151-159)
+                    else if (MODE == EPI_G0_GELU) f[i] = gelu_erf(f[i]);
                     // the reference's combine arithmetic on the bf16-rounded y (processor.cuh:110-169):
                     // term = rne( p~ (x) rne( y / mCw ) ); the bf16 accumulation itself is the REDG below
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) f[i] = a.my_pw * rne_bf16(__fdividef(rne_bf16(f[i]), a.my_mcw));
+                    else if (MODE == EPI_G1_FUSED_ADD) f[i] = pw[h] * rne_bf16(__fdividef(rne_bf16(f[i]), mcw[h]));
                 }
-                uint4 o;
-                o.x = pack_bf16x2(f[0], f[1]); o.y = pack_bf16x2(f[2], f[3]);
-                o.z = pack_bf16x2(f[4], f[5]); o.w = pack_bf16x2(f[6], f[7]);
-                *reinterpret_cast<uint4*>(my_row + (((half * 4 + g) ^ sw) << 4)) = o;
+                const int r = r0 + 8 * h;
+                *reinterpret_cast<uint32_t*>(a.stg + r * EPI_ROW_BYTES + ((j ^ (r & 7)) << 4) + cq * 2) = pack_bf16x2(f[0], f[1]);
             }
         }
         __syncwarp();
         // transposed read-back: 8 lanes cover one row's 128 bytes, 4 rows per instruction, full-line stores
 #pragma unroll
-        for (int it = 0; it < 8; ++it) {
-            const int r = it * 4 + (a.lane >> 3), seg = a.lane & 7;
+        for (int it = 0; it < 4; ++it) {
+            const int r = it * 4 + (lane >> 3), seg = lane & 7;
             const uint4 o = *reinterpret_cast<const uint4*>(a.stg + r * EPI_ROW_BYTES + ((seg ^ (r & 7)) << 4));
-            const int row_in_tile = a.quarter * 32 + r;
+            const int row_in_tile = a.row0 + r;
             if (MODE == EPI_G1_FUSED_ADD || MODE == EPI_G1_FUSED_COPY) {
                 // row -> its token's output row on the source rank (k == 1: plain copy, reference processor.cuh:170-203)
                 const int tok = __shfl_sync(0xffffffffu, a.my_tok, r);
@@ -1490,107 +1333,123 @@ __device__ __forceinline__ void drain_accumulator(const FmParams& p, const Drain
     }
 }
 
-// warps 4-11 of every CTA: TMEM -> registers -> bias/activation -> bf16 -> smem transpose -> coalesced global / peer stores.
-// Warp w reads TMEM lanes [32*(w%4), +32) (a hardware restriction) and the column half (w-4)/4 of the tile.  The
-// release fence and the counter / flag traffic that make a finished tile visible to its consumers are NOT done here:
-// lane 0 of every epilogue warp arrives on pub_full[] and the publisher warp takes over (ffn_publisher).
-template <bool PAIR>
-__device__ __forceinline__ void ffn_epilogue(const FmParams& p, uint8_t* smem, uint64_t* bars, uint32_t tmem_base,
-                                             uint32_t crank) {
-    uint64_t* tmem_full = bars + BAR_TMEM_FULL;
-    uint64_t* tmem_empty = bars + BAR_TMEM_EMPTY;
+// warps 4-11: two consumer warpgroups.  Per tile: wgmma over the k-blocks the producer stages (warpgroup g multiplies A
+// rows [64g, 64g + 64) by the whole B tile into 64 fp32 registers per thread), then the epilogue of this warp's 16 rows.
+// The release fence and the counter / flag traffic that make a finished tile visible to its consumers are NOT done here:
+// lane 0 of every consumer warp arrives on pub_full[] and the publisher warp takes over (ffn_publisher).
+__device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, uint64_t* bars) {
+    uint64_t* full = bars + BAR_FULL;
+    uint64_t* empty = bars + BAR_EMPTY;
     uint64_t* sched_full = bars + BAR_SCHED_FULL;
     uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
     uint64_t* pub_full = bars + BAR_PUB_FULL;
     uint64_t* pub_empty = bars + BAR_PUB_EMPTY;
     const TileInfo* ring = reinterpret_cast<const TileInfo*>(smem + OFF_RING);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int quarter = warp & 3;  // TMEM lanes [32*quarter, 32*quarter+32) are the only ones this warp may read
-    const int chalf = (warp - EPI_WARP0) >> 2;
+    const int wg = (warp - EPI_WARP0) >> 2;
+    const int row0 = wg * 64 + (warp & 3) * 16;   // this warp's 16 rows of the tile
     uint8_t* stg = smem + OFF_EPI + (warp - EPI_WARP0) * EPI_WARP_BYTES;
-    int q = 0, qphase = 0, as = 0, aphase = 0, ps = 0, pphase = 0, ntiles = 0;
+    int q = 0, qphase = 0, stage = 0, phase = 0, ps = 0, pphase = 0, ntiles = 0;
+    const bool stamper = tid == EPI_WARP0 * 32;
     for (;;) {
-        wait_sched_full<PAIR>(p, &sched_full[q], qphase, 100 + q);
+        mbar_wait(&sched_full[q], qphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, 100 + q);
         const TileInfo ti = ring[q];
         __syncwarp();
-        if (lane == 0) release_to_leader<PAIR>(&sched_empty[q], crank);
+        if (lane == 0) mbar_arrive(&sched_empty[q]);
         if (++q == NSCHED) { q = 0; qphase ^= 1; }
         if (ti.kind < 0) break;
+
+        // ---- main loop: one k-block's wgmma group in flight while the previous stage is handed back
+        const int nk = (ti.kind == 0 ? p.H : p.P) / BLOCK_K;
+        float acc[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+        int prev = -1;
+        for (int kb = 0; kb < nk; ++kb) {
+            mbar_wait(&full[stage], phase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, stage);
+            if (kb == 0 && ntiles < 16 && stamper) trace_stamp(p, 32 + ntiles);
+            if (!(p.dbg_flags & 2)) {   // (experiment: no MMA)
+                const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+                const uint64_t da = gmma_smem_desc_sw128(sa + wg * 64 * 128);
+                const uint64_t db = gmma_smem_desc_sw128(sa + A_STAGE_BYTES);
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < BLOCK_K / WGMMA_K; ++kk)
+                    wgmma_m64n128k16_bf16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2));
+                wgmma_commit();
+            }
+            if (prev >= 0) {   // the previous k-block's MMAs have read their stage
+                wgmma_wait<1>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[prev]);
+            }
+            prev = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        __syncwarp();
+        if (lane == 0 && prev >= 0) mbar_arrive(&empty[prev]);
+        if (ntiles < 16 && stamper) trace_stamp(p, 48 + ntiles);
+
         const int N = ti.kind == 0 ? p.P : p.H;
-        const int bn = p.bn[ti.kind];
-        const int n0 = ti.ntile * bn;
-        const int hh = PAIR ? (int)crank : 0;
-        const int my_rows = ti.rows[hh], my_mblk = ti.mblk[hh], my_pkt = ti.pkt[hh], my_src = ti.src[hh];
+        const int n0 = ti.ntile * BLOCK_N;
+        const int my_rows = ti.rows;
         const __nv_bfloat16* bias = ti.kind == 0 ? (p.b_up ? p.b_up + (size_t)ti.le * p.P : nullptr)
                                                  : (p.b_down ? p.b_down + (size_t)ti.le * p.H : nullptr);
         // destination rows: GEMM0 -> local h staging; GEMM1 -> the SOURCE rank's return buffer (peer store),
         // like the reference's GEMM1 epilogue writing into the peer heap (packet.cuh:338-340, processor.cuh:713-720)
         __nv_bfloat16* out_rows;
         if (ti.kind == 0) {
-            out_rows = p.hidden + ((size_t)my_pkt * p.pEC + (size_t)my_mblk * BLOCK_M) * p.P;
+            out_rows = p.hidden + ((size_t)ti.pkt * p.pEC + (size_t)ti.mblk * BLOCK_M) * p.P;
         } else {
             const int e_global = p.rank * p.nLx + ti.le;
-            out_rows = p.peer_ret_y[my_src] + ((size_t)e_global * p.pEC + (size_t)my_mblk * BLOCK_M) * p.H;
+            out_rows = p.peer_ret_y[ti.src] + ((size_t)e_global * p.pEC + (size_t)ti.mblk * BLOCK_M) * p.H;
         }
-        // 64-column chunks of the tile that exist (N is a multiple of 64, not necessarily of the tile width), split
-        // between the two warps of this lane quarter
-        const int per_half = bn / 128;
-        const int nvalid = my_rows > 0 ? min(bn / 64, (N - n0) / 64) : 0;
-        const int c0 = min(chalf * per_half, nvalid), c1 = min(c0 + per_half, nvalid);
-        // fused GEMM1 -> combine: this thread owns accumulator row (quarter*32 + lane); fetch that row's routing record
+        // 64-column chunks of the tile that exist (N is a multiple of 64, not necessarily of the tile width)
+        const int nchunks = row0 < my_rows ? min(BLOCK_N / 64, (N - n0) / 64) : 0;
+        // fused GEMM1 -> combine: lane l < 16 fetches the routing record of tile row (row0 + l)
         const bool fuse = p.fused != 0 && ti.kind == 1;
         int my_tok = 0;
         float my_pw = 0.0f, my_mcw = 1.0f;
         if (fuse && p.dense) {
-            my_tok = my_mblk * BLOCK_M + quarter * 32 + lane;   // row i of the only packet IS token i
-        } else if (fuse && quarter * 32 + lane < my_rows) {
-            const uint4 m = ld_global_v4(p.recv_meta + (size_t)my_pkt * p.pEC + (size_t)my_mblk * BLOCK_M + quarter * 32 + lane);
+            my_tok = ti.mblk * BLOCK_M + row0 + lane;   // row i of the only packet IS token i
+        } else if (fuse && lane < 16 && row0 + lane < my_rows) {
+            const uint4 m = ld_global_v4(p.recv_meta + (size_t)ti.pkt * p.pEC + (size_t)ti.mblk * BLOCK_M + row0 + lane);
             my_tok = (int)m.x;
             my_pw = __uint_as_float(m.y);
             my_mcw = __uint_as_float(m.z);
         }
-        __nv_bfloat16* acc_base = fuse ? p.peer_out_acc[my_src] : nullptr;
-
-        mbar_wait(&tmem_full[as], aphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_TMEM_FULL, as);
-        tcgen05_fence_after();
         if (ntiles == 0 && p.W > 1 && (p.phase_mask & 1u))   // the staging area served as warp 2's window for the remote rows
             asm volatile("bar.sync 7, 288;" ::: "memory");
-        const bool stamp_tile = ntiles < 16 && tid == EPI_WARP0 * 32;
-        if (stamp_tile) trace_stamp(p, 64 + ntiles);
-        const uint32_t t_row = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)as * BLOCK_N;
-        if (c1 > c0) {
+        if (ntiles < 16 && stamper) trace_stamp(p, 64 + ntiles);
+        if (nchunks > 0) {
             DrainArgs da;
-            da.stg = stg; da.t_row = t_row; da.c0 = c0; da.c1 = c1; da.lane = lane; da.quarter = quarter;
-            da.my_rows = my_rows; da.N = N; da.n0 = n0; da.bias = bias; da.out_rows = out_rows; da.acc_base = acc_base;
-            da.my_tok = my_tok; da.my_pw = my_pw; da.my_mcw = my_mcw; da.release_bar = &tmem_empty[as]; da.crank = crank;
-            da.stamp = false;
+            da.stg = stg; da.nchunks = nchunks; da.lane = lane; da.row0 = row0; da.my_rows = my_rows; da.N = N; da.n0 = n0;
+            da.bias = bias; da.out_rows = out_rows; da.acc_base = fuse ? p.peer_out_acc[ti.src] : nullptr;
+            da.my_tok = my_tok; da.my_pw = my_pw; da.my_mcw = my_mcw;
             // one specialised instantiation per (epilogue kind, bias) pair: no per-element or per-group branching
             const int mode = ti.kind == 0 ? (p.act == 0 ? EPI_G0_RELU : EPI_G0_GELU)
                                           : (!fuse ? EPI_G1_STORE : (p.k > 1 ? EPI_G1_FUSED_ADD : EPI_G1_FUSED_COPY));
             if (bias == nullptr) {
                 switch (mode) {
-                    case EPI_G0_RELU: drain_accumulator<EPI_G0_RELU, false, PAIR>(p, da); break;
-                    case EPI_G0_GELU: drain_accumulator<EPI_G0_GELU, false, PAIR>(p, da); break;
-                    case EPI_G1_STORE: drain_accumulator<EPI_G1_STORE, false, PAIR>(p, da); break;
-                    case EPI_G1_FUSED_ADD: drain_accumulator<EPI_G1_FUSED_ADD, false, PAIR>(p, da); break;
-                    default: drain_accumulator<EPI_G1_FUSED_COPY, false, PAIR>(p, da); break;
+                    case EPI_G0_RELU: drain_accumulator<EPI_G0_RELU, false>(p, da, acc); break;
+                    case EPI_G0_GELU: drain_accumulator<EPI_G0_GELU, false>(p, da, acc); break;
+                    case EPI_G1_STORE: drain_accumulator<EPI_G1_STORE, false>(p, da, acc); break;
+                    case EPI_G1_FUSED_ADD: drain_accumulator<EPI_G1_FUSED_ADD, false>(p, da, acc); break;
+                    default: drain_accumulator<EPI_G1_FUSED_COPY, false>(p, da, acc); break;
                 }
             } else {
                 switch (mode) {
-                    case EPI_G0_RELU: drain_accumulator<EPI_G0_RELU, true, PAIR>(p, da); break;
-                    case EPI_G0_GELU: drain_accumulator<EPI_G0_GELU, true, PAIR>(p, da); break;
-                    case EPI_G1_STORE: drain_accumulator<EPI_G1_STORE, true, PAIR>(p, da); break;
-                    case EPI_G1_FUSED_ADD: drain_accumulator<EPI_G1_FUSED_ADD, true, PAIR>(p, da); break;
-                    default: drain_accumulator<EPI_G1_FUSED_COPY, true, PAIR>(p, da); break;
+                    case EPI_G0_RELU: drain_accumulator<EPI_G0_RELU, true>(p, da, acc); break;
+                    case EPI_G0_GELU: drain_accumulator<EPI_G0_GELU, true>(p, da, acc); break;
+                    case EPI_G1_STORE: drain_accumulator<EPI_G1_STORE, true>(p, da, acc); break;
+                    case EPI_G1_FUSED_ADD: drain_accumulator<EPI_G1_FUSED_ADD, true>(p, da, acc); break;
+                    default: drain_accumulator<EPI_G1_FUSED_COPY, true>(p, da, acc); break;
                 }
             }
-        } else {  // nothing to drain for this warp (row block or columns past the end): still release the accumulator
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) release_to_leader<PAIR>(&tmem_empty[as], crank);
         }
-        if (stamp_tile) trace_stamp(p, 80 + ntiles);
-        if (++as == 2) { as = 0; aphase ^= 1; }
+        if (ntiles < 16 && stamper) trace_stamp(p, 80 + ntiles);
 
         // hand the tile to the publisher: this warp's stores are issued (h will be read through the async proxy)
         if (ti.kind == 0) fence_proxy_async_global();
@@ -1604,13 +1463,12 @@ __device__ __forceinline__ void ffn_epilogue(const FmParams& p, uint8_t* smem, u
     }
 }
 
-// warp 2 of every CTA: makes finished tiles visible.  For every tile of the ring, once all epilogue warps of this CTA
-// have issued their stores: GEMM0 -> release-add on the row block's h counter (reference notifyNext's tSA counter,
-// processor.cuh:490-615); GEMM1 -> system-scope fence, then the packet / row-block counter and, from the last tile, the
-// flag on the source rank (reference processor.cuh:722-750).  The fences wait for the stores / REDs to drain (1-2 us,
-// more over NVLink); here they overlap the next tile's epilogue instead of delaying it.
-template <bool PAIR>
-__device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, uint64_t* bars, uint32_t crank) {
+// warp 2: makes finished tiles visible.  For every tile of the ring, once all consumer warps have issued their stores:
+// GEMM0 -> release-add on the row block's h counter (reference notifyNext's tSA counter, processor.cuh:490-615);
+// GEMM1 -> system-scope fence, then the packet / row-block counter and, from the last tile, the flag on the source rank
+// (reference processor.cuh:722-750).  The fences wait for the stores / REDs to drain (1-2 us, more over NVLink); here
+// they overlap the next tile's MMA instead of delaying it.
+__device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, uint64_t* bars) {
     uint64_t* sched_full = bars + BAR_SCHED_FULL;
     uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
     uint64_t* pub_full = bars + BAR_PUB_FULL;
@@ -1621,13 +1479,12 @@ __device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, 
     for (;;) {
         int kind = -1;
         if (lane == 0) {
-            wait_sched_full<PAIR>(p, &sched_full[q], qphase, 400 + q);
+            mbar_wait(&sched_full[q], qphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, 400 + q);
             const TileInfo ti = ring[q];
-            release_to_leader<PAIR>(&sched_empty[q], crank);
+            mbar_arrive(&sched_empty[q]);
             kind = ti.kind;
             if (kind >= 0) {
-                const int hh = PAIR ? (int)crank : 0;
-                const int my_rows = ti.rows[hh], my_mblk = ti.mblk[hh], my_pkt = ti.pkt[hh], my_src = ti.src[hh];
+                const int my_rows = ti.rows, my_mblk = ti.mblk, my_pkt = ti.pkt, my_src = ti.src;
                 mbar_wait(&pub_full[ps], pphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, 10 + ps);
                 mbar_arrive(&pub_empty[ps]);
                 if (my_rows > 0) {
@@ -1641,7 +1498,7 @@ __device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, 
                         } else {
                         fence_acq_rel_sys();   // this tile's adds are performed before the packet counter moves
                         const unsigned int old = atom_acq_rel_gpu_add_u32(p.pkt_done + my_pkt, 1u);
-                        const unsigned int want = (unsigned int)(((ti.cnt[hh] + BLOCK_M - 1) / BLOCK_M) * p.TN1);
+                        const unsigned int want = (unsigned int)(((ti.cnt + BLOCK_M - 1) / BLOCK_M) * p.TN1);
                         if (old + 1u == want) {   // every GEMM1 tile of packet (src, le) has been added into src's output
                             st_release_sys_u64(p.peer_done_flag[my_src] + (size_t)(p.rank * p.nLx + ti.le),
                                                (unsigned long long)p.epoch << 32);
@@ -1670,89 +1527,62 @@ __device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, 
     }
 }
 
-// kernel prologue: barriers of every later phase + TMEM; runs before the router so it costs nothing on the critical path
-template <bool PAIR>
+// kernel prologue: barriers of every later phase; runs before the router so it costs nothing on the critical path
 __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BARS);
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + OFF_TMEM_PTR);
     const int tid = threadIdx.x, warp = tid >> 5;
     if (warp == 1 && (tid & 31) == 0) {
-        // arrival counts: full = leader's expect_tx; empty / tmem_full = one tcgen05.commit; tmem_empty = one lane per
-        // epilogue warp (of both CTAs); pub_full = one lane per epilogue warp of this CTA; sched_empty = every ring reader
-        const int nc = PAIR ? 2 : 1;
-        const int nfull = (PAIR && (p.dbg_flags & 17)) ? 2 : 1;
-        for (int i = 0; i < MAX_STAGES; ++i) { mbar_init(&bars[BAR_FULL + i], nfull); mbar_init(&bars[BAR_EMPTY + i], 1); }
+        // arrival counts: full = the producer's expect_tx; empty = one lane per consumer warp; pub_full = one lane per
+        // consumer warp; sched_empty = every ring reader (producer, publisher, consumer warps)
+        for (int i = 0; i < STAGES; ++i) { mbar_init(&bars[BAR_FULL + i], 1); mbar_init(&bars[BAR_EMPTY + i], NUM_EPI_WARPS); }
         for (int i = 0; i < 2; ++i) {
-            mbar_init(&bars[BAR_TMEM_FULL + i], 1);
-            mbar_init(&bars[BAR_TMEM_EMPTY + i], NUM_EPI_WARPS * nc);
             mbar_init(&bars[BAR_PUB_FULL + i], NUM_EPI_WARPS);
             mbar_init(&bars[BAR_PUB_EMPTY + i], 1);
         }
         for (int i = 0; i < NSCHED; ++i) {
             mbar_init(&bars[BAR_SCHED_FULL + i], 1);
-            mbar_init(&bars[BAR_SCHED_EMPTY + i], 1 + (2 + NUM_EPI_WARPS) * nc);   // MMA lane + per CTA: producer, publisher, epilogue warps
+            mbar_init(&bars[BAR_SCHED_EMPTY + i], 2 + NUM_EPI_WARPS);
             mbar_init(&bars[BAR_PROD_TAKE + i], 1);
         }
         mbar_init(&bars[BAR_XROWS], 1);
         mbar_init(&bars[BAR_DISP_DONE], 1);
         mbar_init(&bars[BAR_WG], 1);
         mbar_init(&bars[BAR_REMOTE], 1);
-        for (int i = 0; i < GATE_STAGES; ++i) { mbar_init(&bars[BAR_GFULL + i], 1); mbar_init(&bars[BAR_GEMPTY + i], 1); }
-        mbar_init(&bars[BAR_GACC], 1);
+        for (int i = 0; i < GATE_STAGES; ++i) { mbar_init(&bars[BAR_GFULL + i], 1); mbar_init(&bars[BAR_GEMPTY + i], NUM_EPI_WARPS); }
         fence_mbar_init();
     }
     if (warp == 0 && (tid & 31) == 0) {
         tma_prefetch_desc(&p.tm_a0); tma_prefetch_desc(&p.tm_b0);
         tma_prefetch_desc(&p.tm_a1); tma_prefetch_desc(&p.tm_b1);
     }
-    if (warp == 3 && (tid & 31) == 0 && (p.phase_mask & 3u) == 3u && (!PAIR || (blockIdx.x & 1) == 0)) {
-        // Warm L2 with the weight tile this pair will most likely claim first (item id = pair index: the first wave is
+    if (warp == 3 && (tid & 31) == 0 && (p.phase_mask & 3u) == 3u) {
+        // Warm L2 with the weight tile this CTA will most likely claim first (item id = CTA index: the first wave is
         // claimed in arrival order), pipeline depth only: HBM is idle during the router and the first tile's loads are
-        // then L2 hits.  A wrong guess costs nothing -- the tile is needed by some pair of the first wave anyway.
-        const int id = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
+        // then L2 hits.  A wrong guess costs nothing -- the tile is needed by some CTA of the first wave anyway.
+        const int id = (int)blockIdx.x;
         if (id < p.total_items) {
             int cur = 0;
             while (id >= p.blocks[cur + 1].start) ++cur;
             const TileBlock blk = p.blocks[cur];
             const int local = id - blk.start;
-            const bool cross = PAIR && blk.pkt2 >= 0;
-            const int m_items = (PAIR && !cross) ? (p.TCM + 1) / 2 : p.TCM;
-            const int nt = local / m_items, le = blk.pkt % p.nLx, bn_w = p.bn[blk.kind];
+            const int nt = local / p.TCM, le = blk.pkt % p.nLx;
             const CUtensorMap* tb = blk.kind == 0 ? &p.tm_b0 : &p.tm_b1;
-            const int b0 = (blk.kind == 0 ? le * 2 * p.P : (le * 2 + 1) * p.H) + nt * bn_w;
-            const int nk_w = (blk.kind == 0 ? p.H : p.P) / BLOCK_K, step = PAIR ? bn_w / 2 : bn_w;
-            for (int kb = 0; kb < min(nk_w, PipeCfg<PAIR>::STAGES); ++kb)
-                for (int r = 0; r < bn_w; r += step) tma_prefetch_l2_2d(tb, kb * BLOCK_K, b0 + r);
+            const int b0 = (blk.kind == 0 ? le * 2 * p.P : (le * 2 + 1) * p.H) + nt * BLOCK_N;
+            const int nk_w = (blk.kind == 0 ? p.H : p.P) / BLOCK_K;
+            for (int kb = 0; kb < min(nk_w, STAGES); ++kb) tma_prefetch_l2_2d(tb, kb * BLOCK_K, b0);
         }
     }
-    if (warp == 2 && ((p.phase_mask & 2u) || p.tc_gate)) { if (PAIR) tmem_alloc_pair(tmem_ptr, TMEM_COLS); else tmem_alloc(tmem_ptr, TMEM_COLS); }
-    tcgen05_fence_before();
 }
 
 // warp roles of the expert-FFN phase (entered per warp as soon as that warp is free; no block-wide sync on entry)
-template <bool PAIR>
-__device__ __forceinline__ void ffn_roles(const FmParams& p, uint8_t* smem, uint32_t crank) {
+__device__ __forceinline__ void ffn_roles(const FmParams& p, uint8_t* smem) {
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BARS);
     const int tid = threadIdx.x, warp = tid >> 5;
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem + OFF_TMEM_PTR);
-    if (warp == 0) ffn_producer<PAIR>(p, smem, bars, crank);
-    else if (warp == 1) { if (crank == 0) ffn_mma<PAIR>(p, smem, bars, tmem_base); }
-    else if (warp == 2) ffn_publisher<PAIR>(p, smem, bars, crank);
-    else if (warp == 3) { if (crank == 0) ffn_scheduler<PAIR>(p, smem, bars); }
-    else if (warp >= EPI_WARP0) ffn_epilogue<PAIR>(p, smem, bars, tmem_base, crank);
-}
-
-template <bool PAIR>
-__device__ __forceinline__ void ffn_teardown(const FmParams& p, uint8_t* smem) {
-    const int tid = threadIdx.x, warp = tid >> 5;
-    tcgen05_fence_before();
-    if (PAIR) cluster_sync_all(); else __syncthreads();   // nobody leaves while the partner may still touch its smem/TMEM
-    if (warp == 2) {
-        tcgen05_fence_after();
-        const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem + OFF_TMEM_PTR);
-        if (PAIR) tmem_dealloc_pair(tmem_base, TMEM_COLS); else tmem_dealloc(tmem_base, TMEM_COLS);
-    }
+    if (warp == 0) ffn_producer(p, smem, bars);
+    else if (warp == 2) ffn_publisher(p, smem, bars);
+    else if (warp == 3) { if ((tid & 31) == 0) ffn_scheduler(p, smem, bars); }
+    else if (warp >= EPI_WARP0) ffn_consumer(p, smem, bars);
+    __syncthreads();
     if (tid == 0) trace_stamp(p, 5);
 }
 
@@ -1908,17 +1738,15 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, uint8_t* smem, 
 }
 
 // ============================================================================================================
-template <bool PAIR>
 __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __grid_constant__ FmParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int tid = threadIdx.x, warp = tid >> 5;
     const int t0 = blockIdx.x * p.tpc;
     const int n_tok = max(0, min(p.tpc, p.S - t0));
-    const uint32_t crank = PAIR ? cluster_ctarank() : 0u;
 
     if (tid == 0) trace_stamp(p, 0);
-    ffn_setup<PAIR>(p, smem);   // mbarriers + TMEM for the later phases (visible to everyone after the next block sync)
+    ffn_setup(p, smem);   // mbarriers for the later phases (visible to everyone after the next block sync)
     if (p.phase_mask & 1u) {
         // per-launch reset of the work counters (reference clearState, moe.cuh:21-70); consumed only after the grid barrier
         if (blockIdx.x == 0) {
@@ -1941,18 +1769,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
             }
             if (tid == 0) *p.claim = 0u;
         }
-        if (p.dense) gate_phase_dense(p, t0, n_tok); else gate_phase<PAIR>(p, smem, t0, n_tok, crank);
+        if (p.dense) gate_phase_dense(p, t0, n_tok); else gate_phase(p, smem, t0, n_tok);
         if (tid == 0) trace_stamp(p, 1);
-        grid_barrier(p);   // also a cluster-wide sync: the partner CTA's barriers are initialised before any remote arrive
+        grid_barrier(p);
         if (tid == 0) trace_stamp(p, 2);
     } else {
         if (blockIdx.x == 0 && tid == 0) *p.claim = 0u;   // debug re-run of later phases on the previous routing
-        if (PAIR) cluster_sync_all(); else __syncthreads();
+        __syncthreads();
     }
 
-    // From here the warps specialise.  Warps 0, 1, 3 (TMA producer, MMA issuer, tile scheduler) enter their FFN roles at
-    // once -- the scheduler claims its first tile and spins on the packet flag while warps 2, 4-7 dispatch this CTA's rows;
-    // warps 4-7 then become the epilogue.
+    // From here the warps specialise.  Warps 0 and 3 (TMA producer, tile scheduler) enter their FFN roles at once -- the
+    // scheduler claims its first tile and spins on the packet flag while warps 2, 4-11 dispatch this CTA's rows; warps
+    // 4-11 then become the consumer warpgroups.
     const bool disp_warp = (warp == 2) || (warp >= EPI_WARP0);
     if ((p.phase_mask & 1u) && disp_warp) {
         if (!p.dense) dispatch_phase(p, smem, t0, n_tok);
@@ -1962,10 +1790,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
     }
     if (p.phase_mask & 2u) {
         if (tid == EPI_WARP0 * 32) trace_stamp(p, 4);
-        ffn_roles<PAIR>(p, smem, crank);
-        ffn_teardown<PAIR>(p, smem);
-    } else if (p.tc_gate && (p.phase_mask & 1u)) {
-        ffn_teardown<PAIR>(p, smem);   // (router-only debug launch: the tensor-core router allocated TMEM)
+        ffn_roles(p, smem);
     }
 
     if (p.phase_mask & 4u) {

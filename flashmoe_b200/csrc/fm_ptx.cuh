@@ -1,4 +1,4 @@
-// fm_ptx.cuh -- thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM),
+// fm_ptx.cuh -- thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma,
 // scoped acquire/release accesses used by the cross-CTA and cross-GPU flag protocol.
 // Hand-written for this project (no CUTLASS/CuTe on the hot path -- BASELINE.json north_star).
 #pragma once
@@ -26,8 +26,7 @@ enum : unsigned int {
     FM_TRAP_NONE = 0,
     FM_TRAP_MBAR_FULL = 1,
     FM_TRAP_MBAR_EMPTY = 2,
-    FM_TRAP_MBAR_TMEM_FULL = 3,
-    FM_TRAP_MBAR_TMEM_EMPTY = 4,
+    // 3, 4: no longer used
     FM_TRAP_MBAR_SCHED_FULL = 5,
     FM_TRAP_MBAR_SCHED_EMPTY = 6,
     FM_TRAP_GRID_BARRIER = 7,
@@ -244,190 +243,72 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, in
 }
 
 // ----------------------------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA issue, commit, TMEM loads
+// wgmma: warpgroup MMA (four consecutive warps), both operands in shared memory, fp32 accumulators in registers
 // ----------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // same warp that allocated
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16 inputs with fp32 accumulation
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives row (lane base + i), columns [c, c+32)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
+// accumulator registers written by other instructions -> visible to the following wgmma.mma_async
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait until at most N committed groups of this thread are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
+// D[64 x N] += A[64 x 16] * B[N x 16]^T, bf16 inputs (both K-major), fp32 accumulation.  Thread t of the warpgroup
+// holds, per 8-column group j, d[4j + 0..1] = row 16*(t/32) + (t%32)/4, columns 8j + 2*(t%4) + {0, 1}, and d[4j + 2..3]
+// = the same columns of row + 8.
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t desc_a, uint64_t desc_b) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(1));
 }
-
-// ----------------------------------------------------------------------------------------------------------------
-// thread-block clusters / CTA pairs (cta_group::2): the two CTAs of a cluster run one 256-row UMMA together
-// ----------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {  // every thread of every CTA in the cluster
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cta address -> shared::cluster address of the same offset in CTA `cta` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t cta) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(cta));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {  // arrive on CTA `cta`'s copy
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(mapa_shared(smem_u32(bar), cta))
-                 : "memory");
-}
-// barrier-only signal to another CTA (no data published by this thread): default semantics, no cluster-scope release
-// fence (a .release.cluster arrive per k-block made the CTA-pair pipeline ~2x slower)
-__device__ __forceinline__ void mbar_arrive_cluster_plain(uint64_t* bar, uint32_t cta) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(mapa_shared(smem_u32(bar), cta)) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {  // acquire at cluster scope
-    uint32_t ok;
+__device__ __forceinline__ void wgmma_m64n64k16_bf16(float (&d)[32], uint64_t desc_a, uint64_t desc_b) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity, DebugRecord* dbg,
-                                                  unsigned long long timeout_ns, unsigned int code, unsigned int info) {
-    SpinGuard g;
-    while (!mbar_try_wait_cluster(bar, parity)) g.tick(dbg, timeout_ns, code, info, parity, 1);
-}
-__device__ __forceinline__ void st_shared_cluster_v4(uint32_t cluster_addr, const uint4& v) {
-    asm volatile("st.shared::cluster.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(cluster_addr), "r"(v.x), "r"(v.y), "r"(v.z),
-                 "r"(v.w)
-                 : "memory");
-}
-// TMA load issued by either CTA of a pair; completion bytes are credited to the mbarrier at `bar_cluster_addr`, a
-// shared::cluster address (mapa_shared(smem_u32(bar), 0) = the LEADER CTA's copy of the barrier)
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const void* tmap, int32_t c0, int32_t c1,
-                                                 uint32_t bar_cluster_addr) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-        : "memory");
-}
-// TMA gather: four arbitrary rows (r0..r3) of a 2-D tensor, `box` columns starting at column c0, land as four
-// consecutive 128-byte rows at smem_dst (tensor map encoded with box {64, 1}, 128-byte swizzle -- the swizzle is a
-// function of the shared-memory address, so a 512-byte aligned destination inside a tile keeps the tile's layout).
-__device__ __forceinline__ void tma_gather4(void* smem_dst, const void* tmap, int32_t c0, int32_t r0, int32_t r1, int32_t r2,
-                                            int32_t r3, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes.cta_group::1 "
-        "[%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
-        : "memory");
-}
-// CTA-pair form: issued by either CTA, completion bytes credited to the barrier at `bar_cluster_addr` (the leader's copy)
-__device__ __forceinline__ void tma_gather4_pair(void* smem_dst, const void* tmap, int32_t c0, int32_t r0, int32_t r1,
-                                                 int32_t r2, int32_t r3, uint32_t bar_cluster_addr) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes.cta_group::2 "
-        "[%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(bar_cluster_addr), "r"(c0), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result, uint32_t ncols) {  // same warp id in both CTAs
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// 256 x N x 16 MMA across the CTA pair (issued by the leader only): rows 0-127 accumulate in the leader's TMEM, rows
-// 128-255 in the peer's; A comes from each CTA's own smem, B rows [0,N/2) from the leader's smem and [N/2,N) from the peer's
-__device__ __forceinline__ void umma_bf16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                  uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {  // arrives on the barrier at this offset in BOTH CTAs
-    const unsigned short mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(mask)
-                 : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(desc_a), "l"(desc_b), "r"(1));
 }
 
-// ----------------------------------------------------------------------------------------------------------------
-// UMMA descriptors (PTX ISA "tcgen05 matrix / instruction descriptors")
-// ----------------------------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a K-major bf16 operand tile stored as rows of 128 bytes (64 bf16) with the
-// 128-byte swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_128B):
+// Shared-memory matrix descriptor (PTX ISA "Matrix Descriptor Format" for wgmma) for a K-major bf16 operand tile
+// stored as rows of 128 bytes (64 bf16) with the 128-byte swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_128B):
 //   bits  0-13  start address >> 4            bits 16-29  leading-dim byte offset >> 4 (unused for swizzled K-major)
 //   bits 32-45  stride-dim byte offset >> 4 = 1024 B (8 rows x 128 B swizzle atom) >> 4
-//   bits 46-47  descriptor version = 1 (sm_100)     bits 61-63  layout: 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t smem_addr) {
+//   bits 62-63  layout: 1 = SWIZZLE_128B
+// Advancing K by 16 elements inside the swizzle row adds 32 bytes (2 in the address field).
+__device__ __forceinline__ uint64_t gmma_smem_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+    d |= static_cast<uint64_t>(1) << 16;
     d |= static_cast<uint64_t>(1024u >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
-}
-// Instruction descriptor, kind::f16: D fp32 (bits 4-5 = 1), A/B bf16 (bits 7-9 / 10-12 = 1), both K-major
-// (bits 15/16 = 0), N >> 3 at bits 17-22, M >> 4 at bits 24-28.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_f32(uint32_t M, uint32_t N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 // ----------------------------------------------------------------------------------------------------------------

@@ -42,7 +42,7 @@ def launch_workers(config_path: str, n_processes: int = 1, processes_per_node: i
                    hostfile: Optional[str] = None, extra_args: Optional[List[str]] = None,
                    timeout: Optional[float] = None) -> subprocess.CompletedProcess:
     cmd = build_command(config_path, n_processes, processes_per_node, hostfile, extra_args)
-    print("Launching FlashMoE (B200) with:", " ".join(cmd), flush=True)
+    print("Launching FlashMoE (H100) with:", " ".join(cmd), flush=True)
     env = dict(os.environ)
     env["PYTHONPATH"] = str(Path(__file__).resolve().parent.parent) + os.pathsep + env.get("PYTHONPATH", "")
     res = subprocess.run(cmd, capture_output=True, text=True, env=env, timeout=timeout)

@@ -1,5 +1,5 @@
 /*
- * flashmoe_b200.h -- C-ABI of the B200-native fused distributed-MoE forward path.
+ * flashmoe_b200.h -- C-ABI of the H100-native (sm_90a) fused distributed-MoE forward path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch types.  It replaces what the reference binds
  * through pybind in csrc/python_bindings.cu (reference paths below are relative to osayamenja/FlashMoE):
@@ -72,7 +72,7 @@ typedef struct fm_dims {
     int32_t k, EC, pEC, TCM;
     int32_t world, rank, num_local_experts;
     int32_t num_sms, smem_bytes;
-    int32_t grid; /* CTAs of the persistent kernel (= num_sms, rounded down to even for CTA pairs); rows of FM_BUF_TRACE */
+    int32_t grid; /* CTAs of the persistent kernel (= num_sms); rows of FM_BUF_TRACE */
 } fm_dims_t;
 
 typedef struct fm_ctx fm_ctx_t;

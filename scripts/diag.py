@@ -1,4 +1,4 @@
-"""GPU bring-up diagnostic: runs the fused kernel phase by phase on one B200 and compares every intermediate
+"""GPU bring-up diagnostic: runs the fused kernel phase by phase on one H100 and compares every intermediate
 buffer with the CPU oracle.  Usage: python scripts/diag.py [--cfg small|A|B] [--stage all|gate|ffn|combine|full|time]
 Each stage runs in its own process when invoked with --stage all (a device trap poisons the CUDA context)."""
 import argparse, json, os, subprocess, sys, time

@@ -1,6 +1,6 @@
 // Peer-write bandwidth probe (2 GPUs, one process): how fast can SM-side code push rows into another GPU's memory over
 // NVLink, by method and transfer size?  Feeds the dispatch design (DESIGN.md section 4, item 3).
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o scripts/bin/peer_bw_probe scripts/peer_bw_probe.cu
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o scripts/bin/peer_bw_probe scripts/peer_bw_probe.cu
 //   scripts/bin/peer_bw_probe            (needs >= 2 GPUs with peer access)
 // Methods: bulk = cp.async.bulk shared -> peer global of `chunk` bytes per operation (one issuing lane per operation, 32
 // lanes of one warp per CTA, everything in flight, like the dispatch's remote mover); st = 16-byte st.global from all
@@ -71,7 +71,9 @@ int main() {
         CK(cudaMemset(s[d].buf, 0, total * 2));
         CK(cudaFuncSetAttribute(k_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * 1024));
     }
-    const int G = 148, iters = 10;
+    int G = 0;   // one CTA per SM
+    CK(cudaDeviceGetAttribute(&G, cudaDevAttrMultiProcessorCount, 0));
+    const int iters = 10;
     auto run = [&](const char* name, int dirs, auto launch) {
         // dirs = 1: GPU 0 writes to GPU 1; dirs = 2: both write to each other at the same time
         float ms[2] = {0, 0};

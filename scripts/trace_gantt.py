@@ -1,7 +1,7 @@
 """Per-tile timeline of the fused kernel from its own %globaltimer stamps (fm_set_trace): where the time of the expert-FFN
 phase goes.  Usage: python scripts/trace_gantt.py [--cfg B] [--world-note ...]   (environment knobs FM_* apply).
-Prints medians over the leader CTAs of: claim -> dependencies resolved -> first k-block landed -> last MMA issued ->
-accumulator complete -> epilogue stores issued -> published, per GEMM kind, plus the idle gaps between tiles."""
+Prints medians over all CTAs of: claim -> dependencies resolved -> first k-block landed -> MMA complete -> epilogue
+start -> epilogue stores issued -> published, per GEMM kind, plus the idle gaps between tiles."""
 import argparse
 import os
 import sys
@@ -28,57 +28,50 @@ def analyse(tr, cfg, label=""):
         v = us(tr[:, i][tr[:, i] > 0])
         if len(v):
             print(f"  {nm:14s} {v.min():8.1f} {np.median(v):8.1f} {v.max():8.1f}")
-    lead = tr[0::2]  # leader CTAs of the pairs hold the scheduler / MMA stamps
-    part = tr[1::2]
     rows = []
-    for c in range(lead.shape[0]):
-        n = int((lead[c, 32:48] > 0).sum())
+    for c in range(tr.shape[0]):   # every CTA runs its own scheduler, producer and consumer warpgroups
+        n = int((tr[c, 32:48] > 0).sum())
         for i in range(n):
-            rows.append(dict(c=c, i=i, claim=lead[c, 112 + i], ready=lead[c, 16 + i], first=lead[c, 32 + i], last=lead[c, 48 + i],
-                             acc=lead[c, 64 + i], stores=lead[c, 80 + i], pub=lead[c, 96 + i],
-                             p_acc=part[c, 64 + i], p_stores=part[c, 80 + i], p_pub=part[c, 96 + i],
-                             prev_last=lead[c, 48 + i - 1] if i else lead[c, 4], prev_acc=lead[c, 64 + i - 1] if i else 0))
+            rows.append(dict(c=c, i=i, claim=tr[c, 112 + i], ready=tr[c, 16 + i], first=tr[c, 32 + i], mma=tr[c, 48 + i],
+                             epi=tr[c, 64 + i], stores=tr[c, 80 + i], pub=tr[c, 96 + i],
+                             prev_mma=tr[c, 48 + i - 1] if i else tr[c, 4]))
     if not rows:
         print("  no tile stamps")
         return
-    span = np.array([r["acc"] - r["first"] for r in rows]) / 1e3
-    thr = 2.0 * np.median(span) if len(span) else 0
+    span = np.array([r["mma"] - r["first"] for r in rows]) / 1e3
     nk = {0: cfg.H // 64, 1: cfg.P // 64}
     kinds = np.array([1 if s > 0.6 * span.max() and span.max() > 1.8 * span.min() else 0 for s in span])
-    ffn0 = np.median(lead[:, 4][lead[:, 4] > 0])
-    ffn_end = tr[:, 5].max()
-    print(f"--- {label} tiles recorded (first 16 per pair): {len(rows)}; GEMM0-like {int((kinds == 0).sum())}, GEMM1-like {int((kinds == 1).sum())}")
+    print(f"--- {label} tiles recorded (first 16 per CTA): {len(rows)}; GEMM0-like {int((kinds == 0).sum())}, GEMM1-like {int((kinds == 1).sum())}")
     for kd in (0, 1):
         sel = [r for r, k in zip(rows, kinds) if k == kd]
         if not sel:
             continue
         f = lambda a, b: np.array([r[a] - r[b] for r in sel]) / 1e3  # noqa: E731
-        main = f("acc", "first")
-        issue = f("last", "first")
+        main = f("mma", "first")
         print(f"  GEMM{kd} (nk={nk[kd]}): n={len(sel)}")
         for nm, v in (("claim->ready", f("ready", "claim")), ("ready->first k-block landed", f("first", "ready")),
-                      ("first landed->last MMA issued", issue), ("first landed->accumulator complete", main),
+                      ("first landed->MMA complete", main),
                       ("  per k-block (us)", main / nk[kd]),
-                      ("accumulator complete->stores issued (leader epi)", f("stores", "acc")),
-                      ("stores issued->published (leader)", f("pub", "stores")),
-                      ("accumulator complete->stores issued (partner epi)", f("p_stores", "p_acc")),
-                      ("MMA idle before this tile (first landed - prev last issued)", f("first", "prev_last")),
+                      ("MMA complete->epilogue start", f("epi", "mma")),
+                      ("epilogue start->stores issued", f("stores", "epi")),
+                      ("stores issued->published", f("pub", "stores")),
+                      ("MMA idle before this tile (first landed - prev MMA complete)", f("first", "prev_mma")),
                       ):
             v = v[np.isfinite(v)]
             print(f"    {nm:62s} med {np.median(v):7.2f}  p10 {np.percentile(v, 10):7.2f}  p90 {np.percentile(v, 90):7.2f}")
     t0rows = [r for r in rows if r["i"] == 0]
     if t0rows:
         g = lambda key: np.median([(r[key] - t00) / 1e3 for r in t0rows])  # noqa: E731
-        print(f"  per pair, first tile: claimed {g('claim'):.1f}, rows ready {g('ready'):.1f}, first k-block landed {g('first'):.1f} us (medians)")
-    # tensor-busy fraction per pair over the FFN phase (first 16 tiles only are stamped; config B has <= 10 per pair)
+        print(f"  per CTA, first tile: claimed {g('claim'):.1f}, rows ready {g('ready'):.1f}, first k-block landed {g('first'):.1f} us (medians)")
+    # tensor-busy time per CTA over the FFN phase (only the first 16 tiles of a CTA are stamped)
     busy = {}
     for r in rows:
-        busy[r["c"]] = busy.get(r["c"], 0) + (r["acc"] - r["first"])
+        busy[r["c"]] = busy.get(r["c"], 0) + (r["mma"] - r["first"])
     b = np.array(list(busy.values())) / 1e3
     t_first = np.array([min(r["first"] for r in rows if r["c"] == c) for c in busy]) - t00
-    t_lastacc = np.array([max(r["acc"] for r in rows if r["c"] == c) for c in busy]) - t00
-    print(f"  per pair: mainloop-busy med {np.median(b):.1f} us; first k-block landed at med {np.median(t_first) / 1e3:.1f} "
-          f"(min {t_first.min() / 1e3:.1f}, max {t_first.max() / 1e3:.1f}) us; last accumulator complete med {np.median(t_lastacc) / 1e3:.1f} max {t_lastacc.max() / 1e3:.1f} us; "
+    t_last = np.array([max(r["mma"] for r in rows if r["c"] == c) for c in busy]) - t00
+    print(f"  per CTA: mainloop-busy med {np.median(b):.1f} us; first k-block landed at med {np.median(t_first) / 1e3:.1f} "
+          f"(min {t_first.min() / 1e3:.1f}, max {t_first.max() / 1e3:.1f}) us; last MMA complete med {np.median(t_last) / 1e3:.1f} max {t_last.max() / 1e3:.1f} us; "
           f"kernel end {us(tr[:, 6].max()):.1f} us")
 
 

@@ -53,22 +53,21 @@ def main():
     tr = ctx.read("trace").astype(np.int64)
     t00 = tr[:, 0].min()
     us = lambda a: (a - t00) / 1e3  # noqa: E731
-    lead = tr[0::2]
     rec = {}
     for key, col, red in (("start_spread", 0, "max"), ("gate_done", 1, "med"), ("barrier", 2, "med"), ("disp_prefix", 8, "med"),
                           ("disp_rows_done", 9, "med"), ("dispatch_end_max", 3, "max"), ("ffn_end_med", 5, "med"),
                           ("done_flags_seen", 14, "med"), ("kernel_end", 6, "max")):
         v = tr[:, col][tr[:, col] > 0]
         rec[key] = float(us(np.median(v) if red == "med" else v.max())) if len(v) else float("nan")
-    first_landed = lead[:, 32][lead[:, 32] > 0]
+    first_landed = tr[:, 32][tr[:, 32] > 0]
     rec["first_tile_kb0_landed_min"] = float(us(first_landed.min())) if len(first_landed) else float("nan")
     rec["first_tile_kb0_landed_med"] = float(us(np.median(first_landed))) if len(first_landed) else float("nan")
-    rem = lead[:, 13][lead[:, 13] > 0]
+    rem = tr[:, 13][tr[:, 13] > 0]
     rec["first_remote_tile_ready_min"] = float(us(rem.min())) if len(rem) else float("nan")
     pub = tr[:, 96:112]
     rec["last_tile_published"] = float(us(pub.max())) if (pub > 0).any() else float("nan")
-    acc = lead[:, 64:80]
-    rec["last_accumulator_complete"] = float(us(acc.max())) if (acc > 0).any() else float("nan")
+    mma = tr[:, 48:64]   # MMA complete, per tile
+    rec["last_mma_complete"] = float(us(mma.max())) if (mma > 0).any() else float("nan")
     rec["abs_start_ns"] = int(t00)
     allr = [None] * world
     dist.all_gather_object(allr, rec)

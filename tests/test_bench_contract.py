@@ -1,5 +1,5 @@
 """bench.py's output contract on the CPU-only legs: the reference arm prints one JSON line with the agreed keys, and the
-multi-rank convention (only rank 0 works and prints) holds.  The GPU arm is exercised on the B200 box by the driver."""
+multi-rank convention (only rank 0 works and prints) holds.  The GPU arm needs an H100."""
 import json
 import os
 import subprocess

@@ -1,6 +1,6 @@
 """Parity tests proper: the CUDA path, called through the C-ABI (MoEContext -> ctypes -> libflashmoe_b200.so), against
 the CPU oracle on the same seeded inputs, against the committed golden fixtures, and -- at BASELINE.json's full
-single-GPU size -- through size-independent properties.  Needs a B200 (pytest -m gpu)."""
+single-GPU size -- through size-independent properties.  Needs an H100 (pytest -m gpu)."""
 import glob
 import os
 
@@ -71,6 +71,9 @@ CASES = {
     "E32_k2": MoEConfig(num_experts=32, expert_top_k=2, sequence_len=1024, hidden_size=512, intermediate_size=512),
     "E64_k4": MoEConfig(num_experts=64, expert_top_k=4, sequence_len=512, hidden_size=256, intermediate_size=256),
     "E128_k2": MoEConfig(num_experts=128, expert_top_k=2, sequence_len=1024, hidden_size=256, intermediate_size=256),
+    # more than 128 experts: the tensor-core router takes a second pass over d_model for experts 128..E-1
+    "E160_k2": MoEConfig(num_experts=160, expert_top_k=2, sequence_len=2048, hidden_size=256, intermediate_size=256),
+    "E256_k2": MoEConfig(num_experts=256, expert_top_k=2, sequence_len=2048, hidden_size=256, intermediate_size=256),
     # 139 tokens per CTA: the tensor-core router walks two sub-chunks (128 + 11 tokens) with different numbers of x boxes
     # (the 64k-token sweep point has four; a stage layout that followed the sub-chunk's row count broke its last one)
     "E32_router_subchunks": MoEConfig(num_experts=32, expert_top_k=2, sequence_len=20480, hidden_size=128,
@@ -91,17 +94,19 @@ def test_parity_with_oracle(name):
     _compare(cfg, _run(cfg, x, wg, we), run_oracle(cfg, x, wg, we))
 
 
-@pytest.mark.parametrize("pair,fused", [(0, 1), (1, 0), (0, 0)])
+@pytest.mark.parametrize("gather,fused", [(0, 1), (1, 0), (0, 0), (2, 1), (2, 0)])
 @pytest.mark.parametrize("name", ["small_drop", "odd_row_blocks", "configA_top1", "ragged_dims"])
-def test_alternate_kernel_modes(monkeypatch, name, pair, fused):
-    """The solo-CTA (cta_group::1) FFN path and the gather-combine path stay parity-green (defaults: CTA pairs + fused)."""
+def test_alternate_kernel_modes(monkeypatch, name, gather, fused):
+    """The row gather from x for GEMM0 tiles (FM_GATHER=1: tiles claimed before their rows landed, timing-dependent;
+    FM_GATHER=2: every local GEMM0 tile, so the gather path always runs) and the gather-combine path stay parity-green
+    (defaults: no row gather, fused combine)."""
     cases = dict(CASES)
     cases["odd_row_blocks"] = MoEConfig(num_experts=4, expert_top_k=2, sequence_len=768, hidden_size=256,
-                                        intermediate_size=512)  # TCM = 3: the last CTA pair has an empty partner
+                                        intermediate_size=512)  # TCM = 3: an odd number of row blocks per packet
     cfg = cases[name]
-    monkeypatch.setenv("FM_PAIR", str(pair))
+    monkeypatch.setenv("FM_GATHER", str(gather))
     monkeypatch.setenv("FM_FUSED_COMBINE", str(fused))
-    x, wg, we, _, _ = make_inputs(cfg, seed=300 + pair * 2 + fused)
+    x, wg, we, _, _ = make_inputs(cfg, seed=300 + gather * 2 + fused)
     _compare(cfg, _run(cfg, x, wg, we), run_oracle(cfg, x, wg, we))
 
 
@@ -210,9 +215,9 @@ def test_host_buffer_entry_point_equals_device_path():
     ctx.close()
 
 
-@pytest.mark.parametrize("name", ["small_drop", "ragged_dims", "E64_k4", "E128_k2"])
+@pytest.mark.parametrize("name", ["small_drop", "ragged_dims", "E64_k4", "E128_k2", "E160_k2"])
 def test_router_cuda_core_path(monkeypatch, name):
-    """The router's logits come from tcgen05.mma by default (E <= 256); FM_TC_GATE=0 selects the register-blocked
+    """The router's logits come from wgmma by default (17 <= E <= 256); FM_TC_GATE=0 selects the register-blocked
     CUDA-core GEMV (the only path for E > 256), which must stay parity-green too."""
     monkeypatch.setenv("FM_TC_GATE", "0")
     cfg = CASES[name]
@@ -222,8 +227,8 @@ def test_router_cuda_core_path(monkeypatch, name):
 
 @pytest.mark.parametrize("name", ["tiny", "small_drop", "ragged_dims", "configA_top1", "multi_seq"])
 def test_router_tensor_core_path_small_expert_counts(monkeypatch, name):
-    """FM_TC_GATE=1 forces the tcgen05 router where the default (E <= 16) is the CUDA-core GEMV: padded expert columns
-    (E = 2, 4, 6, 8 -> 16), 8-row halves of Wg per CTA of a pair, chunks of fewer than 32 tokens."""
+    """FM_TC_GATE=1 forces the wgmma router where the default (E <= 16) is the CUDA-core GEMV: padded expert columns
+    (E = 2, 4, 6, 8 -> 64), chunks of fewer than 32 tokens."""
     monkeypatch.setenv("FM_TC_GATE", "1")
     cfg = CASES[name]
     x, wg, we, _, _ = make_inputs(cfg, seed=500 + len(name))

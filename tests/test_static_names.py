@@ -9,7 +9,7 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FILES = ["bench.py", "__graft_entry__.py", "flashmoe_b200/runtime.py", "flashmoe_b200/worker.py", "flashmoe_b200/_C.py",
          "flashmoe_b200/launcher.py", "flashmoe_b200/layer.py", "flashmoe_b200/ops.py", "flashmoe_b200/_lib.py", "flashmoe_b200/_build.py",
-         "scripts/diag.py", "scripts/trace_gantt.py", "scripts/trace_multi.py", "scripts/ncu_summarize.py", "tests/multi_gpu_worker.py"]
+         "scripts/diag.py", "scripts/trace_gantt.py", "scripts/trace_multi.py", "tests/multi_gpu_worker.py"]
 
 
 def _bound_names(node):
