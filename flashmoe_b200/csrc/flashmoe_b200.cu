@@ -485,7 +485,7 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
     ctx->num_pkts = world * nLx;
 
     // Work list.  Sources in the order own rank, rank+1, ... (local rows need no NVLink hop, so they are ready first).
-    // A work item is one 128 x 128 output tile of one packet.
+    // A work item is one 128 x 256 output tile of one packet.
     struct Unit { int pkt; bool local; };
     std::vector<Unit> units;
     for (int j = 0; j < world; ++j)

@@ -19,7 +19,7 @@
 //
 // CTA = 384 threads, one CTA per SM, all co-resident (cooperative launch).  After the grid barrier the warps specialise:
 // warp 0 = TMA producer, warp 3 = tile scheduler, warps 2 and 4-11 = dispatch, then warps 4-11 = two consumer warpgroups
-// (wgmma into register accumulators, warpgroup g owns rows [64g, 64g + 64) of the 128 x 128 tile, then the epilogue:
+// (wgmma into register accumulators, warpgroup g owns rows [64g, 64g + 64) of the 128 x 256 tile, then the epilogue:
 // bias/activation/combine scaling -> bf16 -> swizzled smem transpose -> 16-byte global / peer stores or adds) and
 // warp 2 = publisher (the release fence + counter / flag traffic of every finished tile, off the consumer warps'
 // critical path).  Warp 1 has no role in phase F.
@@ -35,7 +35,7 @@
 namespace fm {
 
 constexpr int BLOCK_M = 128;   // token rows per tile (= reference BLOCK_M)
-constexpr int BLOCK_N = 128;   // output columns per tile: 64 fp32 accumulators per consumer thread
+constexpr int BLOCK_N = 256;   // output columns per tile: 128 fp32 accumulators per consumer thread
 constexpr int BLOCK_K = 64;    // 64 bf16 = 128 B = one swizzle row
 constexpr int WGMMA_K = 16;
 constexpr int NSCHED = 4;
@@ -50,15 +50,15 @@ constexpr int TRACE_SLOTS = 128; // per CTA: [0..6] phase stamps, [8..14] sub-ph
                                  // [96+i] published, [112+i] claimed (scheduler)
 
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;                  // 16 KiB
-constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;                  // 16 KiB
+constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;                  // 32 KiB
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-constexpr int STAGES = 6;
+constexpr int STAGES = 4;
 constexpr int PIPE_BYTES = STAGES * STAGE_BYTES;                      // 192 KiB
 constexpr int EPI_ROW_BYTES = 128;                                    // 64 bf16; 16-byte pieces XOR-swizzled by (row & 7)
 constexpr int EPI_WARP_BYTES = 32 * EPI_ROW_BYTES;                    // 4 KiB per epilogue warp
 constexpr int OFF_EPI = PIPE_BYTES;                                   // 196608
 constexpr int OFF_BARS = OFF_EPI + NUM_EPI_WARPS * EPI_WARP_BYTES;    // 229376
-// barriers: full[6] empty[6] sched_full[4] sched_empty[4] prod_take[4] xrows disp_done pub_full[2] pub_empty[2] wg remote
+// barriers: full[4] empty[4] sched_full[4] sched_empty[4] prod_take[4] xrows disp_done pub_full[2] pub_empty[2] wg remote
 //           gfull[8] gempty[8]
 constexpr int BAR_FULL = 0, BAR_EMPTY = STAGES;
 constexpr int BAR_SCHED_FULL = 2 * STAGES, BAR_SCHED_EMPTY = BAR_SCHED_FULL + NSCHED;
@@ -72,7 +72,7 @@ constexpr int BAR_REMOTE = BAR_WG + 1;                                // dispatc
 constexpr int GATE_STAGES = 8;                                        // router GEMM on tensor cores: up to 8 smem stages
 constexpr int BAR_GFULL = BAR_REMOTE + 1;                             // full / empty per stage
 constexpr int BAR_GEMPTY = BAR_GFULL + GATE_STAGES;
-constexpr int NUM_BARS = BAR_GEMPTY + GATE_STAGES;                    // 48
+constexpr int NUM_BARS = BAR_GEMPTY + GATE_STAGES;                    // 44
 constexpr int OFF_RING = OFF_BARS + NUM_BARS * 8;                     // 16-byte aligned
 constexpr int SMEM_USED = OFF_RING + NSCHED * 64;
 constexpr int SMEM_BYTES = SMEM_USED + 1024;                          // + slack for manual 1 KiB alignment
@@ -1267,7 +1267,7 @@ enum : int { EPI_G0_RELU = 0, EPI_G0_GELU = 1, EPI_G1_STORE = 2, EPI_G1_FUSED_AD
 
 struct DrainArgs {
     uint8_t* stg;                  // this warp's transpose tile: 16 rows of 128 B (16-byte pieces XOR-swizzled by row & 7)
-    int nchunks;                   // 64-column chunks of the tile that exist (1 or 2)
+    int nchunks;                   // 64-column chunks of the tile that exist (1 to 4)
     int lane, row0, my_rows, N, n0;
     const __nv_bfloat16* bias;     // [N] or nullptr
     __nv_bfloat16* out_rows;       // row 0 of the destination row block (h staging or return buffer)
@@ -1280,7 +1280,7 @@ struct DrainArgs {
 // activation / combine scaling in fp32 -> bf16 (RNE) -> smem transpose -> full-line 16-byte global stores (or REDG adds).
 // 64 accumulator columns per step.
 template <int MODE, bool HAS_BIAS>
-__device__ __forceinline__ void drain_accumulator(const FmParams& p, const DrainArgs& a, const float (&acc)[64]) {
+__device__ __forceinline__ void drain_accumulator(const FmParams& p, const DrainArgs& a, const float (&acc)[128]) {
     const int lane = a.lane, r0 = lane >> 2, cq = (lane & 3) * 2;
     float pw[2], mcw[2];
 #pragma unroll
@@ -1289,7 +1289,7 @@ __device__ __forceinline__ void drain_accumulator(const FmParams& p, const Drain
         mcw[h] = __shfl_sync(0xffffffffu, a.my_mcw, r0 + 8 * h);
     }
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
+    for (int c = 0; c < BLOCK_N / 64; ++c) {
         if (c >= a.nchunks) break;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {   // 8 columns -> one 4-byte smem store per fragment row
@@ -1334,7 +1334,7 @@ __device__ __forceinline__ void drain_accumulator(const FmParams& p, const Drain
 }
 
 // warps 4-11: two consumer warpgroups.  Per tile: wgmma over the k-blocks the producer stages (warpgroup g multiplies A
-// rows [64g, 64g + 64) by the whole B tile into 64 fp32 registers per thread), then the epilogue of this warp's 16 rows.
+// rows [64g, 64g + 64) by the whole B tile into 128 fp32 registers per thread), then the epilogue of this warp's 16 rows.
 // The release fence and the counter / flag traffic that make a finished tile visible to its consumers are NOT done here:
 // lane 0 of every consumer warp arrives on pub_full[] and the publisher warp takes over (ffn_publisher).
 __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, uint64_t* bars) {
@@ -1361,9 +1361,9 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, u
 
         // ---- main loop: one k-block's wgmma group in flight while the previous stage is handed back
         const int nk = (ti.kind == 0 ? p.H : p.P) / BLOCK_K;
-        float acc[64];
+        float acc[128];
 #pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+        for (int i = 0; i < 128; ++i) acc[i] = 0.0f;
         int prev = -1;
         for (int kb = 0; kb < nk; ++kb) {
             mbar_wait(&full[stage], phase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, stage);
@@ -1375,7 +1375,7 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, u
                 wgmma_fence();
 #pragma unroll
                 for (int kk = 0; kk < BLOCK_K / WGMMA_K; ++kk)
-                    wgmma_m64n128k16_bf16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2));
+                    wgmma_m64n256k16_bf16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2));
                 wgmma_commit();
             }
             if (prev >= 0) {   // the previous k-block's MMAs have read their stage
@@ -1556,7 +1556,7 @@ __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
         tma_prefetch_desc(&p.tm_a1); tma_prefetch_desc(&p.tm_b1);
     }
     if (warp == 3 && (tid & 31) == 0 && (p.phase_mask & 3u) == 3u) {
-        // Warm L2 with the weight tile this CTA will most likely claim first (item id = CTA index: the first wave is
+        // Warm L2 with the 256-row weight tile this CTA will most likely claim first (item id = CTA index: the first wave is
         // claimed in arrival order), pipeline depth only: HBM is idle during the router and the first tile's loads are
         // then L2 hits.  A wrong guess costs nothing -- the tile is needed by some CTA of the first wave anyway.
         const int id = (int)blockIdx.x;
@@ -1574,15 +1574,38 @@ __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
     }
 }
 
-// warp roles of the expert-FFN phase (entered per warp as soon as that warp is free; no block-wide sync on entry)
+// Register split of the expert-FFN phase.  __launch_bounds__(384, 1) gives every warp 168 registers (65536 / 384, rounded
+// down to a multiple of 8); the producer warpgroup (warps 0-3: TMA producer, idle warp 1, publisher, scheduler) needs few
+// of them, the consumer warpgroups hold 128 fp32 accumulators per thread.  128 * REGS_PROD + 256 * REGS_CONS <= 65536.
+// 80 / 208 keeps the consumers' k-block loop free of local-memory traffic; with fewer registers for warps 0-3 the
+// scheduler and producer code spill heavily (DESIGN.md section 4).  Warps 0, 1 and 3 alone free 8448 registers, the
+// consumers take 10240: one consumer warpgroup completes its increase only when warp 2 has given its registers up, after
+// dispatch.  With one rank that is at once; with several it waits for the remote row stream (80 / 200 avoids the wait
+// and measured about 3 % slower on one GPU).
+constexpr int REGS_ALL = 168, REGS_PROD = 80, REGS_CONS = 208;
+static_assert(REGS_ALL == (65536 / NUM_THREADS) / 8 * 8, "the even split __launch_bounds__(NUM_THREADS, 1) gives every warp");
+static_assert(128 * REGS_PROD + 256 * REGS_CONS <= 65536, "register file of one SM");
+
+// warp roles of the expert-FFN phase (entered per warp as soon as that warp is free; no block-wide sync on entry).  Every
+// warp of a warpgroup executes the same setmaxnreg: warps 0-3 give registers up on entry, warps 4-11 (here after the
+// router and dispatch, which they run with the even split) take them.  Phase C runs on all 384 threads with the even
+// split again: the consumers hand their registers back before the block sync, warps 0-3 take theirs back after it (an
+// increase waits for free registers, so it must not come before every consumer's decrease).
 __device__ __forceinline__ void ffn_roles(const FmParams& p, uint8_t* smem) {
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BARS);
     const int tid = threadIdx.x, warp = tid >> 5;
-    if (warp == 0) ffn_producer(p, smem, bars);
-    else if (warp == 2) ffn_publisher(p, smem, bars);
-    else if (warp == 3) { if ((tid & 31) == 0) ffn_scheduler(p, smem, bars); }
-    else if (warp >= EPI_WARP0) ffn_consumer(p, smem, bars);
+    if (warp < EPI_WARP0) {
+        setmaxnreg_dec<REGS_PROD>();
+        if (warp == 0) ffn_producer(p, smem, bars);
+        else if (warp == 2) ffn_publisher(p, smem, bars);
+        else if (warp == 3) { if ((tid & 31) == 0) ffn_scheduler(p, smem, bars); __syncwarp(); }
+    } else {
+        setmaxnreg_inc<REGS_CONS>();
+        ffn_consumer(p, smem, bars);
+        setmaxnreg_dec<REGS_ALL>();
+    }
     __syncthreads();
+    if (warp < EPI_WARP0) setmaxnreg_inc<REGS_ALL>();
     if (tid == 0) trace_stamp(p, 5);
 }
 
