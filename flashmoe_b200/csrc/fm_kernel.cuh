@@ -55,11 +55,17 @@ constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
 constexpr int STAGES = 4;
 constexpr int PIPE_BYTES = STAGES * STAGE_BYTES;                      // 192 KiB
 constexpr int EPI_ROW_BYTES = 128;                                    // 64 bf16; 16-byte pieces XOR-swizzled by (row & 7)
-constexpr int EPI_WARP_BYTES = 32 * EPI_ROW_BYTES;                    // 4 KiB per epilogue warp
-constexpr int OFF_EPI = PIPE_BYTES;                                   // 196608
-constexpr int OFF_BARS = OFF_EPI + NUM_EPI_WARPS * EPI_WARP_BYTES;    // 229376
+// The epilogue staging area: two h chunk buffers of 128 rows x 128 B (64 columns of a GEMM0 tile in the TMA's
+// SWIZZLE_128B layout).  Consumer warp w owns rows [(w - 4) * 16, +16) of each buffer: it stages its rows of a GEMM0
+// chunk there (the publisher warp stores the whole chunk with one TMA store), and its GEMM1 transpose tile is its rows
+// of buffer 0.  No warp ever writes another warp's rows, so warps need no ordering among themselves here.
+constexpr int EPI_CHUNK_BYTES = BLOCK_M * EPI_ROW_BYTES;              // 16 KiB
+constexpr int EPI_BUFS = 2;
+constexpr int EPI_BYTES = EPI_BUFS * EPI_CHUNK_BYTES;                 // 32 KiB
+constexpr int OFF_EPI = PIPE_BYTES;                                   // 196608 (1 KiB aligned, as SWIZZLE_128B needs)
+constexpr int OFF_BARS = OFF_EPI + EPI_BYTES;                         // 229376
 // barriers: full[4] empty[4] sched_full[4] sched_empty[4] prod_take[4] xrows disp_done pub_full[2] pub_empty[2] wg remote
-//           gfull[8] gempty[8]
+//           gfull[8] gempty[8] stg_full[2] stg_free[2]
 constexpr int BAR_FULL = 0, BAR_EMPTY = STAGES;
 constexpr int BAR_SCHED_FULL = 2 * STAGES, BAR_SCHED_EMPTY = BAR_SCHED_FULL + NSCHED;
 constexpr int BAR_PROD_TAKE = BAR_SCHED_EMPTY + NSCHED;
@@ -72,7 +78,9 @@ constexpr int BAR_REMOTE = BAR_WG + 1;                                // dispatc
 constexpr int GATE_STAGES = 8;                                        // router GEMM on tensor cores: up to 8 smem stages
 constexpr int BAR_GFULL = BAR_REMOTE + 1;                             // full / empty per stage
 constexpr int BAR_GEMPTY = BAR_GFULL + GATE_STAGES;
-constexpr int NUM_BARS = BAR_GEMPTY + GATE_STAGES;                    // 44
+constexpr int BAR_STG_FULL = BAR_GEMPTY + GATE_STAGES;                // consumer warps -> publisher: h chunk staged
+constexpr int BAR_STG_FREE = BAR_STG_FULL + EPI_BUFS;                 // publisher -> consumer warps: chunk read by the TMA
+constexpr int NUM_BARS = BAR_STG_FREE + EPI_BUFS;                     // 48
 constexpr int OFF_RING = OFF_BARS + NUM_BARS * 8;                     // 16-byte aligned
 constexpr int SMEM_USED = OFF_RING + NSCHED * 64;
 constexpr int SMEM_BYTES = SMEM_USED + 1024;                          // + slack for manual 1 KiB alignment
@@ -102,7 +110,7 @@ struct TileBlock {  // one contiguous run of work items: all tiles of one GEMM o
 struct FmParams {
     CUtensorMap tm_a0;  // recv_x  as [W*nLx*pEC, H]  box {64, 128}
     CUtensorMap tm_b0;  // expert_weights as [nLx*2*P, H]  box {64, 128}  (W_up rows)
-    CUtensorMap tm_a1;  // hidden  as [W*nLx*pEC, P]  box {64, 128}
+    CUtensorMap tm_a1;  // hidden  as [W*nLx*pEC, P]  box {64, 128}: GEMM1's A loads and GEMM0's h stores
     CUtensorMap tm_b1;  // expert_weights as [nLx*2*H, P]  box {64, 128}  (W_down rows)
     CUtensorMap tm_gx;  // router on tensor cores: x as [S, H], box {64, 32}
     CUtensorMap tm_gw;  // router on tensor cores: Wg_eff [E, H], box {64, min(128, E rounded up to 64)}
@@ -945,7 +953,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
         // kept (token, pick) pair of those tokens that belongs to another rank is one bulk store of a whole row to that
         // rank's receive buffer, and when the engine has read the window the next run follows.  The link paces the stores.
         uint8_t* win = smem + OFF_EPI + 8192;
-        const int win_bytes = NUM_EPI_WARPS * EPI_WARP_BYTES - 8192;
+        const int win_bytes = EPI_BYTES - 8192;
         const int rows_win = max(1, win_bytes / row_bytes);
         uint64_t* rbar = reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_REMOTE;
         uint32_t rphase = 0;
@@ -1265,23 +1273,89 @@ __device__ __noinline__ float gelu_erf(float v) {   // GELU, erf form (cutlass::
 
 enum : int { EPI_G0_RELU = 0, EPI_G0_GELU = 1, EPI_G1_STORE = 2, EPI_G1_FUSED_ADD = 3, EPI_G1_FUSED_COPY = 4 };
 
+// registers (wgmma fragment: rows r0 = lane/4 and r0 + 8 of this warp's 16, column pairs 8j + 2*(lane%4)) of the 64
+// accumulator columns [64c, 64c + 64) -> bias / activation / combine scaling in fp32 -> bf16 (RNE) -> 16 rows of 128 B
+// at `stg`, 16-byte piece j of row r at piece j ^ (r & 7) (the TMA's 128-byte swizzle when `stg` is 1 KiB aligned).
+// `bias` points at the chunk's first column (or is unused).
+template <int MODE, bool HAS_BIAS>
+__device__ __forceinline__ void chunk_to_smem(const float (&acc)[128], int c, uint8_t* stg, const __nv_bfloat16* bias,
+                                              int lane, const float (&pw)[2], const float (&mcw)[2]) {
+    const int r0 = lane >> 2, cq = (lane & 3) * 2;
+    // Rows r0 and r0 + 8 share r & 7 = r0, and `stg` is 128-byte aligned, so piece j of either row is one XOR of bits
+    // 4-6 away from piece 0 ^ r0 of row r0: one address register instead of sixteen precomputed ones (which the
+    // compiler would otherwise keep live, or spill, beside the 128 accumulators).
+    const uint32_t row_addr = smem_u32(stg) + r0 * EPI_ROW_BYTES + (r0 << 4) + cq * 2;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {   // 8 columns -> one 4-byte smem store per fragment row
+        const uint32_t addr = xor_u32(row_addr, j << 4);
+        float2 bv = make_float2(0.0f, 0.0f);
+        if (HAS_BIAS) bv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(bias + j * 8 + cq));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float f[2] = {acc[c * 32 + j * 4 + 2 * h], acc[c * 32 + j * 4 + 2 * h + 1]};
+            if (HAS_BIAS) { f[0] += bv.x; f[1] += bv.y; }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                if (MODE == EPI_G0_RELU) f[i] = fmaxf(f[i], 0.0f);                 // ReLU (types.cuh:151-159)
+                else if (MODE == EPI_G0_GELU) f[i] = gelu_erf(f[i]);
+                // the reference's combine arithmetic on the bf16-rounded y (processor.cuh:110-169):
+                // term = rne( p~ (x) rne( y / mCw ) ); the bf16 accumulation itself is the REDG in drain_accumulator
+                else if (MODE == EPI_G1_FUSED_ADD) f[i] = pw[h] * rne_bf16(__fdividef(rne_bf16(f[i]), mcw[h]));
+            }
+            st_shared_u32(addr + h * 8 * EPI_ROW_BYTES, pack_bf16x2(f[0], f[1]));   // row r0 + 8h
+        }
+    }
+}
+
+// GEMM0 epilogue of one consumer warp: each 64-column chunk of h goes through one of the two staging buffers and is
+// stored by the publisher warp (ffn_publisher) with a TMA tensor store.  `chunk` counts the chunks this warp has handed
+// over so far; every consumer warp stages the same sequence, so chunk & 1 names the buffer and chunk >> 1 its use.
+//
+// Hand-off: wait stg_free[b] (the TMA has read the buffer's previous chunk), write this warp's 16 rows, make the
+// generic-proxy smem writes visible to the async proxy (fence.proxy.async.shared::cta by every writing lane, then
+// __syncwarp), and arrive on stg_full[b].  The warp never waits for a store to complete and never publishes g0_done
+// itself: its next tile can be a GEMM1 tile of this CTA over the same row block, whose dependency wait (the scheduler
+// spinning on g0_done) must be satisfied without the consumers -- they are then blocked on that tile's first `full`
+// barrier, and waiting here would deadlock until the SpinGuard fires.  The publisher issues the stores, waits for them
+// (cp.async.bulk.wait_group 0: the async-proxy writes are complete), orders them before its generic-proxy release with
+// fence.proxy.async.global, and then red.release.gpu's g0_done; the scheduler's ld.acquire.gpu of g0_done plus the
+// producer's fence.proxy.async.global before its TMA loads of h complete the chain on the reading side.
+// Rows at or beyond the block's valid rows are staged and stored too: they lie in the packet's pEC padding of h, and
+// GEMM1 multiplies them row-independently and drops their results.
+template <int MODE, bool HAS_BIAS>
+__device__ __forceinline__ void stage_h(const FmParams& p, uint8_t* smem, uint64_t* bars, const float (&acc)[128],
+                                        const __nv_bfloat16* bias, int nchunks, int row0, int lane, uint32_t& chunk) {
+    const float one[2] = {1.0f, 1.0f};
+#pragma unroll
+    for (int c = 0; c < BLOCK_N / 64; ++c) {
+        if (c >= nchunks) break;
+        const int b = chunk & 1;
+        mbar_wait(&bars[BAR_STG_FREE + b], ((chunk >> 1) & 1) ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, 20 + b);
+        chunk_to_smem<MODE, HAS_BIAS>(acc, c, smem + OFF_EPI + b * EPI_CHUNK_BYTES + row0 * EPI_ROW_BYTES,
+                                      HAS_BIAS ? bias + c * 64 : nullptr, lane, one, one);
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars[BAR_STG_FULL + b]);
+        ++chunk;
+    }
+}
+
 struct DrainArgs {
     uint8_t* stg;                  // this warp's transpose tile: 16 rows of 128 B (16-byte pieces XOR-swizzled by row & 7)
     int nchunks;                   // 64-column chunks of the tile that exist (1 to 4)
     int lane, row0, my_rows, N, n0;
     const __nv_bfloat16* bias;     // [N] or nullptr
-    __nv_bfloat16* out_rows;       // row 0 of the destination row block (h staging or return buffer)
+    __nv_bfloat16* out_rows;       // row 0 of the destination row block in the return buffer
     __nv_bfloat16* acc_base;       // fused GEMM1: the source rank's output accumulator
     int my_tok;                    // fused GEMM1, lanes 0-15: token of tile row (row0 + lane)
     float my_pw, my_mcw;
 };
 
-// registers (wgmma fragment: rows r0 = lane/4 and r0 + 8 of this warp's 16, column pairs 8j + 2*(lane%4)) -> bias /
-// activation / combine scaling in fp32 -> bf16 (RNE) -> smem transpose -> full-line 16-byte global stores (or REDG adds).
-// 64 accumulator columns per step.
+// GEMM1 epilogue: 64 accumulator columns per step through chunk_to_smem, then the transposed read-back and full-line
+// 16-byte global stores (or REDG adds) straight from the warp.
 template <int MODE, bool HAS_BIAS>
 __device__ __forceinline__ void drain_accumulator(const FmParams& p, const DrainArgs& a, const float (&acc)[128]) {
-    const int lane = a.lane, r0 = lane >> 2, cq = (lane & 3) * 2;
+    const int lane = a.lane, r0 = lane >> 2;
     float pw[2], mcw[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -1291,26 +1365,7 @@ __device__ __forceinline__ void drain_accumulator(const FmParams& p, const Drain
 #pragma unroll
     for (int c = 0; c < BLOCK_N / 64; ++c) {
         if (c >= a.nchunks) break;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {   // 8 columns -> one 4-byte smem store per fragment row
-            float2 bv = make_float2(0.0f, 0.0f);
-            if (HAS_BIAS) bv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(a.bias + a.n0 + c * 64 + j * 8 + cq));
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                float f[2] = {acc[c * 32 + j * 4 + 2 * h], acc[c * 32 + j * 4 + 2 * h + 1]};
-                if (HAS_BIAS) { f[0] += bv.x; f[1] += bv.y; }
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    if (MODE == EPI_G0_RELU) f[i] = fmaxf(f[i], 0.0f);                 // ReLU (types.cuh:151-159)
-                    else if (MODE == EPI_G0_GELU) f[i] = gelu_erf(f[i]);
-                    // the reference's combine arithmetic on the bf16-rounded y (processor.cuh:110-169):
-                    // term = rne( p~ (x) rne( y / mCw ) ); the bf16 accumulation itself is the REDG below
-                    else if (MODE == EPI_G1_FUSED_ADD) f[i] = pw[h] * rne_bf16(__fdividef(rne_bf16(f[i]), mcw[h]));
-                }
-                const int r = r0 + 8 * h;
-                *reinterpret_cast<uint32_t*>(a.stg + r * EPI_ROW_BYTES + ((j ^ (r & 7)) << 4) + cq * 2) = pack_bf16x2(f[0], f[1]);
-            }
-        }
+        chunk_to_smem<MODE, HAS_BIAS>(acc, c, a.stg, HAS_BIAS ? a.bias + a.n0 + c * 64 : nullptr, lane, pw, mcw);
         __syncwarp();
         // transposed read-back: 8 lanes cover one row's 128 bytes, 4 rows per instruction, full-line stores
 #pragma unroll
@@ -1325,7 +1380,7 @@ __device__ __forceinline__ void drain_accumulator(const FmParams& p, const Drain
                     __nv_bfloat16* dst = a.acc_base + (size_t)tok * a.N + a.n0 + c * 64 + seg * 8;
                     if (MODE == EPI_G1_FUSED_ADD) red_add_bf16x8(dst, o); else st_global_v4(dst, o);
                 }
-            } else if (row_in_tile < a.my_rows) {
+            } else if (row_in_tile < a.my_rows) {   // EPI_G1_STORE: the return buffer on the source rank
                 st_global_v4(a.out_rows + (size_t)row_in_tile * a.N + a.n0 + c * 64 + seg * 8, o);
             }
         }
@@ -1335,8 +1390,9 @@ __device__ __forceinline__ void drain_accumulator(const FmParams& p, const Drain
 
 // warps 4-11: two consumer warpgroups.  Per tile: wgmma over the k-blocks the producer stages (warpgroup g multiplies A
 // rows [64g, 64g + 64) by the whole B tile into 128 fp32 registers per thread), then the epilogue of this warp's 16 rows.
-// The release fence and the counter / flag traffic that make a finished tile visible to its consumers are NOT done here:
-// lane 0 of every consumer warp arrives on pub_full[] and the publisher warp takes over (ffn_publisher).
+// The consumers do not wait for their stores, nor fence or publish: a GEMM0 tile's h chunks are handed to the publisher
+// warp through the staging buffers (stage_h), and after a GEMM1 tile lane 0 of every consumer warp arrives on pub_full[];
+// the publisher warp takes over from there (ffn_publisher).
 __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, uint64_t* bars) {
     uint64_t* full = bars + BAR_FULL;
     uint64_t* empty = bars + BAR_EMPTY;
@@ -1348,19 +1404,20 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, u
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int wg = (warp - EPI_WARP0) >> 2;
     const int row0 = wg * 64 + (warp & 3) * 16;   // this warp's 16 rows of the tile
-    uint8_t* stg = smem + OFF_EPI + (warp - EPI_WARP0) * EPI_WARP_BYTES;
+    uint8_t* stg = smem + OFF_EPI + row0 * EPI_ROW_BYTES;   // GEMM1 transpose tile: this warp's rows of buffer 0
     int q = 0, qphase = 0, stage = 0, phase = 0, ps = 0, pphase = 0, ntiles = 0;
+    uint32_t chunk = 0;   // GEMM0 h chunks this warp has staged so far (stage_h)
     const bool stamper = tid == EPI_WARP0 * 32;
     for (;;) {
         mbar_wait(&sched_full[q], qphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, 100 + q);
-        const TileInfo ti = ring[q];
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sched_empty[q]);
-        if (++q == NSCHED) { q = 0; qphase ^= 1; }
-        if (ti.kind < 0) break;
+        // The tile's ring slot stays ours until its epilogue is set up (sched_empty is arrived on below): the per-tile
+        // fields are read from shared memory after the k-block loop instead of being kept live (spilled) across it.
+        const TileInfo* ti = ring + q;
+        const int kind = ti->kind;
+        if (kind < 0) break;
 
         // ---- main loop: one k-block's wgmma group in flight while the previous stage is handed back
-        const int nk = (ti.kind == 0 ? p.H : p.P) / BLOCK_K;
+        const int nk = (kind == 0 ? p.H : p.P) / BLOCK_K;
         float acc[128];
 #pragma unroll
         for (int i = 0; i < 128; ++i) acc[i] = 0.0f;
@@ -1386,63 +1443,77 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, u
             prev = stage;
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
+        // While the last k-block's MMAs run: the tile's fields from its ring slot and, for the fused GEMM1 epilogue,
+        // lane l < 16's routing record of tile row (row0 + l), so that nothing is fetched after the final wait.
+        const int ntile = ti->ntile, le = ti->le, pkt = ti->pkt, mblk = ti->mblk, my_rows = ti->rows, src = ti->src;
+        const bool fuse = p.fused != 0 && kind == 1;
+        int my_tok = 0;
+        float my_pw = 0.0f, my_mcw = 1.0f;
+        if (fuse && p.dense) {
+            my_tok = mblk * BLOCK_M + row0 + lane;   // row i of the only packet IS token i
+        } else if (fuse && lane < 16 && row0 + lane < my_rows) {
+            const uint4 m = ld_global_v4(p.recv_meta + (size_t)pkt * p.pEC + (size_t)mblk * BLOCK_M + row0 + lane);
+            my_tok = (int)m.x;
+            my_pw = __uint_as_float(m.y);
+            my_mcw = __uint_as_float(m.z);
+        }
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
         __syncwarp();
         if (lane == 0 && prev >= 0) mbar_arrive(&empty[prev]);
         if (ntiles < 16 && stamper) trace_stamp(p, 48 + ntiles);
 
-        const int N = ti.kind == 0 ? p.P : p.H;
-        const int n0 = ti.ntile * BLOCK_N;
-        const int my_rows = ti.rows;
-        const __nv_bfloat16* bias = ti.kind == 0 ? (p.b_up ? p.b_up + (size_t)ti.le * p.P : nullptr)
-                                                 : (p.b_down ? p.b_down + (size_t)ti.le * p.H : nullptr);
-        // destination rows: GEMM0 -> local h staging; GEMM1 -> the SOURCE rank's return buffer (peer store),
-        // like the reference's GEMM1 epilogue writing into the peer heap (packet.cuh:338-340, processor.cuh:713-720)
-        __nv_bfloat16* out_rows;
-        if (ti.kind == 0) {
-            out_rows = p.hidden + ((size_t)ti.pkt * p.pEC + (size_t)ti.mblk * BLOCK_M) * p.P;
-        } else {
-            const int e_global = p.rank * p.nLx + ti.le;
-            out_rows = p.peer_ret_y[ti.src] + ((size_t)e_global * p.pEC + (size_t)ti.mblk * BLOCK_M) * p.H;
-        }
-        // 64-column chunks of the tile that exist (N is a multiple of 64, not necessarily of the tile width)
-        const int nchunks = row0 < my_rows ? min(BLOCK_N / 64, (N - n0) / 64) : 0;
-        // fused GEMM1 -> combine: lane l < 16 fetches the routing record of tile row (row0 + l)
-        const bool fuse = p.fused != 0 && ti.kind == 1;
-        int my_tok = 0;
-        float my_pw = 0.0f, my_mcw = 1.0f;
-        if (fuse && p.dense) {
-            my_tok = ti.mblk * BLOCK_M + row0 + lane;   // row i of the only packet IS token i
-        } else if (fuse && lane < 16 && row0 + lane < my_rows) {
-            const uint4 m = ld_global_v4(p.recv_meta + (size_t)ti.pkt * p.pEC + (size_t)ti.mblk * BLOCK_M + row0 + lane);
-            my_tok = (int)m.x;
-            my_pw = __uint_as_float(m.y);
-            my_mcw = __uint_as_float(m.z);
-        }
         if (ntiles == 0 && p.W > 1 && (p.phase_mask & 1u))   // the staging area served as warp 2's window for the remote rows
             asm volatile("bar.sync 7, 288;" ::: "memory");
+        if (lane == 0) mbar_arrive(&sched_empty[q]);   // every lane has read the slot (the __syncwarp above)
+        if (++q == NSCHED) { q = 0; qphase ^= 1; }
         if (ntiles < 16 && stamper) trace_stamp(p, 64 + ntiles);
+
+        const int n0 = ntile * BLOCK_N;
+        if (kind == 0) {
+            // h: every warp stages its 16 rows of each 64-column chunk (N is a multiple of 64, not necessarily of the
+            // tile width) and goes straight on to the next tile; the publisher warp stores and publishes them
+            const int nchunks = min(BLOCK_N / 64, (p.P - n0) / 64);
+            const __nv_bfloat16* bias = p.b_up ? p.b_up + (size_t)le * p.P + n0 : nullptr;
+            if (bias == nullptr) {
+                if (p.act == 0) stage_h<EPI_G0_RELU, false>(p, smem, bars, acc, bias, nchunks, row0, lane, chunk);
+                else stage_h<EPI_G0_GELU, false>(p, smem, bars, acc, bias, nchunks, row0, lane, chunk);
+            } else {
+                if (p.act == 0) stage_h<EPI_G0_RELU, true>(p, smem, bars, acc, bias, nchunks, row0, lane, chunk);
+                else stage_h<EPI_G0_GELU, true>(p, smem, bars, acc, bias, nchunks, row0, lane, chunk);
+            }
+            if (ntiles < 16 && stamper) trace_stamp(p, 80 + ntiles);
+            ++ntiles;
+            continue;
+        }
+
+        // GEMM1: the destination rows are the SOURCE rank's return buffer (peer store), like the reference's GEMM1
+        // epilogue writing into the peer heap (packet.cuh:338-340, processor.cuh:713-720), or with `fuse` the tokens'
+        // output rows there
+        const int N = p.H;
+        const int e_global = p.rank * p.nLx + le;
+        __nv_bfloat16* out_rows = p.peer_ret_y[src] + ((size_t)e_global * p.pEC + (size_t)mblk * BLOCK_M) * p.H;
+        const __nv_bfloat16* bias = p.b_down ? p.b_down + (size_t)le * p.H : nullptr;
+        const int nchunks = row0 < my_rows ? min(BLOCK_N / 64, (N - n0) / 64) : 0;
+        // this warp's transpose tile is its rows of chunk buffer 0, which the TMA may still be reading for the last
+        // GEMM0 tile: wait as stage_h would before buffer 0's next use (chunk `next0`; the wait consumes nothing)
+        const uint32_t next0 = (chunk + 1) & ~1u;
+        mbar_wait(&bars[BAR_STG_FREE], ((next0 >> 1) & 1) ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, 22);
         if (nchunks > 0) {
             DrainArgs da;
             da.stg = stg; da.nchunks = nchunks; da.lane = lane; da.row0 = row0; da.my_rows = my_rows; da.N = N; da.n0 = n0;
-            da.bias = bias; da.out_rows = out_rows; da.acc_base = fuse ? p.peer_out_acc[ti.src] : nullptr;
+            da.bias = bias; da.out_rows = out_rows; da.acc_base = fuse ? p.peer_out_acc[src] : nullptr;
             da.my_tok = my_tok; da.my_pw = my_pw; da.my_mcw = my_mcw;
             // one specialised instantiation per (epilogue kind, bias) pair: no per-element or per-group branching
-            const int mode = ti.kind == 0 ? (p.act == 0 ? EPI_G0_RELU : EPI_G0_GELU)
-                                          : (!fuse ? EPI_G1_STORE : (p.k > 1 ? EPI_G1_FUSED_ADD : EPI_G1_FUSED_COPY));
+            const int mode = !fuse ? EPI_G1_STORE : (p.k > 1 ? EPI_G1_FUSED_ADD : EPI_G1_FUSED_COPY);
             if (bias == nullptr) {
                 switch (mode) {
-                    case EPI_G0_RELU: drain_accumulator<EPI_G0_RELU, false>(p, da, acc); break;
-                    case EPI_G0_GELU: drain_accumulator<EPI_G0_GELU, false>(p, da, acc); break;
                     case EPI_G1_STORE: drain_accumulator<EPI_G1_STORE, false>(p, da, acc); break;
                     case EPI_G1_FUSED_ADD: drain_accumulator<EPI_G1_FUSED_ADD, false>(p, da, acc); break;
                     default: drain_accumulator<EPI_G1_FUSED_COPY, false>(p, da, acc); break;
                 }
             } else {
                 switch (mode) {
-                    case EPI_G0_RELU: drain_accumulator<EPI_G0_RELU, true>(p, da, acc); break;
-                    case EPI_G0_GELU: drain_accumulator<EPI_G0_GELU, true>(p, da, acc); break;
                     case EPI_G1_STORE: drain_accumulator<EPI_G1_STORE, true>(p, da, acc); break;
                     case EPI_G1_FUSED_ADD: drain_accumulator<EPI_G1_FUSED_ADD, true>(p, da, acc); break;
                     default: drain_accumulator<EPI_G1_FUSED_COPY, true>(p, da, acc); break;
@@ -1451,8 +1522,7 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, u
         }
         if (ntiles < 16 && stamper) trace_stamp(p, 80 + ntiles);
 
-        // hand the tile to the publisher: this warp's stores are issued (h will be read through the async proxy)
-        if (ti.kind == 0) fence_proxy_async_global();
+        // hand the tile to the publisher: this warp's stores / REDs are issued
         __syncwarp();
         if (lane == 0) {
             mbar_wait(&pub_empty[ps], pphase ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, ps);
@@ -1463,19 +1533,24 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, u
     }
 }
 
-// warp 2: makes finished tiles visible.  For every tile of the ring, once all consumer warps have issued their stores:
-// GEMM0 -> release-add on the row block's h counter (reference notifyNext's tSA counter, processor.cuh:490-615);
-// GEMM1 -> system-scope fence, then the packet / row-block counter and, from the last tile, the flag on the source rank
-// (reference processor.cuh:722-750).  The fences wait for the stores / REDs to drain (1-2 us, more over NVLink); here
-// they overlap the next tile's MMA instead of delaying it.
+// warp 2: writes h and makes finished tiles visible.  For every tile of the ring:
+// GEMM0 -> one TMA tensor store per 64-column chunk the consumer warps have staged (stage_h), each buffer handed back as
+// soon as the TMA has read it; then, once the stores are complete, the release-add on the row block's h counter
+// (reference notifyNext's tSA counter, processor.cuh:490-615).
+// GEMM1 -> once all consumer warps have issued their stores / REDs: system-scope fence, then the packet / row-block
+// counter and, from the last tile, the flag on the source rank (reference processor.cuh:722-750).  The fences and the
+// store completion take 1-2 us (more over NVLink); here they overlap the next tile's MMA instead of delaying it.
 __device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, uint64_t* bars) {
     uint64_t* sched_full = bars + BAR_SCHED_FULL;
     uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
     uint64_t* pub_full = bars + BAR_PUB_FULL;
     uint64_t* pub_empty = bars + BAR_PUB_EMPTY;
+    uint64_t* stg_full = bars + BAR_STG_FULL;
+    uint64_t* stg_free = bars + BAR_STG_FREE;
     const TileInfo* ring = reinterpret_cast<const TileInfo*>(smem + OFF_RING);
     const int lane = threadIdx.x & 31;
     int q = 0, qphase = 0, ps = 0, pphase = 0, ntiles = 0;
+    uint32_t chunk = 0;   // h chunks stored so far, in the consumers' staging order
     for (;;) {
         int kind = -1;
         if (lane == 0) {
@@ -1483,44 +1558,59 @@ __device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, 
             const TileInfo ti = ring[q];
             mbar_arrive(&sched_empty[q]);
             kind = ti.kind;
-            if (kind >= 0) {
-                const int my_rows = ti.rows, my_mblk = ti.mblk, my_pkt = ti.pkt, my_src = ti.src;
-                mbar_wait(&pub_full[ps], pphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, 10 + ps);
-                mbar_arrive(&pub_empty[ps]);
-                if (my_rows > 0) {
-                    if (kind == 0) {
-                        fence_proxy_async_global();
-                        red_release_gpu_add_u32(p.g0_done + (size_t)my_pkt * p.TCM + my_mblk, 1u);
-                    } else if (p.fused) {
-                        if (my_src == p.rank && p.out_acc == p.out) {
-                            // local packet, output left in place: nobody waits for a flag (see finish_fused) -- no fence,
-                            // no counter, no flag; kernel completion covers these adds
-                        } else {
-                        fence_acq_rel_sys();   // this tile's adds are performed before the packet counter moves
-                        const unsigned int old = atom_acq_rel_gpu_add_u32(p.pkt_done + my_pkt, 1u);
-                        const unsigned int want = (unsigned int)(((ti.cnt + BLOCK_M - 1) / BLOCK_M) * p.TN1);
-                        if (old + 1u == want) {   // every GEMM1 tile of packet (src, le) has been added into src's output
-                            st_release_sys_u64(p.peer_done_flag[my_src] + (size_t)(p.rank * p.nLx + ti.le),
-                                               (unsigned long long)p.epoch << 32);
-                        }
-                        }
-                    } else {
-                        fence_acq_rel_sys();
-                        const unsigned int old = atom_acq_rel_gpu_add_u32(p.g1_done + (size_t)my_pkt * p.TCM + my_mblk, 1u);
-                        if (old == (unsigned int)p.TN1 - 1u) {  // whole rows of this block are on the source rank
-                            fence_acq_rel_sys();
-                            const int e_global = p.rank * p.nLx + ti.le;
-                            st_release_sys_u64(p.peer_ret_flag[my_src] + (size_t)e_global * p.TCM + my_mblk,
-                                               ((unsigned long long)p.epoch << 32) | (unsigned int)my_rows);
-                        }
+            const int my_rows = ti.rows, my_mblk = ti.mblk, my_pkt = ti.pkt, my_src = ti.src;
+            if (kind == 0) {
+                const int n0 = ti.ntile * BLOCK_N, nchunks = min(BLOCK_N / 64, (p.P - n0) / 64);
+                const int row = my_pkt * p.pEC + my_mblk * BLOCK_M;
+                // both buffers' stores in flight: chunk c is issued as soon as it is staged, and only then does the
+                // warp wait for the TMA to have read chunk c - 1, whose buffer the consumers refill with chunk c + 1
+                for (int c = 0; c < nchunks; ++c, ++chunk) {
+                    const int b = chunk & 1;
+                    mbar_wait(&stg_full[b], (chunk >> 1) & 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, 30 + b);
+                    tma_store_2d(&p.tm_a1, smem + OFF_EPI + b * EPI_CHUNK_BYTES, n0 + c * 64, row);
+                    bulk_commit_group();
+                    if (c > 0) {
+                        bulk_wait_group_read<1>();   // chunk c - 1 has been read: its buffer may be refilled
+                        mbar_arrive(&stg_free[b ^ 1]);
                     }
                 }
-                if (ntiles < 16) trace_stamp(p, 96 + ntiles);
+                bulk_wait_group_read<0>();
+                mbar_arrive(&stg_free[(chunk - 1) & 1]);
+                bulk_wait_group0();            // the tile's h writes (async proxy) are complete ...
+                fence_proxy_async_global();    // ... and ordered before the generic-proxy release below
+                red_release_gpu_add_u32(p.g0_done + (size_t)my_pkt * p.TCM + my_mblk, 1u);
+            } else if (kind == 1) {
+                mbar_wait(&pub_full[ps], pphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, 10 + ps);
+                mbar_arrive(&pub_empty[ps]);
+                if (++ps == 2) { ps = 0; pphase ^= 1; }
+                if (p.fused) {
+                    if (my_src == p.rank && p.out_acc == p.out) {
+                        // local packet, output left in place: nobody waits for a flag (see finish_fused) -- no fence,
+                        // no counter, no flag; kernel completion covers these adds
+                    } else {
+                    fence_acq_rel_sys();   // this tile's adds are performed before the packet counter moves
+                    const unsigned int old = atom_acq_rel_gpu_add_u32(p.pkt_done + my_pkt, 1u);
+                    const unsigned int want = (unsigned int)(((ti.cnt + BLOCK_M - 1) / BLOCK_M) * p.TN1);
+                    if (old + 1u == want) {   // every GEMM1 tile of packet (src, le) has been added into src's output
+                        st_release_sys_u64(p.peer_done_flag[my_src] + (size_t)(p.rank * p.nLx + ti.le),
+                                           (unsigned long long)p.epoch << 32);
+                    }
+                    }
+                } else {
+                    fence_acq_rel_sys();
+                    const unsigned int old = atom_acq_rel_gpu_add_u32(p.g1_done + (size_t)my_pkt * p.TCM + my_mblk, 1u);
+                    if (old == (unsigned int)p.TN1 - 1u) {  // whole rows of this block are on the source rank
+                        fence_acq_rel_sys();
+                        const int e_global = p.rank * p.nLx + ti.le;
+                        st_release_sys_u64(p.peer_ret_flag[my_src] + (size_t)e_global * p.TCM + my_mblk,
+                                           ((unsigned long long)p.epoch << 32) | (unsigned int)my_rows);
+                    }
+                }
             }
+            if (kind >= 0 && ntiles < 16) trace_stamp(p, 96 + ntiles);
         }
         kind = __shfl_sync(0xffffffffu, kind, 0);
         if (++q == NSCHED) { q = 0; qphase ^= 1; }
-        if (++ps == 2) { ps = 0; pphase ^= 1; }
         ++ntiles;
         if (kind < 0) break;
         __syncwarp();
@@ -1532,12 +1622,17 @@ __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BARS);
     const int tid = threadIdx.x, warp = tid >> 5;
     if (warp == 1 && (tid & 31) == 0) {
-        // arrival counts: full = the producer's expect_tx; empty = one lane per consumer warp; pub_full = one lane per
-        // consumer warp; sched_empty = every ring reader (producer, publisher, consumer warps)
+        // arrival counts: full = the producer's expect_tx; empty = one lane per consumer warp; pub_full and stg_full =
+        // one lane per consumer warp; stg_free = the publisher; sched_empty = every ring reader (producer, publisher,
+        // consumer warps)
         for (int i = 0; i < STAGES; ++i) { mbar_init(&bars[BAR_FULL + i], 1); mbar_init(&bars[BAR_EMPTY + i], NUM_EPI_WARPS); }
         for (int i = 0; i < 2; ++i) {
             mbar_init(&bars[BAR_PUB_FULL + i], NUM_EPI_WARPS);
             mbar_init(&bars[BAR_PUB_EMPTY + i], 1);
+        }
+        for (int i = 0; i < EPI_BUFS; ++i) {
+            mbar_init(&bars[BAR_STG_FULL + i], NUM_EPI_WARPS);
+            mbar_init(&bars[BAR_STG_FREE + i], 1);
         }
         for (int i = 0; i < NSCHED; ++i) {
             mbar_init(&bars[BAR_SCHED_FULL + i], 1);

@@ -222,6 +222,9 @@ __device__ __forceinline__ void bulk_store_1d(void* gdst, const void* smem_src, 
 }
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// until at most N committed bulk groups of this thread still have to read their smem source
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 // shared-memory only: generic-proxy accesses to smem <-> async-proxy (TMA) accesses to the same smem; does not wait for
@@ -240,6 +243,13 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, in
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
+}
+// 2-D tiled bulk tensor store, shared -> global, tracked with bulk async-groups (bulk_commit_group / bulk_wait_group*).
+// The smem source must hold the box in the tensor map's swizzled layout; rows outside the tensor are not written.
+__device__ __forceinline__ void tma_store_2d(const void* tmap, const void* smem_src, int32_t c0, int32_t c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(tmap), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+                 : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -367,6 +377,16 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
     return *reinterpret_cast<uint32_t*>(&v);
 }
 __device__ __forceinline__ float bf16_bits_to_f32(uint32_t bits16) { return __uint_as_float(bits16 << 16); }
+// a ^ b that the compiler cannot hoist or fold into precomputed values (keeps swizzled smem addresses out of registers
+// across loops)
+__device__ __forceinline__ uint32_t xor_u32(uint32_t a, uint32_t b) {
+    uint32_t r;
+    asm volatile("xor.b32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(b));
+    return r;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
 __device__ __forceinline__ float rne_bf16(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
 
 }  // namespace fm
