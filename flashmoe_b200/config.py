@@ -108,7 +108,12 @@ class MoEConfig:
 
     @property
     def EC(self) -> int:  # expert capacity in token-expert pairs per source rank (types.cuh:497)
-        base = _ceil_div(self.S, self.E) if self.drop_tokens else self.S
+        return self.EC_of(self.S)
+
+    def EC_of(self, n_tokens: int) -> int:
+        """Expert capacity of a forward over `n_tokens` tokens (MoEContext.forward_tokens): what a config with
+        S = n_tokens has as EC."""
+        base = _ceil_div(n_tokens, self.E) if self.drop_tokens else n_tokens
         return base * self.capacity_factor * self.k
 
     @property

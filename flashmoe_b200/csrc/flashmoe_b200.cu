@@ -102,7 +102,9 @@ struct fm_ctx {
     int device = 0;
     int grid = 0;
     int tpc = 0;
-    int TN0 = 0, TN1 = 0, num_pkts = 0, num_blocks = 0, total_items = 0;
+    int TN0 = 0, TN1 = 0, num_pkts = 0, num_blocks = 0;
+    int g0_blocks = 0, g1_blocks = 0;   // GEMM0 / GEMM1 blocks of the work list (items = their tiles x row blocks per packet)
+    int last_tokens = 0;                // token count of the last launch (a partial-phase launch reuses its routing)
     int claim_ahead_kb = 16;
     int dbg_flags = 0;
     bool coop = true;    // cooperative launch attribute (validates co-residency of the persistent grid)
@@ -143,12 +145,14 @@ struct fm_ctx {
     bool fused = false;   // GEMM1 epilogue adds straight into the source rank's output (no return buffer / gather)
     bool dense = false;   // E == 1: GEMM0 reads x in place, no router GEMV, no dispatch copy (reference fffn.cuh:31-167)
     float* aux = nullptr; // is_training: [2][2E+1] {gML, gMeC, loss} by epoch parity
-    const void* cached_x = nullptr;
+    const void* cached_x = nullptr;     // the maps over the caller's x (tm_a0 when dense, tm_gx) are keyed on pointer AND
+    int cached_x_rows = 0;              // row count: a map with more rows than this call's x would read past it
     int* recv_tok = nullptr;            // [nLx, pEC] slot -> token of the local packets (gather-mode source rows)
     unsigned int* tok_rows = nullptr;   // [2, nLx, TCM]
     int gather = 0;                     // FM_GATHER: 0 off, 1 early tiles only, 2 every local GEMM0 tile (tests)
     bool tc_gate = false;               // router logits on the tensor cores (E <= 256)
     const void* cached_gx = nullptr;
+    int cached_gx_rows = 0;
     const void* cached_gw = nullptr;
     CUtensorMap tm_gx, tm_gw;
     unsigned int* pkt_done = nullptr;
@@ -166,6 +170,11 @@ struct fm_ctx {
 };
 
 namespace {
+
+// expert capacity of n tokens in token-expert pairs per (source rank, expert) packet (reference types.cuh:497)
+long long expert_capacity(const fm_config_t& c, long long n) {
+    return (c.drop_tokens ? (n + c.num_experts - 1) / c.num_experts : n) * c.capacity_factor * c.expert_top_k;
+}
 
 int validate_config(const fm_config_t& c, int world, fm_dims_t* d) {
     if (c.torch_dtype != 2) return fail(FM_EINVAL, "torch_dtype=%d: this build computes in bf16 only (2)", c.torch_dtype);
@@ -193,8 +202,7 @@ int validate_config(const fm_config_t& c, int world, fm_dims_t* d) {
     d->PX = ceil_div(c.num_experts, 64) * 64;
     d->element_size = 2;
     d->k = c.expert_top_k;
-    const long long ec = (long long)(c.drop_tokens ? ceil_div((int)S, c.num_experts) : (int)S) * c.capacity_factor *
-                         c.expert_top_k;
+    const long long ec = expert_capacity(c, S);
     if (ec > (1ll << 24)) return fail(FM_EINVAL, "expert capacity %lld too large", ec);
     d->EC = (int)ec;
     d->pEC = ceil_div(d->EC, 128) * 128;
@@ -249,10 +257,15 @@ int check_kernel_status(fm_ctx* c) {
     return FM_OK;
 }
 
-int launch(fm_ctx* c, const void* x, const void* gate_w, const void* expert_w, const void* bias_up,
+// One forward of n_tok tokens (0 <= n_tok <= S): the call computes exactly what a context created for n_tok tokens
+// would -- capacity EC(n_tok), tokens per CTA ceil(n_tok / grid), maps over x with n_tok rows -- while every buffer keeps
+// its create-time (maximum) size and stride.
+int launch(fm_ctx* c, const void* x, int n_tok, const void* gate_w, const void* expert_w, const void* bias_up,
            const void* bias_down, void* out, cudaStream_t stream, uint32_t phase_mask) {
     if (c == nullptr) return fail(FM_EINVAL, "null context");
-    if (x == nullptr || gate_w == nullptr || expert_w == nullptr || out == nullptr)
+    if ((phase_mask & 1u) == 0u) n_tok = c->last_tokens;   // later phases only: the previous launch's routing and count
+    if (n_tok < 0 || n_tok > c->d.S) return fail(FM_EINVAL, "n_tokens = %d not in [0, S = %d]", n_tok, c->d.S);
+    if (gate_w == nullptr || expert_w == nullptr || (n_tok > 0 && (x == nullptr || out == nullptr)))
         return fail(FM_EINVAL, "x, gate_w, expert_w and out must be non-null device pointers");
     {   // TMA tensor maps, cp.async.bulk row copies and the 16-byte vector accesses all need 16-byte aligned bases
         const void* ptrs[] = {x, gate_w, expert_w, bias_up, bias_down, out};
@@ -268,17 +281,21 @@ int launch(fm_ctx* c, const void* x, const void* gate_w, const void* expert_w, c
     const fm_dims_t& d = c->d;
     const int nLx = d.num_local_experts;
     int rc;
-    if (c->dense && c->cached_x != x) {   // E == 1: the A operand of GEMM0 is the caller's x itself
-        if ((rc = make_tmap(&c->tm_a0, x, (uint64_t)d.S, d.H, fm::BLOCK_M))) return rc;
+    // The maps over the caller's x have exactly n_tok rows (a box taller than that reads the missing rows as zero).  With
+    // no tokens nothing reads x, and no map is encoded.
+    if (c->dense && n_tok > 0 && (c->cached_x != x || c->cached_x_rows != n_tok)) {   // E == 1: GEMM0's A operand is x
+        if ((rc = make_tmap(&c->tm_a0, x, (uint64_t)n_tok, d.H, fm::BLOCK_M))) return rc;
         c->cached_x = x;
+        c->cached_x_rows = n_tok;
     }
     if (c->tc_gate) {
-        // router on tensor cores: x as [S, H] in 32-row boxes, Wg_eff = the [H, E] tensor read flat as [E, H]
+        // router on tensor cores: x as [n_tok, H] in 32-row boxes, Wg_eff = the [H, E] tensor read flat as [E, H]
         // (python_bindings.cu:93-99, moe.cuh:107-109) in boxes of min(128, E rounded up to 64) rows; rows past E read as
         // zero
-        if (c->cached_gx != x) {
-            if ((rc = make_tmap(&c->tm_gx, x, (uint64_t)d.S, d.H, 32))) return rc;
+        if (n_tok > 0 && (c->cached_gx != x || c->cached_gx_rows != n_tok)) {
+            if ((rc = make_tmap(&c->tm_gx, x, (uint64_t)n_tok, d.H, 32))) return rc;
             c->cached_gx = x;
+            c->cached_gx_rows = n_tok;
         }
         if (c->cached_gw != gate_w) {
             const uint32_t e64 = (uint32_t)((d.E + 63) / 64 * 64);
@@ -307,10 +324,14 @@ int launch(fm_ctx* c, const void* x, const void* gate_w, const void* expert_w, c
     p.tm_a0 = c->tm_a0; p.tm_b0 = c->tm_b0; p.tm_a1 = c->tm_a1; p.tm_b1 = c->tm_b1;
     if (c->tc_gate) { p.tm_gx = c->tm_gx; p.tm_gw = c->tm_gw; }
     p.tc_gate = c->tc_gate ? 1 : 0;
-    p.S = d.S; p.H = d.H; p.P = d.P; p.E = d.E; p.k = d.k; p.W = d.world; p.rank = d.rank; p.nLx = nLx;
-    p.EC = d.EC; p.pEC = d.pEC; p.TCM = d.TCM; p.act = c->cfg.hidden_act;
-    p.TN0 = c->TN0; p.TN1 = c->TN1; p.tpc = c->tpc; p.num_pkts = c->num_pkts; p.num_blocks = c->num_blocks;
-    p.total_items = c->total_items;
+    const int ec = (int)expert_capacity(c->cfg, n_tok);
+    p.S = n_tok; p.H = d.H; p.P = d.P; p.E = d.E; p.k = d.k; p.W = d.world; p.rank = d.rank; p.nLx = nLx;
+    p.EC = ec; p.pEC = d.pEC; p.TCM = d.TCM; p.act = c->cfg.hidden_act;
+    p.TN0 = c->TN0; p.TN1 = c->TN1; p.tpc = ceil_div(n_tok, c->grid); p.num_pkts = c->num_pkts; p.num_blocks = c->num_blocks;
+    // one rank knows every packet's capacity, so the work list shrinks to this call's row blocks; a receiver with peers
+    // does not know their token counts and keeps the maximum (the empty row blocks are skipped by the scheduler)
+    p.tcm_items = d.world == 1 ? ceil_div(ec, fm::BLOCK_M) : d.TCM;
+    p.total_items = (c->g0_blocks * c->TN0 + c->g1_blocks * c->TN1) * p.tcm_items;
     p.claim_ahead_kb = c->claim_ahead_kb; p.dbg_flags = c->dbg_flags; p.prefetch_kb = c->prefetch_kb;
     // the epoch and the grid-barrier target advance only when the launch has been accepted (see below): a failed launch
     // must not leave the host ahead of the device counter and of the peers
@@ -368,6 +389,7 @@ int launch(fm_ctx* c, const void* x, const void* gate_w, const void* expert_w, c
     lc.attrs = attrs;
     lc.numAttrs = na;
     FM_CUDA(cudaLaunchKernelEx(&lc, fm::fm_moe_forward_kernel, p));
+    c->last_tokens = n_tok;
     c->epoch = epoch;
     c->bar_count = bar_count;
     c->launches += 1;
@@ -485,18 +507,19 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
     ctx->num_pkts = world * nLx;
 
     // Work list.  Sources in the order own rank, rank+1, ... (local rows need no NVLink hop, so they are ready first).
-    // A work item is one 128 x 256 output tile of one packet.
+    // A work item is one 128 x 256 output tile of one packet.  The table stores, per block, how many GEMM0 and GEMM1 blocks
+    // precede it; the kernel derives the block's first item from the call's row blocks per packet (fm::block_start).
     struct Unit { int pkt; bool local; };
     std::vector<Unit> units;
     for (int j = 0; j < world; ++j)
         for (int le = 0; le < nLx; ++le) units.push_back({((rank + j) % world) * nLx + le, j == 0});
     std::vector<fm::TileBlock> blocks;
-    int start = 0;
+    int n_g[2] = {0, 0};
     auto push = [&](int kind, const Unit& u) {
         fm::TileBlock b;
-        b.kind = kind; b.pkt = u.pkt; b.start = start; b.pad = 0;
+        b.kind = kind; b.pkt = u.pkt; b.g0 = n_g[0]; b.g1 = n_g[1];
         blocks.push_back(b);
-        start += d.TCM * (kind == 0 ? ctx->TN0 : ctx->TN1);
+        ++n_g[kind];
     };
     // GEMM0: local sources first (their rows are acknowledged first), then rank+1, rank+2, ...  GEMM1: REMOTE sources
     // first, local last -- the outputs of remote packets cross NVLink as reductions and their done flags have a link round
@@ -538,9 +561,10 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
         for (const Unit& u : g1_units) push(1, u);
     }
     ctx->num_blocks = (int)blocks.size();
-    ctx->total_items = start;
+    ctx->g0_blocks = n_g[0];
+    ctx->g1_blocks = n_g[1];
     fm::TileBlock sentinel;
-    sentinel.kind = -1; sentinel.pkt = 0; sentinel.start = start; sentinel.pad = 0;
+    sentinel.kind = -1; sentinel.pkt = 0; sentinel.g0 = n_g[0]; sentinel.g1 = n_g[1];
     blocks.push_back(sentinel);
 
 #define FM_TRY(expr)          \
@@ -731,15 +755,22 @@ FM_API int fm_symm_attach_ptrs(fm_ctx_t* ctx, void* const* peer_bases) {
     return FM_OK;
 }
 
+FM_API int fm_moe_forward_tokens(fm_ctx_t* ctx, const void* x, int n_tokens, const void* gate_w, const void* expert_w,
+                                 const void* bias_up, const void* bias_down, void* out, void* stream) {
+    return launch(ctx, x, n_tokens, gate_w, expert_w, bias_up, bias_down, out, static_cast<cudaStream_t>(stream), 7u);
+}
+
 FM_API int fm_moe_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, const void* expert_w, const void* bias_up,
                           const void* bias_down, void* out, void* stream) {
-    return launch(ctx, x, gate_w, expert_w, bias_up, bias_down, out, static_cast<cudaStream_t>(stream), 7u);
+    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
+    return fm_moe_forward_tokens(ctx, x, ctx->d.S, gate_w, expert_w, bias_up, bias_down, out, stream);
 }
 
 FM_API int fm_debug_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, const void* expert_w,
                             const void* bias_up, const void* bias_down, void* out, void* stream, uint32_t phase_mask) {
     if (phase_mask == 0 || phase_mask > 7u) return fail(FM_EINVAL, "phase_mask must be in [1, 7]");
-    return launch(ctx, x, gate_w, expert_w, bias_up, bias_down, out, static_cast<cudaStream_t>(stream), phase_mask);
+    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
+    return launch(ctx, x, ctx->d.S, gate_w, expert_w, bias_up, bias_down, out, static_cast<cudaStream_t>(stream), phase_mask);
 }
 
 // ---- host-buffer entry points -----------------------------------------------------------------------------------
@@ -777,7 +808,7 @@ FM_API int fm_host_submit(fm_ctx_t* ctx, const void* x_host, const void* gate_w,
     FM_CUDA(cudaMemcpyAsync(ctx->x_stage[slot], x_host, bytes, cudaMemcpyHostToDevice, ctx->s_h2d));
     FM_CUDA(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
     FM_CUDA(cudaStreamWaitEvent(s, ctx->ev_h2d[slot], 0));
-    if ((rc = launch(ctx, ctx->x_stage[slot], gate_w, expert_w, bias_up, bias_down, ctx->out_stage[slot], s, 7u))) return rc;
+    if ((rc = launch(ctx, ctx->x_stage[slot], ctx->d.S, gate_w, expert_w, bias_up, bias_down, ctx->out_stage[slot], s, 7u))) return rc;
     FM_CUDA(cudaEventRecord(ctx->ev_kernel[slot], s));
     FM_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_kernel[slot], 0));
     FM_CUDA(cudaMemcpyAsync(out_host, ctx->out_stage[slot], bytes, cudaMemcpyDeviceToHost, ctx->s_d2h));

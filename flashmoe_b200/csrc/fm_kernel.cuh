@@ -103,8 +103,7 @@ static_assert(G_OFF_BASE + 12288 <= OFF_EPI, "gate scratch must fit in the stage
 struct TileBlock {  // one contiguous run of work items: all tiles of one GEMM of one packet (or of a packet pair)
     int kind;       // 0 = GEMM0 (x.W_up^T), 1 = GEMM1 (h.W_down^T)
     int pkt;        // local packet index = src * nLx + le
-    int start;      // first global item id of this block
-    int pad;
+    int g0, g1;     // GEMM0 / GEMM1 blocks before this one in the work list (block_start)
 };
 
 struct FmParams {
@@ -112,11 +111,14 @@ struct FmParams {
     CUtensorMap tm_b0;  // expert_weights as [nLx*2*P, H]  box {64, 128}  (W_up rows)
     CUtensorMap tm_a1;  // hidden  as [W*nLx*pEC, P]  box {64, 128}: GEMM1's A loads and GEMM0's h stores
     CUtensorMap tm_b1;  // expert_weights as [nLx*2*H, P]  box {64, 128}  (W_down rows)
-    CUtensorMap tm_gx;  // router on tensor cores: x as [S, H], box {64, 32}
+    CUtensorMap tm_gx;  // router on tensor cores: x as [S, H] (S = this call's tokens), box {64, 32}
     CUtensorMap tm_gw;  // router on tensor cores: Wg_eff [E, H], box {64, min(128, E rounded up to 64)}
     int tc_gate;        // 1 = logits by wgmma (E <= 256); 0 = register-blocked CUDA-core GEMV
+    // Per call: S = this call's tokens (<= the context's maximum), EC = its capacity, tpc = ceil(S / grid).  pEC and TCM
+    // are the context's maximum and are only strides of the per-packet buffers.
     int S, H, P, E, k, W, rank, nLx, EC, pEC, TCM, act;
     int TN0, TN1, tpc, num_pkts, num_blocks, total_items;
+    int tcm_items;      // row blocks per packet in the work list: TCM of this call's EC at W == 1, the maximum TCM at W > 1
     int claim_ahead_kb; // the scheduler claims the next tile when this many k-blocks of the current one remain
     int prefetch_kb;    // L2 prefetch distance of the TMA producer in k-blocks (0 = off)
     int dbg_flags;      // experiments only (results are garbage for bits 0-3): bit0 = skip all TMA loads, bit1 = skip MMA
@@ -137,7 +139,7 @@ struct FmParams {
     unsigned int* g1_done;     // [num_pkts, TCM]
     unsigned long long* grid_bar;
     int* recv_cnt;             // [num_pkts]
-    const TileBlock* blocks;   // [num_blocks + 1] (sentinel start = total_items)
+    const TileBlock* blocks;   // [num_blocks + 1] (the sentinel's block_start = total_items)
     __nv_bfloat16* hidden;     // [W*nLx*pEC, P]
     __nv_bfloat16* recv_x;     // local symmetric: [W, nLx, pEC, H]
     unsigned long long* recv_flag;  // [W, nLx]  {epoch, rows}: published as soon as the source rank knows the count
@@ -172,6 +174,12 @@ struct FmParams {
     DebugRecord* dbg;
     unsigned long long* trace;  // optional [grid][TRACE_SLOTS] %globaltimer stamps (nullptr = off)
 };
+
+// first work item of block b: every earlier block holds tcm_items row blocks times its GEMM's column tiles, so the item
+// space follows the call's row-block count without rebuilding the table
+__device__ __forceinline__ int block_start(const FmParams& p, const TileBlock& b) {
+    return (b.g0 * p.TN0 + b.g1 * p.TN1) * p.tcm_items;
+}
 
 // ------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void trace_stamp(const FmParams& p, int slot) {
@@ -333,9 +341,9 @@ __device__ __forceinline__ void gate_phase_dense(const FmParams& p, int t0, int 
         p.slot[t] = t;
     }
     if (blockIdx.x == 0 && tid == 0) {
-        p.counts[0] = p.S;
+        p.counts[0] = p.S;   // this call's tokens
         p.recv_cnt[0] = p.S;
-        if (p.aux != nullptr) {   // mean probability 1, routed fraction 1, loss 1 * 1 / 1
+        if (p.aux != nullptr && p.S > 0) {   // mean probability 1, routed fraction 1, loss 1 * 1 / 1 (no tokens: all zero)
             float* a = p.aux + (size_t)(p.epoch & 1u) * 3;
             a[0] = 1.0f; a[1] = 1.0f; a[2] = 1.0f;
         }
@@ -683,7 +691,7 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, uint8_t* smem, int
         mbar_arrive_expect_tx(xbar, (uint32_t)(rows0 * row_bytes));
         bulk_load_1d(smem, p.x + (size_t)t0 * H, (uint32_t)(rows0 * row_bytes), xbar);
     }
-    if (p.aux != nullptr) {   // gML[e] += (sum over this chunk) / S   (gate.cuh:628-634: atomicAdd(gML + e, colAgg / S))
+    if (p.aux != nullptr && p.S > 0) {   // gML[e] += (sum over this chunk) / S   (gate.cuh:628-634: atomicAdd(gML + e, colAgg / S))
         float* gml = p.aux + (size_t)(p.epoch & 1u) * (2 * E + 1);
         for (int e = tid; e < E; e += NUM_THREADS) atomicAdd(gml + e, __fdividef(aux_s[e], (float)p.S));
     }
@@ -807,7 +815,8 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
         const int owner = e / p.nLx, le = e - owner * p.nLx;
         st_relaxed_sys_u64(p.peer_recv_flag[owner] + (size_t)p.rank * p.nLx + le,
                            ((unsigned long long)p.epoch << 32) | (unsigned int)rows);
-        if (p.aux != nullptr) {
+        if (owner == p.rank) p.recv_cnt[p.rank * p.nLx + le] = rows;   // (also when the work list is empty: S = 0)
+        if (p.aux != nullptr && p.S > 0) {   // (S = 0: the buffer stays as cleared, all zero)
             // gMeC[e] = selections of e / S (gate.cuh:698-706 adds each tile's count / S; the chunk totals are summed
             // first here), loss += gML[e] * gMeC[e] / E (gate.cuh:763-773).  Every CTA's gML atomics precede its arrival
             // at the grid barrier, so gML is complete here.
@@ -1039,9 +1048,10 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
 // ============================================================================================================
 // Phase F: expert FFN.  Work items (global order, claimed with one atomic counter by the scheduler warp):
 //   packets in the order (own rank first, then rank+1, ...); all GEMM0 blocks, then the GEMM1 blocks (host knob FM_G1_LAG
-//   interleaves them with a lag instead).  item -> (row block m fastest, column tile n).  The item list is a static
-//   superset: row blocks beyond the packet's row count are skipped once the packet flag is known.  A GEMM1 tile waits for
-//   g0_done[pkt][m] == TN0.
+//   interleaves them with a lag instead).  item -> (row block m fastest, column tile n).  Every packet holds tcm_items row
+//   blocks per column tile: on one rank the TCM of this call's capacity, with several ranks (where a receiver does not
+//   know its peers' token counts) the context's maximum.  Either way the list is a superset: row blocks beyond the
+//   packet's row count are skipped once the packet flag is known.  A GEMM1 tile waits for g0_done[pkt][m] == TN0.
 // ============================================================================================================
 struct TileInfo {     // written by the scheduler warp, read by the producer / consumer / publisher warps
     int kind;         // 0 GEMM0, 1 GEMM1, -1 stop
@@ -1080,14 +1090,14 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, uint8_t* smem, 
             const int id = (int)atomicAdd(p.claim, 1u);
             if (id >= p.total_items) break;
             if (n < 16) trace_stamp(p, 112 + n);   // claim time of tile n (ready time is slot 16+n)
-            while (id >= p.blocks[cursor + 1].start) ++cursor;
+            while (id >= block_start(p, p.blocks[cursor + 1])) ++cursor;
             const TileBlock blk = p.blocks[cursor];
-            const int local = id - blk.start;
-            const int mb = local % p.TCM, nt = local / p.TCM;   // row blocks fastest
+            const int local = id - block_start(p, blk);
+            const int mb = local % p.tcm_items, nt = local / p.tcm_items;   // row blocks fastest
             const int pkt = blk.pkt, le = pkt % p.nLx, src = pkt / p.nLx;
             const bool same_gpu = src == p.rank;   // flag and counters written from this GPU: gpu scope suffices
             // wait for the packet (src, le): flag = {epoch, rows}  (reference subscriber.cuh:52-185)
-            unsigned long long f = ((unsigned long long)p.epoch << 32) | (unsigned int)p.S;   // dense: all S rows, in x
+            unsigned long long f = ((unsigned long long)p.epoch << 32) | (unsigned int)p.S;   // dense: all of the call's rows, in x
             bool stale = false;
             if (!p.dense) {
                 SpinGuard g;
@@ -1647,7 +1657,8 @@ __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
         fence_mbar_init();
     }
     if (warp == 0 && (tid & 31) == 0) {
-        tma_prefetch_desc(&p.tm_a0); tma_prefetch_desc(&p.tm_b0);
+        if (!p.dense || p.S > 0) tma_prefetch_desc(&p.tm_a0);   // (dense, no tokens: no map over x was encoded)
+        tma_prefetch_desc(&p.tm_b0);
         tma_prefetch_desc(&p.tm_a1); tma_prefetch_desc(&p.tm_b1);
     }
     if (warp == 3 && (tid & 31) == 0 && (p.phase_mask & 3u) == 3u) {
@@ -1657,10 +1668,10 @@ __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
         const int id = (int)blockIdx.x;
         if (id < p.total_items) {
             int cur = 0;
-            while (id >= p.blocks[cur + 1].start) ++cur;
+            while (id >= block_start(p, p.blocks[cur + 1])) ++cur;
             const TileBlock blk = p.blocks[cur];
-            const int local = id - blk.start;
-            const int nt = local / p.TCM, le = blk.pkt % p.nLx;
+            const int local = id - block_start(p, blk);
+            const int nt = local / p.tcm_items, le = blk.pkt % p.nLx;
             const CUtensorMap* tb = blk.kind == 0 ? &p.tm_b0 : &p.tm_b1;
             const int b0 = (blk.kind == 0 ? le * 2 * p.P : (le * 2 + 1) * p.H) + nt * BLOCK_N;
             const int nk_w = (blk.kind == 0 ? p.H : p.P) / BLOCK_K;

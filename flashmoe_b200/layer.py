@@ -14,9 +14,9 @@ from .runtime import MoEContext
 
 class MoEOutput(NamedTuple):
     out: torch.Tensor                 # [B, T, H] bf16
-    topk_idx: torch.Tensor            # [S, k] int32   expert picked per token, in pick order
-    topk_weight: torch.Tensor         # [S, k] bf16    gateOut[t, e_j] (bf16-rounded softmax probability)
-    slot: torch.Tensor                # [S, k] int32   slot in the (rank, expert) packet; >= capacity means dropped
+    topk_idx: torch.Tensor            # [B*T, k] int32   expert picked per token, in pick order
+    topk_weight: torch.Tensor         # [B*T, k] bf16    gateOut[t, e_j] (bf16-rounded softmax probability)
+    slot: torch.Tensor                # [B*T, k] int32   slot in the (rank, expert) packet; >= capacity means dropped
     aux_loss: Optional[torch.Tensor] = None   # is_training = 1: f32 [2E+1] = gML[E] | gMeC[E] | load-balancing loss
 
 
@@ -49,15 +49,20 @@ class FlashMoELayer(torch.nn.Module):
 
     @torch.no_grad()
     def forward(self, x: torch.Tensor, return_routing: bool = False):
-        """x [B, T, H] bf16 on this layer's device with B*T == S.  Asynchronous on torch's current stream unless
-        `return_routing` (reading the routing tables synchronises)."""
-        out = self.ctx.forward(x, self.gate_weight, self.expert_weight, bias_up=self.bias_up, bias_down=self.bias_down)
+        """x [B, T, H] bf16 on this layer's device with B*T <= S (the capacity is that of B*T tokens,
+        `cfg.EC_of(B*T)`).  Asynchronous on torch's current stream unless `return_routing` (reading the routing tables
+        synchronises)."""
+        if x.dim() != 3:
+            raise RuntimeError("Input must be 3D [batch, seq, H]")
+        out = self.ctx.forward_tokens(x, self.gate_weight, self.expert_weight, bias_up=self.bias_up,
+                                      bias_down=self.bias_down)
         if not return_routing:
             return out
         self.ctx.synchronize()
-        idx = torch.from_numpy(self.ctx.read("topk_idx"))
-        w = torch.from_numpy(self.ctx.read("topk_w").view("int16")).view(torch.bfloat16)
-        slot = torch.from_numpy(self.ctx.read("slot"))
+        n = self.ctx.last_tokens
+        idx = torch.from_numpy(self.ctx.read("topk_idx")[:n].copy())
+        w = torch.from_numpy(self.ctx.read("topk_w")[:n].view("int16").copy()).view(torch.bfloat16)
+        slot = torch.from_numpy(self.ctx.read("slot")[:n].copy())
         aux = torch.from_numpy(self.ctx.read("aux_loss")) if self.cfg.is_training else None
         return MoEOutput(out, idx, w, slot, aux)
 

@@ -102,6 +102,7 @@ class MoEContext:
         self.cfg = cfg if cfg is not None else _lib.compiled_config()
         if timeout_ms is not None:
             _lib.check(self._L.fm_set_timeout_ms(self._ctx, int(timeout_ms)))
+        self.last_tokens = 0   # tokens of the last forward (valid rows of the routing tables `read` returns)
         self.symmetric = (symmetric or os.environ.get("FM_SYMM") or "ipc").lower()
         self._symm_tensor = None   # keeps an externally allocated slab alive
         if world > 1:
@@ -171,18 +172,36 @@ class MoEContext:
             raise RuntimeError(f"Expert weights must be [*, 2, P={d['P']}, H={d['H']}]. Got [*, 2, "
                                f"{expert_weights.size(2)}, {expert_weights.size(3)}]")
 
-    def _validate(self, input: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor) -> None:
-        """Same conditions as the reference's TORCH_CHECKs (python_bindings.cu:22-65) plus dtype and alignment checks."""
+    def _validate(self, input: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor,
+                  exact_s: bool = True) -> int:
+        """Same conditions as the reference's TORCH_CHECKs (python_bindings.cu:22-65) plus dtype and alignment checks.
+        `exact_s`: the input is [batch, seq, H] with batch*seq == S (forward); otherwise any [..., H] holding at most S
+        tokens (forward_tokens).  Returns the number of tokens."""
         d = self.dims
         _check_tensor("Input", input, self.device)
-        if input.dim() != 3:
-            raise RuntimeError("Input must be 3D [batch, seq, H]")
-        if input.size(0) * input.size(1) != d["S"]:
-            raise RuntimeError(f"Input batch*seq must equal compiled S={d['S']}. Got batch={input.size(0)}, "
-                               f"seq={input.size(1)} (product={input.size(0) * input.size(1)})")
-        if input.size(2) != d["H"]:
-            raise RuntimeError(f"Input hidden_size must equal compiled H={d['H']}. Got {input.size(2)}")
+        if exact_s:
+            if input.dim() != 3:
+                raise RuntimeError("Input must be 3D [batch, seq, H]")
+            if input.size(0) * input.size(1) != d["S"]:
+                raise RuntimeError(f"Input batch*seq must equal compiled S={d['S']}. Got batch={input.size(0)}, "
+                                   f"seq={input.size(1)} (product={input.size(0) * input.size(1)})")
+        elif input.dim() < 1:
+            raise RuntimeError("Input must be [..., H]")
+        if input.size(-1) != d["H"]:
+            raise RuntimeError(f"Input hidden_size must equal compiled H={d['H']}. Got {input.size(-1)}")
+        n = input.numel() // d["H"]
+        if n > d["S"]:
+            raise RuntimeError(f"Input holds {n} tokens, more than the context's S={d['S']}")
         self._validate_weights(gate_weights, expert_weights)
+        return n
+
+    def _output(self, input: torch.Tensor, out: Optional[torch.Tensor]) -> torch.Tensor:
+        if out is None:
+            return torch.empty_like(input)
+        _check_tensor("out", out, self.device)
+        if out.shape != input.shape:
+            raise RuntimeError("out must have the input's shape")
+        return out
 
     def _bias_ptrs(self, bias_up, bias_down):
         d = self.dims
@@ -201,12 +220,7 @@ class MoEContext:
         """Enqueue one fused forward on torch's current stream; returns the [B,T,H] output tensor (async)."""
         self._validate(input, gate_weights, expert_weights)
         bu, bd = self._bias_ptrs(bias_up, bias_down)
-        if out is None:
-            out = torch.empty_like(input)
-        else:
-            _check_tensor("out", out, self.device)
-            if out.shape != input.shape:
-                raise RuntimeError("out must have the input's shape")
+        out = self._output(input, out)
         stream = torch.cuda.current_stream(self.device).cuda_stream
         if phase_mask == 7:
             rc = self._L.fm_moe_forward(self._ctx, input.data_ptr(), gate_weights.data_ptr(),
@@ -215,6 +229,27 @@ class MoEContext:
             rc = self._L.fm_debug_forward(self._ctx, input.data_ptr(), gate_weights.data_ptr(),
                                           expert_weights.data_ptr(), bu, bd, out.data_ptr(), stream, phase_mask)
         _lib.check(rc)
+        if phase_mask & 1:
+            self.last_tokens = self.dims["S"]
+        return out
+
+    def forward_tokens(self, x: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor,
+                       bias_up: Optional[torch.Tensor] = None, bias_down: Optional[torch.Tensor] = None,
+                       out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Enqueue one fused forward over the n = x.numel() // H tokens of `x` (contiguous bf16 [..., H], 0 <= n <= S)
+        on torch's current stream; returns `out` (default: a tensor like `x`), async.  The result is exactly what a
+        context created for S = n computes: routing, capacity `cfg.EC_of(n)`, drops, outputs and, in training mode, the
+        auxiliary loss over the n tokens.  Nothing past row n of `out` is written.  With world > 1 every rank passes its
+        own n (n = 0 included) and all ranks call the same number of times.  The routing tables `read` returns then
+        hold `last_tokens` valid rows."""
+        n = self._validate(x, gate_weights, expert_weights, exact_s=False)
+        bu, bd = self._bias_ptrs(bias_up, bias_down)
+        out = self._output(x, out)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self._L.fm_moe_forward_tokens(self._ctx, x.data_ptr() if n else None, n, gate_weights.data_ptr(),
+                                                 expert_weights.data_ptr(), bu, bd, out.data_ptr() if n else None,
+                                                 stream))
+        self.last_tokens = n
         return out
 
     def _host_args(self, input_host, gate_weights, expert_weights, out_host, bias_up, bias_down):

@@ -113,6 +113,17 @@ FM_API int fm_symm_use_external(fm_ctx_t* ctx, void* base, size_t bytes);
 FM_API int fm_moe_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, const void* expert_w,
                           const void* bias_up, const void* bias_down, void* out, void* stream);
 
+/* Same, on n_tokens tokens (0 <= n_tokens <= S; any count, not only multiples of 128): x and out are [n_tokens, H] and
+ * may be exactly that long.  The context's S is the maximum; the call computes exactly what a context created with
+ * sequence_len * mini_batch = n_tokens computes -- routing, capacity EC(n) = (drop_tokens ? ceil(n/E) : n) * CF * k,
+ * slots, drops, outputs, and with is_training = 1 the auxiliary loss averaged over n (all zero at n = 0).  Nothing is
+ * written to out at or beyond row n_tokens.  With n_tokens = 0, x and out may be NULL; the call still launches and takes
+ * part in the collective.  With world > 1 every rank passes its own count (counts may differ between ranks and between
+ * calls; every rank still calls the same number of times).  fm_moe_forward(...) is fm_moe_forward_tokens(..., S, ...).
+ * FM_EINVAL for n_tokens < 0 or > S.  The routing tables read back with fm_read_buffer hold n_tokens valid rows. */
+FM_API int fm_moe_forward_tokens(fm_ctx_t* ctx, const void* x, int n_tokens, const void* gate_w, const void* expert_w,
+                                 const void* bias_up, const void* bias_down, void* out, void* stream);
+
 /* world > 1: the [S,H] bf16 region of this rank's symmetric slab into which the experts (local and remote) accumulate
  * this rank's output rows.  Passing exactly this pointer as `out` to fm_moe_forward leaves the result there and skips
  * the final copy into a caller tensor (zero-copy output, like registering a user buffer with NVSHMEM); it is
