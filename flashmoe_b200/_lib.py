@@ -24,7 +24,7 @@ EXPORTED_SYMBOLS = (
     "fm_symm_local_ptr", "fm_symm_export", "fm_symm_attach_ipc", "fm_symm_attach_ptrs", "fm_symm_use_external",
     "fm_moe_forward", "fm_moe_forward_tokens", "fm_output_buffer", "fm_moe_forward_host", "fm_host_submit", "fm_host_wait", "fm_check", "fm_set_timeout_ms", "fm_set_trace", "fm_launch_count",
     "fm_buffer_bytes",
-    "fm_read_buffer", "fm_debug_forward", "fm_last_error", "fm_version",
+    "fm_read_buffer", "fm_last_error", "fm_version",
 )
 
 
@@ -78,7 +78,6 @@ def load() -> ctypes.CDLL:
     L.fm_output_buffer.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t)]
     L.fm_host_submit.argtypes = [vp, cvp, cvp, cvp, cvp, cvp, vp, vp, ctypes.POINTER(ctypes.c_uint64)]
     L.fm_host_wait.argtypes = [vp, ctypes.c_uint64]
-    L.fm_debug_forward.argtypes = [vp, cvp, cvp, cvp, cvp, cvp, vp, vp, ctypes.c_uint32]
     L.fm_check.argtypes = [vp]
     L.fm_set_timeout_ms.argtypes = [vp, ctypes.c_uint32]
     L.fm_set_trace.argtypes = [vp, ctypes.c_int]

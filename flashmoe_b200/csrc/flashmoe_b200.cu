@@ -104,11 +104,7 @@ struct fm_ctx {
     int tpc = 0;
     int TN0 = 0, TN1 = 0, num_pkts = 0, num_blocks = 0;
     int g0_blocks = 0, g1_blocks = 0;   // GEMM0 / GEMM1 blocks of the work list (items = their tiles x row blocks per packet)
-    int last_tokens = 0;                // token count of the last launch (a partial-phase launch reuses its routing)
-    int claim_ahead_kb = 16;
     int dbg_flags = 0;
-    bool coop = true;    // cooperative launch attribute (validates co-residency of the persistent grid)
-    int prefetch_kb = 0;
     uint32_t epoch = 0;
     unsigned long long bar_count = 0;
     // in-kernel waits give up after this long (fm_set_timeout_ms): generous by default so that ordinary rank skew (a peer
@@ -147,9 +143,6 @@ struct fm_ctx {
     float* aux = nullptr; // is_training: [2][2E+1] {gML, gMeC, loss} by epoch parity
     const void* cached_x = nullptr;     // the maps over the caller's x (tm_a0 when dense, tm_gx) are keyed on pointer AND
     int cached_x_rows = 0;              // row count: a map with more rows than this call's x would read past it
-    int* recv_tok = nullptr;            // [nLx, pEC] slot -> token of the local packets (gather-mode source rows)
-    unsigned int* tok_rows = nullptr;   // [2, nLx, TCM]
-    int gather = 0;                     // FM_GATHER: 0 off, 1 early tiles only, 2 every local GEMM0 tile (tests)
     bool tc_gate = false;               // router logits on the tensor cores (E <= 256)
     const void* cached_gx = nullptr;
     int cached_gx_rows = 0;
@@ -261,9 +254,8 @@ int check_kernel_status(fm_ctx* c) {
 // would -- capacity EC(n_tok), tokens per CTA ceil(n_tok / grid), maps over x with n_tok rows -- while every buffer keeps
 // its create-time (maximum) size and stride.
 int launch(fm_ctx* c, const void* x, int n_tok, const void* gate_w, const void* expert_w, const void* bias_up,
-           const void* bias_down, void* out, cudaStream_t stream, uint32_t phase_mask) {
+           const void* bias_down, void* out, cudaStream_t stream) {
     if (c == nullptr) return fail(FM_EINVAL, "null context");
-    if ((phase_mask & 1u) == 0u) n_tok = c->last_tokens;   // later phases only: the previous launch's routing and count
     if (n_tok < 0 || n_tok > c->d.S) return fail(FM_EINVAL, "n_tokens = %d not in [0, S = %d]", n_tok, c->d.S);
     if (gate_w == nullptr || expert_w == nullptr || (n_tok > 0 && (x == nullptr || out == nullptr)))
         return fail(FM_EINVAL, "x, gate_w, expert_w and out must be non-null device pointers");
@@ -275,8 +267,6 @@ int launch(fm_ctx* c, const void* x, int n_tok, const void* gate_w, const void* 
                 return fail(FM_EINVAL, "%s must be 16-byte aligned (got %p)", names[i], ptrs[i]);
     }
     if (!c->attached) return fail(FM_ESTATE, "peers not attached: call fm_symm_attach_ipc/ptrs before fm_moe_forward");
-    if ((phase_mask & 1u) == 0u && c->d.world != 1) return fail(FM_EINVAL, "partial-phase launches are single-rank only");
-    if ((phase_mask & 1u) == 0u && c->epoch == 0) return fail(FM_ESTATE, "no previous routing to reuse");
     FM_CUDA(cudaSetDevice(c->device));
     const fm_dims_t& d = c->d;
     const int nLx = d.num_local_experts;
@@ -332,13 +322,12 @@ int launch(fm_ctx* c, const void* x, int n_tok, const void* gate_w, const void* 
     // does not know their token counts and keeps the maximum (the empty row blocks are skipped by the scheduler)
     p.tcm_items = d.world == 1 ? ceil_div(ec, fm::BLOCK_M) : d.TCM;
     p.total_items = (c->g0_blocks * c->TN0 + c->g1_blocks * c->TN1) * p.tcm_items;
-    p.claim_ahead_kb = c->claim_ahead_kb; p.dbg_flags = c->dbg_flags; p.prefetch_kb = c->prefetch_kb;
+    p.dbg_flags = c->dbg_flags;
     // the epoch and the grid-barrier target advance only when the launch has been accepted (see below): a failed launch
     // must not leave the host ahead of the device counter and of the peers
-    const uint32_t epoch = c->epoch + ((phase_mask & 1u) ? 1u : 0u);
-    const unsigned long long bar_count = c->bar_count + ((phase_mask & 1u) ? (unsigned long long)c->grid : 0ull);
+    const uint32_t epoch = c->epoch + 1u;
+    const unsigned long long bar_count = c->bar_count + (unsigned long long)c->grid;
     p.epoch = epoch;
-    p.phase_mask = phase_mask;
     p.bar_target = bar_count;
     p.timeout_ns = c->timeout_ns;
     p.x = static_cast<const __nv_bfloat16*>(x);
@@ -368,9 +357,6 @@ int launch(fm_ctx* c, const void* x, int n_tok, const void* gate_w, const void* 
     if (d.world == 1) p.peer_out_acc[0] = p.out;
     p.aux = c->aux;
     p.dense = c->dense ? 1 : 0;
-    p.gather = c->gather;
-    p.recv_tok = c->recv_tok;
-    p.tok_rows = c->tok_rows;
     p.dbg = c->dbg_dev;
     p.trace = c->trace_on ? c->trace : nullptr;
 
@@ -379,17 +365,14 @@ int launch(fm_ctx* c, const void* x, int n_tok, const void* gate_w, const void* 
     lc.blockDim = dim3(fm::NUM_THREADS);
     lc.dynamicSmemBytes = (size_t)fm::SMEM_BYTES;
     lc.stream = stream;
-    cudaLaunchAttribute attrs[1];
-    int na = 0;
-    if (c->coop) {
-        attrs[na].id = cudaLaunchAttributeCooperative;   // all CTAs co-resident: in-kernel spin waits + grid barrier
-        attrs[na].val.cooperative = 1;
-        ++na;
-    }
-    lc.attrs = attrs;
-    lc.numAttrs = na;
+    // The persistent grid spins on flags, counters and one grid barrier, so every CTA must be resident: the launch is
+    // cooperative (the driver then refuses to start it unless the whole grid fits, also next to other work on the GPU).
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeCooperative;
+    attr.val.cooperative = 1;
+    lc.attrs = &attr;
+    lc.numAttrs = 1;
     FM_CUDA(cudaLaunchKernelEx(&lc, fm::fm_moe_forward_kernel, p));
-    c->last_tokens = n_tok;
     c->epoch = epoch;
     c->bar_count = bar_count;
     c->launches += 1;
@@ -464,7 +447,7 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
     ctx->cfg = c;
     ctx->d = d;
     ctx->device = device;
-    // tuning knobs (scheduler look-ahead, work order); environment overrides are for experiments
+    // path choices (combine, dense E = 1, router, work order); environment overrides are for tests and experiments
     auto env_int = [](const char* name, int dflt) {
         const char* v = getenv(name);
         return (v != nullptr && *v) ? atoi(v) : dflt;
@@ -481,11 +464,6 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
         // d_model 2048, 8192 tokens); up to 256 experts, 128 per pass over d_model.  Default: from 17 experts up (at a
         // handful of experts the GEMV is latency-, not flop-bound).
         ctx->tc_gate = !ctx->dense && d.E <= 256 && env_int("FM_TC_GATE", d.E > 16 ? 1 : 0) != 0;
-        // gather of local rows straight from x (by token index, in the producer warp) for tiles claimed before their row
-        // copies landed: correct, but off by default -- a gather tile loads its A operand through one warp's registers
-        // instead of the TMA engine, which costs more than the earlier start buys.  FM_GATHER=2 gathers every local
-        // GEMM0 tile (deterministic coverage of that path)
-        ctx->gather = ctx->dense ? 0 : std::min(2, std::max(0, env_int("FM_GATHER", 0)));
         ctx->d.grid = ctx->grid;
     }
     ctx->tpc = ceil_div(d.S, ctx->grid);
@@ -494,14 +472,7 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
         return fail(FM_EINVAL, "tokens-per-CTA * k = %d exceeds the router scratch (%d)", ctx->tpc * d.k, fm::G_SEL_MAX);
     }
     const int nLx = d.num_local_experts;
-    ctx->claim_ahead_kb = env_int("FM_CLAIM_AHEAD_KB", 16);
     ctx->dbg_flags = env_int("FM_DBG_FLAGS", 0);
-    // The persistent grid spins on flags, counters and one grid barrier, so every CTA must be resident: the launch is
-    // cooperative (the driver then refuses to start it unless the whole grid fits, also next to other work on the GPU).
-    ctx->coop = env_int("FM_COOP", 1) != 0;
-    ctx->prefetch_kb = env_int("FM_PREFETCH_KB", 0);
-    if (ctx->prefetch_kb < 0) ctx->prefetch_kb = 0;
-    if (ctx->claim_ahead_kb < 0) ctx->claim_ahead_kb = 0;
     ctx->TN0 = ceil_div(d.P, fm::BLOCK_N);
     ctx->TN1 = ceil_div(d.H, fm::BLOCK_N);
     ctx->num_pkts = world * nLx;
@@ -543,7 +514,7 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
             if ((int)i >= lag) push(1, units[i - lag]);
         }
         for (size_t i = units.size() - lag; i < units.size(); ++i) push(1, units[i]);
-    } else if (world >= 4 && lag < 0 && env_int("FM_LOCAL_FIRST", 1) != 0) {   // (0: the two-rank order, for A/B runs)
+    } else if (world >= 4 && lag < 0) {
         std::vector<Unit> loc, rem;
         for (const Unit& u : units) (u.local ? loc : rem).push_back(u);
         for (const Unit& u : loc) push(0, u);
@@ -601,10 +572,6 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
     FM_TRY(dev_alloc(&ctx->hidden, (size_t)ctx->num_pkts * d.pEC * d.P));
     FM_TRY(dev_alloc(&ctx->trace, (size_t)ctx->grid * fm::TRACE_SLOTS));
     if (c.is_training) FM_TRY(dev_alloc(&ctx->aux, (size_t)2 * (2 * d.E + 1)));
-    if (ctx->gather) {
-        FM_TRY(dev_alloc(&ctx->recv_tok, (size_t)nLx * d.pEC));
-        FM_TRY(dev_alloc(&ctx->tok_rows, (size_t)2 * nLx * d.TCM));
-    }
 
     // symmetric slab: [recv_x | ret_y | recv_flag | ret_flag]  (reference heap + flags, bootstrap.cuh:348-362)
     size_t off = 0;
@@ -651,7 +618,7 @@ FM_API int fm_destroy(fm_ctx_t* ctx) {
         if (ctx->peer_opened[r] && ctx->peer_base[r] != nullptr) cudaIpcCloseMemHandle(ctx->peer_base[r]);
     void* bufs[] = {ctx->topk_idx, ctx->topk_w, ctx->mcw, ctx->slot, ctx->counts, ctx->gate_out, ctx->chunk_counts,
                     ctx->ctrl, ctx->g0_done, ctx->g1_done, ctx->pkt_done, ctx->recv_cnt, ctx->blocks, ctx->hidden, ctx->trace,
-                    ctx->aux, ctx->recv_tok, ctx->tok_rows};
+                    ctx->aux};
     for (void* b : bufs)
         if (b != nullptr) cudaFree(b);
     for (int i = 0; i < FM_HOST_SLOTS; ++i) {
@@ -757,20 +724,13 @@ FM_API int fm_symm_attach_ptrs(fm_ctx_t* ctx, void* const* peer_bases) {
 
 FM_API int fm_moe_forward_tokens(fm_ctx_t* ctx, const void* x, int n_tokens, const void* gate_w, const void* expert_w,
                                  const void* bias_up, const void* bias_down, void* out, void* stream) {
-    return launch(ctx, x, n_tokens, gate_w, expert_w, bias_up, bias_down, out, static_cast<cudaStream_t>(stream), 7u);
+    return launch(ctx, x, n_tokens, gate_w, expert_w, bias_up, bias_down, out, static_cast<cudaStream_t>(stream));
 }
 
 FM_API int fm_moe_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, const void* expert_w, const void* bias_up,
                           const void* bias_down, void* out, void* stream) {
     if (ctx == nullptr) return fail(FM_EINVAL, "null context");
     return fm_moe_forward_tokens(ctx, x, ctx->d.S, gate_w, expert_w, bias_up, bias_down, out, stream);
-}
-
-FM_API int fm_debug_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, const void* expert_w,
-                            const void* bias_up, const void* bias_down, void* out, void* stream, uint32_t phase_mask) {
-    if (phase_mask == 0 || phase_mask > 7u) return fail(FM_EINVAL, "phase_mask must be in [1, 7]");
-    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
-    return launch(ctx, x, ctx->d.S, gate_w, expert_w, bias_up, bias_down, out, static_cast<cudaStream_t>(stream), phase_mask);
 }
 
 // ---- host-buffer entry points -----------------------------------------------------------------------------------
@@ -808,7 +768,7 @@ FM_API int fm_host_submit(fm_ctx_t* ctx, const void* x_host, const void* gate_w,
     FM_CUDA(cudaMemcpyAsync(ctx->x_stage[slot], x_host, bytes, cudaMemcpyHostToDevice, ctx->s_h2d));
     FM_CUDA(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
     FM_CUDA(cudaStreamWaitEvent(s, ctx->ev_h2d[slot], 0));
-    if ((rc = launch(ctx, ctx->x_stage[slot], ctx->d.S, gate_w, expert_w, bias_up, bias_down, ctx->out_stage[slot], s, 7u))) return rc;
+    if ((rc = launch(ctx, ctx->x_stage[slot], ctx->d.S, gate_w, expert_w, bias_up, bias_down, ctx->out_stage[slot], s))) return rc;
     FM_CUDA(cudaEventRecord(ctx->ev_kernel[slot], s));
     FM_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_kernel[slot], 0));
     FM_CUDA(cudaMemcpyAsync(out_host, ctx->out_stage[slot], bytes, cudaMemcpyDeviceToHost, ctx->s_d2h));

@@ -39,6 +39,7 @@ constexpr int BLOCK_N = 256;   // output columns per tile: 128 fp32 accumulators
 constexpr int BLOCK_K = 64;    // 64 bf16 = 128 B = one swizzle row
 constexpr int WGMMA_K = 16;
 constexpr int NSCHED = 4;
+constexpr int CLAIM_AHEAD_KB = 16;   // the scheduler claims the next tile when this many k-blocks of the current one remain
 constexpr int NUM_THREADS = 384;
 constexpr int NUM_WARPS = NUM_THREADS / 32;
 constexpr int EPI_WARP0 = 4;   // warps 4..11: warpgroup (warp - 4) / 4 owns tile rows [64g, 64g + 64), warp % 4 its 16-row slice
@@ -119,11 +120,9 @@ struct FmParams {
     int S, H, P, E, k, W, rank, nLx, EC, pEC, TCM, act;
     int TN0, TN1, tpc, num_pkts, num_blocks, total_items;
     int tcm_items;      // row blocks per packet in the work list: TCM of this call's EC at W == 1, the maximum TCM at W > 1
-    int claim_ahead_kb; // the scheduler claims the next tile when this many k-blocks of the current one remain
-    int prefetch_kb;    // L2 prefetch distance of the TMA producer in k-blocks (0 = off)
-    int dbg_flags;      // experiments only (results are garbage for bits 0-3): bit0 = skip all TMA loads, bit1 = skip MMA
-                        // issue, bit2 = skip the A loads, bit3 = skip the B loads, bit5 = ignore BAR_DISP_DONE
-    unsigned int epoch, phase_mask;
+    int dbg_flags;      // experiments only (results are garbage): bit0 = skip all TMA loads, bit1 = skip MMA issue,
+                        // bit2 = skip the A loads, bit3 = skip the B loads
+    unsigned int epoch;
     unsigned long long bar_target, timeout_ns;
     const __nv_bfloat16 *x, *wg, *b_up, *b_down;
     __nv_bfloat16* out;
@@ -164,11 +163,6 @@ struct FmParams {
     __nv_bfloat16* peer_out_acc[FM_MAX_WORLD];
     // training mode (is_training = 1): [2][2E+1] f32 by epoch parity = {gML[E] mean gate probability per expert,
     // gMeC[E] mean routed fraction per expert, loss} (reference moe/gate.cuh:608-635,698-706,763-773); nullptr otherwise
-    // local packets (source = this rank): token of every slot, acknowledged BEFORE the row copies, so a GEMM0 tile
-    // claimed early can gather its A rows straight from x instead of waiting for the copies to land
-    int* recv_tok;             // [nLx, pEC] (local packets only, indexed by local expert)
-    unsigned int* tok_rows;    // [2, nLx, TCM] rows of block b whose token entry is written, by epoch parity
-    int gather;                // 0 = off, 1 = when a tile's rows have not landed yet, 2 = every local GEMM0 tile
     float* aux;
     int dense;          // E == 1: no router GEMV, no dispatch copy; GEMM0 reads x in place (reference moe/fffn.cuh:31-167)
     DebugRecord* dbg;
@@ -827,31 +821,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
             atomicAdd(a + 2 * E, __fdividef(me * ce, (float)E));
         }
     }
-    // Local packets first get their token table (slot -> token) and an acknowledgement of it: a GEMM0 tile claimed before
-    // the row copies below have landed gathers its rows from x by these indices (ffn_producer).
     const unsigned int par = p.epoch & 1u;
-    if (p.gather) {
-        const int first_local = p.rank * p.nLx;
-        for (int i = tid; i < n_tok * k; i += DISP_THREADS) {
-            const int e = sel_e[i];
-            const int le = e - first_local;
-            if (le >= 0 && le < p.nLx) {
-                const int s = base_s[e] + rank_s[i];
-                if (s < p.EC) p.recv_tok[(size_t)le * p.pEC + s] = t0 + i / k;
-            }
-        }
-        disp_sync();
-        for (int le = tid; le < p.nLx; le += DISP_THREADS) {
-            const int e = first_local + le;
-            const int lo = base_s[e];
-            const int hi = min(lo + own_s[e], p.EC);
-            if (hi > lo) {
-                unsigned int* ctr = p.tok_rows + ((size_t)par * p.nLx + le) * p.TCM;
-                for (int b = lo / BLOCK_M; b <= (hi - 1) / BLOCK_M; ++b)
-                    red_release_gpu_add_u32(ctr + b, (unsigned int)(min(hi, (b + 1) * BLOCK_M) - max(lo, b * BLOCK_M)));
-            }
-        }
-    }
     // Row copies.
     //   * Rows for experts on THIS rank (warps 4-11): the chunk's token rows are contiguous in x, so one bulk load stages up
     //     to 128 KiB of them in shared memory (the first group was requested at the end of the router) and every kept
@@ -1058,13 +1028,12 @@ struct TileInfo {     // written by the scheduler warp, read by the producer / c
     int ntile;
     int le;           // local expert
     int b_row;        // TMA row coordinate of the B tile
-    int gather;       // GEMM0, local packet: 1 = the A rows are gathered from x (their row copies had not landed yet)
     int pkt;          // local packet index src * nLx + le
     int mblk;         // 128-row block of that packet
     int rows;         // valid rows of that block
     int src;          // source rank of the packet
     int cnt;          // rows of the whole packet
-    int pad[2];
+    int pad[3];
 };
 static_assert(sizeof(TileInfo) <= 64, "a ring slot is 64 bytes");
 
@@ -1084,8 +1053,8 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, uint8_t* smem, 
             mbar_wait(&prod_take[pq], ((n - 1) / NSCHED) & 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_EMPTY, 200 + pq);
         }
         TileInfo ti;
-        ti.kind = -1; ti.ntile = 0; ti.le = 0; ti.b_row = 0; ti.gather = 0; ti.pkt = 0; ti.mblk = 0; ti.rows = 0;
-        ti.src = 0; ti.cnt = 0; ti.pad[0] = ti.pad[1] = 0;
+        ti.kind = -1; ti.ntile = 0; ti.le = 0; ti.b_row = 0; ti.pkt = 0; ti.mblk = 0; ti.rows = 0;
+        ti.src = 0; ti.cnt = 0; ti.pad[0] = ti.pad[1] = ti.pad[2] = 0;
         for (;;) {
             const int id = (int)atomicAdd(p.claim, 1u);
             if (id >= p.total_items) break;
@@ -1120,34 +1089,19 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, uint8_t* smem, 
                 st_release_sys_u64(p.peer_done_flag[src] + (size_t)(p.rank * p.nLx + le), (unsigned long long)p.epoch << 32);
             const int rows = max(0, min(BLOCK_M, cnt - mb * BLOCK_M));
             if (rows == 0) continue;   // an empty row block of the static superset
-            int gather = 0;
             SpinGuard g;
-            const unsigned int* rctr = p.recv_rows + ((size_t)(p.epoch & 1u) * p.num_pkts + pkt) * p.TCM + mb;
             if (blk.kind == 1) {  // GEMM1 needs the whole h row block (reference notifyNext, processor.cuh:490-615)
                 const unsigned int* ctr = p.g0_done + (size_t)pkt * p.TCM + mb;
                 while (ld_acquire_gpu_u32(ctr) < (unsigned int)p.TN0) g.tick(p.dbg, p.timeout_ns, FM_TRAP_G0_DONE, pkt, mb, 0);
-                if (p.gather && p.fused && same_gpu && (p.phase_mask & 1u)) {
-                    // the block's GEMM0 tiles may all have run in gather mode, i.e. before its row copies and routing
-                    // records landed: the combine epilogue reads those records, so order behind their ack
-                    while (ld_acquire_gpu_u32(rctr) < (unsigned int)rows)
-                        g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_ROWS, pkt, mb, rows);
-                }
-            } else if ((p.phase_mask & 1u) && !p.dense) {  // GEMM0 needs the rows of this block to have landed (dispatch acks)
-                // local packet: the token table of the block is acknowledged before its row copies -- if it is complete
-                // while the rows are not, the producer gathers the rows from x itself (FM_GATHER=1); FM_GATHER=2 gathers
-                // every local GEMM0 tile, so the gather path runs whatever the timing
-                const unsigned int* tctr = (p.gather && same_gpu)
-                    ? p.tok_rows + ((size_t)(p.epoch & 1u) * p.nLx + le) * p.TCM + mb : nullptr;
+            } else if (!p.dense) {  // GEMM0 needs the rows of this block to have landed (dispatch acks)
+                const unsigned int* rctr = p.recv_rows + ((size_t)(p.epoch & 1u) * p.num_pkts + pkt) * p.TCM + mb;
                 for (;;) {
-                    if (p.gather != 2 || tctr == nullptr) {
-                        const unsigned int got = same_gpu ? ld_acquire_gpu_u32(rctr) : ld_acquire_sys_u32(rctr);
-                        if (got >= (unsigned int)rows) break;
-                    }
-                    if (tctr != nullptr && ld_acquire_gpu_u32(tctr) >= (unsigned int)rows) { gather = 1; break; }
+                    const unsigned int got = same_gpu ? ld_acquire_gpu_u32(rctr) : ld_acquire_sys_u32(rctr);
+                    if (got >= (unsigned int)rows) break;
                     g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_ROWS, pkt, mb, rows);
                 }
             }
-            ti.kind = blk.kind; ti.ntile = nt; ti.le = le; ti.gather = gather; ti.pkt = pkt; ti.mblk = mb; ti.rows = rows;
+            ti.kind = blk.kind; ti.ntile = nt; ti.le = le; ti.pkt = pkt; ti.mblk = mb; ti.rows = rows;
             ti.src = src; ti.cnt = cnt;
             // expert_weights [nLx,2,P,H]: W_up(le) starts at row le*2*P of the [.,H] view; W_down(le) (the [P,H]
             // block flat-viewed as [H,P]) starts at row (le*2+1)*H of the [.,P] view.
@@ -1168,22 +1122,6 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, uint8_t* smem, 
     }
 }
 
-// gather mode: the 128 A rows of k-block kb come straight from x by token index (lane l owns rows 4l .. 4l+3), stored
-// with the 128-byte swizzle the TMA would have applied (16-byte piece c of row r at piece c ^ (r & 7))
-__device__ __forceinline__ void gather_a_rows(const FmParams& p, uint8_t* sa, int kb, int lane, const int4& tok) {
-    const int toks[4] = {tok.x, tok.y, tok.z, tok.w};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int row = lane * 4 + i;
-        const __nv_bfloat16* src = p.x + (size_t)toks[i] * p.H + kb * BLOCK_K;
-        uint4 v[8];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) v[c] = ld_global_nc_v4(src + c * 8);
-#pragma unroll
-        for (int c = 0; c < 8; ++c) *reinterpret_cast<uint4*>(sa + row * 128 + ((c ^ (row & 7)) << 4)) = v[c];
-    }
-}
-
 // warp 0: TMA producer
 __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem, uint64_t* bars) {
     uint64_t* full = bars + BAR_FULL;
@@ -1196,34 +1134,19 @@ __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem, u
     int stage = 0, phase = 0, q = 0, qphase = 0;
     bool first = true, stamped = false;
     for (;;) {
-        int kind = -1, gather = 0, g_base = 0, g_rows = 0;
+        int kind = -1;
         TileInfo ti;
         if (lane == 0) {
             mbar_wait(&sched_full[q], qphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, 300 + q);
             ti = ring[q];
             mbar_arrive(&sched_empty[q]);
             kind = ti.kind;
-            gather = ti.gather;
-            g_base = ti.le * p.pEC + ti.mblk * BLOCK_M;   // the block's first slot in the local token table
-            g_rows = ti.rows;
         }
         kind = __shfl_sync(0xffffffffu, kind, 0);
         if (kind < 0) break;
-        gather = __shfl_sync(0xffffffffu, gather, 0);
-        // gather mode (GEMM0 tile of a local packet whose row copies have not landed): every lane owns four rows of the
-        // A tile and fetches them from x by token index, k-block by k-block
-        int4 tok = make_int4(0, 0, 0, 0);
-        if (gather) {
-            g_base = __shfl_sync(0xffffffffu, g_base, 0);
-            g_rows = __shfl_sync(0xffffffffu, g_rows, 0);
-            if (lane * 4 < g_rows) tok = ld_global_cg_i4(p.recv_tok + g_base + lane * 4);
-            if (lane * 4 + 1 >= g_rows) tok.y = 0;   // padding rows of the last block: any valid row (results are dropped)
-            if (lane * 4 + 2 >= g_rows) tok.z = 0;
-            if (lane * 4 + 3 >= g_rows) tok.w = 0;
-        }
         int nk = 0;
         if (lane == 0) {
-            if (first && (p.phase_mask & 1u) && !(p.dbg_flags & 32))   // the stage area doubles as the dispatch staging buffer
+            if (first)   // the stage area doubles as the dispatch staging buffer
                 mbar_wait(&bars[BAR_DISP_DONE], 0, p.dbg, p.timeout_ns, FM_TRAP_MBAR_EMPTY, 901);
             first = false;
             fence_proxy_async_global();  // rows written by generic-proxy stores (peers / other SMs) -> TMA reads
@@ -1232,41 +1155,21 @@ __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem, u
         nk = __shfl_sync(0xffffffffu, nk, 0);
         const CUtensorMap* ta = kind == 0 ? &p.tm_a0 : &p.tm_a1;
         const CUtensorMap* tb = kind == 0 ? &p.tm_b0 : &p.tm_b1;
-        const int take_at = min(nk - 1, max(0, nk - p.claim_ahead_kb));
+        const int take_at = min(nk - 1, max(0, nk - CLAIM_AHEAD_KB));
         int a_row = 0, b_row = 0;
         if (lane == 0) {
             a_row = ti.pkt * p.pEC + ti.mblk * BLOCK_M;
             b_row = ti.b_row;
-            const int pf = p.prefetch_kb;
-            if (pf > 0) {   // warm L2 for the k-blocks just beyond the smem pipeline
-                for (int kb = STAGES; kb < min(nk, STAGES + pf); ++kb) {
-                    tma_prefetch_l2_2d(ta, kb * BLOCK_K, a_row);
-                    tma_prefetch_l2_2d(tb, kb * BLOCK_K, b_row);
-                }
-            }
         }
         for (int kb = 0; kb < nk; ++kb) {
             uint8_t* sa = smem + stage * STAGE_BYTES;
             const bool ld_a = (p.dbg_flags & 5) == 0, ld_b = (p.dbg_flags & 9) == 0;   // experiments only
             if (lane == 0) {
-                const int pf = p.prefetch_kb;
-                if (pf > 0 && kb + STAGES + pf < nk) {
-                    tma_prefetch_l2_2d(ta, (kb + STAGES + pf) * BLOCK_K, a_row);
-                    tma_prefetch_l2_2d(tb, (kb + STAGES + pf) * BLOCK_K, b_row);
-                }
                 if (kb == take_at) mbar_arrive(&prod_take[q]);  // lets the scheduler claim the next tile
                 mbar_wait(&empty[stage], phase ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_EMPTY, stage);
-            }
-            if (gather) {   // warp-uniform: the A rows are in shared memory before the stage's barrier can complete
-                __syncwarp();   // lane 0 has seen the stage empty
-                if (ld_a) gather_a_rows(p, sa, kb, lane, tok);
-                fence_proxy_async_smem();   // generic-proxy smem writes -> the consumers' wgmma (async proxy) reads
-                __syncwarp();
-            }
-            if (lane == 0) {
-                const uint32_t tx = (ld_a && !gather ? (uint32_t)A_STAGE_BYTES : 0u) + (ld_b ? (uint32_t)B_STAGE_BYTES : 0u);
+                const uint32_t tx = (ld_a ? (uint32_t)A_STAGE_BYTES : 0u) + (ld_b ? (uint32_t)B_STAGE_BYTES : 0u);
                 if (tx) mbar_arrive_expect_tx(&full[stage], tx); else mbar_arrive(&full[stage]);
-                if (ld_a && !gather) tma_load_2d(sa, ta, kb * BLOCK_K, a_row, &full[stage]);
+                if (ld_a) tma_load_2d(sa, ta, kb * BLOCK_K, a_row, &full[stage]);
                 if (ld_b) tma_load_2d(sa + A_STAGE_BYTES, tb, kb * BLOCK_K, b_row, &full[stage]);
                 if (!stamped) { trace_stamp(p, 7); stamped = true; }   // first loads of the first tile issued
             }
@@ -1473,7 +1376,7 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, u
         if (lane == 0 && prev >= 0) mbar_arrive(&empty[prev]);
         if (ntiles < 16 && stamper) trace_stamp(p, 48 + ntiles);
 
-        if (ntiles == 0 && p.W > 1 && (p.phase_mask & 1u))   // the staging area served as warp 2's window for the remote rows
+        if (ntiles == 0 && p.W > 1)   // the staging area served as warp 2's window for the remote rows
             asm volatile("bar.sync 7, 288;" ::: "memory");
         if (lane == 0) mbar_arrive(&sched_empty[q]);   // every lane has read the slot (the __syncwarp above)
         if (++q == NSCHED) { q = 0; qphase ^= 1; }
@@ -1661,7 +1564,7 @@ __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
         tma_prefetch_desc(&p.tm_b0);
         tma_prefetch_desc(&p.tm_a1); tma_prefetch_desc(&p.tm_b1);
     }
-    if (warp == 3 && (tid & 31) == 0 && (p.phase_mask & 3u) == 3u) {
+    if (warp == 3 && (tid & 31) == 0) {
         // Warm L2 with the 256-row weight tile this CTA will most likely claim first (item id = CTA index: the first wave is
         // claimed in arrival order), pipeline depth only: HBM is idle during the router and the first tile's loads are
         // then L2 hits.  A wrong guess costs nothing -- the tile is needed by some CTA of the first wave anyway.
@@ -1876,59 +1779,46 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
 
     if (tid == 0) trace_stamp(p, 0);
     ffn_setup(p, smem);   // mbarriers for the later phases (visible to everyone after the next block sync)
-    if (p.phase_mask & 1u) {
-        // per-launch reset of the work counters (reference clearState, moe.cuh:21-70); consumed only after the grid barrier
-        if (blockIdx.x == 0) {
-            for (int i = tid; i < p.num_pkts * p.TCM; i += NUM_THREADS) {
-                p.g0_done[i] = 0u;
-                p.g1_done[i] = 0u;
-            }
-            for (int i = tid; i < p.num_pkts; i += NUM_THREADS) p.pkt_done[i] = 0u;
-            // the arrival counters of the NEXT epoch's parity: nobody reads them any more (launch epoch-1 is over) and no
-            // peer can write them yet (a rank starts forward epoch+1 only after this launch has returned all its rows)
-            unsigned int* next_rows = p.recv_rows + (size_t)((p.epoch + 1u) & 1u) * p.num_pkts * p.TCM;
-            for (int i = tid; i < p.num_pkts * p.TCM; i += NUM_THREADS) next_rows[i] = 0u;
-            if (p.gather) {
-                unsigned int* next_tok = p.tok_rows + (size_t)((p.epoch + 1u) & 1u) * p.nLx * p.TCM;
-                for (int i = tid; i < p.nLx * p.TCM; i += NUM_THREADS) next_tok[i] = 0u;
-            }
-            if (p.aux != nullptr) {   // the loss buffers of the next launch (reference clearState, moe.cuh:49-54)
-                float* next_aux = p.aux + (size_t)((p.epoch + 1u) & 1u) * (2 * p.E + 1);
-                for (int i = tid; i < 2 * p.E + 1; i += NUM_THREADS) next_aux[i] = 0.0f;
-            }
-            if (tid == 0) *p.claim = 0u;
+    // per-launch reset of the work counters (reference clearState, moe.cuh:21-70); consumed only after the grid barrier
+    if (blockIdx.x == 0) {
+        for (int i = tid; i < p.num_pkts * p.TCM; i += NUM_THREADS) {
+            p.g0_done[i] = 0u;
+            p.g1_done[i] = 0u;
         }
-        if (p.dense) gate_phase_dense(p, t0, n_tok); else gate_phase(p, smem, t0, n_tok);
-        if (tid == 0) trace_stamp(p, 1);
-        grid_barrier(p);
-        if (tid == 0) trace_stamp(p, 2);
-    } else {
-        if (blockIdx.x == 0 && tid == 0) *p.claim = 0u;   // debug re-run of later phases on the previous routing
-        __syncthreads();
+        for (int i = tid; i < p.num_pkts; i += NUM_THREADS) p.pkt_done[i] = 0u;
+        // the arrival counters of the NEXT epoch's parity: nobody reads them any more (launch epoch-1 is over) and no
+        // peer can write them yet (a rank starts forward epoch+1 only after this launch has returned all its rows)
+        unsigned int* next_rows = p.recv_rows + (size_t)((p.epoch + 1u) & 1u) * p.num_pkts * p.TCM;
+        for (int i = tid; i < p.num_pkts * p.TCM; i += NUM_THREADS) next_rows[i] = 0u;
+        if (p.aux != nullptr) {   // the loss buffers of the next launch (reference clearState, moe.cuh:49-54)
+            float* next_aux = p.aux + (size_t)((p.epoch + 1u) & 1u) * (2 * p.E + 1);
+            for (int i = tid; i < 2 * p.E + 1; i += NUM_THREADS) next_aux[i] = 0.0f;
+        }
+        if (tid == 0) *p.claim = 0u;
     }
+    if (p.dense) gate_phase_dense(p, t0, n_tok); else gate_phase(p, smem, t0, n_tok);
+    if (tid == 0) trace_stamp(p, 1);
+    grid_barrier(p);
+    if (tid == 0) trace_stamp(p, 2);
 
     // From here the warps specialise.  Warps 0 and 3 (TMA producer, tile scheduler) enter their FFN roles at once -- the
     // scheduler claims its first tile and spins on the packet flag while warps 2, 4-11 dispatch this CTA's rows; warps
     // 4-11 then become the consumer warpgroups.
     const bool disp_warp = (warp == 2) || (warp >= EPI_WARP0);
-    if ((p.phase_mask & 1u) && disp_warp) {
+    if (disp_warp) {
         if (!p.dense) dispatch_phase(p, smem, t0, n_tok);
         else if (warp == 2 && (tid & 31) == 0)   // nothing to copy: GEMM0's TMA reads x in place; release the producer
             mbar_arrive(reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_DISP_DONE);
         if (warp == 2 && (tid & 31) == 0) trace_stamp(p, 3);
     }
-    if (p.phase_mask & 2u) {
-        if (tid == EPI_WARP0 * 32) trace_stamp(p, 4);
-        ffn_roles(p, smem);
-    }
+    if (tid == EPI_WARP0 * 32) trace_stamp(p, 4);
+    ffn_roles(p, smem);
 
-    if (p.phase_mask & 4u) {
-        __syncthreads();
-        if (p.fused) finish_fused(p, t0, n_tok);
-        else combine_phase(p, smem, t0, n_tok);
-        __syncthreads();
-        if (tid == 0) trace_stamp(p, 6);
-    }
+    __syncthreads();
+    if (p.fused) finish_fused(p, t0, n_tok);
+    else combine_phase(p, smem, t0, n_tok);
+    __syncthreads();
+    if (tid == 0) trace_stamp(p, 6);
 }
 
 }  // namespace fm

@@ -216,21 +216,15 @@ class MoEContext:
 
     def forward(self, input: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor,
                 bias_up: Optional[torch.Tensor] = None, bias_down: Optional[torch.Tensor] = None,
-                out: Optional[torch.Tensor] = None, phase_mask: int = 7) -> torch.Tensor:
+                out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Enqueue one fused forward on torch's current stream; returns the [B,T,H] output tensor (async)."""
         self._validate(input, gate_weights, expert_weights)
         bu, bd = self._bias_ptrs(bias_up, bias_down)
         out = self._output(input, out)
         stream = torch.cuda.current_stream(self.device).cuda_stream
-        if phase_mask == 7:
-            rc = self._L.fm_moe_forward(self._ctx, input.data_ptr(), gate_weights.data_ptr(),
-                                        expert_weights.data_ptr(), bu, bd, out.data_ptr(), stream)
-        else:
-            rc = self._L.fm_debug_forward(self._ctx, input.data_ptr(), gate_weights.data_ptr(),
-                                          expert_weights.data_ptr(), bu, bd, out.data_ptr(), stream, phase_mask)
-        _lib.check(rc)
-        if phase_mask & 1:
-            self.last_tokens = self.dims["S"]
+        _lib.check(self._L.fm_moe_forward(self._ctx, input.data_ptr(), gate_weights.data_ptr(),
+                                          expert_weights.data_ptr(), bu, bd, out.data_ptr(), stream))
+        self.last_tokens = self.dims["S"]
         return out
 
     def forward_tokens(self, x: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor,

@@ -172,12 +172,6 @@ enum fm_buffer {
 FM_API int fm_buffer_bytes(const fm_ctx_t* ctx, int which, size_t* bytes);
 FM_API int fm_read_buffer(fm_ctx_t* ctx, int which, void* host_dst, size_t bytes);
 
-/* Debug: run only the phases in `phase_mask` (bit0 gate+dispatch, bit1 expert FFN, bit2 combine).  A launch that
- * omits bit0 reuses the previous launch's routing and epoch (single rank only). */
-FM_API int fm_debug_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, const void* expert_w,
-                            const void* bias_up, const void* bias_down, void* out, void* stream,
-                            uint32_t phase_mask);
-
 FM_API const char* fm_last_error(void);
 FM_API const char* fm_version(void);
 

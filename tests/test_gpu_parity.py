@@ -94,19 +94,21 @@ def test_parity_with_oracle(name):
     _compare(cfg, _run(cfg, x, wg, we), run_oracle(cfg, x, wg, we))
 
 
-@pytest.mark.parametrize("gather,fused", [(0, 1), (1, 0), (0, 0), (2, 1), (2, 0)])
+@pytest.mark.parametrize("g1_lag,fused", [(0, 1), (1, 0), (0, 0), (2, 1), (2, 0)])
 @pytest.mark.parametrize("name", ["small_drop", "odd_row_blocks", "configA_top1", "ragged_dims"])
-def test_alternate_kernel_modes(monkeypatch, name, gather, fused):
-    """The row gather from x for GEMM0 tiles (FM_GATHER=1: tiles claimed before their rows landed, timing-dependent;
-    FM_GATHER=2: every local GEMM0 tile, so the gather path always runs) and the gather-combine path stay parity-green
-    (defaults: no row gather, fused combine)."""
+def test_alternate_kernel_modes(monkeypatch, name, g1_lag, fused):
+    """The work order with GEMM1 of an expert interleaved g1_lag experts behind its GEMM0 (FM_G1_LAG=1, 2; 0 = the
+    default, all GEMM0 tiles first; a lag of at least E, as 2 at configA_top1's two experts, keeps the default) and the
+    gather-combine path (FM_FUSED_COMBINE=0; the default for k <= 2 is the fused GEMM1 -> combine epilogue) stay
+    parity-green."""
     cases = dict(CASES)
     cases["odd_row_blocks"] = MoEConfig(num_experts=4, expert_top_k=2, sequence_len=768, hidden_size=256,
                                         intermediate_size=512)  # TCM = 3: an odd number of row blocks per packet
     cfg = cases[name]
-    monkeypatch.setenv("FM_GATHER", str(gather))
+    if g1_lag:
+        monkeypatch.setenv("FM_G1_LAG", str(g1_lag))
     monkeypatch.setenv("FM_FUSED_COMBINE", str(fused))
-    x, wg, we, _, _ = make_inputs(cfg, seed=300 + gather * 2 + fused)
+    x, wg, we, _, _ = make_inputs(cfg, seed=300 + g1_lag * 2 + fused)
     _compare(cfg, _run(cfg, x, wg, we), run_oracle(cfg, x, wg, we))
 
 

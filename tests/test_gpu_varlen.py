@@ -62,7 +62,7 @@ def test_parity_with_oracle_over_token_counts(E):
 
 
 # every kernel path that a token count could reach differently: router (CUDA cores / tensor cores, one and two passes
-# over d_model), combine (fused / gather, k = 3), the dense E = 1 path, the row gather from x, bias + GELU
+# over d_model), combine (fused / gather, k = 3), the dense E = 1 path, bias + GELU
 PATHS = {
     "router_cuda_cores": (BASE, {}),
     "router_tensor_cores_E32": (BASE.replace(num_experts=32), {}),
@@ -70,7 +70,6 @@ PATHS = {
     "gather_combine": (BASE, {"FM_FUSED_COMBINE": "0"}),
     "gather_combine_k3": (BASE.replace(expert_top_k=3), {}),
     "dense_E1": (BASE.replace(num_experts=1, expert_top_k=1), {}),
-    "row_gather_from_x": (BASE, {"FM_GATHER": "2"}),
     "bias_gelu": (BASE.replace(hidden_act=1), {}),
 }
 
