@@ -1,0 +1,600 @@
+"""Inputs on which fp32 arithmetic is exact, a float64 reference of every stage of the forward, and per-stage checkers.
+
+Every input is a small integer times a power of two: x on a grid of 1, the gate weights on 2^-6, W_up on 2^-3, W_down on
+2^-5, the biases on the grid of the product they are added to.  When, for every output element, sum |a_i * b_i| stays
+below 2^24 grid units, every partial sum in any order is an fp32 number, so the router logits and the pre-rounding values
+of `h` and `y` are exact whatever the tile shape, k-block order or wgmma reduction tree.  On such inputs float64 numpy
+computes the exact answer, and a correct kernel has freedom only in three documented approximations:
+
+  1. the softmax: ex2.approx.ftz on fl(z * log2e), the fma recurrence of the denominator and __fdividef
+     (gate_out, topk_w, mcw);
+  2. GELU: erff and three fp32 operations;
+  3. the combine's __fdividef(y, mcw).
+
+For those the reference is an interval: each rounding step is monotone, so the ends run through the kernel's own sequence
+of roundings, and the device value must lie inside.  Everything else (ReLU, bias adds, the RNE conversions, the bf16
+products and the bf16 accumulation of the combine) is checked bit for bit.  Top-k is decided exactly: distinct logits
+differ by at least one grid step, ties are exact, and an expert whose probability flushes to zero is picked in index
+order behind the others.
+
+The checkers raise AssertionError naming the stage, the first failing (token, pick) or (packet, row, column), and the
+device and reference bits.  No pytest in here: tests/test_exact_reference.py and tests/test_gpu_exact.py use it.
+"""
+from __future__ import annotations
+
+import dataclasses
+import functools
+from typing import Dict, Optional, Sequence
+
+import numpy as np
+import torch
+
+from flashmoe_b200.config import MoEConfig
+
+# ----------------------------------------------------------------------------- grids and fp32 limits
+X_GRID, WG_GRID, WUP_GRID, WDOWN_GRID = 0, -6, -3, -5   # log2 of the grid step of each operand
+EXACT_UNITS = 2 ** 24                                   # sum |a b| below this many product-grid units: fp32-exact sums
+
+LOG2E_F32 = np.float32(1.4426950408889634)              # the constant fast_expf multiplies by (fm_ptx.cuh)
+FLUSH_T = -126.0                                        # ex2.approx.ftz: a result below 2^-126 is flushed to +0
+FLUSH_MARGIN = 0.01                                     # no logit gap within this of the flush threshold
+MIN_PROB = 2.0 ** -120                                  # non-flushed probabilities stay well inside the normal range
+
+# Error bounds of the three approximations (relative, for normal fp32 values).
+#   ex2.approx.ftz.f32: the PTX ISA documents a maximum relative error of about 2 ulp (2^-22) over the normal range;
+#     taken as 2^-21.
+EPS_EX2 = 2.0 ** -21
+#   __fdividef(x, y): 2 ulp for 2^-126 <= |y| <= 2^126 (CUDA C++ Programming Guide, intrinsic functions) -> 2^-22.
+EPS_DIV = 2.0 ** -22
+#   GELU 0.5f * v * (1.0f + erff(v * 0.70710678f)) for v >= 0 (the generator keeps GELU pre-activations >= 0):
+#     fl(v * c) with c = fl32(1/sqrt 2): 2^-24 + 2^-24; erf is concave on [0, inf), so a relative error d of its
+#     argument moves erf by at most d relative -> 2^-23; erff itself 2 ulp (Programming Guide, standard functions)
+#     -> 2^-22; 1 + e rounds once (2^-24) and does not amplify e's relative error since e >= 0; the final product
+#     rounds once (2^-24; 0.5f * v is exact).  Total 7 * 2^-24, taken as 8 * 2^-24.
+EPS_GELU = 8 * 2.0 ** -24
+U32 = 2.0 ** -24                                        # one fp32 rounding (RNE)
+
+
+# ----------------------------------------------------------------------------- bf16 bit helpers
+def to_bits(t: torch.Tensor) -> np.ndarray:
+    assert t.dtype == torch.bfloat16
+    return t.detach().cpu().contiguous().view(torch.int16).numpy().view(np.uint16).copy()
+
+
+def from_bits(a: np.ndarray) -> torch.Tensor:
+    return torch.from_numpy(np.ascontiguousarray(a).view(np.int16).copy()).view(torch.bfloat16)
+
+
+def bits_to_f64(a: np.ndarray) -> np.ndarray:
+    return (np.asarray(a, dtype=np.uint16).astype(np.uint32) << 16).view(np.float32).astype(np.float64)
+
+
+def f32_to_bf16(a32: np.ndarray) -> np.ndarray:
+    """fp32 -> bf16 bits, round to nearest even (no NaNs occur here)."""
+    u = np.ascontiguousarray(a32, dtype=np.float32).view(np.uint32).astype(np.uint64)
+    return ((u + 0x7FFF + ((u >> 16) & 1)) >> 16).astype(np.uint16)
+
+
+def f64_to_bf16(a: np.ndarray) -> np.ndarray:
+    """float64 -> fp32 (RNE) -> bf16 (RNE): a single rounding for values that are fp32 numbers, and monotone always."""
+    return f32_to_bf16(np.asarray(a, dtype=np.float64).astype(np.float32))
+
+
+def f64_to_bf16_trunc(a: np.ndarray) -> np.ndarray:
+    """Round toward zero instead of to nearest even (planted fault)."""
+    u = np.ascontiguousarray(np.asarray(a, dtype=np.float64).astype(np.float32)).view(np.uint32)
+    return (u >> 16).astype(np.uint16)
+
+
+def order_key(bits: np.ndarray) -> np.ndarray:
+    """Integer key monotone in the bf16 value (+0 and -0 share key 0); one bf16 ulp = 1."""
+    b = np.asarray(bits, dtype=np.uint16).astype(np.int32)
+    mag = b & 0x7FFF
+    return np.where(b & 0x8000, -mag, mag)
+
+
+def grid_log2(a: np.ndarray) -> int:
+    """Largest q such that every element of `a` (bf16 values as float64) is a multiple of 2^q (0 for an all-zero array)."""
+    v = np.abs(np.asarray(a, dtype=np.float64))
+    v = v[v != 0]
+    if v.size == 0:
+        return 0
+    m, e = np.frexp(v)                       # v = m 2^e, m in [0.5, 1); bf16 has 8 significant bits
+    mi = np.rint(m * 256).astype(np.int64)
+    assert np.array_equal(mi.astype(np.float64) / 256, m), "not a bf16 value"
+    tz = np.zeros_like(mi)
+    r = mi.copy()
+    for _ in range(8):
+        even = (r & 1) == 0
+        tz += even
+        r = np.where(even, r >> 1, r)
+    return int((e - 8 + tz).min())
+
+
+def _fmt(bits) -> str:
+    b = int(bits)
+    return f"0x{b:04x} ({float(bits_to_f64(np.array([b]))[0]):.9g})"
+
+
+# ----------------------------------------------------------------------------- inputs
+@dataclasses.dataclass
+class ExactInputs:
+    cfg: MoEConfig
+    x: torch.Tensor                 # [mini_batch, seq, H] bf16 (CPU)
+    wg: torch.Tensor                # [H, E] bf16, flat view = Wg_eff [E, H]
+    we: torch.Tensor                # [E, 2, P, H] bf16; the down block is W_down_eff [H, P] reinterpreted
+    bu: Optional[torch.Tensor]      # [E, P] or None
+    bd: Optional[torch.Tensor]      # [E, H] or None
+    underflow_tokens: np.ndarray    # token indices built to flush all but one expert
+    zero_tokens: np.ndarray         # token indices with x = 0 (all logits tie)
+
+    @functools.cached_property
+    def x64(self) -> np.ndarray:
+        return self.x.reshape(-1, self.cfg.H).double().numpy()
+
+    @functools.cached_property
+    def wg_eff64(self) -> np.ndarray:
+        return self.wg.reshape(-1).reshape(self.cfg.E, self.cfg.H).double().numpy()
+
+    @functools.cached_property
+    def w_up64(self) -> np.ndarray:
+        return self.we[:, 0].double().numpy()
+
+    @functools.cached_property
+    def w_down64(self) -> np.ndarray:   # [E, H, P]: the [P, H] block viewed flat as [H, P]
+        E, _, P, H = self.we.shape
+        return self.we[:, 1].reshape(E, -1).reshape(E, H, P).double().numpy()
+
+    def bias64(self, which: str) -> Optional[np.ndarray]:
+        b = self.bu if which == "up" else self.bd
+        return None if b is None else b.double().numpy()
+
+    def device(self, dev):
+        return tuple(None if t is None else t.to(dev) for t in (self.x, self.wg, self.we, self.bu, self.bd))
+
+
+def exact_inputs(cfg: MoEConfig, seed: int, *, x_range: int = 8, wg_range: int = 4, up_range: int = 8,
+                 down_range: int = 4, bias: bool = False, gelu_friendly: bool = False,
+                 ties: Sequence[Sequence[int]] = (), boost_frac: float = 0.3, tie_boost: int = 16,
+                 zero_tokens: int = 0, underflow_tokens: int = 0, first_choice: Optional[np.ndarray] = None,
+                 route_gain: int = 32) -> ExactInputs:
+    """Seeded exact inputs for `cfg` (CPU bf16 tensors).
+
+    x: integers in [-x_range, x_range]; Wg_eff: integers in [-wg_range, wg_range] * 2^-6; W_up: integers in
+    [-up_range, up_range] * 2^-3; W_down: integers in [-down_range, down_range] * 2^-5; b_up on 2^-3, b_down on 2^-8.
+
+    Routing controls (x columns 0, 1 and 2 .. 2 + E are reserved for them when used):
+      ties         expert groups whose Wg_eff rows are made identical (exact logit ties for every token); a
+                   `boost_frac` share of the tokens gets x[:, 0] in {1, 2} and the tied experts a weight of
+                   `tie_boost` there, which lifts the tied groups into those tokens' top-k.
+      zero_tokens  tokens with x = 0: every logit is 0, p = 1/E, picks 0 .. k-1.
+      underflow_tokens  tokens with x[:, 1] = 1; expert E-1 weighs 192 there and leads by more than 88 logit units,
+                   so every other probability flushes to 0 and the rest of the top-k is picked in index order.
+      first_choice planned routing: token t has x[t, 2 + first_choice[t]] = 1, and expert e weighs `route_gain` in
+                   column 2 + e, so first_choice[t] leads every other expert (exact packet sizes for k = 1).
+    gelu_friendly: x >= 0, sparse W_up >= 0 and b_up >= 0, so GELU pre-activations are >= 0 and the GELU error bound
+    applies, and h keeps a grid coarse enough for GEMM1 to stay exact."""
+    g = np.random.default_rng(seed)
+    S, H, P, E = cfg.S, cfg.H, cfg.P, cfg.E
+    if gelu_friendly:
+        x = g.integers(0, x_range + 1, size=(S, H)).astype(np.float64)
+        up = g.integers(1, up_range + 1, size=(E, P, H)) * (g.random((E, P, H)) < 4.0 / H)
+    else:
+        x = g.integers(-x_range, x_range + 1, size=(S, H)).astype(np.float64)
+        up = g.integers(-up_range, up_range + 1, size=(E, P, H))
+    wg = g.integers(-wg_range, wg_range + 1, size=(E, H)).astype(np.float64) * 2.0 ** WG_GRID
+    up = up.astype(np.float64) * 2.0 ** WUP_GRID
+    down = g.integers(-down_range, down_range + 1, size=(E, H, P)).astype(np.float64) * 2.0 ** WDOWN_GRID
+    bu = bd = None
+    if bias:
+        lo = 0 if gelu_friendly else -16
+        bu = g.integers(lo, 17, size=(E, P)).astype(np.float64) * 2.0 ** WUP_GRID
+        bd = g.integers(-256, 257, size=(E, H)).astype(np.float64) * 2.0 ** (WUP_GRID + WDOWN_GRID)
+
+    reserved = 2 + (E if first_choice is not None else 0)
+    if ties or underflow_tokens or first_choice is not None:
+        assert H > reserved, f"H={H} leaves no room for the routing columns"
+        x[:, :reserved] = 0
+        wg[:, :reserved] = 0
+    if first_choice is not None:
+        fc = np.asarray(first_choice)
+        assert fc.shape == (S,)
+        x[np.arange(S), 2 + fc] = 1
+        wg[np.arange(E), 2 + np.arange(E)] = route_gain
+    tied = sorted({e for grp in ties for e in grp})
+    for grp in ties:
+        for e in grp[1:]:
+            wg[e] = wg[grp[0]]
+    if ties:
+        boosted = g.random(S) < boost_frac
+        x[boosted, 0] = g.integers(1, 3, size=int(boosted.sum()))
+        wg[tied, 0] = tie_boost
+    under = np.sort(g.choice(S, size=underflow_tokens, replace=False)) if underflow_tokens else np.zeros(0, np.int64)
+    if underflow_tokens:
+        x[under, 0] = 0
+        x[under, 1] = 1
+        wg[E - 1, 1] = 192
+    zeros = np.setdiff1d(np.arange(S), under)
+    zeros = np.sort(g.choice(zeros, size=zero_tokens, replace=False)) if zero_tokens else np.zeros(0, np.int64)
+    x[zeros] = 0
+
+    def bf(a):
+        t = torch.from_numpy(np.ascontiguousarray(a)).bfloat16()
+        assert np.array_equal(t.double().numpy(), a), "generator produced a value that is not a bf16 number"
+        return t
+
+    we = np.stack([up, down.reshape(E, -1).reshape(E, P, H)], axis=1)
+    return ExactInputs(cfg, bf(x).reshape(cfg.mini_batch, cfg.sequence_len, H), bf(wg.reshape(-1).reshape(H, E)),
+                       bf(we), None if bu is None else bf(bu), None if bd is None else bf(bd), under, zeros)
+
+
+# ----------------------------------------------------------------------------- preconditions
+def assert_exact_sums(a: np.ndarray, b: np.ndarray, bias: Optional[np.ndarray], what: str) -> None:
+    """a [M, K] @ b[N, K]^T (+ bias [N]) has every partial sum exact in fp32: all values on a common product grid and
+    sum |a b| + |bias| below 2^24 grid units for every output element."""
+    if a.size == 0 or b.size == 0:
+        return
+    q = grid_log2(a) + grid_log2(b)
+    tot = np.abs(a) @ np.abs(b).T
+    if bias is not None:
+        assert grid_log2(bias) >= q or not np.any(bias), f"{what}: bias is off the product grid 2^{q}"
+        tot = tot + np.abs(bias)[None, :]
+    worst = float(tot.max())
+    assert worst < EXACT_UNITS * 2.0 ** q, (f"{what}: sum |ab| reaches {worst:.6g} = {worst / 2.0 ** q:.4g} units of "
+                                            f"2^{q}, not below 2^24: fp32 partial sums would not be exact")
+
+
+# ----------------------------------------------------------------------------- router reference
+@dataclasses.dataclass
+class RouterRef:
+    logits: np.ndarray     # float64 [n, E], exact
+    flushed: np.ndarray    # bool [n, E]: probability exactly +0
+    topk: np.ndarray       # int32 [n, k]
+    p_lo: np.ndarray       # float64 [n, E] bounds of the device's fp32 probability
+    p_hi: np.ndarray
+    go_lo: np.ndarray      # bf16 bits [n, E] bounds of gate_out
+    go_hi: np.ndarray
+
+    def mcw_bounds(self):
+        k = self.topk.shape[1]
+        rows = np.arange(self.topk.shape[0])[:, None]
+        lo = self.p_lo[rows, self.topk].sum(1) * (1 - U32) ** k
+        hi = self.p_hi[rows, self.topk].sum(1) * (1 + U32) ** k
+        return lo, hi
+
+
+def router_reference(x: np.ndarray, wg_eff: np.ndarray, k: int) -> RouterRef:
+    n, E = x.shape[0], wg_eff.shape[0]
+    assert_exact_sums(x, wg_eff, None, "router logits")
+    logits = x @ wg_eff.T
+    if n == 0:
+        z = np.zeros((0, E))
+        return RouterRef(z, z.astype(bool), np.zeros((0, k), np.int32), z, z, z.astype(np.uint16), z.astype(np.uint16))
+    m = logits.max(axis=1, keepdims=True)
+    d32 = (logits - m).astype(np.float32)                       # exact: both on the 2^-6 grid, far below 2^24 units
+    t32 = (d32 * LOG2E_F32).astype(np.float64)                 # fl(z * log2e), the argument of ex2 in the final pass
+    near = np.abs(t32 - FLUSH_T) < FLUSH_MARGIN * float(LOG2E_F32)
+    assert not near.any(), f"token {int(np.argwhere(near)[0][0])}: a logit gap lies within {FLUSH_MARGIN} of the flush threshold"
+    flushed = t32 < FLUSH_T
+    # denominator: the recurrence dI = fma(dI, ex2(t(pM - mI)), ex2(t(l_e - mI))) against D = sum 2^((l_e - m) c):
+    #   every ex2 call is within EPS_EX2 and a term passes through at most E of them, every fma rounds once (E * U32);
+    #   the t() roundings along a term's path add exponent errors that telescope to at most U32 * c * (m - l_e), i.e.
+    #   a relative 2^-24 * (m - l_e); terms and rescale factors that flush in the recurrence change dI by < 2^-126 * E.
+    c = float(LOG2E_F32)
+    D = np.where(flushed, 0.0, np.exp2(d32.astype(np.float64) * c)).sum(axis=1)
+    spread = np.where(flushed, 0.0, -d32.astype(np.float64)).max(axis=1)
+    dD = (E + 1) * (EPS_EX2 + U32) + U32 * spread + E * 2.0 ** -126
+    D_lo, D_hi = D * (1 - dD), D * (1 + dD)
+    num = np.exp2(t32)
+    p_lo = np.where(flushed, 0.0, num * (1 - EPS_EX2) / D_hi[:, None] * (1 - EPS_DIV))
+    p_hi = np.where(flushed, 0.0, num * (1 + EPS_EX2) / D_lo[:, None] * (1 + EPS_DIV))
+    small = ~flushed & (p_lo < MIN_PROB)
+    assert not small.any(), f"token {int(np.argwhere(small)[0][0])}: a probability leaves the normal fp32 range"
+    # top-k: strict '>' in ascending expert order, i.e. larger p first and the lower index on equal p.  Distinct
+    # logits give distinct p (they differ by >= 2^-6 in the exponent's argument, 1.6 %, far beyond the error bounds),
+    # equal logits give identical device p, and flushed experts all have p = +0.
+    key = np.where(flushed, -np.inf, logits)
+    topk = np.argsort(-key, axis=1, kind="stable")[:, :k].astype(np.int32)
+    return RouterRef(logits, flushed, topk, p_lo, p_hi, f64_to_bf16(p_lo), f64_to_bf16(p_hi))
+
+
+# ----------------------------------------------------------------------------- bookkeeping
+def slots_from_topk(topk: np.ndarray, E: int, EC: int):
+    """slot [n, k]: position of (t, j) among all selections of its expert in ascending (token, pick) order, dropped ones
+    counted; counts [E]: all selections; recv_cnt [E] = min(counts, EC); kept = slot < EC."""
+    flat = np.asarray(topk, dtype=np.int64).reshape(-1)
+    assert flat.size == 0 or (flat.min() >= 0 and flat.max() < E), "expert index out of range"
+    counts = np.bincount(flat, minlength=E).astype(np.int32)
+    order = np.argsort(flat, kind="stable")
+    start = np.concatenate([[0], np.cumsum(counts)[:-1]])
+    slot = np.empty(flat.size, dtype=np.int32)
+    slot[order] = np.arange(flat.size) - start[flat[order]]
+    slot = slot.reshape(topk.shape)
+    return slot, counts, np.minimum(counts, EC).astype(np.int32), slot < EC
+
+
+def packet_tokens(topk: np.ndarray, slot: np.ndarray, E: int, EC: int):
+    """For every expert, the token of each kept slot in slot order (rows of its packet)."""
+    out = []
+    for e in range(E):
+        t, j = np.nonzero((topk == e) & (slot < EC))
+        out.append(t[np.argsort(slot[t, j])])
+    return out
+
+
+# ----------------------------------------------------------------------------- expert FFN reference
+@dataclasses.dataclass
+class Rounded:
+    lo: np.ndarray          # bf16 bits
+    hi: np.ndarray
+    exact: np.ndarray       # float64 value before the final rounding (the midpoint for intervals)
+
+
+def gemm0_reference(rows: np.ndarray, w_up: np.ndarray, b_up: Optional[np.ndarray], act: int, what: str) -> Rounded:
+    """h = RNE(act(rows . w_up^T + b_up)); ReLU is exact, GELU an interval (EPS_GELU, pre-activations >= 0)."""
+    assert_exact_sums(rows, w_up, b_up, what)
+    v = rows @ w_up.T
+    if b_up is not None:
+        v = v + b_up[None, :]
+    if act == 0:
+        a = np.maximum(v, 0.0)
+        b = f64_to_bf16(a)
+        return Rounded(b, b, a)
+    from scipy.special import erf
+
+    assert (v >= 0).all(), f"{what}: a GELU pre-activation is negative; the GELU error bound assumes v >= 0"
+    gl = 0.5 * v * (1.0 + erf(v / np.sqrt(2.0)))
+    return Rounded(f64_to_bf16(gl * (1 - EPS_GELU)), f64_to_bf16(gl * (1 + EPS_GELU)), gl)
+
+
+def gemm1_reference(h_bits: np.ndarray, w_down: np.ndarray, b_down: Optional[np.ndarray], what: str) -> Rounded:
+    """y = RNE(h . w_down^T + b_down) for the given h (bf16 bits) -- exact."""
+    h = bits_to_f64(h_bits)
+    assert_exact_sums(h, w_down, b_down, what)
+    v = h @ w_down.T
+    if b_down is not None:
+        v = v + b_down[None, :]
+    b = f64_to_bf16(v)
+    return Rounded(b, b, v)
+
+
+# ----------------------------------------------------------------------------- combine reference
+def combine_tokens(y_of: np.ndarray, kept: np.ndarray, pw_bits: np.ndarray, mcw: np.ndarray) -> Rounded:
+    """out [n, H] for n tokens: y_of bf16 bits [n, k, H] (the y row of each pick; ignored where not kept), kept bool
+    [n, k], pw_bits bf16 [n, k] (topk_w), mcw fp32 [n].
+      k == 1: out = y, unscaled; a dropped pick gives +0.
+      k >= 2: term_j = RNE(pw_j * RNE(__fdividef(y_j, mcw))), out = bf16 accumulation of the kept terms in pick order
+              from +0, each add rounded to fp32 and then to bf16 (combine_rows; for k = 2 the order is immaterial).
+    Only __fdividef is approximate (EPS_DIV); both ends of every step go through the same roundings."""
+    n, k, H = y_of.shape
+    if k == 1:
+        b = np.where(kept[:, :, None], y_of, 0).astype(np.uint16)[:, 0]
+        return Rounded(b, b, bits_to_f64(b))
+    m = np.asarray(mcw, dtype=np.float32).astype(np.float64)[:, None]
+    acc_lo = np.zeros((n, H))
+    acc_hi = np.zeros((n, H))
+    real = np.zeros((n, H))   # the combine in real arithmetic, for the rounding statistics
+    for j in range(k):
+        y = bits_to_f64(y_of[:, j])
+        q = y / m
+        qa, qb = q * (1 - EPS_DIV), q * (1 + EPS_DIV)
+        ql_b, qh_b = f64_to_bf16(np.minimum(qa, qb)), f64_to_bf16(np.maximum(qa, qb))
+        assert (order_key(qh_b) - order_key(ql_b) <= 1).all(), "combine: RNE(y / mcw) interval wider than one ulp"
+        ql, qh = bits_to_f64(ql_b), bits_to_f64(qh_b)
+        pw = bits_to_f64(pw_bits[:, j])[:, None]
+        tl, th = bits_to_f64(f64_to_bf16(pw * ql)), bits_to_f64(f64_to_bf16(pw * qh))
+        keep = kept[:, j][:, None]
+        real += np.where(keep, pw * q, 0.0)
+        acc_lo = np.where(keep, bits_to_f64(f64_to_bf16(acc_lo + tl)), acc_lo)
+        acc_hi = np.where(keep, bits_to_f64(f64_to_bf16(acc_hi + th)), acc_hi)
+    return Rounded(f64_to_bf16(acc_lo), f64_to_bf16(acc_hi), real)
+
+
+# ----------------------------------------------------------------------------- statistics
+class Stats:
+    """Per stage: elements checked, elements whose exact value needed rounding, intervals of nonzero width."""
+
+    def __init__(self):
+        self.d: Dict[str, np.ndarray] = {}
+
+    def add(self, stage: str, checked: int, rounded: int = 0, wide: int = 0) -> None:
+        self.d.setdefault(stage, np.zeros(3, np.int64))
+        self.d[stage] += (checked, rounded, wide)
+
+    def merge(self, other: "Stats") -> None:
+        for s, v in other.d.items():
+            self.d.setdefault(s, np.zeros(3, np.int64))
+            self.d[s] += v
+
+    def line(self) -> str:
+        return "; ".join(f"{s}: {v[0]} checked, {v[1]} rounded, {v[2]} wide" for s, v in self.d.items())
+
+
+def rounded_count(r: Rounded) -> int:
+    """Elements whose exact (or midpoint) value is not the bf16 value it was rounded to."""
+    return int((bits_to_f64(r.lo) != r.exact).sum())
+
+
+# ----------------------------------------------------------------------------- checkers
+def _interval_check(got_bits: np.ndarray, r: Rounded, what: str, labels: Sequence[str],
+                    index_of=lambda i: i, max_width: Optional[int] = 1) -> int:
+    """got inside [lo, hi] elementwise (+0 == -0); the interval is at most `max_width` bf16 ulps wide (None: any width;
+    the combine's sums can cancel, so one ulp of a term may be several of the sum).  Returns the number of intervals of
+    nonzero width."""
+    g, lo, hi = order_key(got_bits), order_key(r.lo), order_key(r.hi)
+    width = hi - lo
+    assert (width >= 0).all() and (max_width is None or (width <= max_width).all()), (
+        f"{what}: reference interval wider than one bf16 ulp at {_where(np.argwhere((width < 0) | (width > 1))[0], labels, index_of)}")
+    bad = (g < lo) | (g > hi)
+    if bad.any():
+        i = tuple(np.argwhere(bad)[0])
+        raise AssertionError(f"{what}: {int(bad.sum())} of {bad.size} elements outside the reference; first at "
+                             f"{_where(i, labels, index_of)}: device {_fmt(got_bits[i])}, reference "
+                             f"[{_fmt(r.lo[i])}, {_fmt(r.hi[i])}]")
+    return int((width > 0).sum())
+
+
+def _where(i, labels, index_of) -> str:
+    i = index_of(tuple(int(v) for v in i))
+    return ", ".join(f"{n} {v}" for n, v in zip(labels, i))
+
+
+def check_topk(got: np.ndarray, ref: RouterRef, what: str = "topk_idx") -> None:
+    bad = (got != ref.topk).any(axis=1)
+    if bad.any():
+        t = int(np.flatnonzero(bad)[0])
+        j = int(np.flatnonzero(got[t] != ref.topk[t])[0])
+        raise AssertionError(f"{what}: {int(bad.sum())} tokens differ; first token {t} pick {j}: device {got[t].tolist()}, "
+                             f"reference {ref.topk[t].tolist()} (logits of those experts: "
+                             f"{ref.logits[t, got[t]].tolist()} vs {ref.logits[t, ref.topk[t]].tolist()})")
+
+
+def check_equal(got: np.ndarray, want: np.ndarray, what: str, labels: Sequence[str], signed_zero: bool = True) -> None:
+    got, want = np.asarray(got), np.asarray(want)
+    assert got.shape == want.shape, f"{what}: shape {got.shape} != {want.shape}"
+    bad = got != want
+    if not signed_zero and got.dtype == np.uint16:   # an exact zero sum may carry either sign
+        bad &= order_key(got) != order_key(want)
+    if bad.any():
+        i = tuple(int(v) for v in np.argwhere(bad)[0])
+        gv, wv = (_fmt(got[i]), _fmt(want[i])) if got.dtype == np.uint16 else (got[i], want[i])
+        raise AssertionError(f"{what}: {int(bad.sum())} of {bad.size} differ; first at "
+                             f"{', '.join(f'{n} {v}' for n, v in zip(labels, i))}: device {gv}, reference {wv}")
+
+
+@dataclasses.dataclass
+class Device:
+    """What one launch left behind (host copies); `n` tokens valid."""
+    out: np.ndarray        # bf16 bits [n, H]
+    topk_idx: np.ndarray   # [n, k]
+    topk_w: np.ndarray     # bf16 bits [n, k]
+    mcw: np.ndarray        # fp32 [n]
+    gate_out: np.ndarray   # bf16 bits [n, E]
+    slot: np.ndarray       # [n, k]
+    counts: np.ndarray     # [E]
+    recv_cnt: Optional[np.ndarray]
+    recv_x: Optional[np.ndarray]   # [E, pEC, H] or None (the dense path copies nothing)
+    hidden: np.ndarray     # [E, pEC, P]
+    ret_y: Optional[np.ndarray]    # [E, pEC, H] (gather path) or None
+
+
+def check_forward(inp: ExactInputs, dev: Device, EC: int, n: Optional[int] = None, stats: Optional[Stats] = None):
+    """Every stage of one launch over the first n tokens of `inp` (default all), in pipeline order; GEMM1 and the
+    combine are referenced from the device's own hidden, topk_w and mcw, so a failure names the stage that broke."""
+    cfg = inp.cfg
+    E, k, H = cfg.E, cfg.k, cfg.H
+    st = stats if stats is not None else Stats()
+    x = inp.x64[: (cfg.S if n is None else n)]
+    n = x.shape[0]
+    ref = router_reference(x, inp.wg_eff64, k)
+    check_topk(dev.topk_idx, ref)
+    st.add("topk_idx", ref.topk.size)
+    w1 = _interval_check(dev.gate_out, Rounded(ref.go_lo, ref.go_hi, 0.5 * (ref.p_lo + ref.p_hi)), "gate_out",
+                         ("token", "expert"))
+    st.add("gate_out", ref.go_lo.size, int((ref.p_lo != bits_to_f64(ref.go_lo)).sum()), w1)
+    rows = np.arange(n)[:, None]
+    check_equal(dev.topk_w, dev.gate_out[rows, dev.topk_idx], "topk_w vs gate_out[t, topk_idx]", ("token", "pick"))
+    st.add("topk_w", dev.topk_w.size)
+    lo, hi = ref.mcw_bounds()
+    bad = ~((dev.mcw >= lo) & (dev.mcw <= hi))
+    assert not bad.any(), (f"mcw: token {int(np.flatnonzero(bad)[0])}: device {dev.mcw[bad][0]!r} outside "
+                           f"[{lo[bad][0]!r}, {hi[bad][0]!r}]")
+    st.add("mcw", n)
+
+    slot, counts, recv_cnt, kept = slots_from_topk(dev.topk_idx, E, EC)
+    check_equal(dev.slot, slot, "slot", ("token", "pick"))
+    check_equal(dev.counts, counts, "counts", ("expert",))
+    if dev.recv_cnt is not None:
+        check_equal(dev.recv_cnt, recv_cnt, "recv_cnt", ("expert",))
+    st.add("slot/counts/recv_cnt", slot.size + 2 * E)
+
+    toks = packet_tokens(dev.topk_idx, slot, E, EC)
+    xb = f64_to_bf16(x)
+    y_dev_ref = np.zeros((E, max(1, int(recv_cnt.max(initial=0))), H), np.uint16)
+    for e in range(E):
+        c = len(toks[e])
+        if c == 0:
+            continue
+        if dev.recv_x is not None:
+            check_equal(dev.recv_x[e, :c], xb[toks[e]], f"recv_x of expert {e}", ("slot", "column"))
+            st.add("recv_x", c * H)
+        h_ref = gemm0_reference(x[toks[e]], inp.w_up64[e], None if inp.bu is None else inp.bias64("up")[e],
+                                cfg.hidden_act, f"GEMM0 of expert {e}")
+        h_dev = dev.hidden[e, :c]
+        if cfg.hidden_act == 0:
+            check_equal(h_dev, h_ref.lo, f"hidden of expert {e}", ("slot", "column"), signed_zero=False)
+            st.add("hidden", h_dev.size, rounded_count(h_ref))
+        else:
+            w = _interval_check(h_dev, h_ref, f"hidden of expert {e}", ("slot", "column"))
+            st.add("hidden", h_dev.size, rounded_count(h_ref), w)
+        y_ref = gemm1_reference(h_dev, inp.w_down64[e], None if inp.bd is None else inp.bias64("down")[e],
+                                f"GEMM1 of expert {e}")
+        y_dev_ref[e, :c] = y_ref.lo
+        if dev.ret_y is not None:
+            check_equal(dev.ret_y[e, :c], y_ref.lo, f"ret_y of expert {e}", ("slot", "column"), signed_zero=False)
+            st.add("ret_y", c * H, rounded_count(y_ref))
+        else:
+            st.add("y (in the fused epilogue)", 0, rounded_count(y_ref))
+
+    y_of = y_dev_ref[dev.topk_idx, np.where(kept, slot, 0)]          # [n, k, H]
+    out_ref = combine_tokens(y_of, kept, dev.topk_w, dev.mcw)
+    w = _interval_check(dev.out, out_ref, "out", ("token", "column"), max_width=None)
+    st.add("out", dev.out.size, rounded_count(out_ref) if k > 1 else 0, w)
+    dropped = ~kept.any(axis=1)
+    if dropped.any():
+        check_equal(dev.out[dropped], np.zeros((int(dropped.sum()), H), np.uint16),
+                    "out rows of tokens whose picks were all dropped (+0)", ("row", "column"))
+        st.add("all-dropped rows", int(dropped.sum()) * H)
+    return st
+
+
+def check_preconditions(inp: ExactInputs, EC: int, min_h_rounded: float, min_out_rounded: float,
+                        n: Optional[int] = None, dense: bool = False) -> Stats:
+    """Run the reference alone (the device values replaced by the reference's own) and assert the rounding shares:
+    inputs that never round do not test RNE.  Returns the statistics."""
+    dev = reference_device(inp, EC, n, dense)
+    st = check_forward(inp, dev, EC, n)
+    zero = np.zeros(3, np.int64)   # (a call with no tokens has neither)
+    hs, os_ = st.d.get("hidden", zero), st.d.get("out", zero)
+    if hs[0]:
+        assert hs[1] >= min_h_rounded * hs[0], f"only {hs[1]} of {hs[0]} h elements needed rounding"
+    if os_[0] and inp.cfg.k > 1:
+        assert os_[1] >= min_out_rounded * os_[0], f"only {os_[1]} of {os_[0]} out elements needed rounding"
+    return st
+
+
+def reference_device(inp: ExactInputs, EC: int, n: Optional[int] = None, dense: bool = False) -> Device:
+    """A Device record computed by the reference itself (midpoints of the intervals): what a correct kernel could
+    have produced.  The planted-fault tests start from it."""
+    cfg = inp.cfg
+    E, k, H, P = cfg.E, cfg.k, cfg.H, cfg.P
+    x = inp.x64[: (cfg.S if n is None else n)]
+    n = x.shape[0]
+    ref = router_reference(x, inp.wg_eff64, k)
+    gate_out = ref.go_lo.copy()
+    rows = np.arange(n)[:, None]
+    p_mid = 0.5 * (ref.p_lo + ref.p_hi)
+    mcw = np.zeros(n, np.float32)
+    for j in range(k):
+        mcw = (mcw + p_mid[rows[:, 0], ref.topk[:, j]].astype(np.float32)).astype(np.float32)
+    slot, counts, recv_cnt, kept = slots_from_topk(ref.topk, E, EC)
+    toks = packet_tokens(ref.topk, slot, E, EC)
+    rmax = max(1, int(recv_cnt.max(initial=0)))
+    recv_x = np.zeros((E, rmax, H), np.uint16)
+    hidden = np.zeros((E, rmax, P), np.uint16)
+    ret_y = np.zeros((E, rmax, H), np.uint16)
+    for e in range(E):
+        c = len(toks[e])
+        if c == 0:
+            continue
+        recv_x[e, :c] = f64_to_bf16(x[toks[e]])
+        h = gemm0_reference(x[toks[e]], inp.w_up64[e], inp.bias64("up")[e] if inp.bu is not None else None,
+                            cfg.hidden_act, "GEMM0")
+        hidden[e, :c] = h.lo
+        ret_y[e, :c] = gemm1_reference(h.lo, inp.w_down64[e], inp.bias64("down")[e] if inp.bd is not None else None,
+                                       "GEMM1").lo
+    topk_w = gate_out[rows, ref.topk]
+    y_of = ret_y[ref.topk, np.where(kept, slot, 0)]
+    out = combine_tokens(y_of, kept, topk_w, mcw).lo
+    return Device(out, ref.topk.copy(), topk_w, mcw, gate_out, slot, counts, recv_cnt, None if dense else recv_x,
+                  hidden, ret_y)

@@ -1,0 +1,188 @@
+"""CPU checks of tests/exact.py: the C oracle agrees with the float64 reference on exact inputs, every case the GPU file
+runs satisfies the exactness preconditions and actually rounds, and every checker catches the faults it exists for --
+including an output fault that the seeded-randn acceptance rule (tests/util.py::check_output) lets through."""
+import numpy as np
+import pytest
+
+from oracle import moe_oracle as mo
+from tests import exact as ex
+from tests import test_gpu_exact as gx
+from tests.util import check_output
+
+
+def _oracle(inp, EC, act):
+    cfg = inp.cfg
+    up, down = mo.split_expert_weights(ex.to_bits(inp.we))
+    return mo.forward(ex.to_bits(inp.x.reshape(cfg.S, cfg.H)),
+                      mo.gate_weights_effective(ex.to_bits(inp.wg), cfg.E, cfg.H), up, down, k=cfg.k, EC=EC, act=act,
+                      b_up=None if inp.bu is None else ex.to_bits(inp.bu),
+                      b_down=None if inp.bd is None else ex.to_bits(inp.bd))
+
+
+@pytest.mark.parametrize("name", ["router_E8_k2_tc0", "router_E64_k4_tc0", "router_E129_k2_tc0", "k3", "fused_k1",
+                                  "bias_relu", "bias_gelu", "packet_cut_at_EC"])
+def test_oracle_agrees_with_exact_reference(name):
+    """Top-k, slots and counts identical; h and y bit-identical; gate_out, mcw and out inside the reference intervals."""
+    cfg, gen, _ = gx.CASES[name]
+    inp = ex.exact_inputs(cfg, seed=7 + len(name), **gen)
+    o = _oracle(inp, cfg.EC, cfg.hidden_act)
+    ref = ex.router_reference(inp.x64, inp.wg_eff64, cfg.k)
+    ex.check_topk(o.topk_idx, ref, "oracle topk_idx")
+    slot, counts, _, kept = ex.slots_from_topk(ref.topk, cfg.E, cfg.EC)
+    assert np.array_equal(o.slot, slot) and np.array_equal(o.counts, counts) and np.array_equal(o.kept.astype(bool), kept)
+    ex._interval_check(o.gate_out, ex.Rounded(ref.go_lo, ref.go_hi, ref.p_lo), "oracle gate_out", ("token", "expert"))
+    lo, hi = ref.mcw_bounds()
+    assert ((o.mcw >= lo) & (o.mcw <= hi)).all()
+    # h and y: the oracle's expert FFN on every packet against the reference
+    xb = ex.to_bits(inp.x.reshape(cfg.S, cfg.H))
+    up, down = mo.split_expert_weights(ex.to_bits(inp.we))
+    toks = ex.packet_tokens(ref.topk, slot, cfg.E, cfg.EC)
+    y_all = np.zeros((cfg.E, max(1, max(len(t) for t in toks)), cfg.H), np.uint16)
+    for e in range(cfg.E):
+        if not len(toks[e]):
+            continue
+        h_o, y_o = mo.expert_ffn(xb[toks[e]], up[e], down[e], act=cfg.hidden_act,
+                                 b_up=None if inp.bu is None else ex.to_bits(inp.bu)[e],
+                                 b_down=None if inp.bd is None else ex.to_bits(inp.bd)[e])
+        h = ex.gemm0_reference(inp.x64[toks[e]], inp.w_up64[e], None if inp.bu is None else inp.bias64("up")[e],
+                               cfg.hidden_act, "GEMM0")
+        if cfg.hidden_act == 0:
+            ex.check_equal(h_o, h.lo, f"oracle h of expert {e}", ("slot", "column"))
+        else:
+            ex._interval_check(h_o, h, f"oracle h of expert {e}", ("slot", "column"))
+        y = ex.gemm1_reference(h_o, inp.w_down64[e], None if inp.bd is None else inp.bias64("down")[e], "GEMM1")
+        ex.check_equal(y_o, y.lo, f"oracle y of expert {e}", ("slot", "column"))
+        y_all[e, :len(toks[e])] = y_o
+    pw = o.gate_out[np.arange(cfg.S)[:, None], o.topk_idx]
+    out = ex.combine_tokens(y_all[ref.topk, np.where(kept, slot, 0)], kept, pw, o.mcw)
+    ex._interval_check(o.out, out, "oracle out", ("token", "column"), max_width=None)
+
+
+@pytest.mark.parametrize("name", list(gx.CASES))
+def test_gpu_cases_are_exact_and_round(name):
+    cfg, gen, env = gx.CASES[name]
+    inp = ex.exact_inputs(cfg, seed=1000 + sum(map(ord, name)), **gen)   # the GPU test's seed
+    ex.check_preconditions(inp, cfg.EC, gx.MIN_H_ROUNDED, gx.MIN_OUT_ROUNDED, dense=gx._dense(cfg, env))
+
+
+def test_multi_launch_cases_are_exact_and_round():
+    cfg = gx.TOKENS_CFG
+    inp = ex.exact_inputs(cfg, seed=2000, ties=gx.tie_groups(cfg.E), zero_tokens=4, underflow_tokens=8)
+    for n in gx.TOKEN_COUNTS:
+        ex.check_preconditions(inp, cfg.EC_of(n), gx.MIN_H_ROUNDED if n > 30 else 0, gx.MIN_OUT_ROUNDED, n=n)
+    for fused in (1, 0):
+        for i in range(5):
+            cfg = gx.EPILOGUE_ORDER
+            inp = ex.exact_inputs(cfg, seed=3000 + 10 * fused + i, ties=gx.tie_groups(cfg.E), zero_tokens=4)
+            ex.check_preconditions(inp, cfg.EC, gx.MIN_H_ROUNDED, gx.MIN_OUT_ROUNDED)
+
+
+@pytest.mark.parametrize("seed", [4000, 4001, 4002, 4010])
+def test_config_B_inputs_are_exact_and_round(seed):
+    cfg = gx.CONFIG_B
+    ex.check_preconditions(ex.exact_inputs(cfg, seed=seed, **gx.CONFIG_B_GEN), cfg.EC, gx.MIN_H_ROUNDED,
+                           gx.MIN_OUT_ROUNDED)
+
+
+# ----------------------------------------------------------------------------- planted faults
+def _base(name="router_E8_k2_tc0", seed=11):
+    cfg, gen, _ = gx.CASES[name]
+    inp = ex.exact_inputs(cfg, seed=seed, **gen)
+    return cfg, inp, ex.reference_device(inp, cfg.EC)
+
+
+def test_reference_device_passes_its_own_checks():
+    for name in ("router_E8_k2_tc0", "router_E1024_k2", "k3", "bias_gelu"):
+        cfg, inp, dev = _base(name)
+        ex.check_forward(inp, dev, cfg.EC)
+
+
+def test_fault_h_one_ulp():
+    cfg, inp, dev = _base()
+    e = int(np.argmax(dev.counts))
+    dev.hidden[e, 3, 5] += 1
+    with pytest.raises(AssertionError, match=f"hidden of expert {e}"):
+        ex.check_forward(inp, dev, cfg.EC)
+
+
+def test_fault_h_truncated_instead_of_rne():
+    cfg, inp, dev = _base()
+    slot, _, _, _ = ex.slots_from_topk(dev.topk_idx, cfg.E, cfg.EC)
+    toks = ex.packet_tokens(dev.topk_idx, slot, cfg.E, cfg.EC)
+    for e in range(cfg.E):
+        v = np.maximum(inp.x64[toks[e]] @ inp.w_up64[e].T, 0)
+        dev.hidden[e, :len(toks[e])] = ex.f64_to_bf16_trunc(v)
+    with pytest.raises(AssertionError, match="hidden of expert"):
+        ex.check_forward(inp, dev, cfg.EC)
+
+
+def test_fault_recv_x_rows_swapped():
+    cfg, inp, dev = _base()
+    e = int(np.argmax(dev.counts))
+    a, b = 0, next(i for i in range(1, dev.recv_cnt[e]) if not np.array_equal(dev.recv_x[e, 0], dev.recv_x[e, i]))
+    dev.recv_x[e, [a, b]] = dev.recv_x[e, [b, a]]
+    with pytest.raises(AssertionError, match=f"recv_x of expert {e}"):
+        ex.check_forward(inp, dev, cfg.EC)
+
+
+def test_fault_tie_broken_toward_higher_index():
+    cfg, inp, dev = _base()
+    ref = ex.router_reference(inp.x64, inp.wg_eff64, cfg.k)
+    lg = ref.logits[np.arange(cfg.S)[:, None], ref.topk]
+    t = int(np.flatnonzero(lg[:, 0] == lg[:, 1])[0])   # a token whose two picks tie
+    dev.topk_idx[t] = dev.topk_idx[t][::-1]
+    with pytest.raises(AssertionError, match=f"topk_idx: 1 tokens differ; first token {t} "):
+        ex.check_forward(inp, dev, cfg.EC)
+
+
+def test_fault_underflow_tie_broken_by_logit():
+    cfg, inp, dev = _base("router_E64_k4_tc0")
+    ref = ex.router_reference(inp.x64, inp.wg_eff64, cfg.k)
+    t = int(inp.underflow_tokens[0])
+    assert ref.flushed[t].sum() == cfg.E - 1 and ref.topk[t, 0] == cfg.E - 1
+    assert list(ref.topk[t, 1:]) == list(range(cfg.k - 1))   # index order behind the leader
+    by_logit = np.argsort(-np.where(np.arange(cfg.E) == cfg.E - 1, -np.inf, ref.logits[t]), kind="stable")
+    dev.topk_idx[t, 1:] = by_logit[: cfg.k - 1]
+    assert not np.array_equal(dev.topk_idx[t], ref.topk[t])
+    with pytest.raises(AssertionError, match=f"first token {t} "):
+        ex.check_forward(inp, dev, cfg.EC)
+
+
+def test_fault_dropped_pair_contribution_added():
+    cfg, inp, dev = _base("packet_cut_at_EC")   # k = 1, experts cut at EC = 64: dropped tokens must be +0
+    t = int(np.flatnonzero(dev.slot[:, 0] >= cfg.EC)[0])
+    e = int(dev.topk_idx[t, 0])
+    h = ex.gemm0_reference(inp.x64[t:t + 1], inp.w_up64[e], None, 0, "GEMM0")
+    dev.out[t] = ex.gemm1_reference(h.lo, inp.w_down64[e], None, "GEMM1").lo[0]
+    with pytest.raises(AssertionError, match="out"):
+        ex.check_forward(inp, dev, cfg.EC)
+    cfg, inp, dev = _base("router_E8_k2_tc0")   # k = 2: a pair cut at EC still adds its scaled y
+    slot, _, _, kept = ex.slots_from_topk(dev.topk_idx, cfg.E, cfg.EC)
+    t, j = (int(v) for v in np.argwhere(~kept & kept[:, ::-1])[0])   # one pick kept, the other dropped
+    e = int(dev.topk_idx[t, j])
+    h = ex.gemm0_reference(inp.x64[t:t + 1], inp.w_up64[e], None, 0, "GEMM0")
+    y = ex.gemm1_reference(h.lo, inp.w_down64[e], None, "GEMM1").lo
+    y_of = np.stack([dev.ret_y[dev.topk_idx[t, i], slot[t, i] if kept[t, i] else 0] for i in range(cfg.k)])[None]
+    y_of[0, j] = y[0]
+    dev.out[t] = ex.combine_tokens(y_of, np.ones((1, cfg.k), bool), dev.topk_w[t:t + 1], dev.mcw[t:t + 1]).lo[0]
+    with pytest.raises(AssertionError, match=f"out: .* first at token {t},"):
+        ex.check_forward(inp, dev, cfg.EC)
+
+
+def test_fault_one_fragment_of_out_scaled_passes_check_output_but_not_the_exact_check():
+    """Config B's 4096 x 1024 output: one 16-row x 64-column fragment off by 5 % passes the seeded-randn rule
+    (relative Frobenius 7.8e-4 <= 1e-3, 0.024 % of the elements off) -- the gap the exact checks close."""
+    rng = np.random.default_rng(5)
+    n, H = 4096, 1024
+    y_of = ex.f64_to_bf16(rng.integers(-2000, 2001, size=(n, 2, H)) / 256.0)
+    kept = np.ones((n, 2), bool)
+    pw = ex.f64_to_bf16(np.full((n, 2), 0.5))
+    mcw = np.ones(n, np.float32)
+    ref = ex.combine_tokens(y_of, kept, pw, mcw)
+    got = ref.lo.copy()
+    frag = (slice(1024, 1040), slice(256, 320))
+    got[frag] = ex.f64_to_bf16(ex.bits_to_f64(got[frag]) * 1.05)
+    relf = check_output(got, ref.lo)   # accepted by the old rule
+    assert 5e-4 < relf <= 1e-3
+    with pytest.raises(AssertionError, match="out: .* first at token 1024, column 256"):
+        ex._interval_check(got, ref, "out", ("token", "column"), max_width=None)
