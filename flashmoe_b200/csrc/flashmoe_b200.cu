@@ -105,12 +105,10 @@ struct fm_ctx {
     int TN0 = 0, TN1 = 0, num_pkts = 0, num_blocks = 0;
     int g0_blocks = 0, g1_blocks = 0;   // GEMM0 / GEMM1 blocks of the work list (items = their tiles x row blocks per packet)
     int dbg_flags = 0;
-    uint32_t epoch = 0;
-    unsigned long long bar_count = 0;
     // in-kernel waits give up after this long (fm_set_timeout_ms): generous by default so that ordinary rank skew (a peer
     // still loading data, compiling, paused in a debugger) is not turned into a trap -- see fm_ptx.cuh SpinGuard
     unsigned long long timeout_ns = 120ull * 1000ull * 1000ull * 1000ull;
-    uint64_t launches = 0;
+    uint64_t launches = 0;   // launches issued through the API (graph replays are not counted; fm_last_launch counts them)
     // device buffers
     int* topk_idx = nullptr;
     __nv_bfloat16* topk_w = nullptr;
@@ -119,7 +117,8 @@ struct fm_ctx {
     int* counts = nullptr;
     __nv_bfloat16* gate_out = nullptr;
     int* chunk_counts = nullptr;
-    unsigned int* ctrl = nullptr;  // [0] unused, [1] claim, [2..3] grid barrier (u64)
+    // [0] unused, [1] claim, [2..3] grid barrier (u64), [4..5] launch counter (u64), [6] token count of the last launch
+    unsigned int* ctrl = nullptr;
     unsigned int* g0_done = nullptr;
     unsigned int* g1_done = nullptr;
     int* recv_cnt = nullptr;
@@ -234,6 +233,12 @@ void set_peer_pointers(const fm_ctx* c, fm::FmParams& p) {
 }
 
 int check_kernel_status(fm_ctx* c) {
+    if (c->dbg_host != nullptr && c->dbg_host->code == fm::FM_STATUS_BAD_COUNT) {
+        // not a fault: reported once, then the record is cleared and the context stays usable
+        const int n = (int)c->dbg_host->info0, S = (int)c->dbg_host->info1;
+        memset(c->dbg_host, 0, sizeof(fm::DebugRecord));
+        return fail(FM_EINVAL, "device token count n_tokens = %d not in [0, S = %d]: that launch ran on 0 tokens", n, S);
+    }
     if (c->dbg_host != nullptr && c->dbg_host->code != 0) {
         static const char* names[] = {"none", "smem-full mbarrier", "smem-empty mbarrier", "(unused)",
                                       "(unused)", "sched-full mbarrier", "sched-empty mbarrier",
@@ -250,15 +255,20 @@ int check_kernel_status(fm_ctx* c) {
     return FM_OK;
 }
 
-// One forward of n_tok tokens (0 <= n_tok <= S): the call computes exactly what a context created for n_tok tokens
-// would -- capacity EC(n_tok), tokens per CTA ceil(n_tok / grid), maps over x with n_tok rows -- while every buffer keeps
-// its create-time (maximum) size and stride.
-int launch(fm_ctx* c, const void* x, int n_tok, const void* gate_w, const void* expert_w, const void* bias_up,
-           const void* bias_down, void* out, cudaStream_t stream) {
+// One forward of n tokens (0 <= n <= S): the call computes exactly what a context created for n tokens would --
+// capacity EC(n), tokens per CTA ceil(n / grid) -- while every buffer keeps its create-time (maximum) size and stride.
+// n is n_tok, or with n_dev != nullptr the count the kernel reads from *n_dev when it starts (n_tok is then S).  The
+// maps over x have n_tok rows.  The kernel derives everything that depends on n and on the launch's place in the
+// context's sequence of launches itself (fm_kernel.cuh, struct Launch), so the parameters built here are valid for
+// every replay of a captured launch, and this function issues nothing that stream capture forbids.
+int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* gate_w, const void* expert_w,
+           const void* bias_up, const void* bias_down, void* out, cudaStream_t stream) {
     if (c == nullptr) return fail(FM_EINVAL, "null context");
     if (n_tok < 0 || n_tok > c->d.S) return fail(FM_EINVAL, "n_tokens = %d not in [0, S = %d]", n_tok, c->d.S);
     if (gate_w == nullptr || expert_w == nullptr || (n_tok > 0 && (x == nullptr || out == nullptr)))
         return fail(FM_EINVAL, "x, gate_w, expert_w and out must be non-null device pointers");
+    if (reinterpret_cast<uintptr_t>(n_dev) % alignof(int))
+        return fail(FM_EINVAL, "n_tokens_dev must be 4-byte aligned (got %p)", static_cast<const void*>(n_dev));
     {   // TMA tensor maps, cp.async.bulk row copies and the 16-byte vector accesses all need 16-byte aligned bases
         const void* ptrs[] = {x, gate_w, expert_w, bias_up, bias_down, out};
         const char* names[] = {"x", "gate_w", "expert_w", "bias_up", "bias_down", "out"};
@@ -314,22 +324,16 @@ int launch(fm_ctx* c, const void* x, int n_tok, const void* gate_w, const void* 
     p.tm_a0 = c->tm_a0; p.tm_b0 = c->tm_b0; p.tm_a1 = c->tm_a1; p.tm_b1 = c->tm_b1;
     if (c->tc_gate) { p.tm_gx = c->tm_gx; p.tm_gw = c->tm_gw; }
     p.tc_gate = c->tc_gate ? 1 : 0;
-    const int ec = (int)expert_capacity(c->cfg, n_tok);
-    p.S = n_tok; p.H = d.H; p.P = d.P; p.E = d.E; p.k = d.k; p.W = d.world; p.rank = d.rank; p.nLx = nLx;
-    p.EC = ec; p.pEC = d.pEC; p.TCM = d.TCM; p.act = c->cfg.hidden_act;
-    p.TN0 = c->TN0; p.TN1 = c->TN1; p.tpc = ceil_div(n_tok, c->grid); p.num_pkts = c->num_pkts; p.num_blocks = c->num_blocks;
-    // one rank knows every packet's capacity, so the work list shrinks to this call's row blocks; a receiver with peers
-    // does not know their token counts and keeps the maximum (the empty row blocks are skipped by the scheduler)
-    p.tcm_items = d.world == 1 ? ceil_div(ec, fm::BLOCK_M) : d.TCM;
-    p.total_items = (c->g0_blocks * c->TN0 + c->g1_blocks * c->TN1) * p.tcm_items;
+    p.n_tokens = n_tok; p.n_tokens_dev = n_dev;
+    p.H = d.H; p.P = d.P; p.E = d.E; p.k = d.k; p.W = d.world; p.rank = d.rank; p.nLx = nLx;
+    p.pEC = d.pEC; p.TCM = d.TCM; p.act = c->cfg.hidden_act;
+    p.TN0 = c->TN0; p.TN1 = c->TN1; p.num_pkts = c->num_pkts; p.num_blocks = c->num_blocks;
+    p.drop_tokens = c->cfg.drop_tokens; p.ec_mult = c->cfg.capacity_factor * d.k;   // EC(n), as expert_capacity
+    p.items_per_rb = c->g0_blocks * c->TN0 + c->g1_blocks * c->TN1;
     p.dbg_flags = c->dbg_flags;
-    // the epoch and the grid-barrier target advance only when the launch has been accepted (see below): a failed launch
-    // must not leave the host ahead of the device counter and of the peers
-    const uint32_t epoch = c->epoch + 1u;
-    const unsigned long long bar_count = c->bar_count + (unsigned long long)c->grid;
-    p.epoch = epoch;
-    p.bar_target = bar_count;
     p.timeout_ns = c->timeout_ns;
+    p.launch_ctr = reinterpret_cast<unsigned long long*>(c->ctrl + 4);
+    p.launch_tokens = reinterpret_cast<int*>(c->ctrl + 6);
     p.x = static_cast<const __nv_bfloat16*>(x);
     p.wg = static_cast<const __nv_bfloat16*>(gate_w);
     p.b_up = static_cast<const __nv_bfloat16*>(bias_up);
@@ -373,9 +377,18 @@ int launch(fm_ctx* c, const void* x, int n_tok, const void* gate_w, const void* 
     lc.attrs = &attr;
     lc.numAttrs = 1;
     FM_CUDA(cudaLaunchKernelEx(&lc, fm::fm_moe_forward_kernel, p));
-    c->epoch = epoch;
-    c->bar_count = bar_count;
     c->launches += 1;
+    return FM_OK;
+}
+
+// the device's launch record: launches run so far (replays included) and the token count of the last one.  Synchronises.
+int read_launch_record(fm_ctx* c, uint64_t* launches, int32_t* n_tokens) {
+    FM_CUDA(cudaSetDevice(c->device));
+    FM_CUDA(cudaDeviceSynchronize());
+    unsigned int w[3];
+    FM_CUDA(cudaMemcpy(w, c->ctrl + 4, sizeof(w), cudaMemcpyDeviceToHost));
+    if (launches != nullptr) *launches = (uint64_t)w[0] | ((uint64_t)w[1] << 32);
+    if (n_tokens != nullptr) *n_tokens = (int32_t)w[2];
     return FM_OK;
 }
 
@@ -724,7 +737,23 @@ FM_API int fm_symm_attach_ptrs(fm_ctx_t* ctx, void* const* peer_bases) {
 
 FM_API int fm_moe_forward_tokens(fm_ctx_t* ctx, const void* x, int n_tokens, const void* gate_w, const void* expert_w,
                                  const void* bias_up, const void* bias_down, void* out, void* stream) {
-    return launch(ctx, x, n_tokens, gate_w, expert_w, bias_up, bias_down, out, static_cast<cudaStream_t>(stream));
+    return launch(ctx, x, n_tokens, nullptr, gate_w, expert_w, bias_up, bias_down, out, static_cast<cudaStream_t>(stream));
+}
+
+FM_API int fm_moe_forward_tokens_dev(fm_ctx_t* ctx, const void* x, const int32_t* n_tokens_dev, const void* gate_w,
+                                     const void* expert_w, const void* bias_up, const void* bias_down, void* out,
+                                     void* stream) {
+    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
+    if (n_tokens_dev == nullptr) return fail(FM_EINVAL, "n_tokens_dev must be a device pointer to one int32");
+    if (x == nullptr || out == nullptr)
+        return fail(FM_EINVAL, "x and out must be non-null device pointers to S = %d rows", ctx->d.S);
+    return launch(ctx, x, ctx->d.S, n_tokens_dev, gate_w, expert_w, bias_up, bias_down, out,
+                  static_cast<cudaStream_t>(stream));
+}
+
+FM_API int fm_last_launch(fm_ctx_t* ctx, uint64_t* launches, int32_t* n_tokens) {
+    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
+    return read_launch_record(ctx, launches, n_tokens);
 }
 
 FM_API int fm_moe_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, const void* expert_w, const void* bias_up,
@@ -768,7 +797,7 @@ FM_API int fm_host_submit(fm_ctx_t* ctx, const void* x_host, const void* gate_w,
     FM_CUDA(cudaMemcpyAsync(ctx->x_stage[slot], x_host, bytes, cudaMemcpyHostToDevice, ctx->s_h2d));
     FM_CUDA(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
     FM_CUDA(cudaStreamWaitEvent(s, ctx->ev_h2d[slot], 0));
-    if ((rc = launch(ctx, ctx->x_stage[slot], ctx->d.S, gate_w, expert_w, bias_up, bias_down, ctx->out_stage[slot], s))) return rc;
+    if ((rc = launch(ctx, ctx->x_stage[slot], ctx->d.S, nullptr, gate_w, expert_w, bias_up, bias_down, ctx->out_stage[slot], s))) return rc;
     FM_CUDA(cudaEventRecord(ctx->ev_kernel[slot], s));
     FM_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_kernel[slot], 0));
     FM_CUDA(cudaMemcpyAsync(out_host, ctx->out_stage[slot], bytes, cudaMemcpyDeviceToHost, ctx->s_d2h));
@@ -841,7 +870,8 @@ static int buffer_desc(const fm_ctx_t* c, int which, const void** ptr, size_t* b
         case FM_BUF_TRACE: *ptr = c->trace; *bytes = (size_t)c->grid * fm::TRACE_SLOTS * 8; break;
         case FM_BUF_AUX_LOSS:
             if (c->aux == nullptr) return fail(FM_EINVAL, "the auxiliary loss exists only with is_training = 1");
-            *ptr = c->aux + (size_t)(c->epoch & 1u) * (2 * d.E + 1); *bytes = (size_t)(2 * d.E + 1) * 4; break;
+            // the last launch's half of the [2][2E+1] buffer: fm_read_buffer adds its offset from the device's launch count
+            *ptr = c->aux; *bytes = (size_t)(2 * d.E + 1) * 4; break;
         default: return fail(FM_EINVAL, "unknown buffer id %d", which);
     }
     return FM_OK;
@@ -864,6 +894,11 @@ FM_API int fm_read_buffer(fm_ctx_t* ctx, int which, void* host_dst, size_t bytes
     cudaError_t e = cudaDeviceSynchronize();
     if ((rc = check_kernel_status(ctx))) return rc;
     if (e != cudaSuccess) return fail(FM_ECUDA, "cudaDeviceSynchronize failed: %s", cudaGetErrorString(e));
+    if (which == FM_BUF_AUX_LOSS) {   // launch L wrote parity L & 1
+        uint64_t launches = 0;
+        if ((rc = read_launch_record(ctx, &launches, nullptr))) return rc;
+        p = static_cast<const float*>(p) + (size_t)(launches & 1u) * (2 * ctx->d.E + 1);
+    }
     FM_CUDA(cudaMemcpy(host_dst, p, n, cudaMemcpyDeviceToHost));
     return FM_OK;
 }

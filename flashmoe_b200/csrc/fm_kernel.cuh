@@ -83,7 +83,8 @@ constexpr int BAR_STG_FULL = BAR_GEMPTY + GATE_STAGES;                // consume
 constexpr int BAR_STG_FREE = BAR_STG_FULL + EPI_BUFS;                 // publisher -> consumer warps: chunk read by the TMA
 constexpr int NUM_BARS = BAR_STG_FREE + EPI_BUFS;                     // 48
 constexpr int OFF_RING = OFF_BARS + NUM_BARS * 8;                     // 16-byte aligned
-constexpr int SMEM_USED = OFF_RING + NSCHED * 64;
+constexpr int OFF_LAUNCH = OFF_RING + NSCHED * 64;                    // this launch's Launch record (below)
+constexpr int SMEM_USED = OFF_LAUNCH + 64;
 constexpr int SMEM_BYTES = SMEM_USED + 1024;                          // + slack for manual 1 KiB alignment
 static_assert(OFF_RING % 16 == 0, "ring entries are 16-byte aligned");
 static_assert(SMEM_BYTES <= 232448, "227 KiB of dynamic shared memory per CTA");
@@ -112,18 +113,24 @@ struct FmParams {
     CUtensorMap tm_b0;  // expert_weights as [nLx*2*P, H]  box {64, 128}  (W_up rows)
     CUtensorMap tm_a1;  // hidden  as [W*nLx*pEC, P]  box {64, 128}: GEMM1's A loads and GEMM0's h stores
     CUtensorMap tm_b1;  // expert_weights as [nLx*2*H, P]  box {64, 128}  (W_down rows)
-    CUtensorMap tm_gx;  // router on tensor cores: x as [S, H] (S = this call's tokens), box {64, 32}
+    CUtensorMap tm_gx;  // router on tensor cores: x as [n_tokens, H], box {64, 32}
     CUtensorMap tm_gw;  // router on tensor cores: Wg_eff [E, H], box {64, min(128, E rounded up to 64)}
     int tc_gate;        // 1 = logits by wgmma (E <= 256); 0 = register-blocked CUDA-core GEMV
-    // Per call: S = this call's tokens (<= the context's maximum), EC = its capacity, tpc = ceil(S / grid).  pEC and TCM
-    // are the context's maximum and are only strides of the per-packet buffers.
-    int S, H, P, E, k, W, rank, nLx, EC, pEC, TCM, act;
-    int TN0, TN1, tpc, num_pkts, num_blocks, total_items;
-    int tcm_items;      // row blocks per packet in the work list: TCM of this call's EC at W == 1, the maximum TCM at W > 1
+    // The call's token count and everything derived from it are resolved on the device (resolve_launch, struct Launch).
+    // n_tokens: the count itself, or with n_tokens_dev the context's S -- the rows of the maps over x and the bound of
+    // *n_tokens_dev, which the kernel reads when it starts.  pEC and TCM are the context's maximum and are only strides
+    // of the per-packet buffers.
+    int n_tokens;
+    const int* n_tokens_dev;
+    int H, P, E, k, W, rank, nLx, pEC, TCM, act;
+    int TN0, TN1, num_pkts, num_blocks;
+    int drop_tokens, ec_mult;   // capacity EC(n) = (drop_tokens ? ceil(n / E) : n) * ec_mult, ec_mult = capacity_factor * k
+    int items_per_rb;   // work items per row block of every packet: GEMM0 blocks * TN0 + GEMM1 blocks * TN1
     int dbg_flags;      // experiments only (results are garbage): bit0 = skip all TMA loads, bit1 = skip MMA issue,
                         // bit2 = skip the A loads, bit3 = skip the B loads
-    unsigned int epoch;
-    unsigned long long bar_target, timeout_ns;
+    unsigned long long timeout_ns;
+    unsigned long long* launch_ctr;   // [1] launches this context has run (CTA 0 advances it after the grid barrier)
+    int* launch_tokens;               // [1] the token count the last launch ran with
     const __nv_bfloat16 *x, *wg, *b_up, *b_down;
     __nv_bfloat16* out;
     int* topk_idx;             // [S,k]
@@ -169,10 +176,52 @@ struct FmParams {
     unsigned long long* trace;  // optional [grid][TRACE_SLOTS] %globaltimer stamps (nullptr = off)
 };
 
+// Launch state.  Nothing that changes from launch to launch is a kernel parameter, so a launch captured in a CUDA graph
+// computes the right values on every replay: every CTA reads the context's launch counter (and, for a device-side count,
+// the count) when it starts and derives the rest.  Launch L = counter + 1 has epoch (uint32) L -- the tag of every flag
+// it publishes -- and waits at the grid barrier for the monotonic arrival count L * grid.  CTA 0 stores L after the grid
+// barrier, when every CTA of the launch has read the old value; the next launch on the stream sees the new one.
+struct Launch {
+    unsigned long long launch;       // L
+    unsigned long long bar_target;   // L * grid
+    unsigned int epoch;              // (uint32) L
+    int S;                           // this call's tokens (0 when a device-side count is out of range)
+    int EC;                          // its capacity EC(S)
+    int tpc;                         // tokens per CTA, ceil(S / grid)
+    int tcm_items;                   // row blocks per packet in the work list: TCM of EC at W == 1, the maximum TCM at W > 1
+    int total_items;                 // work items of the launch
+};
+static_assert(sizeof(Launch) <= SMEM_USED - OFF_LAUNCH, "the Launch record's shared-memory slot");
+
+// one thread per CTA, before the prologue's block sync
+__device__ __forceinline__ void resolve_launch(const FmParams& p, Launch* L) {
+    const unsigned long long launch = *reinterpret_cast<const volatile unsigned long long*>(p.launch_ctr) + 1ull;
+    int n = p.n_tokens;
+    if (p.n_tokens_dev != nullptr) {
+        const int v = *reinterpret_cast<const volatile int*>(p.n_tokens_dev);
+        n = (v < 0 || v > p.n_tokens) ? 0 : v;
+        // an out-of-range count must not trap (every rank takes part in the collective): the launch runs as n = 0 and
+        // the host reports the count at its next check
+        if (n != v && blockIdx.x == 0) fm_record(p.dbg, FM_STATUS_BAD_COUNT, (unsigned int)v, (unsigned int)p.n_tokens, 0, 0);
+    }
+    const int G = (int)gridDim.x;
+    const int ec = (p.drop_tokens ? (n + p.E - 1) / p.E : n) * p.ec_mult;
+    L->launch = launch;
+    L->bar_target = launch * (unsigned long long)G;
+    L->epoch = (unsigned int)launch;
+    L->S = n;
+    L->EC = ec;
+    L->tpc = (n + G - 1) / G;
+    // one rank knows every packet's capacity, so the work list shrinks to this call's row blocks; a receiver with peers
+    // does not know their token counts and keeps the maximum (the empty row blocks are skipped by the scheduler)
+    L->tcm_items = p.W == 1 ? (ec + BLOCK_M - 1) / BLOCK_M : p.TCM;
+    L->total_items = p.items_per_rb * L->tcm_items;
+}
+
 // first work item of block b: every earlier block holds tcm_items row blocks times its GEMM's column tiles, so the item
 // space follows the call's row-block count without rebuilding the table
-__device__ __forceinline__ int block_start(const FmParams& p, const TileBlock& b) {
-    return (b.g0 * p.TN0 + b.g1 * p.TN1) * p.tcm_items;
+__device__ __forceinline__ int block_start(const FmParams& p, const Launch& L, const TileBlock& b) {
+    return (b.g0 * p.TN0 + b.g1 * p.TN1) * L.tcm_items;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -181,12 +230,12 @@ __device__ __forceinline__ void trace_stamp(const FmParams& p, int slot) {
         p.trace[(size_t)blockIdx.x * TRACE_SLOTS + slot] = globaltimer_ns();
 }
 
-__device__ __forceinline__ void grid_barrier(const FmParams& p) {
+__device__ __forceinline__ void grid_barrier(const FmParams& p, const Launch& L) {
     __syncthreads();
     if (threadIdx.x == 0) {
         atom_acq_rel_gpu_add_u64(p.grid_bar, 1ull);
         SpinGuard g;
-        while (ld_acquire_gpu_u64(p.grid_bar) < p.bar_target)
+        while (ld_acquire_gpu_u64(p.grid_bar) < L.bar_target)
             g.tick(p.dbg, p.timeout_ns, FM_TRAP_GRID_BARRIER, 0, 0, 0);
     }
     __syncthreads();
@@ -324,7 +373,7 @@ __device__ __forceinline__ void gate_logits_tc(const FmParams& p, uint8_t* smem,
 
 // E == 1 (reference: the dense fffn kernel is selected instead of the MoE kernel, moe.cuh:174-177): every token goes to
 // expert 0 with probability 1, slot = token index, nothing is dropped (EC >= S).  No GEMV, no softmax.
-__device__ __forceinline__ void gate_phase_dense(const FmParams& p, int t0, int n_tok) {
+__device__ __forceinline__ void gate_phase_dense(const FmParams& p, const Launch& L, int t0, int n_tok) {
     const int tid = threadIdx.x;
     for (int i = tid; i < n_tok; i += NUM_THREADS) {
         const int t = t0 + i;
@@ -335,16 +384,16 @@ __device__ __forceinline__ void gate_phase_dense(const FmParams& p, int t0, int 
         p.slot[t] = t;
     }
     if (blockIdx.x == 0 && tid == 0) {
-        p.counts[0] = p.S;   // this call's tokens
-        p.recv_cnt[0] = p.S;
-        if (p.aux != nullptr && p.S > 0) {   // mean probability 1, routed fraction 1, loss 1 * 1 / 1 (no tokens: all zero)
-            float* a = p.aux + (size_t)(p.epoch & 1u) * 3;
+        p.counts[0] = L.S;   // this call's tokens
+        p.recv_cnt[0] = L.S;
+        if (p.aux != nullptr && L.S > 0) {   // mean probability 1, routed fraction 1, loss 1 * 1 / 1 (no tokens: all zero)
+            float* a = p.aux + (size_t)(L.epoch & 1u) * 3;
             a[0] = 1.0f; a[1] = 1.0f; a[2] = 1.0f;
         }
     }
 }
 
-__device__ __forceinline__ void gate_phase(const FmParams& p, uint8_t* smem, int t0, int n_tok) {
+__device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int E = p.E, H = p.H, k = p.k;
     __nv_bfloat16* wg_s = reinterpret_cast<__nv_bfloat16*>(smem + G_OFF_WG);
@@ -374,7 +423,7 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, uint8_t* smem, int
         const int n_sub = min(TS, n_tok - s0);
         if (tc) {
             if (s0 > 0) __syncthreads();   // the logits scratch is reused: everybody is done with the previous sub-chunk
-            gate_logits_tc(p, smem, t0, s0, n_sub, min(TS, p.tpc), logit_s, ldl, tcs);
+            gate_logits_tc(p, smem, t0, s0, n_sub, min(TS, L.tpc), logit_s, ldl, tcs);
         } else {
         for (int i = tid; i < n_sub * ldl; i += NUM_THREADS) logit_s[i] = 0.0f;
         for (int eg0 = 0; eg0 < E; eg0 += EG) {
@@ -685,9 +734,9 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, uint8_t* smem, int
         mbar_arrive_expect_tx(xbar, (uint32_t)(rows0 * row_bytes));
         bulk_load_1d(smem, p.x + (size_t)t0 * H, (uint32_t)(rows0 * row_bytes), xbar);
     }
-    if (p.aux != nullptr && p.S > 0) {   // gML[e] += (sum over this chunk) / S   (gate.cuh:628-634: atomicAdd(gML + e, colAgg / S))
-        float* gml = p.aux + (size_t)(p.epoch & 1u) * (2 * E + 1);
-        for (int e = tid; e < E; e += NUM_THREADS) atomicAdd(gml + e, __fdividef(aux_s[e], (float)p.S));
+    if (p.aux != nullptr && L.S > 0) {   // gML[e] += (sum over this chunk) / S   (gate.cuh:628-634: atomicAdd(gML + e, colAgg / S))
+        float* gml = p.aux + (size_t)(L.epoch & 1u) * (2 * E + 1);
+        for (int e = tid; e < E; e += NUM_THREADS) atomicAdd(gml + e, __fdividef(aux_s[e], (float)L.S));
     }
     // position of every (token, pick) among this chunk's selections of the same expert, ascending (token, pick) order.
     // One warp walks the entries 32 at a time: lanes holding the same expert find each other with match.any, the rank
@@ -729,8 +778,9 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, uint8_t* smem, int
 constexpr int DISP_THREADS = 288;   // warps 2, 4..11; warps 0, 1, 3 are already in their FFN roles (producer / MMA / scheduler)
 __device__ __forceinline__ void disp_sync() { asm volatile("bar.sync 2, 288;" ::: "memory"); }
 
-__device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem, int t0, int n_tok) {
+__device__ __forceinline__ void dispatch_phase(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int EC = L.EC;
     const int tid = (warp == 2 ? 0 : (warp - 3) * 32) + lane;   // 0..287 within the dispatch subset
     const int E = p.E, H = p.H, k = p.k, G = gridDim.x;
     const int16_t* sel_e = reinterpret_cast<const int16_t*>(smem + G_OFF_SEL);
@@ -805,23 +855,23 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
     for (int e = (int)blockIdx.x + tid * G; e < E; e += DISP_THREADS * G) {
         const int tot = total_s[e];
         p.counts[e] = tot;
-        const int rows = tot < p.EC ? tot : p.EC;
+        const int rows = tot < EC ? tot : EC;
         const int owner = e / p.nLx, le = e - owner * p.nLx;
         st_relaxed_sys_u64(p.peer_recv_flag[owner] + (size_t)p.rank * p.nLx + le,
-                           ((unsigned long long)p.epoch << 32) | (unsigned int)rows);
+                           ((unsigned long long)L.epoch << 32) | (unsigned int)rows);
         if (owner == p.rank) p.recv_cnt[p.rank * p.nLx + le] = rows;   // (also when the work list is empty: S = 0)
-        if (p.aux != nullptr && p.S > 0) {   // (S = 0: the buffer stays as cleared, all zero)
+        if (p.aux != nullptr && L.S > 0) {   // (S = 0: the buffer stays as cleared, all zero)
             // gMeC[e] = selections of e / S (gate.cuh:698-706 adds each tile's count / S; the chunk totals are summed
             // first here), loss += gML[e] * gMeC[e] / E (gate.cuh:763-773).  Every CTA's gML atomics precede its arrival
             // at the grid barrier, so gML is complete here.
-            float* a = p.aux + (size_t)(p.epoch & 1u) * (2 * E + 1);
-            const float ce = __fdividef((float)tot, (float)p.S);
+            float* a = p.aux + (size_t)(L.epoch & 1u) * (2 * E + 1);
+            const float ce = __fdividef((float)tot, (float)L.S);
             a[E + e] = ce;
             const float me = *reinterpret_cast<volatile float*>(a + e);
             atomicAdd(a + 2 * E, __fdividef(me * ce, (float)E));
         }
     }
-    const unsigned int par = p.epoch & 1u;
+    const unsigned int par = L.epoch & 1u;
     // Row copies.
     //   * Rows for experts on THIS rank (warps 4-11): the chunk's token rows are contiguous in x, so one bulk load stages up
     //     to 128 KiB of them in shared memory (the first group was requested at the end of the router) and every kept
@@ -869,7 +919,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
                 const int e = sel_e[ti * k + j];
                 const int s = base_s[e] + rank_s[ti * k + j];
                 p.slot[(size_t)t * k + j] = s;
-                if (s < p.EC) {
+                if (s < EC) {
                     const int owner = e / p.nLx, le = e - owner * p.nLx;
                     const size_t row = (size_t)(p.rank * p.nLx + le) * p.pEC + s;
                     if (p.fused) {   // what the expert's GEMM1 epilogue needs to combine this row
@@ -901,7 +951,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
         if (ltid == 0) trace_stamp(p, 9);
         if (any_remote) asm volatile("bar.sync 5, 288;" ::: "memory");   // warp 2 has taken what it needs from the stage area
         if (ltid < 32) {   // warp 4: acknowledge the local experts, then hand the stage area to the TMA producer
-            for (int e = first_local + ltid; e < first_local + p.nLx; e += 32) ack(e, base_s[e], min(base_s[e] + own_s[e], p.EC), true);
+            for (int e = first_local + ltid; e < first_local + p.nLx; e += 32) ack(e, base_s[e], min(base_s[e] + own_s[e], EC), true);
             __syncwarp();
             // (more than 256 experts on several ranks: warp 2 still needs base / own for its acknowledgements and releases)
             if (ltid == 0 && (!any_remote || E <= 256)) mbar_arrive(reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_DISP_DONE);
@@ -920,7 +970,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
         const int e = lane + 32 * i;
         const bool remote = in_regs && e < E && (e < first_local || e >= first_local + p.nLx);
         rlo[i] = remote ? base_s[e] : 0;
-        rhi[i] = remote ? min(base_s[e] + own_s[e], p.EC) : 0;
+        rhi[i] = remote ? min(base_s[e] + own_s[e], EC) : 0;
     }
     __syncwarp();
     if (in_regs) asm volatile("bar.arrive 5, 288;" ::: "memory");   // done with the stage area
@@ -944,7 +994,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
             for (int i = lane; i < rows * k; i += 32) {
                 const size_t gi = (size_t)(t0 + tw) * k + i;
                 const int owner = p.topk_idx[gi] / p.nLx;
-                mine |= owner != p.rank && p.slot[gi] < p.EC;
+                mine |= owner != p.rank && p.slot[gi] < EC;
             }
             const unsigned int anyone = __ballot_sync(0xffffffffu, mine);
             if (anyone == 0u) continue;
@@ -961,7 +1011,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
                     const int e = p.topk_idx[gi];
                     const int owner = e / p.nLx;
                     const int sl = p.slot[gi];
-                    if (owner != p.rank && sl < p.EC)
+                    if (owner != p.rank && sl < EC)
                         bulk_store_1d(p.peer_recv_x[owner] + ((size_t)(p.rank * p.nLx + (e - owner * p.nLx)) * p.pEC + sl) * H,
                                       win + (size_t)(i / k) * row_bytes, (uint32_t)row_bytes);
                 }
@@ -984,7 +1034,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
                         const int e = p.topk_idx[gi];
                         const int owner = e / p.nLx;
                         const int sl = p.slot[gi];
-                        if (owner != p.rank && sl < p.EC)
+                        if (owner != p.rank && sl < EC)
                             bulk_store_1d(reinterpret_cast<uint8_t*>(p.peer_recv_x[owner] +
                                               ((size_t)(p.rank * p.nLx + (e - owner * p.nLx)) * p.pEC + sl) * H) + off,
                                           win, (uint32_t)nb);
@@ -1008,7 +1058,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, uint8_t* smem,
         for (int i = 0; i < RMAX; ++i) ack(lane + 32 * i, rlo[i], rhi[i], false);
     } else {
         for (int e = lane; e < E; e += 32)
-            if (e < first_local || e >= first_local + p.nLx) ack(e, base_s[e], min(base_s[e] + own_s[e], p.EC), false);
+            if (e < first_local || e >= first_local + p.nLx) ack(e, base_s[e], min(base_s[e] + own_s[e], EC), false);
         __syncwarp();
         asm volatile("bar.arrive 5, 288;" ::: "memory");
         if (lane == 0) mbar_arrive(reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_DISP_DONE);
@@ -1040,7 +1090,7 @@ static_assert(sizeof(TileInfo) <= 64, "a ring slot is 64 bytes");
 // warp 3, lane 0: claims work items and resolves their dependencies AHEAD of the TMA producer, so the atomic, the
 // packet-flag and the h-row-block-counter round trips overlap the previous tile's loads (the job of the reference's OS
 // CTA: subscriber decode + scheduler doorbells, os/subscriber.cuh, os/scheduler.cuh -- here one thread, no queues).
-__device__ __forceinline__ void ffn_scheduler(const FmParams& p, uint8_t* smem, uint64_t* bars) {
+__device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L, uint8_t* smem, uint64_t* bars) {
     uint64_t* sched_full = bars + BAR_SCHED_FULL;
     uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
     uint64_t* prod_take = bars + BAR_PROD_TAKE;
@@ -1057,28 +1107,31 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, uint8_t* smem, 
         ti.src = 0; ti.cnt = 0; ti.pad[0] = ti.pad[1] = ti.pad[2] = 0;
         for (;;) {
             const int id = (int)atomicAdd(p.claim, 1u);
-            if (id >= p.total_items) break;
+            if (id >= L.total_items) break;
             if (n < 16) trace_stamp(p, 112 + n);   // claim time of tile n (ready time is slot 16+n)
-            while (id >= block_start(p, p.blocks[cursor + 1])) ++cursor;
+            while (id >= block_start(p, L, p.blocks[cursor + 1])) ++cursor;
             const TileBlock blk = p.blocks[cursor];
-            const int local = id - block_start(p, blk);
-            const int mb = local % p.tcm_items, nt = local / p.tcm_items;   // row blocks fastest
+            const int local = id - block_start(p, L, blk);
+            const int mb = local % L.tcm_items, nt = local / L.tcm_items;   // row blocks fastest
             const int pkt = blk.pkt, le = pkt % p.nLx, src = pkt / p.nLx;
             const bool same_gpu = src == p.rank;   // flag and counters written from this GPU: gpu scope suffices
+            const unsigned int epoch = L.epoch;
             // wait for the packet (src, le): flag = {epoch, rows}  (reference subscriber.cuh:52-185)
-            unsigned long long f = ((unsigned long long)p.epoch << 32) | (unsigned int)p.S;   // dense: all of the call's rows, in x
+            // dense: all of the call's rows, in x (the map over x may have more rows -- a device-side count reads S rows --
+            // and the rows past the call's count only reach h's padding rows, which GEMM1's epilogue drops: rows below)
+            unsigned long long f = ((unsigned long long)epoch << 32) | (unsigned int)L.S;
             bool stale = false;
             if (!p.dense) {
                 SpinGuard g;
                 for (;;) {
                     f = same_gpu ? ld_acquire_gpu_u64(p.recv_flag + pkt) : ld_acquire_sys_u64(p.recv_flag + pkt);
-                    const int ahead = (int)((unsigned int)(f >> 32) - p.epoch);
+                    const int ahead = (int)((unsigned int)(f >> 32) - epoch);
                     if (ahead == 0) break;
                     // The source rank is already in a LATER forward: it only gets there after every real tile of
                     // this packet has been returned to it, so whatever item of the static superset is left here
                     // is an empty row block.
                     if (ahead > 0) { stale = true; break; }
-                    g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_FLAG, pkt, (unsigned int)(f >> 32), p.epoch);
+                    g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_FLAG, pkt, (unsigned int)(f >> 32), epoch);
                 }
             }
             if (stale) continue;
@@ -1086,7 +1139,7 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, uint8_t* smem, 
             // once per packet and GEMM (its first item): bookkeeping that needs the count
             if (local == 0 && blk.kind == 0 && !p.dense) p.recv_cnt[pkt] = cnt;
             if (p.fused && local == 0 && blk.kind == 1 && cnt == 0)   // nothing to contribute: tell the source now
-                st_release_sys_u64(p.peer_done_flag[src] + (size_t)(p.rank * p.nLx + le), (unsigned long long)p.epoch << 32);
+                st_release_sys_u64(p.peer_done_flag[src] + (size_t)(p.rank * p.nLx + le), (unsigned long long)epoch << 32);
             const int rows = max(0, min(BLOCK_M, cnt - mb * BLOCK_M));
             if (rows == 0) continue;   // an empty row block of the static superset
             SpinGuard g;
@@ -1094,7 +1147,7 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, uint8_t* smem, 
                 const unsigned int* ctr = p.g0_done + (size_t)pkt * p.TCM + mb;
                 while (ld_acquire_gpu_u32(ctr) < (unsigned int)p.TN0) g.tick(p.dbg, p.timeout_ns, FM_TRAP_G0_DONE, pkt, mb, 0);
             } else if (!p.dense) {  // GEMM0 needs the rows of this block to have landed (dispatch acks)
-                const unsigned int* rctr = p.recv_rows + ((size_t)(p.epoch & 1u) * p.num_pkts + pkt) * p.TCM + mb;
+                const unsigned int* rctr = p.recv_rows + ((size_t)(epoch & 1u) * p.num_pkts + pkt) * p.TCM + mb;
                 for (;;) {
                     const unsigned int got = same_gpu ? ld_acquire_gpu_u32(rctr) : ld_acquire_sys_u32(rctr);
                     if (got >= (unsigned int)rows) break;
@@ -1453,7 +1506,7 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, u
 // GEMM1 -> once all consumer warps have issued their stores / REDs: system-scope fence, then the packet / row-block
 // counter and, from the last tile, the flag on the source rank (reference processor.cuh:722-750).  The fences and the
 // store completion take 1-2 us (more over NVLink); here they overlap the next tile's MMA instead of delaying it.
-__device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, uint64_t* bars) {
+__device__ __forceinline__ void ffn_publisher(const FmParams& p, const Launch& L, uint8_t* smem, uint64_t* bars) {
     uint64_t* sched_full = bars + BAR_SCHED_FULL;
     uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
     uint64_t* pub_full = bars + BAR_PUB_FULL;
@@ -1506,7 +1559,7 @@ __device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, 
                     const unsigned int want = (unsigned int)(((ti.cnt + BLOCK_M - 1) / BLOCK_M) * p.TN1);
                     if (old + 1u == want) {   // every GEMM1 tile of packet (src, le) has been added into src's output
                         st_release_sys_u64(p.peer_done_flag[my_src] + (size_t)(p.rank * p.nLx + ti.le),
-                                           (unsigned long long)p.epoch << 32);
+                                           (unsigned long long)L.epoch << 32);
                     }
                     }
                 } else {
@@ -1516,7 +1569,7 @@ __device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, 
                         fence_acq_rel_sys();
                         const int e_global = p.rank * p.nLx + ti.le;
                         st_release_sys_u64(p.peer_ret_flag[my_src] + (size_t)e_global * p.TCM + my_mblk,
-                                           ((unsigned long long)p.epoch << 32) | (unsigned int)my_rows);
+                                           ((unsigned long long)L.epoch << 32) | (unsigned int)my_rows);
                     }
                 }
             }
@@ -1530,7 +1583,8 @@ __device__ __forceinline__ void ffn_publisher(const FmParams& p, uint8_t* smem, 
     }
 }
 
-// kernel prologue: barriers of every later phase; runs before the router so it costs nothing on the critical path
+// kernel prologue: barriers of every later phase; runs before the router so it costs nothing on the critical path.
+// Warp 3's L2 warm-up needs this launch's work list, so it runs after the block sync that publishes the Launch record.
 __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BARS);
     const int tid = threadIdx.x, warp = tid >> 5;
@@ -1560,21 +1614,24 @@ __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
         fence_mbar_init();
     }
     if (warp == 0 && (tid & 31) == 0) {
-        if (!p.dense || p.S > 0) tma_prefetch_desc(&p.tm_a0);   // (dense, no tokens: no map over x was encoded)
+        if (!p.dense || p.n_tokens > 0) tma_prefetch_desc(&p.tm_a0);   // (dense, no tokens: no map over x was encoded)
         tma_prefetch_desc(&p.tm_b0);
         tma_prefetch_desc(&p.tm_a1); tma_prefetch_desc(&p.tm_b1);
     }
-    if (warp == 3 && (tid & 31) == 0) {
+}
+
+__device__ __forceinline__ void ffn_warm_l2(const FmParams& p, const Launch& L) {
+    if (threadIdx.x == 3 * 32) {
         // Warm L2 with the 256-row weight tile this CTA will most likely claim first (item id = CTA index: the first wave is
         // claimed in arrival order), pipeline depth only: HBM is idle during the router and the first tile's loads are
         // then L2 hits.  A wrong guess costs nothing -- the tile is needed by some CTA of the first wave anyway.
         const int id = (int)blockIdx.x;
-        if (id < p.total_items) {
+        if (id < L.total_items) {
             int cur = 0;
-            while (id >= block_start(p, p.blocks[cur + 1])) ++cur;
+            while (id >= block_start(p, L, p.blocks[cur + 1])) ++cur;
             const TileBlock blk = p.blocks[cur];
-            const int local = id - block_start(p, blk);
-            const int nt = local / p.tcm_items, le = blk.pkt % p.nLx;
+            const int local = id - block_start(p, L, blk);
+            const int nt = local / L.tcm_items, le = blk.pkt % p.nLx;
             const CUtensorMap* tb = blk.kind == 0 ? &p.tm_b0 : &p.tm_b1;
             const int b0 = (blk.kind == 0 ? le * 2 * p.P : (le * 2 + 1) * p.H) + nt * BLOCK_N;
             const int nk_w = (blk.kind == 0 ? p.H : p.P) / BLOCK_K;
@@ -1600,14 +1657,14 @@ static_assert(128 * REGS_PROD + 256 * REGS_CONS <= 65536, "register file of one 
 // router and dispatch, which they run with the even split) take them.  Phase C runs on all 384 threads with the even
 // split again: the consumers hand their registers back before the block sync, warps 0-3 take theirs back after it (an
 // increase waits for free registers, so it must not come before every consumer's decrease).
-__device__ __forceinline__ void ffn_roles(const FmParams& p, uint8_t* smem) {
+__device__ __forceinline__ void ffn_roles(const FmParams& p, const Launch& L, uint8_t* smem) {
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BARS);
     const int tid = threadIdx.x, warp = tid >> 5;
     if (warp < EPI_WARP0) {
         setmaxnreg_dec<REGS_PROD>();
         if (warp == 0) ffn_producer(p, smem, bars);
-        else if (warp == 2) ffn_publisher(p, smem, bars);
-        else if (warp == 3) { if ((tid & 31) == 0) ffn_scheduler(p, smem, bars); __syncwarp(); }
+        else if (warp == 2) ffn_publisher(p, L, smem, bars);
+        else if (warp == 3) { if ((tid & 31) == 0) ffn_scheduler(p, L, smem, bars); __syncwarp(); }
     } else {
         setmaxnreg_inc<REGS_CONS>();
         ffn_consumer(p, smem, bars);
@@ -1627,7 +1684,7 @@ __device__ __forceinline__ void ffn_roles(const FmParams& p, uint8_t* smem) {
 // exactly because bf16 addition commutes and 0 + a is exact.
 // ============================================================================================================
 template <int KMAX, int PIECES>
-__device__ __forceinline__ void combine_rows(const FmParams& p, int t0, int n_tok, const int* c_e, const int* c_s,
+__device__ __forceinline__ void combine_rows(const FmParams& p, int EC, int t0, int n_tok, const int* c_e, const int* c_s,
                                              const float* c_w, const float* c_m) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int H = p.H, k = p.k;
@@ -1644,7 +1701,7 @@ __device__ __forceinline__ void combine_rows(const FmParams& p, int t0, int n_to
             if (j < k) {
                 const int s = c_s[ti * k + j];
                 pw[j] = c_w[ti * k + j];
-                keep[j] = s < p.EC;
+                keep[j] = s < EC;
                 yrow[j] = p.ret_y + ((size_t)c_e[ti * k + j] * p.pEC + (keep[j] ? s : 0)) * H;
             }
         }
@@ -1689,7 +1746,7 @@ __device__ __forceinline__ void combine_rows(const FmParams& p, int t0, int n_to
 
 // fused path: the output rows were accumulated by the GEMM1 epilogues; wait until every expert (local or remote) has
 // reported all of its contributions, then (W > 1) move my rows from the symmetric accumulator to the caller's tensor
-__device__ __forceinline__ void finish_fused(const FmParams& p, int t0, int n_tok) {
+__device__ __forceinline__ void finish_fused(const FmParams& p, const Launch& L, int t0, int n_tok) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     // Contributions of experts on THIS GPU need no flag when the rows are left where they were accumulated (out == the
     // accumulation target): they are complete when the kernel is, and nobody reads them before.  Only the experts on other
@@ -1699,7 +1756,7 @@ __device__ __forceinline__ void finish_fused(const FmParams& p, int t0, int n_to
     for (int e = tid; e < p.E; e += NUM_THREADS) {
         if (!need_local && e / p.nLx == p.rank) continue;
         SpinGuard g;
-        while ((ld_acquire_sys_u64(p.done_flag + e) >> 32) != p.epoch)
+        while ((ld_acquire_sys_u64(p.done_flag + e) >> 32) != L.epoch)
             g.tick(p.dbg, p.timeout_ns, FM_TRAP_RET_FLAG, e, 0xD0E, 0);
     }
     __syncthreads();
@@ -1725,9 +1782,9 @@ __device__ __forceinline__ void finish_fused(const FmParams& p, int t0, int n_to
     }
 }
 
-__device__ __forceinline__ void combine_phase(const FmParams& p, uint8_t* smem, int t0, int n_tok) {
+__device__ __forceinline__ void combine_phase(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int H = p.H, k = p.k;
+    const int H = p.H, k = p.k, EC = L.EC;
     // the pipeline stage area is free again: stage this chunk's routing records, and let one thread per (token, pick)
     // poll its return flag so the waits overlap instead of chaining per token
     int* c_e = reinterpret_cast<int*>(smem);
@@ -1742,10 +1799,10 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, uint8_t* smem, 
         c_e[i] = e;
         c_s[i] = s;
         c_w[i] = __bfloat162float(p.topk_w[gi]);
-        if (s < p.EC) {
+        if (s < EC) {
             const unsigned long long* fl = p.ret_flag + (size_t)e * p.TCM + (s / BLOCK_M);
             SpinGuard g;
-            while ((ld_acquire_sys_u64(fl) >> 32) != p.epoch)
+            while ((ld_acquire_sys_u64(fl) >> 32) != L.epoch)
                 g.tick(p.dbg, p.timeout_ns, FM_TRAP_RET_FLAG, e, s, t0 + i / k);
         }
     }
@@ -1753,7 +1810,7 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, uint8_t* smem, 
     __syncthreads();
     if (k == 1) {
         for (int ti = warp; ti < n_tok; ti += NUM_WARPS) {
-            const bool keep = c_s[ti] < p.EC;
+            const bool keep = c_s[ti] < EC;
             const __nv_bfloat16* yrow = p.ret_y + ((size_t)c_e[ti] * p.pEC + (keep ? c_s[ti] : 0)) * H;
             __nv_bfloat16* orow = p.out + (size_t)(t0 + ti) * H;
             for (int h = lane * 8; h < H; h += 256) {
@@ -1763,9 +1820,9 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, uint8_t* smem, 
             }
         }
     } else if (k == 2) {
-        combine_rows<2, 4>(p, t0, n_tok, c_e, c_s, c_w, c_m);
+        combine_rows<2, 4>(p, EC, t0, n_tok, c_e, c_s, c_w, c_m);
     } else {
-        combine_rows<8, 1>(p, t0, n_tok, c_e, c_s, c_w, c_m);
+        combine_rows<8, 1>(p, EC, t0, n_tok, c_e, c_s, c_w, c_m);
     }
 }
 
@@ -1774,11 +1831,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int tid = threadIdx.x, warp = tid >> 5;
-    const int t0 = blockIdx.x * p.tpc;
-    const int n_tok = max(0, min(p.tpc, p.S - t0));
+    Launch* launch_s = reinterpret_cast<Launch*>(smem + OFF_LAUNCH);
 
     if (tid == 0) trace_stamp(p, 0);
+    if (tid == 2 * 32) resolve_launch(p, launch_s);   // (warp 2 has no part in the prologue)
     ffn_setup(p, smem);   // mbarriers for the later phases (visible to everyone after the next block sync)
+    __syncthreads();
+    const Launch& L = *launch_s;
+    const int t0 = blockIdx.x * L.tpc;
+    const int n_tok = max(0, min(L.tpc, L.S - t0));
+    ffn_warm_l2(p, L);
     // per-launch reset of the work counters (reference clearState, moe.cuh:21-70); consumed only after the grid barrier
     if (blockIdx.x == 0) {
         for (int i = tid; i < p.num_pkts * p.TCM; i += NUM_THREADS) {
@@ -1788,35 +1850,41 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
         for (int i = tid; i < p.num_pkts; i += NUM_THREADS) p.pkt_done[i] = 0u;
         // the arrival counters of the NEXT epoch's parity: nobody reads them any more (launch epoch-1 is over) and no
         // peer can write them yet (a rank starts forward epoch+1 only after this launch has returned all its rows)
-        unsigned int* next_rows = p.recv_rows + (size_t)((p.epoch + 1u) & 1u) * p.num_pkts * p.TCM;
+        unsigned int* next_rows = p.recv_rows + (size_t)((L.epoch + 1u) & 1u) * p.num_pkts * p.TCM;
         for (int i = tid; i < p.num_pkts * p.TCM; i += NUM_THREADS) next_rows[i] = 0u;
         if (p.aux != nullptr) {   // the loss buffers of the next launch (reference clearState, moe.cuh:49-54)
-            float* next_aux = p.aux + (size_t)((p.epoch + 1u) & 1u) * (2 * p.E + 1);
+            float* next_aux = p.aux + (size_t)((L.epoch + 1u) & 1u) * (2 * p.E + 1);
             for (int i = tid; i < 2 * p.E + 1; i += NUM_THREADS) next_aux[i] = 0.0f;
         }
         if (tid == 0) *p.claim = 0u;
     }
-    if (p.dense) gate_phase_dense(p, t0, n_tok); else gate_phase(p, smem, t0, n_tok);
+    if (p.dense) gate_phase_dense(p, L, t0, n_tok); else gate_phase(p, L, smem, t0, n_tok);
     if (tid == 0) trace_stamp(p, 1);
-    grid_barrier(p);
+    grid_barrier(p, L);
     if (tid == 0) trace_stamp(p, 2);
+    // every CTA has read the launch counter (resolve_launch, before its arrival at the barrier): advance it for the next
+    // launch on the stream, and record this launch's token count beside it (fm_last_launch)
+    if (blockIdx.x == 0 && tid == 0) {
+        *p.launch_ctr = L.launch;
+        *p.launch_tokens = L.S;
+    }
 
     // From here the warps specialise.  Warps 0 and 3 (TMA producer, tile scheduler) enter their FFN roles at once -- the
     // scheduler claims its first tile and spins on the packet flag while warps 2, 4-11 dispatch this CTA's rows; warps
     // 4-11 then become the consumer warpgroups.
     const bool disp_warp = (warp == 2) || (warp >= EPI_WARP0);
     if (disp_warp) {
-        if (!p.dense) dispatch_phase(p, smem, t0, n_tok);
+        if (!p.dense) dispatch_phase(p, L, smem, t0, n_tok);
         else if (warp == 2 && (tid & 31) == 0)   // nothing to copy: GEMM0's TMA reads x in place; release the producer
             mbar_arrive(reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_DISP_DONE);
         if (warp == 2 && (tid & 31) == 0) trace_stamp(p, 3);
     }
     if (tid == EPI_WARP0 * 32) trace_stamp(p, 4);
-    ffn_roles(p, smem);
+    ffn_roles(p, L, smem);
 
     __syncthreads();
-    if (p.fused) finish_fused(p, t0, n_tok);
-    else combine_phase(p, smem, t0, n_tok);
+    if (p.fused) finish_fused(p, L, t0, n_tok);
+    else combine_phase(p, L, smem, t0, n_tok);
     __syncthreads();
     if (tid == 0) trace_stamp(p, 6);
 }

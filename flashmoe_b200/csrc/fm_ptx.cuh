@@ -35,17 +35,15 @@ enum : unsigned int {
     FM_TRAP_RET_FLAG = 10,
     FM_TRAP_RECV_ROWS = 11,
     FM_TRAP_MBAR_PUB = 12,
+    // not a trap: the launch read a token count outside [0, S] from device memory and ran on 0 tokens (info0 = the
+    // count, info1 = S).  The host reports it once and clears the record; the context stays usable.
+    FM_STATUS_BAD_COUNT = 13,
 };
 
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-
-__device__ __noinline__ void fm_trap(DebugRecord* dbg, unsigned int code, unsigned int i0, unsigned int i1,
-                                     unsigned int i2, unsigned long long waited) {
-    if (dbg != nullptr) {  // plain stores to pinned host memory (no PCIe atomics needed); first writer wins loosely
+// plain stores to pinned host memory (no PCIe atomics needed); first writer wins loosely
+__device__ __forceinline__ void fm_record(DebugRecord* dbg, unsigned int code, unsigned int i0, unsigned int i1,
+                                          unsigned int i2, unsigned long long waited) {
+    if (dbg != nullptr) {
         volatile DebugRecord* d = dbg;
         if (d->code == 0u) {
             d->block = blockIdx.x;
@@ -58,6 +56,17 @@ __device__ __noinline__ void fm_trap(DebugRecord* dbg, unsigned int code, unsign
             __threadfence_system();
         }
     }
+}
+
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+__device__ __noinline__ void fm_trap(DebugRecord* dbg, unsigned int code, unsigned int i0, unsigned int i1,
+                                     unsigned int i2, unsigned long long waited) {
+    fm_record(dbg, code, i0, i1, i2, waited);
     __trap();
 }
 

@@ -48,18 +48,25 @@ class FlashMoELayer(torch.nn.Module):
             self.bias_down = None
 
     @torch.no_grad()
-    def forward(self, x: torch.Tensor, return_routing: bool = False):
+    def forward(self, x: torch.Tensor, return_routing: bool = False, n_tokens: Optional[torch.Tensor] = None):
         """x [B, T, H] bf16 on this layer's device with B*T <= S (the capacity is that of B*T tokens,
         `cfg.EC_of(B*T)`).  Asynchronous on torch's current stream unless `return_routing` (reading the routing tables
-        synchronises)."""
+        synchronises).  `n_tokens`: a one-element int32 tensor on the device with the token count n; x then holds
+        B*T = S rows of which the first n are the tokens (see `MoEContext.forward_tokens`), and the call can be captured
+        once in a CUDA graph and replayed for any n.  The routing tables then hold the n rows of the last launch."""
         if x.dim() != 3:
             raise RuntimeError("Input must be 3D [batch, seq, H]")
         out = self.ctx.forward_tokens(x, self.gate_weight, self.expert_weight, bias_up=self.bias_up,
-                                      bias_down=self.bias_down)
+                                      bias_down=self.bias_down, n_tokens=n_tokens)
         if not return_routing:
             return out
+        return self.routing(out)
+
+    def routing(self, out: torch.Tensor) -> MoEOutput:
+        """The routing decisions of this layer's last launch -- an eager call or a replay of a captured graph -- next to
+        its output `out`.  Synchronises."""
         self.ctx.synchronize()
-        n = self.ctx.last_tokens
+        n = self.ctx.launch_record()[1]   # (the device's record: right after a replay as after an eager call)
         idx = torch.from_numpy(self.ctx.read("topk_idx")[:n].copy())
         w = torch.from_numpy(self.ctx.read("topk_w")[:n].view("int16").copy()).view(torch.bfloat16)
         slot = torch.from_numpy(self.ctx.read("slot")[:n].copy())

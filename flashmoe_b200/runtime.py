@@ -102,7 +102,9 @@ class MoEContext:
         self.cfg = cfg if cfg is not None else _lib.compiled_config()
         if timeout_ms is not None:
             _lib.check(self._L.fm_set_timeout_ms(self._ctx, int(timeout_ms)))
-        self.last_tokens = 0   # tokens of the last forward (valid rows of the routing tables `read` returns)
+        # tokens of the last forward (valid rows of the routing tables `read` returns); None after a call with a
+        # device-side count (launch_record() has it)
+        self.last_tokens: Optional[int] = 0
         self.symmetric = (symmetric or os.environ.get("FM_SYMM") or "ipc").lower()
         self._symm_tensor = None   # keeps an externally allocated slab alive
         if world > 1:
@@ -229,22 +231,52 @@ class MoEContext:
 
     def forward_tokens(self, x: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor,
                        bias_up: Optional[torch.Tensor] = None, bias_down: Optional[torch.Tensor] = None,
-                       out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                       out: Optional[torch.Tensor] = None, n_tokens: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Enqueue one fused forward over the n = x.numel() // H tokens of `x` (contiguous bf16 [..., H], 0 <= n <= S)
         on torch's current stream; returns `out` (default: a tensor like `x`), async.  The result is exactly what a
         context created for S = n computes: routing, capacity `cfg.EC_of(n)`, drops, outputs and, in training mode, the
         auxiliary loss over the n tokens.  Nothing past row n of `out` is written.  With world > 1 every rank passes its
         own n (n = 0 included) and all ranks call the same number of times.  The routing tables `read` returns then
-        hold `last_tokens` valid rows."""
+        hold `last_tokens` valid rows.
+
+        `n_tokens`: a one-element int32 CUDA tensor on this context's device holding n, read by the kernel when it starts
+        (fm_moe_forward_tokens_dev): no host synchronisation, and one captured CUDA graph serves every n.  `x` must then
+        hold exactly S tokens; its rows n and above may hold anything and affect no result, and rows n and above of
+        `out` are not written.  `last_tokens` is then None -- `launch_record()` returns the count the launch ran with.
+        A count outside [0, S] runs the launch on 0 tokens and makes the next `check` / `synchronize` raise."""
         n = self._validate(x, gate_weights, expert_weights, exact_s=False)
         bu, bd = self._bias_ptrs(bias_up, bias_down)
         out = self._output(x, out)
         stream = torch.cuda.current_stream(self.device).cuda_stream
+        if n_tokens is not None:
+            self._check_count_tensor(n_tokens)
+            if n != self.dims["S"]:
+                raise RuntimeError(f"with a device-side n_tokens, x must hold exactly S={self.dims['S']} tokens (got {n})")
+            _lib.check(self._L.fm_moe_forward_tokens_dev(self._ctx, x.data_ptr(), n_tokens.data_ptr(),
+                                                         gate_weights.data_ptr(), expert_weights.data_ptr(), bu, bd,
+                                                         out.data_ptr(), stream))
+            self.last_tokens = None
+            return out
         _lib.check(self._L.fm_moe_forward_tokens(self._ctx, x.data_ptr() if n else None, n, gate_weights.data_ptr(),
                                                  expert_weights.data_ptr(), bu, bd, out.data_ptr() if n else None,
                                                  stream))
         self.last_tokens = n
         return out
+
+    def _check_count_tensor(self, t: torch.Tensor) -> None:
+        """Metadata only (no .item(): a check must not synchronise, and may run under stream capture)."""
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != self.device:
+            raise RuntimeError(f"n_tokens must be a CUDA tensor on {self.device}")
+        if t.dtype != torch.int32 or t.numel() != 1:
+            raise RuntimeError(f"n_tokens must be a one-element torch.int32 tensor, got {t.dtype} with {t.numel()} elements")
+
+    def launch_record(self) -> Tuple[int, int]:
+        """(launches, n_tokens): how many launches this context has run on the device -- graph replays included, unlike
+        `launch_count` -- and the token count the last one ran with (0 after an out-of-range device count).
+        Synchronises the device."""
+        launches, n = ctypes.c_uint64(), ctypes.c_int32()
+        _lib.check(self._L.fm_last_launch(self._ctx, ctypes.byref(launches), ctypes.byref(n)))
+        return int(launches.value), int(n.value)
 
     def _host_args(self, input_host, gate_weights, expert_weights, out_host, bias_up, bias_down):
         d = self.dims
@@ -346,6 +378,7 @@ class MoEContext:
 
     @property
     def launch_count(self) -> int:
+        """Launches issued through this API (graph replays are not counted; see `launch_record`)."""
         return int(self._L.fm_launch_count(self._ctx))
 
     def close(self) -> None:

@@ -124,6 +124,32 @@ FM_API int fm_moe_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, cons
 FM_API int fm_moe_forward_tokens(fm_ctx_t* ctx, const void* x, int n_tokens, const void* gate_w, const void* expert_w,
                                  const void* bias_up, const void* bias_down, void* out, void* stream);
 
+/* Same, with the token count in DEVICE memory: the kernel reads n = *n_tokens_dev (one int32) when it starts, so the
+ * count may be produced on the GPU (no host synchronisation) and one captured CUDA graph serves every count.  x and out
+ * are buffers of S rows; the result is bit-identical to fm_moe_forward_tokens(ctx, x, n, ...) -- routing tables and
+ * auxiliary loss included.  Rows n and above of x may hold anything (NaN included) and affect no result; rows n and
+ * above of out are never written.  A count outside [0, S] does not fault: that launch runs on 0 tokens (it still takes
+ * part in the collective) and the next fm_check / fm_read_buffer / fm_host_wait returns FM_EINVAL once, naming the
+ * count; the context stays usable.  fm_last_launch returns the count a launch ran with. */
+FM_API int fm_moe_forward_tokens_dev(fm_ctx_t* ctx, const void* x, const int32_t* n_tokens_dev, const void* gate_w,
+                                     const void* expert_w, const void* bias_up, const void* bias_down, void* out,
+                                     void* stream);
+
+/* ---- CUDA graphs ----
+ * Every forward entry point on device buffers (fm_moe_forward, fm_moe_forward_tokens, fm_moe_forward_tokens_dev) may
+ * be captured into a CUDA graph and the graph replayed any number of times, interleaved with eager calls on the same
+ * context.  A launch keeps no per-launch state in its parameters: the kernel takes its epoch, grid-barrier target and
+ * token-dependent sizes from the context's device-side launch counter (and the device-side count) when it starts.
+ * What is fixed at capture: the pointers (x, out, weights, biases, n_tokens_dev), a host-side n_tokens, and the
+ * fm_set_trace and fm_set_timeout_ms settings.  Replays of launches on one context must run in stream order, one at a
+ * time, like eager calls.  With world > 1 every rank issues the same number of launches, eager calls and replays
+ * together, in the same order.  The host-buffer entry points (fm_moe_forward_host, fm_host_submit) cannot be captured.
+ *
+ * fm_last_launch synchronises the device and returns the number of launches the context has run (graph replays
+ * included) and the token count the last one ran with (0 for an out-of-range device count).  Either pointer may be
+ * NULL. */
+FM_API int fm_last_launch(fm_ctx_t* ctx, uint64_t* launches, int32_t* n_tokens);
+
 /* world > 1: the [S,H] bf16 region of this rank's symmetric slab into which the experts (local and remote) accumulate
  * this rank's output rows.  Passing exactly this pointer as `out` to fm_moe_forward leaves the result there and skips
  * the final copy into a caller tensor (zero-copy output, like registering a user buffer with NVSHMEM); it is
@@ -149,6 +175,7 @@ FM_API int fm_host_wait(fm_ctx_t* ctx, uint64_t ticket);
 /* Check the kernel's host-mapped status record after a synchronise; FM_EKERNEL + message if a wait timed out. */
 FM_API int fm_check(fm_ctx_t* ctx);
 FM_API int fm_set_timeout_ms(fm_ctx_t* ctx, uint32_t ms);
+/* Launches issued through this API (a captured launch counts once, at capture; graph replays are not counted). */
 FM_API uint64_t fm_launch_count(const fm_ctx_t* ctx);
 /* Per-CTA phase / tile time stamps into FM_BUF_TRACE (profiling aid; off by default). */
 FM_API int fm_set_trace(fm_ctx_t* ctx, int enable);
