@@ -393,30 +393,277 @@ __device__ __forceinline__ void gate_phase_dense(const FmParams& p, const Launch
     }
 }
 
+// Router logits on the CUDA cores: logits[t, e] = sum_h x[t,h] * Wg_eff[e,h] for one sub-chunk of n_sub tokens of this
+// CTA, accumulated into the logits scratch.  Wg_eff is staged by the TMA engine in groups of up to 128 experts by chunks
+// of H; the x rows are read straight from global memory.
+__device__ __forceinline__ void gate_logits_gemv(const FmParams& p, uint8_t* smem, int t0, int s0, int n_sub,
+                                                 float* logit_s, int ldl, uint32_t& wgphase) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int E = p.E, H = p.H;
+    __nv_bfloat16* wg_s = reinterpret_cast<__nv_bfloat16*>(smem + G_OFF_WG);
+    uint64_t* wgbar = reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_WG;   // initialised in the kernel prologue
+    const int EG = E < 128 ? E : 128;                      // experts staged per group
+    int Hc = (G_WG_BYTES / (EG * 2)) & ~255;               // H columns staged per chunk (multiple of 256)
+    if (Hc > H) Hc = H;
+    for (int i = tid; i < n_sub * ldl; i += NUM_THREADS) logit_s[i] = 0.0f;
+    for (int eg0 = 0; eg0 < E; eg0 += EG) {
+        const int eg_len = min(EG, E - eg0);
+        for (int hc0 = 0; hc0 < H; hc0 += Hc) {
+            const int hc_len = min(Hc, H - hc0);
+            __syncthreads();  // previous users of wg_s are done (also orders the logit_s zero fill)
+            // stage Wg_eff[eg0 .. eg0+eg_len, hc0 .. hc0+hc_len) -> wg_s[e][Hc] through the TMA engine (1-D bulk copies,
+            // one per expert row, or a single one when the rows are contiguous on both sides): no register round trip,
+            // and the copy runs under the x loads issued below
+            if (warp == 0) {
+                if (lane == 0) {
+                    fence_proxy_async_smem();   // earlier generic accesses to this scratch -> async-proxy writes
+                    mbar_arrive_expect_tx(wgbar, (uint32_t)(eg_len * hc_len * 2));
+                }
+                __syncwarp();
+                if (hc_len == H && Hc == H) {
+                    if (lane == 0) bulk_load_1d(wg_s, p.wg + (size_t)eg0 * H, (uint32_t)(eg_len * H * 2), wgbar);
+                } else {
+                    for (int e = lane; e < eg_len; e += 32)
+                        bulk_load_1d(wg_s + (size_t)e * Hc, p.wg + (size_t)(eg0 + e) * H + hc0, (uint32_t)(hc_len * 2), wgbar);
+                }
+            }
+            const bool single = hc_len <= 1024;
+            uint4 xv[4][4];
+            // the first token block's x rows (HBM) are requested while Wg is in flight, so both latencies overlap
+            if (single && warp * 4 < n_sub) {
+                const int ntk0 = min(4, n_sub - warp * 4);
+                const __nv_bfloat16* xr0 = p.x + (size_t)(t0 + s0 + warp * 4) * H + hc0;
+#pragma unroll
+                for (int tk = 0; tk < 4; ++tk)
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const int h = i * 256 + lane * 8;
+                        xv[tk][i] = (tk < ntk0 && h < hc_len) ? ld_global_nc_v4(xr0 + (size_t)tk * H + h)
+                                                              : make_uint4(0u, 0u, 0u, 0u);
+                    }
+            }
+            mbar_wait(wgbar, wgphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 902);
+            wgphase ^= 1;
+            // register-blocked GEMV: a warp takes 4 tokens x 8 experts at a time (32 accumulators per lane, one per
+            // (token, expert) pair), lanes split the H columns in 16-byte pieces; all of a step's global loads are
+            // issued before the first FMA, and each staged Wg piece is reused by the 4 tokens.
+            for (int tb = warp * 4; tb < n_sub; tb += NUM_WARPS * 4) {
+                const int ntk = min(4, n_sub - tb);
+                const __nv_bfloat16* xr = p.x + (size_t)(t0 + s0 + tb) * H + hc0;
+                if (single && tb != warp * 4) {
+#pragma unroll
+                    for (int tk = 0; tk < 4; ++tk)
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const int h = i * 256 + lane * 8;
+                            xv[tk][i] = (tk < ntk && h < hc_len) ? ld_global_nc_v4(xr + (size_t)tk * H + h)
+                                                                 : make_uint4(0u, 0u, 0u, 0u);
+                        }
+                }
+                for (int g8 = 0; g8 * 8 < eg_len; ++g8) {
+                    const int ne = min(8, eg_len - g8 * 8);
+                    float acc[32];
+#pragma unroll
+                    for (int e = 0; e < 32; ++e) acc[e] = 0.0f;
+                    for (int pg = 0; pg < hc_len; pg += 1024) {
+                        if (!single) {
+#pragma unroll
+                            for (int tk = 0; tk < 4; ++tk)
+#pragma unroll
+                                for (int i = 0; i < 4; ++i) {
+                                    const int h = pg + i * 256 + lane * 8;
+                                    xv[tk][i] = (tk < ntk && h < hc_len) ? ld_global_nc_v4(xr + (size_t)tk * H + h)
+                                                                         : make_uint4(0u, 0u, 0u, 0u);
+                                }
+                        }
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const int h = pg + i * 256 + lane * 8;
+                            if (h < hc_len) {
+                                const __nv_bfloat16* wrow = wg_s + (size_t)(g8 * 8) * Hc + h;
+                                float xf[4][8];   // the 4 tokens' 8 columns, unpacked once per piece
+#pragma unroll
+                                for (int tk = 0; tk < 4; ++tk) unpack8(xv[tk][i], xf[tk]);
+#pragma unroll
+                                for (int e = 0; e < 8; ++e) {
+                                    if (e < ne) {
+                                        float wf[8];
+                                        unpack8(*reinterpret_cast<const uint4*>(wrow + (size_t)e * Hc), wf);
+#pragma unroll
+                                        for (int tk = 0; tk < 4; ++tk)
+#pragma unroll
+                                            for (int q = 0; q < 8; ++q)
+                                                acc[tk * 8 + e] = fmaf(xf[tk][q], wf[q], acc[tk * 8 + e]);
+                                    }
+                                }
+                            }
+                        }
+                    }
+                    const float tot = warp_transpose_reduce(acc, lane);   // lane -> (token lane/8, expert lane%8)
+                    const int tk = lane >> 3, e = lane & 7;
+                    if (tk < ntk && e < ne) logit_s[(tb + tk) * ldl + eg0 + g8 * 8 + e] += tot;
+                }
+            }
+        }
+    }
+}
+
+// The accumulation rows of this chunk's tokens start at zero (reference clearState zeroes the output,
+// moe.cuh:43-48).  Done by the TMA engine from a zeroed piece of the (still unused) epilogue staging area, so no
+// thread stalls on a store queue (as plain stores this cost 1.5-3 us on the router's critical path wherever it was
+// placed), and issued by gate_phase only after the first sub-chunk's logits: the engine works in order, and at the start
+// of the kernel these stores sat in front of the gate-weight load (+5 us).  The LAST warp issues them (softmax_topk
+// fills the warps from 0 upwards: with config B's 28 tokens per CTA warps 7-11 have none, and as warp 4's job
+// the 3 us of this block were on the router's critical path) and waits for them in dispatch_phase before the
+// local rows are acknowledged -- an expert only adds into a token's row after an acknowledgement of this CTA.
+__device__ __forceinline__ void zero_fill_out_rows(const FmParams& p, uint8_t* smem, int t0, int n_tok) {
+    const int lane = threadIdx.x & 31, H = p.H;
+    uint8_t* zbuf = smem + OFF_EPI;
+    const int row_bytes = H * 2, zbytes = min(row_bytes, 8192);
+    for (int i = lane * 16; i < zbytes; i += 512) *reinterpret_cast<uint4*>(zbuf + i) = make_uint4(0u, 0u, 0u, 0u);
+    fence_proxy_async_smem();
+    __syncwarp();
+    const int pieces = row_bytes / zbytes;   // H is a multiple of 64, rows above 8 KiB are multiples of 8 KiB or handled below
+    for (int i = lane; i < n_tok * pieces; i += 32)
+        bulk_store_1d(reinterpret_cast<uint8_t*>(p.out_acc + (size_t)(t0 + i / pieces) * H) + (size_t)(i % pieces) * zbytes, zbuf,
+                      (uint32_t)zbytes);
+    const int rem = row_bytes - pieces * zbytes;   // (row_bytes not a multiple of 8 KiB: the tail of every row)
+    if (rem > 0)
+        for (int i = lane; i < n_tok; i += 32)
+            bulk_store_1d(reinterpret_cast<uint8_t*>(p.out_acc + (size_t)(t0 + i) * H) + (size_t)pieces * zbytes, zbuf, (uint32_t)rem);
+    bulk_commit_group();
+    if (lane == 0) trace_stamp(p, 10);
+}
+
+// Lanes per token of softmax_topk: pow2ceil(E) up to 8 experts (one expert per lane), then 4 / 8 / 16 / 32, so that a
+// lane owns at most 32 experts.
+__device__ __forceinline__ int softmax_topk_lanes(int E) {
+    if (E > 8) return E <= 128 ? 4 : E <= 256 ? 8 : E <= 512 ? 16 : 32;
+    int lpt = 1;
+    while (lpt < E) lpt <<= 1;
+    return lpt;
+}
+
+// Softmax and top-k of one sub-chunk, for every E in [1, 1024]: a group of LPT = softmax_topk_lanes(E) lanes per token,
+// lane `sub` owns experts sub, sub + LPT, ... (C = ceil(E / LPT) <= 32 of them), 32 / LPT tokens per warp, so that a
+// sub-chunk of up to 96 tokens at E > 8 is one round of the CTA's 12 warps (the recurrence is a dependent chain of E
+// steps per token whatever the lane count; one lane per expert would serialise 111 tokens of the 16k-token sweep point
+// into 10 rounds, a thread per token leaves one or two warps doing ~5 E dependent steps each: 17 us at E = 128 with 56
+// tokens).  Every lane of a group runs the reference's sequential online-softmax recurrence (gate.cuh:575-584) itself;
+// a lane scans its own experts in ascending order with a strict '>', the group reduction prefers the larger value and,
+// on equal values, the lower index -- together the reference's ascending scan (gate.cuh:654-670).  A round in which no
+// expert compares greater than -inf (a token with NaN logits) picks expert 0, like the reference's scan.  Writes
+// gate_out, topk_idx, topk_w, mcw and sel_e, and leaves the probabilities in the logits scratch (the training-mode
+// column sums read them).
+__device__ __forceinline__ void softmax_topk(const FmParams& p, float* logit_s, int ldl, int16_t* sel_e, int t0, int s0,
+                                             int n_sub) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int E = p.E, k = p.k;
+    const int LPT = softmax_topk_lanes(E), lg = __ffs(LPT) - 1;   // shifts: the compiler cannot see LPT is a power of 2
+    const int TPW = 32 >> lg, sub = lane & (LPT - 1);
+    for (int tb = warp * TPW; tb < n_sub; tb += NUM_WARPS * TPW) {
+        const int ti_raw = tb + (lane >> lg);
+        const bool valid = ti_raw < n_sub;
+        const int ti = valid ? ti_raw : n_sub - 1;   // (idle groups compute on a copy of the last row, write nothing)
+        float* l = logit_s + ti * ldl;
+        const int t = t0 + s0 + ti;
+        float dI = 0.0f, mI = -INFINITY;
+        // (unrolled so that the loads, the running maxima and the exponentials of 8 steps are in flight together;
+        // the dependent chain is then one max and one fma per step -- same operations in the same order)
+#pragma unroll 8
+        for (int e = 0; e < E; ++e) {
+            const float pM = mI;
+            mI = fmaxf(mI, l[e]);
+            dI = fmaf(dI, fast_expf(pM - mI), fast_expf(l[e] - mI));
+        }
+        __syncwarp();   // every lane of the group has read the logits before they are replaced by probabilities
+        if (valid)
+#pragma unroll 4
+            for (int e = sub; e < E; e += LPT) {
+                const float pe = __fdividef(fast_expf(l[e] - mI), dI);
+                l[e] = pe;
+                p.gate_out[(size_t)t * E + e] = __float2bfloat16_rn(pe);
+            }
+        unsigned int taken = 0u;
+        float sum = 0.0f;
+        for (int i = 0; i < k; ++i) {
+            float bv = -INFINITY;
+            int bi = 0x7fffffff;
+            if (valid) {
+                int c = 0;
+#pragma unroll 4
+                for (int e = sub; e < E; e += LPT, ++c) {
+                    const float v = l[e];
+                    if (v > bv && !((taken >> c) & 1u)) { bv = v; bi = e; }
+                }
+            }
+            for (int off = LPT >> 1; off >= 1; off >>= 1) {
+                const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
+                const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
+                if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+            }
+            if (bi == 0x7fffffff) { bi = 0; }   // nothing comparable left (NaN logits): the reference's default
+            if ((bi & (LPT - 1)) == sub) taken |= 1u << (bi >> lg);
+            sum += bv;
+            if (sub == 0 && valid) {
+                p.topk_idx[(size_t)t * k + i] = bi;
+                p.topk_w[(size_t)t * k + i] = __float2bfloat16_rn(bv);
+                sel_e[(s0 + ti) * k + i] = (int16_t)bi;
+            }
+        }
+        if (sub == 0 && valid) p.mcw[t] = sum;
+        __syncwarp();
+    }
+}
+
+// Position of every (token, pick) among this chunk's selections of the same expert, ascending (token, pick) order, and
+// the chunk's per-expert counts.  One warp walks the entries 32 at a time: lanes holding the same expert find each other
+// with match.any, the rank inside the group is a popcount, the running per-expert count lives in shared memory (O(n)
+// instead of O(n^2); the 64k-token sweep point has 886 entries per CTA).
+__device__ __forceinline__ void slot_ranks(const FmParams& p, uint8_t* smem, int n_tok) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int E = p.E, k = p.k;
+    const int16_t* sel_e = reinterpret_cast<const int16_t*>(smem + G_OFF_SEL);
+    int* rank_s = reinterpret_cast<int*>(smem + G_OFF_SEL + G_SEL_MAX * 2);
+    int* cnt_s = reinterpret_cast<int*>(smem + G_OFF_BASE);
+    for (int e = tid; e < E; e += NUM_THREADS) cnt_s[e] = 0;
+    __syncthreads();
+    const int n_ent = n_tok * k;
+    if (warp == 0) {
+        for (int i0 = 0; i0 < n_ent; i0 += 32) {
+            const int i = i0 + lane;
+            const bool valid = i < n_ent;
+            const int e = valid ? (int)sel_e[i] : (E + lane);        // invalid lanes get unique keys
+            const unsigned int same = __match_any_sync(0xffffffffu, e);
+            const unsigned int before = same & ((1u << lane) - 1u);
+            if (valid) rank_s[i] = cnt_s[e] + __popc(before);
+            __syncwarp();
+            if (valid && before == 0u) cnt_s[e] += __popc(same);    // one lane per distinct expert of the group
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+    for (int e = tid; e < E; e += NUM_THREADS) p.chunk_counts[(size_t)blockIdx.x * E + e] = cnt_s[e];
+}
+
 __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int E = p.E, H = p.H, k = p.k;
-    __nv_bfloat16* wg_s = reinterpret_cast<__nv_bfloat16*>(smem + G_OFF_WG);
+    const int E = p.E, H = p.H;
     float* logit_s = reinterpret_cast<float*>(smem + G_OFF_LOGIT);
     int16_t* sel_e = reinterpret_cast<int16_t*>(smem + G_OFF_SEL);
-    int* rank_s = reinterpret_cast<int*>(smem + G_OFF_SEL + G_SEL_MAX * 2);
 
     float* aux_s = reinterpret_cast<float*>(smem + G_OFF_BASE + 8192);   // training: this chunk's sum_t p[t,e]
     if (p.aux != nullptr)
         for (int e = tid; e < E; e += NUM_THREADS) aux_s[e] = 0.0f;   // ordered by the block syncs of the first stage below
 
-    uint64_t* wgbar = reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_WG;   // initialised in the kernel prologue
-    uint32_t wgphase = 0;
-    const int EG = E < 128 ? E : 128;                      // experts staged per group
-    int Hc = (G_WG_BYTES / (EG * 2)) & ~255;               // H columns staged per chunk (multiple of 256)
-    if (Hc > H) Hc = H;
-    const int ldl = E + 1;                                  // padded logits row (bank spread for thread-per-row)
+    const int ldl = E + 1;                                  // padded logits row (bank spread across a warp's tokens)
     int TS = G_LOGIT_BYTES / (ldl * 4);                     // tokens per sub-chunk
     const bool tc = p.tc_gate != 0;
     if (tc) TS = min(TS, BLOCK_M);                          // two wgmma warpgroups = 128 token rows
     else if (TS > n_tok) TS = n_tok;
     GateTcState tcs;
     tcs.gkb = 0;
+    uint32_t wgphase = 0;
     if (tc) __syncthreads();   // the router's stage barriers (initialised in the prologue) are visible to every warp
 
     for (int s0 = 0; s0 < n_tok; s0 += TS) {
@@ -425,288 +672,12 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, u
             if (s0 > 0) __syncthreads();   // the logits scratch is reused: everybody is done with the previous sub-chunk
             gate_logits_tc(p, smem, t0, s0, n_sub, min(TS, L.tpc), logit_s, ldl, tcs);
         } else {
-        for (int i = tid; i < n_sub * ldl; i += NUM_THREADS) logit_s[i] = 0.0f;
-        for (int eg0 = 0; eg0 < E; eg0 += EG) {
-            const int eg_len = min(EG, E - eg0);
-            for (int hc0 = 0; hc0 < H; hc0 += Hc) {
-                const int hc_len = min(Hc, H - hc0);
-                __syncthreads();  // previous users of wg_s are done (also orders the logit_s zero fill)
-                // stage Wg_eff[eg0 .. eg0+eg_len, hc0 .. hc0+hc_len) -> wg_s[e][Hc] through the TMA engine (1-D bulk copies,
-                // one per expert row, or a single one when the rows are contiguous on both sides): no register round trip,
-                // and the copy runs under the x loads issued below
-                if (warp == 0) {
-                    if (lane == 0) {
-                        fence_proxy_async_smem();   // earlier generic accesses to this scratch -> async-proxy writes
-                        mbar_arrive_expect_tx(wgbar, (uint32_t)(eg_len * hc_len * 2));
-                    }
-                    __syncwarp();
-                    if (hc_len == H && Hc == H) {
-                        if (lane == 0) bulk_load_1d(wg_s, p.wg + (size_t)eg0 * H, (uint32_t)(eg_len * H * 2), wgbar);
-                    } else {
-                        for (int e = lane; e < eg_len; e += 32)
-                            bulk_load_1d(wg_s + (size_t)e * Hc, p.wg + (size_t)(eg0 + e) * H + hc0, (uint32_t)(hc_len * 2), wgbar);
-                    }
-                }
-                const bool single = hc_len <= 1024;
-                uint4 xv[4][4];
-                // the first token block's x rows (HBM) are requested while Wg is in flight, so both latencies overlap
-                if (single && warp * 4 < n_sub) {
-                    const int ntk0 = min(4, n_sub - warp * 4);
-                    const __nv_bfloat16* xr0 = p.x + (size_t)(t0 + s0 + warp * 4) * H + hc0;
-#pragma unroll
-                    for (int tk = 0; tk < 4; ++tk)
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int h = i * 256 + lane * 8;
-                            xv[tk][i] = (tk < ntk0 && h < hc_len) ? ld_global_nc_v4(xr0 + (size_t)tk * H + h)
-                                                                  : make_uint4(0u, 0u, 0u, 0u);
-                        }
-                }
-                mbar_wait(wgbar, wgphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 902);
-                wgphase ^= 1;
-                // register-blocked GEMV: a warp takes 4 tokens x 8 experts at a time (32 accumulators per lane, one per
-                // (token, expert) pair), lanes split the H columns in 16-byte pieces; all of a step's global loads are
-                // issued before the first FMA, and each staged Wg piece is reused by the 4 tokens.
-                for (int tb = warp * 4; tb < n_sub; tb += NUM_WARPS * 4) {
-                    const int ntk = min(4, n_sub - tb);
-                    const __nv_bfloat16* xr = p.x + (size_t)(t0 + s0 + tb) * H + hc0;
-                    if (single && tb != warp * 4) {
-#pragma unroll
-                        for (int tk = 0; tk < 4; ++tk)
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const int h = i * 256 + lane * 8;
-                                xv[tk][i] = (tk < ntk && h < hc_len) ? ld_global_nc_v4(xr + (size_t)tk * H + h)
-                                                                     : make_uint4(0u, 0u, 0u, 0u);
-                            }
-                    }
-                    for (int g8 = 0; g8 * 8 < eg_len; ++g8) {
-                        const int ne = min(8, eg_len - g8 * 8);
-                        float acc[32];
-#pragma unroll
-                        for (int e = 0; e < 32; ++e) acc[e] = 0.0f;
-                        for (int pg = 0; pg < hc_len; pg += 1024) {
-                            if (!single) {
-#pragma unroll
-                                for (int tk = 0; tk < 4; ++tk)
-#pragma unroll
-                                    for (int i = 0; i < 4; ++i) {
-                                        const int h = pg + i * 256 + lane * 8;
-                                        xv[tk][i] = (tk < ntk && h < hc_len) ? ld_global_nc_v4(xr + (size_t)tk * H + h)
-                                                                             : make_uint4(0u, 0u, 0u, 0u);
-                                    }
-                            }
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const int h = pg + i * 256 + lane * 8;
-                                if (h < hc_len) {
-                                    const __nv_bfloat16* wrow = wg_s + (size_t)(g8 * 8) * Hc + h;
-                                    float xf[4][8];   // the 4 tokens' 8 columns, unpacked once per piece
-#pragma unroll
-                                    for (int tk = 0; tk < 4; ++tk) unpack8(xv[tk][i], xf[tk]);
-#pragma unroll
-                                    for (int e = 0; e < 8; ++e) {
-                                        if (e < ne) {
-                                            float wf[8];
-                                            unpack8(*reinterpret_cast<const uint4*>(wrow + (size_t)e * Hc), wf);
-#pragma unroll
-                                            for (int tk = 0; tk < 4; ++tk)
-#pragma unroll
-                                                for (int q = 0; q < 8; ++q)
-                                                    acc[tk * 8 + e] = fmaf(xf[tk][q], wf[q], acc[tk * 8 + e]);
-                                        }
-                                    }
-                                }
-                            }
-                        }
-                        const float tot = warp_transpose_reduce(acc, lane);   // lane -> (token lane/8, expert lane%8)
-                        const int tk = lane >> 3, e = lane & 7;
-                        if (tk < ntk && e < ne) logit_s[(tb + tk) * ldl + eg0 + g8 * 8 + e] += tot;
-                    }
-                }
-            }
+            gate_logits_gemv(p, smem, t0, s0, n_sub, logit_s, ldl, wgphase);
         }
-        }   // GEMV path
         __syncthreads();
         if (tid == 0) trace_stamp(p, 11);
-        if (p.fused && s0 == 0 && warp == NUM_WARPS - 1) {
-        // The accumulation rows of this chunk's tokens start at zero (reference clearState zeroes the output,
-        // moe.cuh:43-48).  Done by the TMA engine from a zeroed piece of the (still unused) epilogue staging area, so no
-        // thread stalls on a store queue (as plain stores this cost 1.5-3 us on the router's critical path wherever it was
-        // placed), and issued only now, after the GEMV: the engine works in order, and at the start of the kernel these
-        // stores sat in front of the gate-weight load (+5 us).  The LAST warp issues them (the softmax / top-k rounds below
-        // fill the warps from 0 upwards: with config B's 28 tokens per CTA warps 7-11 have none, and as warp 4's job
-        // the 3 us of this block were on the router's critical path) and waits for them in dispatch_phase before the
-        // local rows are acknowledged -- an expert only adds into a token's row after an acknowledgement of this CTA.
-        uint8_t* zbuf = smem + OFF_EPI;
-        const int row_bytes = H * 2, zbytes = min(row_bytes, 8192);
-        for (int i = lane * 16; i < zbytes; i += 512) *reinterpret_cast<uint4*>(zbuf + i) = make_uint4(0u, 0u, 0u, 0u);
-        fence_proxy_async_smem();
-        __syncwarp();
-        const int pieces = row_bytes / zbytes;   // H is a multiple of 64, rows above 8 KiB are multiples of 8 KiB or handled below
-        for (int i = lane; i < n_tok * pieces; i += 32)
-            bulk_store_1d(reinterpret_cast<uint8_t*>(p.out_acc + (size_t)(t0 + i / pieces) * H) + (size_t)(i % pieces) * zbytes, zbuf,
-                          (uint32_t)zbytes);
-        const int rem = row_bytes - pieces * zbytes;   // (row_bytes not a multiple of 8 KiB: the tail of every row)
-        if (rem > 0)
-            for (int i = lane; i < n_tok; i += 32)
-                bulk_store_1d(reinterpret_cast<uint8_t*>(p.out_acc + (size_t)(t0 + i) * H) + (size_t)pieces * zbytes, zbuf, (uint32_t)rem);
-        bulk_commit_group();
-        if (lane == 0) trace_stamp(p, 10);
-    }
-        if (E <= 8) {
-            // E <= 8: a group of LPT = pow2ceil(E) lanes per token.  Every lane of the group runs the reference's
-            // sequential online-softmax recurrence itself (gate.cuh:575-584; E <= 32 steps on broadcast smem reads, so the
-            // result is bit-identical to the thread-per-row form), then lane `sub` owns expert `sub`: its probability,
-            // the coalesced gateOut store, and its candidate in the k rounds of argmax -- a shuffle reduction that
-            // keeps the larger value and, on equal values, the lower index = the strict-'>' ascending scan of
-            // gate.cuh:654-670.
-            int LPT = 1;
-            while (LPT < E) LPT <<= 1;
-            const int TPW = 32 / LPT, sub = lane & (LPT - 1);
-            for (int tb = warp * TPW; tb < n_sub; tb += NUM_WARPS * TPW) {
-                const int ti_raw = tb + lane / LPT;
-                const bool valid = ti_raw < n_sub;
-                const int ti = valid ? ti_raw : n_sub - 1;
-                const float* l = logit_s + ti * ldl;
-                const int t = t0 + s0 + ti;
-                float dI = 0.0f, mI = -INFINITY;
-#pragma unroll 8
-                for (int e = 0; e < E; ++e) {
-                    const float pM = mI;
-                    mI = fmaxf(mI, l[e]);
-                    dI = fmaf(dI, fast_expf(pM - mI), fast_expf(l[e] - mI));
-                }
-                const bool own = sub < E;
-                const float pe = own ? __fdividef(fast_expf(l[sub] - mI), dI) : -INFINITY;
-                if (own && valid) p.gate_out[(size_t)t * E + sub] = __float2bfloat16_rn(pe);
-                bool taken = !own;
-                float sum = 0.0f;
-                for (int i = 0; i < k; ++i) {
-                    float bv = taken ? -INFINITY : pe;
-                    int bi = taken ? 0x7fffffff : sub;
-                    for (int off = LPT >> 1; off >= 1; off >>= 1) {
-                        const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
-                        const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
-                        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-                    }
-                    if (bi == sub) taken = true;
-                    sum += bv;
-                    if (sub == 0 && valid) {
-                        p.topk_idx[(size_t)t * k + i] = bi;
-                        p.topk_w[(size_t)t * k + i] = __float2bfloat16_rn(bv);
-                        sel_e[(s0 + ti) * k + i] = (int16_t)bi;
-                    }
-                }
-                if (sub == 0 && valid) p.mcw[t] = sum;
-                __syncwarp();
-                if (own && valid) logit_s[ti * ldl + sub] = pe;   // probabilities (training-mode column sums read them)
-            }
-        } else if (E <= 1024) {
-            // 8 < E <= 1024: the same scheme with C = ceil(E / LPT) <= 32 experts per lane (lane `sub` owns experts sub,
-            // sub + LPT, ...): 8 / 4 / 2 / 1 tokens per warp, so that a sub-chunk of up to 96 tokens is one round of the CTA's
-            // 12 warps (the recurrence is a dependent chain of E steps per token whatever the lane count; one lane per
-            // expert would serialise 111 tokens of the 16k-token sweep point into 10 rounds, a thread per token leaves one
-            // or two warps doing ~5 E dependent steps each: 17 us at E = 128 with 56 tokens).  Every lane of a group runs the sequential
-            // recurrence itself; a lane scans its own experts in ascending order with a strict '>', the group reduction
-            // prefers the larger value and, on equal values, the lower index -- together the reference's ascending scan.
-            const int LPT = E <= 128 ? 4 : E <= 256 ? 8 : E <= 512 ? 16 : 32;
-            const int TPW = 32 / LPT, sub = lane & (LPT - 1);
-            for (int tb = warp * TPW; tb < n_sub; tb += NUM_WARPS * TPW) {
-                const int ti_raw = tb + lane / LPT;
-                const bool valid = ti_raw < n_sub;
-                const int ti = valid ? ti_raw : n_sub - 1;   // (idle groups compute on a copy of the last row, write nothing)
-                float* l = logit_s + ti * ldl;
-                const int t = t0 + s0 + ti;
-                float dI = 0.0f, mI = -INFINITY;
-                // (unrolled so that the loads, the running maxima and the exponentials of 8 steps are in flight together;
-                // the dependent chain is then one max and one fma per step -- same operations in the same order)
-#pragma unroll 8
-                for (int e = 0; e < E; ++e) {
-                    const float pM = mI;
-                    mI = fmaxf(mI, l[e]);
-                    dI = fmaf(dI, fast_expf(pM - mI), fast_expf(l[e] - mI));
-                }
-                __syncwarp();   // every lane of the group has read the logits before they are replaced by probabilities
-                if (valid)
-#pragma unroll 4
-                    for (int e = sub; e < E; e += LPT) {
-                        const float pe = __fdividef(fast_expf(l[e] - mI), dI);
-                        l[e] = pe;
-                        p.gate_out[(size_t)t * E + e] = __float2bfloat16_rn(pe);
-                    }
-                unsigned int taken = 0u;
-                float sum = 0.0f;
-                for (int i = 0; i < k; ++i) {
-                    float bv = -INFINITY;
-                    int bi = 0x7fffffff;
-                    if (valid) {
-                        int c = 0;
-#pragma unroll 4
-                        for (int e = sub; e < E; e += LPT, ++c) {
-                            const float v = l[e];
-                            if (v > bv && !((taken >> c) & 1u)) { bv = v; bi = e; }
-                        }
-                    }
-                    for (int off = LPT >> 1; off >= 1; off >>= 1) {
-                        const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
-                        const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
-                        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-                    }
-                    if (bi == 0x7fffffff) { bi = 0; }   // nothing comparable left (NaN logits): the thread-per-token form's default
-                    if ((bi & (LPT - 1)) == sub) taken |= 1u << (bi / LPT);
-                    sum += bv;
-                    if (sub == 0 && valid) {
-                        p.topk_idx[(size_t)t * k + i] = bi;
-                        p.topk_w[(size_t)t * k + i] = __float2bfloat16_rn(bv);
-                        sel_e[(s0 + ti) * k + i] = (int16_t)bi;
-                    }
-                }
-                if (sub == 0 && valid) p.mcw[t] = sum;
-                __syncwarp();
-            }
-        } else
-        // thread-per-token softmax + top-k, the same per-thread recurrence the reference runs after its transpose
-        for (int ti = tid; ti < n_sub; ti += NUM_THREADS) {
-            float* l = logit_s + ti * ldl;
-            const int t = t0 + s0 + ti;
-            float dI = 0.0f, mI = -INFINITY;
-            for (int e = 0; e < E; ++e) {
-                const float pM = mI;
-                mI = fmaxf(mI, l[e]);
-                dI = fmaf(dI, fast_expf(pM - mI), fast_expf(l[e] - mI));
-            }
-            for (int e = 0; e < E; ++e) {
-                const float pe = __fdividef(fast_expf(l[e] - mI), dI);
-                l[e] = pe;
-                p.gate_out[(size_t)t * E + e] = __float2bfloat16_rn(pe);
-            }
-            int picked[8];
-            float sum = 0.0f;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                picked[i] = -1;
-                if (i < k) {
-                    float sV = -INFINITY;
-                    int sIdx = 0;
-                    for (int j = 0; j < E; ++j) {
-                        bool taken = false;
-#pragma unroll
-                        for (int q = 0; q < 8; ++q) taken |= (q < i) && (picked[q] == j);
-                        if (l[j] > sV && !taken) {
-                            sIdx = j;
-                            sV = l[j];
-                        }
-                    }
-                    picked[i] = sIdx;
-                    sum += sV;
-                    p.topk_idx[(size_t)t * k + i] = sIdx;
-                    p.topk_w[(size_t)t * k + i] = __float2bfloat16_rn(sV);
-                    sel_e[(s0 + ti) * k + i] = (int16_t)sIdx;
-                }
-            }
-            p.mcw[t] = sum;
-        }
+        if (p.fused && s0 == 0 && warp == NUM_WARPS - 1) zero_fill_out_rows(p, smem, t0, n_tok);
+        softmax_topk(p, logit_s, ldl, sel_e, t0, s0, n_sub);
         if (tid == 0) trace_stamp(p, 15);
         __syncthreads();
         if (p.aux != nullptr) {
@@ -738,29 +709,7 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, u
         float* gml = p.aux + (size_t)(L.epoch & 1u) * (2 * E + 1);
         for (int e = tid; e < E; e += NUM_THREADS) atomicAdd(gml + e, __fdividef(aux_s[e], (float)L.S));
     }
-    // position of every (token, pick) among this chunk's selections of the same expert, ascending (token, pick) order.
-    // One warp walks the entries 32 at a time: lanes holding the same expert find each other with match.any, the rank
-    // inside the group is a popcount, the running per-expert count lives in shared memory (O(n) instead of O(n^2);
-    // the 64k-token sweep point has 886 entries per CTA).
-    int* cnt_s = reinterpret_cast<int*>(smem + G_OFF_BASE);
-    for (int e = tid; e < E; e += NUM_THREADS) cnt_s[e] = 0;
-    __syncthreads();
-    const int n_ent = n_tok * k;
-    if (warp == 0) {
-        for (int i0 = 0; i0 < n_ent; i0 += 32) {
-            const int i = i0 + lane;
-            const bool valid = i < n_ent;
-            const int e = valid ? (int)sel_e[i] : (E + lane);        // invalid lanes get unique keys
-            const unsigned int same = __match_any_sync(0xffffffffu, e);
-            const unsigned int before = same & ((1u << lane) - 1u);
-            if (valid) rank_s[i] = cnt_s[e] + __popc(before);
-            __syncwarp();
-            if (valid && before == 0u) cnt_s[e] += __popc(same);    // one lane per distinct expert of the group
-            __syncwarp();
-        }
-    }
-    __syncthreads();
-    for (int e = tid; e < E; e += NUM_THREADS) p.chunk_counts[(size_t)blockIdx.x * E + e] = cnt_s[e];
+    slot_ranks(p, smem, n_tok);
 }
 
 // ============================================================================================================

@@ -120,7 +120,9 @@ FM_API int fm_moe_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, cons
  * written to out at or beyond row n_tokens.  With n_tokens = 0, x and out may be NULL; the call still launches and takes
  * part in the collective.  With world > 1 every rank passes its own count (counts may differ between ranks and between
  * calls; every rank still calls the same number of times).  fm_moe_forward(...) is fm_moe_forward_tokens(..., S, ...).
- * FM_EINVAL for n_tokens < 0 or > S.  The routing tables read back with fm_read_buffer hold n_tokens valid rows. */
+ * FM_EINVAL for n_tokens < 0 or > S.  The routing tables read back with fm_read_buffer hold n_tokens valid rows.  A row
+ * below n_tokens that holds a NaN routes all k of its picks to expert 0, as the reference does; they take capacity of
+ * expert 0 like any other pick. */
 FM_API int fm_moe_forward_tokens(fm_ctx_t* ctx, const void* x, int n_tokens, const void* gate_w, const void* expert_w,
                                  const void* bias_up, const void* bias_down, void* out, void* stream);
 

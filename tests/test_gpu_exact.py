@@ -17,7 +17,7 @@ MIN_H_ROUNDED, MIN_OUT_ROUNDED = 0.02, 0.2   # shares of h / out elements (k >= 
 
 
 def _lpt(E):
-    """Lanes per token of the router's softmax / top-k (fm_kernel.cuh gate_phase)."""
+    """Lanes per token of the router's softmax / top-k (fm_kernel.cuh softmax_topk_lanes)."""
     if E <= 8:
         p = 1
         while p < E:

@@ -248,6 +248,35 @@ def test_router_many_experts_general_path():
     _compare(cfg, _run(cfg, x, wg, we), run_oracle(cfg, x, wg, we))
 
 
+@pytest.mark.parametrize("E,k,tc_gate", [(4, 3, None), (6, 3, None), (8, 2, None), (16, 2, None), (64, 4, None),
+                                         (8, 2, 1)])
+def test_router_nan_token(monkeypatch, E, k, tc_gate):
+    """A NaN in a token's x row makes all its logits NaN: no expert compares greater than -inf in any top-k round, and
+    the token picks expert 0 every time, as the oracle does.  Every index stays in range (E = 6: idle lanes in the
+    lane groups), and the other tokens route, count and combine as usual."""
+    if tc_gate is not None:
+        monkeypatch.setenv("FM_TC_GATE", str(tc_gate))
+    cfg = MoEConfig(num_experts=E, expert_top_k=k, sequence_len=512, hidden_size=256, intermediate_size=512)
+    x, wg, we, _, _ = make_inputs(cfg, seed=600 + E + k)
+    rows = x.view(cfg.S, cfg.H)
+    nan_tokens = [1, 2, 301]
+    rows[1] = float("nan")          # a whole row
+    rows[2, 17] = float("nan")      # one element, in the neighbour of a NaN row
+    rows[301, 0] = float("nan")
+    got = _run(cfg, x, wg, we)
+    ref = run_oracle(cfg, x, wg, we)
+    topk = got["topk_idx"]
+    assert ((topk >= 0) & (topk < E)).all()
+    assert (topk[nan_tokens] == 0).all() and (ref.topk_idx[nan_tokens] == 0).all()
+    slot, counts, recv_cnt, _ = slots_from_topk(topk, E, cfg.EC)
+    assert (got["slot"] == slot).all()
+    assert (got["counts"] == counts).all()
+    assert (got["recv_cnt"] == recv_cnt).all()
+    rows_ok = ~check_topk(topk, ref)
+    rows_ok[nan_tokens] = False
+    check_output(got["out"], ref.out, rows_ok=rows_ok)
+
+
 @pytest.mark.parametrize("fused", [1, 0])
 def test_relaunch_with_changing_inputs_every_launch_checked(monkeypatch, fused):
     """Back-to-back launches on ONE context with different activations (routing, per-expert counts and drops change,
