@@ -182,7 +182,8 @@ int validate_config(const fm_config_t& c, int world, fm_dims_t* d) {
     const long long S = (long long)c.sequence_len * c.mini_batch;
     if (S % 128) return fail(FM_EINVAL, "S = sequence_len*mini_batch = %lld must be a multiple of 128", S);
     if (S > (1ll << 24)) return fail(FM_EINVAL, "S = %lld too large", S);
-    if (c.num_experts < 1 || c.num_experts > 1024) return fail(FM_EINVAL, "num_experts must be in [1, 1024]");
+    if (c.num_experts < 1 || c.num_experts > fm::MAX_EXPERTS)
+        return fail(FM_EINVAL, "num_experts must be in [1, %d]", fm::MAX_EXPERTS);
     if (c.expert_top_k < 1 || c.expert_top_k > c.num_experts || c.expert_top_k > 8)
         return fail(FM_EINVAL, "expert_top_k must be in [1, min(num_experts, 8)]");
     if (world < 1 || world > FM_MAX_WORLD) return fail(FM_EINVAL, "world size %d not in [1, %d]", world, FM_MAX_WORLD);

@@ -88,19 +88,85 @@ constexpr int SMEM_USED = OFF_LAUNCH + 64;
 constexpr int SMEM_BYTES = SMEM_USED + 1024;                          // + slack for manual 1 KiB alignment
 static_assert(OFF_RING % 16 == 0, "ring entries are 16-byte aligned");
 static_assert(SMEM_BYTES <= 232448, "227 KiB of dynamic shared memory per CTA");
-// named barriers (bar.sync ids): 2-7 dispatch / staging hand-over (see dispatch_phase), 8 the router's consumer warpgroups
-constexpr int NAMED_BAR_GATE_MMA = 8;
+constexpr int MAX_EXPERTS = 1024;   // validate_config rejects more; sizes the per-expert arrays below
 
-// gate-phase aliases of the (not yet used) pipeline stage area
-constexpr int G_OFF_WG = 0;              // bf16 [EG][Hc]           <= 64 KiB
-constexpr int G_WG_BYTES = 65536;
-constexpr int G_OFF_LOGIT = 65536;       // f32  [TS][E+1]          <= 64 KiB
-constexpr int G_LOGIT_BYTES = 65536;
-constexpr int G_OFF_SEL = 131072;        // int16 sel_e[tpc*k] then int32 rank[tpc*k]   <= 48 KiB
-constexpr int G_SEL_MAX = 8192;          // max tpc*k
-constexpr int G_OFF_BASE = 131072 + 49152;  // int32 base[E] + total[E] + own[E]   <= 12 KiB (E <= 1024)
-constexpr int G_XROWS_BYTES = 131072;       // dispatch: staged token rows (reuses the Wg / logits scratch)
-static_assert(G_OFF_BASE + 12288 <= OFF_EPI, "gate scratch must fit in the stage area");
+// Shared-memory plan.  Four phases take turns in the stage area [0, PIPE_BYTES) and the epilogue staging area
+// [OFF_EPI, OFF_EPI + EPI_BYTES); every alias below is one of these regions:
+//
+//   bytes             | router (G)               | dispatch (D)              | expert FFN (F)       | gather combine (C)
+//   ------------------+--------------------------+---------------------------+----------------------+-------------------
+//   stage [0, 64K)    | Wg chunks (GEMV) or      | x-row staging, 128 KiB    | pipeline stages,     | routing records
+//                     | tensor-core stages       | (load issued at the end   | after BAR_DISP_DONE  | c_e/c_s/c_w/c_m,
+//                     |                          | of gate_phase)            |                      | 128 KiB
+//   [64K, 128K)       | logits [TS][E+1] f32     | (staging, cont.)          | (stages)             | (records, cont.)
+//                     | (single-pass tensor-core |                           |                      |
+//                     | stages overlay it)       |                           |                      |
+//   [128K, 176K)      | sel_e i16 + rank i32,    | read                      | (stages)             |
+//                     | G_SEL_MAX each           |                           |                      |
+//   [176K, 188K)      | slot_ranks counts (on    | base / total / own,       | (stages)             |
+//                     | base), training column   | MAX_EXPERTS each          |                      |
+//                     | sums (on own)            |                           |                      |
+//   epilogue [0, 8K)  | zero source of the       | read by the fill's bulk   | chunk buffers        |
+//                     | output-row fill (warp 11)| stores until warps 4-11's |                      |
+//                     |                          | wait_group.read           |                      |
+//   epilogue [8K,32K) |                          | warp 2's remote-row       | chunk buffers, after |
+//                     |                          | window (W > 1)            | NAMED_BAR_WINDOW     |
+constexpr int G_OFF_WG = 0;                                // bf16 [EG][Hc] gate-weight chunks, or tensor-core stages
+constexpr int G_WG_BYTES = 64 * 1024;
+constexpr int G_OFF_LOGIT = G_OFF_WG + G_WG_BYTES;         // f32 [TS][E+1]
+constexpr int G_LOGIT_BYTES = 64 * 1024;
+constexpr int G_SEL_MAX = 8192;                            // max tpc * k (the host rejects more)
+constexpr int G_OFF_SEL = G_OFF_LOGIT + G_LOGIT_BYTES;     // int16 sel_e[tpc * k]
+constexpr int G_OFF_RANK = G_OFF_SEL + G_SEL_MAX * 2;      // int32 rank[tpc * k]
+constexpr int D_OFF_BASE = G_OFF_RANK + G_SEL_MAX * 4;     // int32 base[E]: selections of e by lower chunks
+constexpr int D_OFF_TOTAL = D_OFF_BASE + MAX_EXPERTS * 4;  // int32 total[E]: by all chunks
+constexpr int D_OFF_OWN = D_OFF_TOTAL + MAX_EXPERTS * 4;   // int32 own[E]: by this chunk
+constexpr int D_PREFIX_END = D_OFF_OWN + MAX_EXPERTS * 4;
+constexpr int G_OFF_CNT = D_OFF_BASE;                      // int32 [E] slot_ranks' running counts
+constexpr int G_OFF_COLSUM = D_OFF_OWN;                    // f32 [E] training: this chunk's sum_t p[t,e]
+constexpr int D_OFF_XROWS = 0;                             // staged token rows of this chunk
+constexpr int D_XROWS_BYTES = 128 * 1024;
+constexpr int C_OFF_E = 0;                                 // int32 [tpc * k] expert
+constexpr int C_OFF_S = C_OFF_E + G_SEL_MAX * 4;           // int32 [tpc * k] slot
+constexpr int C_OFF_W = C_OFF_S + G_SEL_MAX * 4;           // f32 [tpc * k] combine weight
+constexpr int C_OFF_M = C_OFF_W + G_SEL_MAX * 4;           // f32 [tpc] mCw
+constexpr int C_RECORDS_END = C_OFF_M + G_SEL_MAX * 4;
+constexpr int EPI_OFF_ZERO = OFF_EPI;                      // zero source of the output-row fill
+constexpr int EPI_ZERO_BYTES = 8 * 1024;
+constexpr int D_OFF_WIN = EPI_OFF_ZERO + EPI_ZERO_BYTES;   // warp 2's remote-row window
+constexpr int D_WIN_BYTES = OFF_EPI + EPI_BYTES - D_OFF_WIN;
+static_assert(D_PREFIX_END <= PIPE_BYTES, "router and dispatch scratch within the stage area");
+static_assert(D_OFF_XROWS + D_XROWS_BYTES <= G_OFF_SEL,
+              "x-row staging below sel_e / rank: slot_ranks uses them while the first load is in flight");
+static_assert(C_RECORDS_END <= PIPE_BYTES, "combine records within the stage area");
+static_assert(D_WIN_BYTES > 0 && EPI_ZERO_BYTES + D_WIN_BYTES <= EPI_BYTES,
+              "zero source and remote-row window within the epilogue staging area");
+static_assert(G_OFF_COLSUM + MAX_EXPERTS * (int)sizeof(float) <= D_PREFIX_END, "a column sum per expert");
+
+__device__ __forceinline__ uint64_t* bar(uint8_t* smem, int id) { return reinterpret_cast<uint64_t*>(smem + OFF_BARS) + id; }
+
+// Named barriers (named_sync / named_arrive; id 0 is __syncthreads).  Ids 2-7 are one protocol between warp 2 and warps
+// 4-11, from dispatch into the consumers' first epilogue:
+//
+//   id | threads      | sync / arrive                        | orders
+//   ---+--------------+--------------------------------------+----------------------------------------------------------
+//   2  | DISP_THREADS | warps 2, 4-11                        | prefix arrays zeroed, then complete
+//   3  | DISP_THREADS | 4-11 arrive, 2 syncs                 | this chunk's p.slot is written
+//   4  | EPI_THREADS  | warps 4-11                           | x-row staging reuse; local row stores complete before acks
+//   5  | DISP_THREADS | 2 arrives, 4-11 sync                 | warp 2 is done reading base / own in the stage area
+//   6  | DISP_THREADS | 4-11 arrive, 2 syncs                 | local rows and the zero-fill complete before remote acks
+//   7  | DISP_THREADS | 2 arrives, consumers sync before     | remote-row window handed back
+//      |              | their first epilogue (W > 1)         |
+//   8  | EPI_THREADS  | router consumer warpgroups           | tensor-core stages read before the logits are written
+constexpr int EPI_THREADS = 32 * NUM_EPI_WARPS;    // warps 4-11
+constexpr int DISP_THREADS = 32 + EPI_THREADS;     // warps 2, 4-11
+constexpr int NAMED_BAR_PREFIX = 2;
+constexpr int NAMED_BAR_SLOTS = 3;
+constexpr int NAMED_BAR_LOCAL = 4;
+constexpr int NAMED_BAR_PREFIX_READ = 5;
+constexpr int NAMED_BAR_LOCAL_DONE = 6;
+constexpr int NAMED_BAR_WINDOW = 7;
+constexpr int NAMED_BAR_GATE_MMA = 8;
 
 struct TileBlock {  // one contiguous run of work items: all tiles of one GEMM of one packet (or of a packet pair)
     int kind;       // 0 = GEMM0 (x.W_up^T), 1 = GEMM1 (h.W_down^T)
@@ -283,9 +349,8 @@ __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
 struct GateTcState { int gkb; };
 __device__ __forceinline__ void gate_logits_tc(const FmParams& p, uint8_t* smem, int t0, int s0, int n_sub, int rows_cap,
                                                float* logit_s, int ldl, GateTcState& st) {
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BARS);
-    uint64_t* gfull = bars + BAR_GFULL;
-    uint64_t* gempty = bars + BAR_GEMPTY;
+    uint64_t* gfull = bar(smem, BAR_GFULL);
+    uint64_t* gempty = bar(smem, BAR_GEMPTY);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int E = p.E, E64 = (E + 63) & ~63;
     const int GB = min(128, E64);                                // Wg_eff rows per pass (the tensor map's box height)
@@ -350,7 +415,7 @@ __device__ __forceinline__ void gate_logits_tc(const FmParams& p, uint8_t* smem,
                 if (lane == 0) mbar_arrive(&gempty[s]);
             }
             // both warpgroups are done reading the stages (which may overlap the logits scratch)
-            asm volatile("bar.sync %0, 256;" ::"n"(NAMED_BAR_GATE_MMA) : "memory");
+            named_sync<NAMED_BAR_GATE_MMA, EPI_THREADS>();
             if (active) {
                 const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), cq = (lane & 3) * 2;
 #pragma unroll
@@ -401,7 +466,7 @@ __device__ __forceinline__ void gate_logits_gemv(const FmParams& p, uint8_t* sme
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int E = p.E, H = p.H;
     __nv_bfloat16* wg_s = reinterpret_cast<__nv_bfloat16*>(smem + G_OFF_WG);
-    uint64_t* wgbar = reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_WG;   // initialised in the kernel prologue
+    uint64_t* wgbar = bar(smem, BAR_WG);   // initialised in the kernel prologue
     const int EG = E < 128 ? E : 128;                      // experts staged per group
     int Hc = (G_WG_BYTES / (EG * 2)) & ~255;               // H columns staged per chunk (multiple of 256)
     if (Hc > H) Hc = H;
@@ -518,8 +583,8 @@ __device__ __forceinline__ void gate_logits_gemv(const FmParams& p, uint8_t* sme
 // local rows are acknowledged -- an expert only adds into a token's row after an acknowledgement of this CTA.
 __device__ __forceinline__ void zero_fill_out_rows(const FmParams& p, uint8_t* smem, int t0, int n_tok) {
     const int lane = threadIdx.x & 31, H = p.H;
-    uint8_t* zbuf = smem + OFF_EPI;
-    const int row_bytes = H * 2, zbytes = min(row_bytes, 8192);
+    uint8_t* zbuf = smem + EPI_OFF_ZERO;
+    const int row_bytes = H * 2, zbytes = min(row_bytes, EPI_ZERO_BYTES);
     for (int i = lane * 16; i < zbytes; i += 512) *reinterpret_cast<uint4*>(zbuf + i) = make_uint4(0u, 0u, 0u, 0u);
     fence_proxy_async_smem();
     __syncwarp();
@@ -624,8 +689,8 @@ __device__ __forceinline__ void slot_ranks(const FmParams& p, uint8_t* smem, int
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int E = p.E, k = p.k;
     const int16_t* sel_e = reinterpret_cast<const int16_t*>(smem + G_OFF_SEL);
-    int* rank_s = reinterpret_cast<int*>(smem + G_OFF_SEL + G_SEL_MAX * 2);
-    int* cnt_s = reinterpret_cast<int*>(smem + G_OFF_BASE);
+    int* rank_s = reinterpret_cast<int*>(smem + G_OFF_RANK);
+    int* cnt_s = reinterpret_cast<int*>(smem + G_OFF_CNT);
     for (int e = tid; e < E; e += NUM_THREADS) cnt_s[e] = 0;
     __syncthreads();
     const int n_ent = n_tok * k;
@@ -652,7 +717,7 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, u
     float* logit_s = reinterpret_cast<float*>(smem + G_OFF_LOGIT);
     int16_t* sel_e = reinterpret_cast<int16_t*>(smem + G_OFF_SEL);
 
-    float* aux_s = reinterpret_cast<float*>(smem + G_OFF_BASE + 8192);   // training: this chunk's sum_t p[t,e]
+    float* aux_s = reinterpret_cast<float*>(smem + G_OFF_COLSUM);   // training: this chunk's sum_t p[t,e]
     if (p.aux != nullptr)
         for (int e = tid; e < E; e += NUM_THREADS) aux_s[e] = 0.0f;   // ordered by the block syncs of the first stage below
 
@@ -699,11 +764,11 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, u
     // slot ranks, the grid barrier and the prefix pass instead of after them.
     if (tid == 32 && n_tok > 0) {   // (warp 1: warp 0 is about to compute the slot ranks)
         const int row_bytes = H * 2;
-        const int rows0 = max(1, min(n_tok, G_XROWS_BYTES / row_bytes));
-        uint64_t* xbar = reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_XROWS;
+        const int rows0 = max(1, min(n_tok, D_XROWS_BYTES / row_bytes));
+        uint64_t* xbar = bar(smem, BAR_XROWS);
         fence_proxy_async_smem();
         mbar_arrive_expect_tx(xbar, (uint32_t)(rows0 * row_bytes));
-        bulk_load_1d(smem, p.x + (size_t)t0 * H, (uint32_t)(rows0 * row_bytes), xbar);
+        bulk_load_1d(smem + D_OFF_XROWS, p.x + (size_t)t0 * H, (uint32_t)(rows0 * row_bytes), xbar);
     }
     if (p.aux != nullptr && L.S > 0) {   // gML[e] += (sum over this chunk) / S   (gate.cuh:628-634: atomicAdd(gML + e, colAgg / S))
         float* gml = p.aux + (size_t)(L.epoch & 1u) * (2 * E + 1);
@@ -724,83 +789,67 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, u
 // row blocks are complete, not when the slowest CTA of the source rank has finished.
 // Runs on warps 2, 4-11 only (see the kernel body).
 // ============================================================================================================
-constexpr int DISP_THREADS = 288;   // warps 2, 4..11; warps 0, 1, 3 are already in their FFN roles (producer / MMA / scheduler)
-__device__ __forceinline__ void disp_sync() { asm volatile("bar.sync 2, 288;" ::: "memory"); }
-
-__device__ __forceinline__ void dispatch_phase(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int EC = L.EC;
-    const int tid = (warp == 2 ? 0 : (warp - 3) * 32) + lane;   // 0..287 within the dispatch subset
-    const int E = p.E, H = p.H, k = p.k, G = gridDim.x;
-    const int16_t* sel_e = reinterpret_cast<const int16_t*>(smem + G_OFF_SEL);
-    const int* rank_s = reinterpret_cast<const int*>(smem + G_OFF_SEL + G_SEL_MAX * 2);
-    int* base_s = reinterpret_cast<int*>(smem + G_OFF_BASE);        // selections of e by lower chunks
-    int* total_s = base_s + 1024;                                    // selections of e by all chunks
-    int* own_s = base_s + 2048;                                      // selections of e by this chunk
-
-    // one pass over chunk_counts [G, E] gives the prefix (lower chunks), this chunk's own counts and the totals
-    for (int e = tid; e < E; e += DISP_THREADS) { base_s[e] = 0; total_s[e] = 0; }
-    disp_sync();
-    const int E4 = E >> 2;
-    if ((E & 3) == 0 && E4 <= DISP_THREADS && (DISP_THREADS % E4) == 0) {
-        // 16-byte loads, four experts at a time; a thread always meets the same four (DISP_THREADS is a multiple of E / 4),
-        // so it sums in registers and touches shared memory once.  (E = 128: 2 batches of loads instead of 9.)
-        const int nb4 = (int)blockIdx.x * E4, n4 = G * E4;
-        int pt[4] = {0, 0, 0, 0}, pb[4] = {0, 0, 0, 0};
-        for (int i0 = tid; i0 < n4; i0 += 8 * DISP_THREADS) {
-            int4 v[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-                const int i = i0 + u * DISP_THREADS;
-                v[u] = i < n4 ? ld_global_cg_i4(reinterpret_cast<const int4*>(p.chunk_counts) + i) : make_int4(0, 0, 0, 0);
-            }
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-                const int i = i0 + u * DISP_THREADS;
-                if (i >= n4) break;
-                if (i >= nb4 && i < nb4 + E4) *reinterpret_cast<int4*>(own_s + 4 * (i - nb4)) = v[u];
-                pt[0] += v[u].x; pt[1] += v[u].y; pt[2] += v[u].z; pt[3] += v[u].w;
-                if (i < nb4) { pb[0] += v[u].x; pb[1] += v[u].y; pb[2] += v[u].z; pb[3] += v[u].w; }
-            }
-        }
-        if (tid < n4) {
-            const int e0 = 4 * (tid % E4);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                if (pt[q] != 0) atomicAdd(&total_s[e0 + q], pt[q]);
-                if (pb[q] != 0) atomicAdd(&base_s[e0 + q], pb[q]);
-            }
-        }
-    } else {
-        const int nb = (int)blockIdx.x * E, n = G * E;
-        const bool fixed_e = (E <= DISP_THREADS) && (DISP_THREADS % E) == 0;   // then a thread always meets one e
-        int part_b = 0, part_t = 0, cur_e = -1;
-        for (int i0 = tid; i0 < n; i0 += 8 * DISP_THREADS) {
-            int v[8];
+// The prefix over chunk_counts [G, E]: base (selections of e by lower chunks), total (by all chunks) and own (by this
+// chunk).  Experts go in column groups of V: four with 16-byte loads when E % 4 == 0, else one.  With ncol = E / V groups
+// and ncol <= DISP_THREADS, R = DISP_THREADS / ncol threads share a group and stride over the rows by R; with more groups
+// thread tid owns groups tid, tid + DISP_THREADS, ...  Sums stay in registers and a thread adds each of its groups into
+// total and base once.  These are integer sums: every order gives the same bits.
+template <int V>
+__device__ __forceinline__ void expert_prefix_cols(const FmParams& p, int tid, int* base_s, int* total_s, int* own_s) {
+    const int G = gridDim.x, ncol = p.E / V;
+    const int R = max(1, DISP_THREADS / ncol);
+    if (tid >= R * ncol) return;
+    // group (row r, column group c) is element r * ncol + c of chunk_counts viewed in groups of V
+    const int n = G * ncol, mine = (int)blockIdx.x * ncol, step = R * ncol;
+    for (int c = tid % ncol; c < ncol; c += DISP_THREADS) {
+        int pt[V] = {}, pb[V] = {};
+        for (int i0 = tid / ncol * ncol + c; i0 < n; i0 += 8 * step) {
+            int v[8][V];
 #pragma unroll
             for (int u = 0; u < 8; ++u) {   // all loads of the batch are in flight before the first use
-                const int i = i0 + u * DISP_THREADS;
-                v[u] = i < n ? p.chunk_counts[i] : 0;
+                const int i = i0 + u * step;
+                if constexpr (V == 4) {
+                    const int4 q = i < n ? ld_global_cg_i4(reinterpret_cast<const int4*>(p.chunk_counts) + i) : make_int4(0, 0, 0, 0);
+                    v[u][0] = q.x; v[u][1] = q.y; v[u][2] = q.z; v[u][3] = q.w;
+                } else {
+                    v[u][0] = i < n ? p.chunk_counts[i] : 0;
+                }
             }
 #pragma unroll
             for (int u = 0; u < 8; ++u) {
-                const int i = i0 + u * DISP_THREADS;
+                const int i = i0 + u * step;
                 if (i >= n) break;
-                const int e = i % E;
-                if (i >= nb && i < nb + E) own_s[e] = v[u];
-                if (fixed_e) { part_t += v[u]; if (i < nb) part_b += v[u]; cur_e = e; }
-                else if (v[u] != 0) { atomicAdd(&total_s[e], v[u]); if (i < nb) atomicAdd(&base_s[e], v[u]); }
+                if (i == mine + c) {
+                    if constexpr (V == 4) *reinterpret_cast<int4*>(own_s + 4 * c) = make_int4(v[u][0], v[u][1], v[u][2], v[u][3]);
+                    else own_s[c] = v[u][0];
+                }
+#pragma unroll
+                for (int q = 0; q < V; ++q) {
+                    pt[q] += v[u][q];
+                    if (i < mine) pb[q] += v[u][q];
+                }
             }
         }
-        if (cur_e >= 0) {
-            if (part_t != 0) atomicAdd(&total_s[cur_e], part_t);
-            if (part_b != 0) atomicAdd(&base_s[cur_e], part_b);
+#pragma unroll
+        for (int q = 0; q < V; ++q) {
+            if (pt[q] != 0) atomicAdd(&total_s[c * V + q], pt[q]);
+            if (pb[q] != 0) atomicAdd(&base_s[c * V + q], pb[q]);
         }
     }
-    disp_sync();
-    if (tid == 0) trace_stamp(p, 8);
-    // the count of packet (me, e) is known: CTA (e mod G) tells the owner now.  Nothing precedes this word that the
-    // reader depends on (the rows are acknowledged through recv_rows), so a relaxed system-scope store is enough.
+}
+
+__device__ __forceinline__ void expert_prefix(const FmParams& p, int tid, int* base_s, int* total_s, int* own_s) {
+    for (int e = tid; e < p.E; e += DISP_THREADS) { base_s[e] = 0; total_s[e] = 0; }
+    named_sync<NAMED_BAR_PREFIX, DISP_THREADS>();
+    if (p.E % 4 == 0) expert_prefix_cols<4>(p, tid, base_s, total_s, own_s);
+    else expert_prefix_cols<1>(p, tid, base_s, total_s, own_s);
+    named_sync<NAMED_BAR_PREFIX, DISP_THREADS>();
+}
+
+// The count of packet (me, e) is known: CTA (e mod G) tells the owner now.  Nothing precedes this word that the reader
+// depends on (the rows are acknowledged through recv_rows), so a relaxed system-scope store is enough.
+__device__ __forceinline__ void publish_counts(const FmParams& p, const Launch& L, int tid, const int* total_s) {
+    const int E = p.E, G = gridDim.x, EC = L.EC;
     for (int e = (int)blockIdx.x + tid * G; e < E; e += DISP_THREADS * G) {
         const int tot = total_s[e];
         p.counts[e] = tot;
@@ -820,100 +869,109 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, const Launch& 
             atomicAdd(a + 2 * E, __fdividef(me * ce, (float)E));
         }
     }
-    const unsigned int par = L.epoch & 1u;
-    // Row copies.
-    //   * Rows for experts on THIS rank (warps 4-11): the chunk's token rows are contiguous in x, so one bulk load stages up
-    //     to 128 KiB of them in shared memory (the first group was requested at the end of the router) and every kept
-    //     (token, pick) pair is one cp.async.bulk store of a whole row through the TMA engine (no per-lane chains).  They
-    //     land in ~4 us and are acknowledged at once (gpu-scope release); the stage area is handed to the TMA producer, the
-    //     warps become epilogue warps, and the expert FFN starts on the local packets while
-    //   * rows for experts on OTHER ranks (warp 2, from the moment the slots are known) cross NVLink as 16-byte peer stores
-    //     read straight from x (L2 hits), sixteen pieces per lane in flight.  The link bounds them (S*k*(1-1/W)*H*2 bytes
-    //     at ~770 GB/s) and back-pressures the issuing warp -- which has no other duty until the first tile needs
-    //     publishing; it then waits for the stores with a system-scope release and acknowledges them.
-    uint64_t* xbar = reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_XROWS;   // initialised in the kernel prologue
-    uint8_t* x_s = smem;   // the router's Wg / logits scratch is free now
+}
+
+// This chunk's rows of expert e occupy slots [lo, hi) of packet (me, e): add the rows landed per 128-row block to the
+// owner's arrival counters of epoch parity `par`.  The release covers every store of the threads that met at the
+// preceding barrier.
+__device__ __forceinline__ void ack_rows(const FmParams& p, unsigned int par, int e, int lo, int hi, bool local) {
+    if (hi <= lo) return;
+    const int owner = e / p.nLx, le = e - owner * p.nLx;
+    unsigned int* ctr = p.peer_recv_rows[owner] + ((size_t)par * p.num_pkts + (size_t)(p.rank * p.nLx + le)) * p.TCM;
+    for (int b = lo / BLOCK_M; b <= (hi - 1) / BLOCK_M; ++b) {
+        const int n = min(hi, (b + 1) * BLOCK_M) - max(lo, b * BLOCK_M);
+        if (local) red_release_gpu_add_u32(ctr + b, (unsigned int)n);
+        else red_release_sys_add_u32(ctr + b, (unsigned int)n);
+    }
+}
+
+// Up to RANGES_IN_REGS experts, warp 2 keeps the slot ranges of the remote ones in registers (RMAX per lane) and gives
+// the prefix arrays up before its row stream; beyond that it needs them until its acknowledgements.
+constexpr int RMAX = 8;
+constexpr int RANGES_IN_REGS = 32 * RMAX;
+
+// Warps 4-11: every (token, pick) pair's slot and routing record, and the rows for experts on this rank.
+__device__ __forceinline__ void dispatch_local_rows(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok,
+                                                    const int* base_s, const int* own_s) {
+    const int ltid = threadIdx.x - EPI_WARP0 * 32;
+    const int E = p.E, H = p.H, k = p.k, EC = L.EC;
+    const int16_t* sel_e = reinterpret_cast<const int16_t*>(smem + G_OFF_SEL);
+    const int* rank_s = reinterpret_cast<const int*>(smem + G_OFF_RANK);
+    uint64_t* xbar = bar(smem, BAR_XROWS);   // initialised in the kernel prologue
+    uint8_t* x_s = smem + D_OFF_XROWS;       // the router's Wg / logits scratch is free now
     const int row_bytes = H * 2;
-    const int rows_per_group = max(1, min(n_tok, G_XROWS_BYTES / row_bytes));
+    const int rows_per_group = max(1, min(n_tok, D_XROWS_BYTES / row_bytes));
     const bool any_remote = p.W > 1;
     const int first_local = p.rank * p.nLx;
-    auto ack = [&](int e, int lo, int hi, bool local) {
-        // this chunk's rows of expert e occupy slots [lo, hi) of packet (me, e): add the rows landed per 128-row block.
-        // The release covers every store of the threads that met at the preceding barrier.
-        if (hi <= lo) return;
-        const int owner = e / p.nLx, le = e - owner * p.nLx;
-        unsigned int* ctr = p.peer_recv_rows[owner] + ((size_t)par * p.num_pkts + (size_t)(p.rank * p.nLx + le)) * p.TCM;
-        for (int b = lo / BLOCK_M; b <= (hi - 1) / BLOCK_M; ++b) {
-            const int n = min(hi, (b + 1) * BLOCK_M) - max(lo, b * BLOCK_M);
-            if (local) red_release_gpu_add_u32(ctr + b, (unsigned int)n);
-            else red_release_sys_add_u32(ctr + b, (unsigned int)n);
+    uint32_t xphase = 0;
+    for (int g0 = 0; g0 < n_tok; g0 += rows_per_group) {
+        const int rows = min(rows_per_group, n_tok - g0);
+        if (ltid == 0 && g0 > 0) {   // group 0 was requested at the end of the router (gate_phase)
+            mbar_arrive_expect_tx(xbar, (uint32_t)(rows * row_bytes));
+            bulk_load_1d(x_s, p.x + (size_t)(t0 + g0) * H, (uint32_t)(rows * row_bytes), xbar);
         }
-    };
-    constexpr int LOCAL_THREADS = DISP_THREADS - 32;   // warps 4..11
-    if (warp != 2) {
-        // ---------------------------------------------------------------- warps 4-11: slots, routing records, local rows
-        const int ltid = tid - 32;
-        uint32_t xphase = 0;
-        for (int g0 = 0; g0 < n_tok; g0 += rows_per_group) {
-            const int rows = min(rows_per_group, n_tok - g0);
-            if (ltid == 0 && g0 > 0) {   // group 0 was requested at the end of the router (gate_phase)
-                mbar_arrive_expect_tx(xbar, (uint32_t)(rows * row_bytes));
-                bulk_load_1d(x_s, p.x + (size_t)(t0 + g0) * H, (uint32_t)(rows * row_bytes), xbar);
-            }
-            mbar_wait(xbar, xphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 900);
-            xphase ^= 1;
-            for (int i = ltid; i < rows * k; i += LOCAL_THREADS) {   // one thread per (token, pick)
-                const int tl = i / k, j = i - tl * k;
-                const int ti = g0 + tl, t = t0 + ti;
-                const int e = sel_e[ti * k + j];
-                const int s = base_s[e] + rank_s[ti * k + j];
-                p.slot[(size_t)t * k + j] = s;
-                if (s < EC) {
-                    const int owner = e / p.nLx, le = e - owner * p.nLx;
-                    const size_t row = (size_t)(p.rank * p.nLx + le) * p.pEC + s;
-                    if (p.fused) {   // what the expert's GEMM1 epilogue needs to combine this row
-                        uint4 m;
-                        m.x = (unsigned int)t;
-                        m.y = __float_as_uint(__bfloat162float(p.topk_w[(size_t)t * k + j]));
-                        m.z = __float_as_uint(p.mcw[t]);
-                        m.w = 0u;
-                        st_global_v4(p.peer_recv_meta[owner] + row, m);
-                    }
-                    if (owner == p.rank)
-                        bulk_store_1d(p.recv_x + row * H, x_s + (size_t)tl * row_bytes, (uint32_t)row_bytes);
+        mbar_wait(xbar, xphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 900);
+        xphase ^= 1;
+        for (int i = ltid; i < rows * k; i += EPI_THREADS) {   // one thread per (token, pick)
+            const int tl = i / k, j = i - tl * k;
+            const int ti = g0 + tl, t = t0 + ti;
+            const int e = sel_e[ti * k + j];
+            const int s = base_s[e] + rank_s[ti * k + j];
+            p.slot[(size_t)t * k + j] = s;
+            if (s < EC) {
+                const int owner = e / p.nLx, le = e - owner * p.nLx;
+                const size_t row = (size_t)(p.rank * p.nLx + le) * p.pEC + s;
+                if (p.fused) {   // what the expert's GEMM1 epilogue needs to combine this row
+                    uint4 m;
+                    m.x = (unsigned int)t;
+                    m.y = __float_as_uint(__bfloat162float(p.topk_w[(size_t)t * k + j]));
+                    m.z = __float_as_uint(p.mcw[t]);
+                    m.w = 0u;
+                    st_global_v4(p.peer_recv_meta[owner] + row, m);
                 }
-            }
-            bulk_commit_group();
-            if (g0 + rows_per_group < n_tok) {   // the staging buffer is reused: wait until the bulk stores have read it
-                bulk_wait_group_read0();
-                asm volatile("bar.sync 4, 256;" ::: "memory");
+                if (owner == p.rank)
+                    bulk_store_1d(p.recv_x + row * H, x_s + (size_t)tl * row_bytes, (uint32_t)row_bytes);
             }
         }
-        // (the zero-fill stores, an older bulk group of warp 11, read the first 8 KiB of the epilogue staging area, which
-        // is warp 2's window: they must have been read before warp 2 starts -- all but the newest group, the row stores)
-        asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        if (any_remote) asm volatile("bar.arrive 3, 288;" ::: "memory");   // every slot (p.slot) is written: warp 2 may start
-        bulk_wait_group0();        // this thread's local row stores (and warp 11's zero-fill stores) are complete ...
-        fence_proxy_async_all();   // ... and ordered (async proxy) before the generic-proxy counter traffic below
-        asm volatile("bar.sync 4, 256;" ::: "memory");
-        if (any_remote) asm volatile("bar.arrive 6, 288;" ::: "memory");   // local rows + zero-fill complete (warp 2's acks wait for this)
-        if (ltid == 0) trace_stamp(p, 9);
-        if (any_remote) asm volatile("bar.sync 5, 288;" ::: "memory");   // warp 2 has taken what it needs from the stage area
-        if (ltid < 32) {   // warp 4: acknowledge the local experts, then hand the stage area to the TMA producer
-            for (int e = first_local + ltid; e < first_local + p.nLx; e += 32) ack(e, base_s[e], min(base_s[e] + own_s[e], EC), true);
-            __syncwarp();
-            // (more than 256 experts on several ranks: warp 2 still needs base / own for its acknowledgements and releases)
-            if (ltid == 0 && (!any_remote || E <= 256)) mbar_arrive(reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_DISP_DONE);
+        bulk_commit_group();
+        if (g0 + rows_per_group < n_tok) {   // the staging buffer is reused: wait until the bulk stores have read it
+            bulk_wait_group_read0();
+            named_sync<NAMED_BAR_LOCAL, EPI_THREADS>();
         }
-        return;
     }
-    // -------------------------------------------------------------------- warp 2
-    if (!any_remote) return;
-    // the slot ranges of the remote experts go into registers (E <= 256) before the stage area -- where base / own live --
-    // is released by warp 4; beyond that the release waits for this warp
-    constexpr int RMAX = 8;
+    // (the zero-fill stores, an older bulk group of warp 11, read the first 8 KiB of the epilogue staging area, which
+    // is warp 2's window: they must have been read before warp 2 starts -- all but the newest group, the row stores)
+    bulk_wait_group_read<1>();
+    if (any_remote) named_arrive<NAMED_BAR_SLOTS, DISP_THREADS>();   // every slot (p.slot) is written: warp 2 may start
+    bulk_wait_group0();        // this thread's local row stores (and warp 11's zero-fill stores) are complete ...
+    fence_proxy_async_all();   // ... and ordered (async proxy) before the generic-proxy counter traffic below
+    named_sync<NAMED_BAR_LOCAL, EPI_THREADS>();
+    if (any_remote) named_arrive<NAMED_BAR_LOCAL_DONE, DISP_THREADS>();   // local rows + zero-fill complete (warp 2's acks wait for this)
+    if (ltid == 0) trace_stamp(p, 9);
+    if (any_remote) named_sync<NAMED_BAR_PREFIX_READ, DISP_THREADS>();   // warp 2 has taken what it needs from the stage area
+    if (ltid < 32) {   // warp 4: acknowledge the local experts, then hand the stage area to the TMA producer
+        const unsigned int par = L.epoch & 1u;
+        for (int e = first_local + ltid; e < first_local + p.nLx; e += 32)
+            ack_rows(p, par, e, base_s[e], min(base_s[e] + own_s[e], EC), true);
+        __syncwarp();
+        // (more than RANGES_IN_REGS experts on several ranks: warp 2 still needs base / own for its acknowledgements and
+        // releases)
+        if (ltid == 0 && (!any_remote || E <= RANGES_IN_REGS)) mbar_arrive(bar(smem, BAR_DISP_DONE));
+    }
+}
+
+// Warp 2, several ranks: the rows for experts on other ranks.
+__device__ __forceinline__ void dispatch_remote_rows(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok,
+                                                     const int* base_s, const int* own_s) {
+    const int lane = threadIdx.x & 31;
+    const int E = p.E, H = p.H, k = p.k, EC = L.EC;
+    const int row_bytes = H * 2;
+    const int first_local = p.rank * p.nLx;
+    const unsigned int par = L.epoch & 1u;
+    // the slot ranges of the remote experts go into registers (E <= RANGES_IN_REGS) before the stage area -- where base /
+    // own live -- is released by warp 4; beyond that the release waits for this warp
     int rlo[RMAX], rhi[RMAX];
-    const bool in_regs = E <= 32 * RMAX;
+    const bool in_regs = E <= RANGES_IN_REGS;
 #pragma unroll
     for (int i = 0; i < RMAX; ++i) {
         const int e = lane + 32 * i;
@@ -922,18 +980,18 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, const Launch& 
         rhi[i] = remote ? min(base_s[e] + own_s[e], EC) : 0;
     }
     __syncwarp();
-    if (in_regs) asm volatile("bar.arrive 5, 288;" ::: "memory");   // done with the stage area
-    asm volatile("bar.sync 3, 288;" ::: "memory");                  // every slot of this chunk (p.slot) is written
+    if (in_regs) named_arrive<NAMED_BAR_PREFIX_READ, DISP_THREADS>();   // done with the stage area
+    named_sync<NAMED_BAR_SLOTS, DISP_THREADS>();                        // every slot of this chunk (p.slot) is written
     {
         // Remote rows through the TMA engine (SM-issued peer stores reached only ~400 GB/s over NVLink, bulk stores ~600):
         // a window of the epilogue staging area -- unused until this CTA's first tile is complete; its first 8 KiB hold the
         // zero source of the output zero-fill -- is filled with a run of consecutive token rows of x (one bulk load), every
         // kept (token, pick) pair of those tokens that belongs to another rank is one bulk store of a whole row to that
         // rank's receive buffer, and when the engine has read the window the next run follows.  The link paces the stores.
-        uint8_t* win = smem + OFF_EPI + 8192;
-        const int win_bytes = EPI_BYTES - 8192;
+        uint8_t* win = smem + D_OFF_WIN;
+        const int win_bytes = D_WIN_BYTES;
         const int rows_win = max(1, win_bytes / row_bytes);
-        uint64_t* rbar = reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_REMOTE;
+        uint64_t* rbar = bar(smem, BAR_REMOTE);
         uint32_t rphase = 0;
         const bool fits = row_bytes <= win_bytes;   // (d_model > 12288: rows go piecewise, below)
         for (int tw = 0; tw < n_tok; tw += rows_win) {
@@ -994,24 +1052,47 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, const Launch& 
                 }
             }
         }
-        asm volatile("bar.arrive 7, 288;" ::: "memory");   // the staging area belongs to the epilogue warps from here
+        named_arrive<NAMED_BAR_WINDOW, DISP_THREADS>();   // the staging area belongs to the epilogue warps from here
         bulk_wait_group0();        // the rows have arrived on the other ranks ...
         fence_proxy_async_all();   // ... and are ordered before the generic-proxy acknowledgements
     }
     __syncwarp();
     // the remote acknowledgements also tell the peers that this chunk's output rows are zeroed (TMA stores issued by warp 11
     // in the router, completed before it arrives here) and that the routing records are written
-    asm volatile("bar.sync 6, 288;" ::: "memory");
+    named_sync<NAMED_BAR_LOCAL_DONE, DISP_THREADS>();
     if (in_regs) {
 #pragma unroll
-        for (int i = 0; i < RMAX; ++i) ack(lane + 32 * i, rlo[i], rhi[i], false);
+        for (int i = 0; i < RMAX; ++i) ack_rows(p, par, lane + 32 * i, rlo[i], rhi[i], false);
     } else {
         for (int e = lane; e < E; e += 32)
-            if (e < first_local || e >= first_local + p.nLx) ack(e, base_s[e], min(base_s[e] + own_s[e], EC), false);
+            if (e < first_local || e >= first_local + p.nLx) ack_rows(p, par, e, base_s[e], min(base_s[e] + own_s[e], EC), false);
         __syncwarp();
-        asm volatile("bar.arrive 5, 288;" ::: "memory");
-        if (lane == 0) mbar_arrive(reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_DISP_DONE);
+        named_arrive<NAMED_BAR_PREFIX_READ, DISP_THREADS>();
+        if (lane == 0) mbar_arrive(bar(smem, BAR_DISP_DONE));
     }
+}
+
+__device__ __forceinline__ void dispatch_phase(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int tid = (warp == 2 ? 0 : (warp - 3) * 32) + lane;   // 0..287 within the dispatch subset
+    int* base_s = reinterpret_cast<int*>(smem + D_OFF_BASE);
+    int* total_s = reinterpret_cast<int*>(smem + D_OFF_TOTAL);
+    int* own_s = reinterpret_cast<int*>(smem + D_OFF_OWN);
+    expert_prefix(p, tid, base_s, total_s, own_s);
+    if (tid == 0) trace_stamp(p, 8);
+    publish_counts(p, L, tid, total_s);
+    // Row copies.
+    //   * Rows for experts on THIS rank (warps 4-11): the chunk's token rows are contiguous in x, so one bulk load stages up
+    //     to 128 KiB of them in shared memory (the first group was requested at the end of the router) and every kept
+    //     (token, pick) pair is one cp.async.bulk store of a whole row through the TMA engine (no per-lane chains).  They
+    //     land in ~4 us and are acknowledged at once (gpu-scope release); the stage area is handed to the TMA producer, the
+    //     warps become epilogue warps, and the expert FFN starts on the local packets while
+    //   * rows for experts on OTHER ranks (warp 2, from the moment the slots are known) cross NVLink as 16-byte peer stores
+    //     read straight from x (L2 hits), sixteen pieces per lane in flight.  The link bounds them (S*k*(1-1/W)*H*2 bytes
+    //     at ~770 GB/s) and back-pressures the issuing warp -- which has no other duty until the first tile needs
+    //     publishing; it then waits for the stores with a system-scope release and acknowledges them.
+    if (warp != 2) dispatch_local_rows(p, L, smem, t0, n_tok, base_s, own_s);
+    else if (p.W > 1) dispatch_remote_rows(p, L, smem, t0, n_tok, base_s, own_s);
 }
 
 // ============================================================================================================
@@ -1379,7 +1460,7 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, u
         if (ntiles < 16 && stamper) trace_stamp(p, 48 + ntiles);
 
         if (ntiles == 0 && p.W > 1)   // the staging area served as warp 2's window for the remote rows
-            asm volatile("bar.sync 7, 288;" ::: "memory");
+            named_sync<NAMED_BAR_WINDOW, DISP_THREADS>();
         if (lane == 0) mbar_arrive(&sched_empty[q]);   // every lane has read the slot (the __syncwarp above)
         if (++q == NSCHED) { q = 0; qphase ^= 1; }
         if (ntiles < 16 && stamper) trace_stamp(p, 64 + ntiles);
@@ -1736,10 +1817,10 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, const Launch& L
     const int H = p.H, k = p.k, EC = L.EC;
     // the pipeline stage area is free again: stage this chunk's routing records, and let one thread per (token, pick)
     // poll its return flag so the waits overlap instead of chaining per token
-    int* c_e = reinterpret_cast<int*>(smem);
-    int* c_s = c_e + G_SEL_MAX;
-    float* c_w = reinterpret_cast<float*>(c_s + G_SEL_MAX);
-    float* c_m = c_w + G_SEL_MAX;
+    int* c_e = reinterpret_cast<int*>(smem + C_OFF_E);
+    int* c_s = reinterpret_cast<int*>(smem + C_OFF_S);
+    float* c_w = reinterpret_cast<float*>(smem + C_OFF_W);
+    float* c_m = reinterpret_cast<float*>(smem + C_OFF_M);
     const int n = n_tok * k;
     for (int i = tid; i < n; i += NUM_THREADS) {
         const size_t gi = (size_t)t0 * k + i;
@@ -1825,7 +1906,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
     if (disp_warp) {
         if (!p.dense) dispatch_phase(p, L, smem, t0, n_tok);
         else if (warp == 2 && (tid & 31) == 0)   // nothing to copy: GEMM0's TMA reads x in place; release the producer
-            mbar_arrive(reinterpret_cast<uint64_t*>(smem + OFF_BARS) + BAR_DISP_DONE);
+            mbar_arrive(bar(smem, BAR_DISP_DONE));
         if (warp == 2 && (tid & 31) == 0) trace_stamp(p, 3);
     }
     if (tid == EPI_WARP0 * 32) trace_stamp(p, 4);

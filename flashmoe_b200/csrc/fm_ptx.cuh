@@ -120,6 +120,19 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, DebugR
     while (!mbar_try_wait(bar, parity)) g.tick(dbg, timeout_ns, code, info, parity, 0);
 }
 
+// named CTA barriers (id 0 is __syncthreads): the N threads that take part, whole warps, either wait (sync) or only
+// signal (arrive); id and count are immediates
+template <int ID, int N>
+__device__ __forceinline__ void named_sync() {
+    static_assert(ID > 0 && ID < 16 && N % 32 == 0, "named barrier id 1-15, whole warps");
+    asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(N) : "memory");
+}
+template <int ID, int N>
+__device__ __forceinline__ void named_arrive() {
+    static_assert(ID > 0 && ID < 16 && N % 32 == 0, "named barrier id 1-15, whole warps");
+    asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(N) : "memory");
+}
+
 // ----------------------------------------------------------------------------------------------------------------
 // proxy / memory fences
 // ----------------------------------------------------------------------------------------------------------------
