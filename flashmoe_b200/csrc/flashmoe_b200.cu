@@ -240,12 +240,20 @@ int check_kernel_status(fm_ctx* c) {
         memset(c->dbg_host, 0, sizeof(fm::DebugRecord));
         return fail(FM_EINVAL, "device token count n_tokens = %d not in [0, S = %d]: that launch ran on 0 tokens", n, S);
     }
+    if (c->dbg_host != nullptr && c->dbg_host->code == fm::FM_TRAP_MBAR) {
+        const fm::DebugRecord r = *c->dbg_host;
+        const fm::MbarName b = fm::mbar_name((int)r.info0);
+        return fail(FM_EKERNEL,
+                    "kernel wait timed out on mbarrier %s[%d], parity %u (block %u, warp %u): waited %.1f ms (rank %d, "
+                    "launch %llu)",
+                    b.group != nullptr ? b.group : "unknown", b.index, r.info1, r.block, r.thread / 32,
+                    (double)r.waited_ns * 1e-6, c->d.rank, (unsigned long long)c->launches);
+    }
     if (c->dbg_host != nullptr && c->dbg_host->code != 0) {
-        static const char* names[] = {"none", "smem-full mbarrier", "smem-empty mbarrier", "(unused)",
-                                      "(unused)", "sched-full mbarrier", "sched-empty mbarrier",
+        static const char* names[] = {"none", "mbarrier", "(unused)", "(unused)", "(unused)", "(unused)", "(unused)",
                                       "grid barrier", "dispatch flag (packet never arrived)", "GEMM0 row-block counter",
                                       "return flag (expert output never arrived)",
-                                      "dispatch row acknowledgement (rows of a packet never arrived)", "publisher mbarrier"};
+                                      "dispatch row acknowledgement (rows of a packet never arrived)"};
         const fm::DebugRecord r = *c->dbg_host;
         const char* nm = r.code < sizeof(names) / sizeof(names[0]) ? names[r.code] : "unknown";
         return fail(FM_EKERNEL,

@@ -29,6 +29,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/flashmoe_b200.h"
 #include "fm_ptx.cuh"
 
@@ -44,11 +46,38 @@ constexpr int NUM_THREADS = 384;
 constexpr int NUM_WARPS = NUM_THREADS / 32;
 constexpr int EPI_WARP0 = 4;   // warps 4..11: warpgroup (warp - 4) / 4 owns tile rows [64g, 64g + 64), warp % 4 its 16-row slice
 constexpr int NUM_EPI_WARPS = 8;
-constexpr int TRACE_SLOTS = 128; // per CTA: [0..6] phase stamps, [8..14] sub-phase stamps (13 = first tile of a remote packet
-                                 // ready, 14 = all done flags seen); per tile i < 16 of this CTA:
-                                 // [16+i] dependencies resolved (scheduler), [32+i] first k-block landed, [48+i] last MMA
-                                 // complete (consumers), [64+i] epilogue started, [80+i] epilogue stores issued,
-                                 // [96+i] published, [112+i] claimed (scheduler)
+
+// Trace stamps (%globaltimer, FmParams::trace): TRACE_SLOTS per CTA, phase slots 0-15, then per-tile slots base + i for
+// the first TRACE_TILES tiles of the CTA.  scripts/trace_gantt.py and scripts/trace_multi.py read them through
+// flashmoe_b200/trace_slots.py, which keeps the same names (tests/test_trace_slots.py checks that the two agree).
+constexpr int TRACE_SLOTS = 128;
+constexpr int TRACE_TILES = 16;
+enum TraceSlot : int {
+    TRACE_START = 0,             // kernel entry
+    TRACE_GATE_DONE = 1,         // router done, before the grid barrier
+    TRACE_BARRIER = 2,           // past the grid barrier
+    TRACE_DISPATCH_END = 3,      // warp 2 done with dispatch
+    TRACE_FFN_START = 4,         // warp 4 enters the expert FFN
+    TRACE_FFN_END = 5,           // every FFN role done
+    TRACE_KERNEL_END = 6,
+    TRACE_FIRST_TMA = 7,         // producer: first loads of the first tile issued
+    TRACE_DISP_PREFIX = 8,       // dispatch: prefix over the chunk counts done
+    TRACE_DISP_ROWS_DONE = 9,    // dispatch: local rows and the zero-fill complete (warp 4)
+    TRACE_ZERO_ISSUED = 10,      // router: output-row zero-fill issued (warp 11)
+    TRACE_GATE_LOGITS = 11,      // router: a sub-chunk's logits done
+    TRACE_GATE_TOPK = 12,        // router: every sub-chunk's softmax / top-k done
+    TRACE_FIRST_REMOTE = 13,     // scheduler: first tile of a packet from another rank ready
+    TRACE_DONE_FLAGS = 14,       // fused completion: every expert's done flag seen
+    TRACE_TOPK_WARP0 = 15,       // router: warp 0's softmax / top-k of a sub-chunk done
+    TRACE_TILE_READY = 16,       // scheduler: the tile's dependencies resolved
+    TRACE_TILE_FIRST_KB = 32,    // consumers: first k-block landed
+    TRACE_TILE_MMA_DONE = 48,    // consumers: last MMA complete
+    TRACE_TILE_EPI_START = 64,   // consumers: epilogue started
+    TRACE_TILE_STORES = 80,      // consumers: epilogue stores issued (GEMM0: last h chunk handed over)
+    TRACE_TILE_PUBLISHED = 96,   // publisher: tile published
+    TRACE_TILE_CLAIMED = 112,    // scheduler: tile claimed
+};
+static_assert(TRACE_TILE_CLAIMED + TRACE_TILES == TRACE_SLOTS, "per-tile slots fill the buffer");
 
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;                  // 16 KiB
 constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;                  // 32 KiB
@@ -64,30 +93,8 @@ constexpr int EPI_CHUNK_BYTES = BLOCK_M * EPI_ROW_BYTES;              // 16 KiB
 constexpr int EPI_BUFS = 2;
 constexpr int EPI_BYTES = EPI_BUFS * EPI_CHUNK_BYTES;                 // 32 KiB
 constexpr int OFF_EPI = PIPE_BYTES;                                   // 196608 (1 KiB aligned, as SWIZZLE_128B needs)
-constexpr int OFF_BARS = OFF_EPI + EPI_BYTES;                         // 229376
-// barriers: full[4] empty[4] sched_full[4] sched_empty[4] prod_take[4] xrows disp_done pub_full[2] pub_empty[2] wg remote
-//           gfull[8] gempty[8] stg_full[2] stg_free[2]
-constexpr int BAR_FULL = 0, BAR_EMPTY = STAGES;
-constexpr int BAR_SCHED_FULL = 2 * STAGES, BAR_SCHED_EMPTY = BAR_SCHED_FULL + NSCHED;
-constexpr int BAR_PROD_TAKE = BAR_SCHED_EMPTY + NSCHED;
-constexpr int BAR_XROWS = BAR_PROD_TAKE + NSCHED;                     // dispatch phase: bulk row load
-constexpr int BAR_DISP_DONE = BAR_XROWS + 1;                          // this CTA's dispatch no longer uses the stage area
-constexpr int BAR_PUB_FULL = BAR_DISP_DONE + 1;                       // consumer warps -> publisher: tile's stores issued
-constexpr int BAR_PUB_EMPTY = BAR_PUB_FULL + 2;                       // publisher -> consumer warps: slot consumed
-constexpr int BAR_WG = BAR_PUB_EMPTY + 2;                             // router: bulk-staged gate weights
-constexpr int BAR_REMOTE = BAR_WG + 1;                                // dispatch, warp 2: staged rows for other ranks
+constexpr int OFF_BARS = OFF_EPI + EPI_BYTES;                         // 229376: the mbarriers (table below)
 constexpr int GATE_STAGES = 8;                                        // router GEMM on tensor cores: up to 8 smem stages
-constexpr int BAR_GFULL = BAR_REMOTE + 1;                             // full / empty per stage
-constexpr int BAR_GEMPTY = BAR_GFULL + GATE_STAGES;
-constexpr int BAR_STG_FULL = BAR_GEMPTY + GATE_STAGES;                // consumer warps -> publisher: h chunk staged
-constexpr int BAR_STG_FREE = BAR_STG_FULL + EPI_BUFS;                 // publisher -> consumer warps: chunk read by the TMA
-constexpr int NUM_BARS = BAR_STG_FREE + EPI_BUFS;                     // 48
-constexpr int OFF_RING = OFF_BARS + NUM_BARS * 8;                     // 16-byte aligned
-constexpr int OFF_LAUNCH = OFF_RING + NSCHED * 64;                    // this launch's Launch record (below)
-constexpr int SMEM_USED = OFF_LAUNCH + 64;
-constexpr int SMEM_BYTES = SMEM_USED + 1024;                          // + slack for manual 1 KiB alignment
-static_assert(OFF_RING % 16 == 0, "ring entries are 16-byte aligned");
-static_assert(SMEM_BYTES <= 232448, "227 KiB of dynamic shared memory per CTA");
 constexpr int MAX_EXPERTS = 1024;   // validate_config rejects more; sizes the per-expert arrays below
 
 // Shared-memory plan.  Four phases take turns in the stage area [0, PIPE_BYTES) and the epilogue staging area
@@ -142,6 +149,104 @@ static_assert(C_RECORDS_END <= PIPE_BYTES, "combine records within the stage are
 static_assert(D_WIN_BYTES > 0 && EPI_ZERO_BYTES + D_WIN_BYTES <= EPI_BYTES,
               "zero source and remote-row window within the epilogue staging area");
 static_assert(G_OFF_COLSUM + MAX_EXPERTS * (int)sizeof(float) <= D_PREFIX_END, "a column sum per expert");
+
+// mbarriers (mbar_init / mbar_arrive / bar_wait on bar(smem, id)).  FM_MBARRIERS below declares every group once:
+// X(ID, name, first id, count, arrival count); BAR_<ID> is the group's first id, ffn_setup initialises every barrier
+// from it, and the host names a timed-out wait's barrier with mbar_name.  "+ tx": the arrival is an arrive.expect_tx,
+// and the phase also waits for the TMA's bytes.
+//
+//   group       | arrive                                  | wait                          | orders
+//   ------------+-----------------------------------------+-------------------------------+------------------------------
+//   full        | producer (warp 0), + tx                 | consumer warps                | a pipeline stage's A and B
+//               |                                         |                               | tiles landed
+//   empty       | consumer warps, lane 0                  | producer                      | the MMAs have read the stage
+//   sched_full  | scheduler (warp 3)                      | producer, publisher,          | a scheduler-ring slot's
+//               |                                         | consumer warps                | TileInfo written
+//   sched_empty | producer, publisher, consumer warps     | scheduler                     | every reader is done with
+//               |                                         |                               | the slot
+//   prod_take   | producer, CLAIM_AHEAD_KB k-blocks before| scheduler, before it claims   | bounds the scheduler's
+//               | the end of the slot's tile              | the tile after the next       | look-ahead
+//   xrows       | warp 1 (first group), warp 4 (the       | warps 4-11                    | a group of this chunk's x
+//               | others), + tx                           |                               | rows staged
+//   disp_done   | warp 4, or warp 2 (dense; more than     | producer, before its first    | dispatch is done with the
+//               | RANGES_IN_REGS experts on several ranks)| tile                          | stage area
+//   pub_full    | consumer warps, after a GEMM1 tile      | publisher                     | the tile's stores / adds
+//               |                                         |                               | issued
+//   pub_empty   | publisher                               | consumer warps                | the publisher took the slot
+//   wg          | warp 0, + tx                            | every router thread           | a gate-weight chunk staged
+//   remote      | warp 2, + tx                            | warp 2                        | the remote-row window filled
+//   gfull       | warp 0, + tx                            | consumer warps                | a router tensor-core stage
+//               |                                         |                               | landed
+//   gempty      | consumer warps                          | warp 0                        | the router MMAs have read it
+//   stg_full    | consumer warps, after fencing their     | publisher                     | an h chunk staged
+//               | rows to the async proxy                 |                               |
+//   stg_free    | publisher                               | consumer warps                | the TMA has read the chunk
+//               |                                         |                               | buffer
+#define FM_MBARRIERS(X)                                            \
+    X(FULL,        full,         0, STAGES,      1)                 \
+    X(EMPTY,       empty,        4, STAGES,      NUM_EPI_WARPS)     \
+    X(SCHED_FULL,  sched_full,   8, NSCHED,      1)                 \
+    X(SCHED_EMPTY, sched_empty, 12, NSCHED,      2 + NUM_EPI_WARPS) \
+    X(PROD_TAKE,   prod_take,   16, NSCHED,      1)                 \
+    X(XROWS,       xrows,       20, 1,           1)                 \
+    X(DISP_DONE,   disp_done,   21, 1,           1)                 \
+    X(PUB_FULL,    pub_full,    22, 2,           NUM_EPI_WARPS)     \
+    X(PUB_EMPTY,   pub_empty,   24, 2,           1)                 \
+    X(WG,          wg,          26, 1,           1)                 \
+    X(REMOTE,      remote,      27, 1,           1)                 \
+    X(GFULL,       gfull,       28, GATE_STAGES, 1)                 \
+    X(GEMPTY,      gempty,      36, GATE_STAGES, NUM_EPI_WARPS)     \
+    X(STG_FULL,    stg_full,    44, EPI_BUFS,    NUM_EPI_WARPS)     \
+    X(STG_FREE,    stg_free,    46, EPI_BUFS,    1)
+
+enum : int {
+#define FM_MBAR_ID(ID, name, first, count, arrivals) BAR_##ID = (first),
+    FM_MBARRIERS(FM_MBAR_ID)
+#undef FM_MBAR_ID
+};
+#define FM_MBAR_COUNT(ID, name, first, count, arrivals) +(count)
+constexpr int NUM_BARS = 0 FM_MBARRIERS(FM_MBAR_COUNT);   // 48
+#undef FM_MBAR_COUNT
+
+constexpr bool mbar_groups_contiguous() {
+    int next = 0;
+#define FM_MBAR_NEXT(ID, name, first, count, arrivals) \
+    if ((first) != next) return false;                 \
+    next += (count);
+    FM_MBARRIERS(FM_MBAR_NEXT)
+#undef FM_MBAR_NEXT
+    return true;
+}
+static_assert(mbar_groups_contiguous(), "each mbarrier group starts where the one before it ends, the first at id 0");
+
+// the group and index of barrier `id`, for the host's timeout message
+struct MbarName { const char* group; int index; };
+constexpr MbarName mbar_name(int id) {
+#define FM_MBAR_NAME(ID, name, first, count, arrivals) \
+    if (id >= (first) && id < (first) + (count)) return {#name, id - (first)};
+    FM_MBARRIERS(FM_MBAR_NAME)
+#undef FM_MBAR_NAME
+    return {nullptr, id};
+}
+constexpr bool same_str(const char* a, const char* b) {
+    while (*a != 0 && *a == *b) { ++a; ++b; }
+    return *a == *b;
+}
+static_assert(same_str(mbar_name(0).group, "full") && mbar_name(0).index == 0 &&
+              same_str(mbar_name(BAR_SCHED_FULL + 2).group, "sched_full") && mbar_name(BAR_SCHED_FULL + 2).index == 2 &&
+              same_str(mbar_name(BAR_DISP_DONE).group, "disp_done") && mbar_name(BAR_DISP_DONE).index == 0 &&
+              same_str(mbar_name(NUM_BARS - 1).group, "stg_free") && mbar_name(NUM_BARS - 1).index == EPI_BUFS - 1 &&
+              mbar_name(NUM_BARS).group == nullptr,
+              "mbar_name finds each barrier's group and index");
+
+constexpr int OFF_RING = OFF_BARS + NUM_BARS * 8;                     // the scheduler ring: NSCHED TileInfo slots
+constexpr int OFF_LAUNCH = OFF_RING + NSCHED * 64;                    // this launch's Launch record (below)
+constexpr int SMEM_USED = OFF_LAUNCH + 64;
+constexpr int SMEM_BYTES = SMEM_USED + 1024;                          // + slack for manual 1 KiB alignment
+static_assert(OFF_BARS + NUM_BARS * (int)sizeof(uint64_t) == OFF_RING && OFF_BARS % 8 == 0,
+              "the mbarriers fill [OFF_BARS, OFF_RING)");
+static_assert(OFF_RING % 16 == 0, "ring entries are 16-byte aligned");
+static_assert(SMEM_BYTES <= 232448, "227 KiB of dynamic shared memory per CTA");
 
 __device__ __forceinline__ uint64_t* bar(uint8_t* smem, int id) { return reinterpret_cast<uint64_t*>(smem + OFF_BARS) + id; }
 
@@ -296,6 +401,25 @@ __device__ __forceinline__ void trace_stamp(const FmParams& p, int slot) {
         p.trace[(size_t)blockIdx.x * TRACE_SLOTS + slot] = globaltimer_ns();
 }
 
+// per-tile stamp `base` (TRACE_TILE_*) of this CTA's tile n; only the first TRACE_TILES tiles have slots
+__device__ __forceinline__ void trace_tile(const FmParams& p, int base, int n) {
+    if (n < TRACE_TILES) trace_stamp(p, base + n);
+}
+
+// wait for the phase of parity `parity` of mbarrier `id` to complete; a timeout traps with FM_TRAP_MBAR (id, parity)
+__device__ __forceinline__ void bar_wait(const FmParams& p, uint8_t* smem, int id, uint32_t parity) {
+    mbar_wait(bar(smem, id), parity, p.dbg, p.timeout_ns, (unsigned int)id);
+}
+
+template <int N>
+struct Ring {   // a cursor over a ring of N mbarrier-guarded slots: the slot and the parity of its current phase
+    int i = 0;
+    uint32_t phase = 0;
+    __device__ __forceinline__ void next() {
+        if (++i == N) { i = 0; phase ^= 1u; }
+    }
+};
+
 __device__ __forceinline__ void grid_barrier(const FmParams& p, const Launch& L) {
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -349,8 +473,6 @@ __device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
 struct GateTcState { int gkb; };
 __device__ __forceinline__ void gate_logits_tc(const FmParams& p, uint8_t* smem, int t0, int s0, int n_sub, int rows_cap,
                                                float* logit_s, int ldl, GateTcState& st) {
-    uint64_t* gfull = bar(smem, BAR_GFULL);
-    uint64_t* gempty = bar(smem, BAR_GEMPTY);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int E = p.E, E64 = (E + 63) & ~63;
     const int GB = min(128, E64);                                // Wg_eff rows per pass (the tensor map's box height)
@@ -374,11 +496,12 @@ __device__ __forceinline__ void gate_logits_tc(const FmParams& p, uint8_t* smem,
             for (int kb = 0; kb < nk; ++kb) {
                 const int g = st.gkb + kb, s = g % NS;
                 const uint32_t ph = (uint32_t)(g / NS) & 1u;
-                mbar_wait(&gempty[s], ph ^ 1u, p.dbg, p.timeout_ns, FM_TRAP_MBAR_EMPTY, 910 + s);
+                bar_wait(p, smem, BAR_GEMPTY + s, ph ^ 1u);
                 uint8_t* sa = smem + G_OFF_WG + s * stage_bytes;
-                mbar_arrive_expect_tx(&gfull[s], tx);
-                for (int j = 0; j < nb32; ++j) tma_load_2d(sa + j * 4096, &p.tm_gx, kb * BLOCK_K, t0 + s0 + j * 32, &gfull[s]);
-                tma_load_2d(sa + a_cap, &p.tm_gw, kb * BLOCK_K, e0, &gfull[s]);
+                uint64_t* full = bar(smem, BAR_GFULL + s);
+                mbar_arrive_expect_tx(full, tx);
+                for (int j = 0; j < nb32; ++j) tma_load_2d(sa + j * 4096, &p.tm_gx, kb * BLOCK_K, t0 + s0 + j * 32, full);
+                tma_load_2d(sa + a_cap, &p.tm_gw, kb * BLOCK_K, e0, full);
             }
         } else if (warp >= EPI_WARP0) {        // consumer warpgroups
             const int wg = (warp - EPI_WARP0) >> 2;
@@ -390,7 +513,7 @@ __device__ __forceinline__ void gate_logits_tc(const FmParams& p, uint8_t* smem,
             for (int kb = 0; kb < nk; ++kb) {
                 const int g = st.gkb + kb, s = g % NS;
                 const uint32_t ph = (uint32_t)(g / NS) & 1u;
-                mbar_wait(&gfull[s], ph, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 910 + s);
+                bar_wait(p, smem, BAR_GFULL + s, ph);
                 if (active) {
                     const uint32_t sa = smem_u32(smem + G_OFF_WG + s * stage_bytes);
                     const uint64_t da = gmma_smem_desc_sw128(sa + wg * 64 * 128);
@@ -412,7 +535,7 @@ __device__ __forceinline__ void gate_logits_tc(const FmParams& p, uint8_t* smem,
                     wgmma_fence_regs(acc);
                 }
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&gempty[s]);
+                if (lane == 0) mbar_arrive(bar(smem, BAR_GEMPTY + s));
             }
             // both warpgroups are done reading the stages (which may overlap the logits scratch)
             named_sync<NAMED_BAR_GATE_MMA, EPI_THREADS>();
@@ -507,7 +630,7 @@ __device__ __forceinline__ void gate_logits_gemv(const FmParams& p, uint8_t* sme
                                                               : make_uint4(0u, 0u, 0u, 0u);
                     }
             }
-            mbar_wait(wgbar, wgphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 902);
+            bar_wait(p, smem, BAR_WG, wgphase);
             wgphase ^= 1;
             // register-blocked GEMV: a warp takes 4 tokens x 8 experts at a time (32 accumulators per lane, one per
             // (token, expert) pair), lanes split the H columns in 16-byte pieces; all of a step's global loads are
@@ -597,7 +720,7 @@ __device__ __forceinline__ void zero_fill_out_rows(const FmParams& p, uint8_t* s
         for (int i = lane; i < n_tok; i += 32)
             bulk_store_1d(reinterpret_cast<uint8_t*>(p.out_acc + (size_t)(t0 + i) * H) + (size_t)pieces * zbytes, zbuf, (uint32_t)rem);
     bulk_commit_group();
-    if (lane == 0) trace_stamp(p, 10);
+    if (lane == 0) trace_stamp(p, TRACE_ZERO_ISSUED);
 }
 
 // Lanes per token of softmax_topk: pow2ceil(E) up to 8 experts (one expert per lane), then 4 / 8 / 16 / 32, so that a
@@ -740,10 +863,10 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, u
             gate_logits_gemv(p, smem, t0, s0, n_sub, logit_s, ldl, wgphase);
         }
         __syncthreads();
-        if (tid == 0) trace_stamp(p, 11);
+        if (tid == 0) trace_stamp(p, TRACE_GATE_LOGITS);
         if (p.fused && s0 == 0 && warp == NUM_WARPS - 1) zero_fill_out_rows(p, smem, t0, n_tok);
         softmax_topk(p, logit_s, ldl, sel_e, t0, s0, n_sub);
-        if (tid == 0) trace_stamp(p, 15);
+        if (tid == 0) trace_stamp(p, TRACE_TOPK_WARP0);
         __syncthreads();
         if (p.aux != nullptr) {
             // column sums of the fp32 probabilities of this sub-chunk (the reference block-reduces each gate tile's
@@ -758,7 +881,7 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, u
             __syncthreads();
         }
     }
-    if (tid == 0) trace_stamp(p, 12);
+    if (tid == 0) trace_stamp(p, TRACE_GATE_TOPK);
     // The Wg / logits scratch is free from here on: start staging this chunk's token rows for the dispatch phase now
     // (one bulk load, same barrier and layout dispatch_phase expects for its first group), so the load runs under the
     // slot ranks, the grid barrier and the prefix pass instead of after them.
@@ -910,7 +1033,7 @@ __device__ __forceinline__ void dispatch_local_rows(const FmParams& p, const Lau
             mbar_arrive_expect_tx(xbar, (uint32_t)(rows * row_bytes));
             bulk_load_1d(x_s, p.x + (size_t)(t0 + g0) * H, (uint32_t)(rows * row_bytes), xbar);
         }
-        mbar_wait(xbar, xphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 900);
+        bar_wait(p, smem, BAR_XROWS, xphase);
         xphase ^= 1;
         for (int i = ltid; i < rows * k; i += EPI_THREADS) {   // one thread per (token, pick)
             const int tl = i / k, j = i - tl * k;
@@ -947,7 +1070,7 @@ __device__ __forceinline__ void dispatch_local_rows(const FmParams& p, const Lau
     fence_proxy_async_all();   // ... and ordered (async proxy) before the generic-proxy counter traffic below
     named_sync<NAMED_BAR_LOCAL, EPI_THREADS>();
     if (any_remote) named_arrive<NAMED_BAR_LOCAL_DONE, DISP_THREADS>();   // local rows + zero-fill complete (warp 2's acks wait for this)
-    if (ltid == 0) trace_stamp(p, 9);
+    if (ltid == 0) trace_stamp(p, TRACE_DISP_ROWS_DONE);
     if (any_remote) named_sync<NAMED_BAR_PREFIX_READ, DISP_THREADS>();   // warp 2 has taken what it needs from the stage area
     if (ltid < 32) {   // warp 4: acknowledge the local experts, then hand the stage area to the TMA producer
         const unsigned int par = L.epoch & 1u;
@@ -1011,7 +1134,7 @@ __device__ __forceinline__ void dispatch_remote_rows(const FmParams& p, const La
                     mbar_arrive_expect_tx(rbar, (uint32_t)(rows * row_bytes));
                     bulk_load_1d(win, p.x + (size_t)(t0 + tw) * H, (uint32_t)(rows * row_bytes), rbar);
                 }
-                mbar_wait(rbar, rphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 903);
+                bar_wait(p, smem, BAR_REMOTE, rphase);
                 rphase ^= 1;
                 for (int i = lane; i < rows * k; i += 32) {
                     const size_t gi = (size_t)(t0 + tw) * k + i;
@@ -1034,7 +1157,7 @@ __device__ __forceinline__ void dispatch_remote_rows(const FmParams& p, const La
                         mbar_arrive_expect_tx(rbar, (uint32_t)nb);
                         bulk_load_1d(win, reinterpret_cast<const uint8_t*>(p.x + (size_t)(t0 + tw) * H) + off, (uint32_t)nb, rbar);
                     }
-                    mbar_wait(rbar, rphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, 904);
+                    bar_wait(p, smem, BAR_REMOTE, rphase);
                     rphase ^= 1;
                     for (int i = lane; i < k; i += 32) {
                         const size_t gi = (size_t)(t0 + tw) * k + i;
@@ -1079,7 +1202,7 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, const Launch& 
     int* total_s = reinterpret_cast<int*>(smem + D_OFF_TOTAL);
     int* own_s = reinterpret_cast<int*>(smem + D_OFF_OWN);
     expert_prefix(p, tid, base_s, total_s, own_s);
-    if (tid == 0) trace_stamp(p, 8);
+    if (tid == 0) trace_stamp(p, TRACE_DISP_PREFIX);
     publish_counts(p, L, tid, total_s);
     // Row copies.
     //   * Rows for experts on THIS rank (warps 4-11): the chunk's token rows are contiguous in x, so one bulk load stages up
@@ -1117,20 +1240,49 @@ struct TileInfo {     // written by the scheduler warp, read by the producer / c
 };
 static_assert(sizeof(TileInfo) <= 64, "a ring slot is 64 bytes");
 
+struct WorkItem {     // a work item id, decoded
+    TileBlock blk;
+    int mb;           // row block of the packet
+    int nt;           // column tile
+    int le, src;      // the packet's local expert and source rank
+};
+
+// Item `id` of this launch's work list.  `cursor` is the index of a block at or before the item's; the scheduler keeps it
+// across its (increasing) ids.
+__device__ __forceinline__ WorkItem decode_item(const FmParams& p, const Launch& L, int id, int& cursor) {
+    while (id >= block_start(p, L, p.blocks[cursor + 1])) ++cursor;
+    WorkItem w;
+    w.blk = p.blocks[cursor];
+    const int local = id - block_start(p, L, w.blk);
+    w.mb = local % L.tcm_items;   // row blocks fastest
+    w.nt = local / L.tcm_items;
+    w.le = w.blk.pkt % p.nLx;
+    w.src = w.blk.pkt / p.nLx;
+    return w;
+}
+
+// k-blocks of a tile: GEMM0 reduces over H, GEMM1 over P
+__device__ __forceinline__ int tile_kblocks(const FmParams& p, int kind) { return (kind == 0 ? p.H : p.P) / BLOCK_K; }
+
+// TMA row of column tile nt's B operand.  expert_weights [nLx,2,P,H]: W_up(le) starts at row le*2*P of the [.,H] view;
+// W_down(le) (the [P,H] block flat-viewed as [H,P]) starts at row (le*2+1)*H of the [.,P] view.
+__device__ __forceinline__ int b_tile_row(const FmParams& p, int kind, int le, int nt) {
+    return (kind == 0 ? le * 2 * p.P : (le * 2 + 1) * p.H) + nt * BLOCK_N;
+}
+
 // warp 3, lane 0: claims work items and resolves their dependencies AHEAD of the TMA producer, so the atomic, the
 // packet-flag and the h-row-block-counter round trips overlap the previous tile's loads (the job of the reference's OS
 // CTA: subscriber decode + scheduler doorbells, os/subscriber.cuh, os/scheduler.cuh -- here one thread, no queues).
-__device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L, uint8_t* smem, uint64_t* bars) {
-    uint64_t* sched_full = bars + BAR_SCHED_FULL;
-    uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
-    uint64_t* prod_take = bars + BAR_PROD_TAKE;
+__device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L, uint8_t* smem) {
     TileInfo* ring = reinterpret_cast<TileInfo*>(smem + OFF_RING);
-    int q = 0, qphase = 0, cursor = 0, n = 0;
+    Ring<NSCHED> q;      // the slot of tile n
+    Ring<NSCHED> prev;   // the slot of tile n - 1: one step behind q from tile 1 on
+    int cursor = 0, n = 0;
     bool seen_remote = false;   // trace only: first tile of a packet from another rank
     for (;;) {
         if (n >= 1) {  // bounded look-ahead: wait until the producer is close to finishing tile n-1
-            const int pq = (q + NSCHED - 1) % NSCHED;
-            mbar_wait(&prod_take[pq], ((n - 1) / NSCHED) & 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_EMPTY, 200 + pq);
+            bar_wait(p, smem, BAR_PROD_TAKE + prev.i, prev.phase);
+            prev.next();
         }
         TileInfo ti;
         ti.kind = -1; ti.ntile = 0; ti.le = 0; ti.b_row = 0; ti.pkt = 0; ti.mblk = 0; ti.rows = 0;
@@ -1138,12 +1290,11 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L
         for (;;) {
             const int id = (int)atomicAdd(p.claim, 1u);
             if (id >= L.total_items) break;
-            if (n < 16) trace_stamp(p, 112 + n);   // claim time of tile n (ready time is slot 16+n)
-            while (id >= block_start(p, L, p.blocks[cursor + 1])) ++cursor;
-            const TileBlock blk = p.blocks[cursor];
-            const int local = id - block_start(p, L, blk);
-            const int mb = local % L.tcm_items, nt = local / L.tcm_items;   // row blocks fastest
-            const int pkt = blk.pkt, le = pkt % p.nLx, src = pkt / p.nLx;
+            trace_tile(p, TRACE_TILE_CLAIMED, n);
+            const WorkItem w = decode_item(p, L, id, cursor);
+            const TileBlock& blk = w.blk;
+            const int mb = w.mb, nt = w.nt, pkt = blk.pkt, le = w.le, src = w.src;
+            const bool first_item = mb == 0 && nt == 0;   // the packet's first item of this GEMM
             const bool same_gpu = src == p.rank;   // flag and counters written from this GPU: gpu scope suffices
             const unsigned int epoch = L.epoch;
             // wait for the packet (src, le): flag = {epoch, rows}  (reference subscriber.cuh:52-185)
@@ -1167,8 +1318,8 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L
             if (stale) continue;
             const int cnt = (int)(f & 0xffffffffull);
             // once per packet and GEMM (its first item): bookkeeping that needs the count
-            if (local == 0 && blk.kind == 0 && !p.dense) p.recv_cnt[pkt] = cnt;
-            if (p.fused && local == 0 && blk.kind == 1 && cnt == 0)   // nothing to contribute: tell the source now
+            if (first_item && blk.kind == 0 && !p.dense) p.recv_cnt[pkt] = cnt;
+            if (p.fused && first_item && blk.kind == 1 && cnt == 0)   // nothing to contribute: tell the source now
                 st_release_sys_u64(p.peer_done_flag[src] + (size_t)(p.rank * p.nLx + le), (unsigned long long)epoch << 32);
             const int rows = max(0, min(BLOCK_M, cnt - mb * BLOCK_M));
             if (rows == 0) continue;   // an empty row block of the static superset
@@ -1186,43 +1337,37 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L
             }
             ti.kind = blk.kind; ti.ntile = nt; ti.le = le; ti.pkt = pkt; ti.mblk = mb; ti.rows = rows;
             ti.src = src; ti.cnt = cnt;
-            // expert_weights [nLx,2,P,H]: W_up(le) starts at row le*2*P of the [.,H] view; W_down(le) (the [P,H]
-            // block flat-viewed as [H,P]) starts at row (le*2+1)*H of the [.,P] view.
-            ti.b_row = (blk.kind == 0 ? le * 2 * p.P : (le * 2 + 1) * p.H) + nt * BLOCK_N;
+            ti.b_row = b_tile_row(p, blk.kind, le, nt);
             break;
         }
-        if (ti.kind >= 0 && n < 16) trace_stamp(p, 16 + n);
+        if (ti.kind >= 0) trace_tile(p, TRACE_TILE_READY, n);
         if (ti.kind >= 0 && ti.src != p.rank && !seen_remote) {
             seen_remote = true;
-            trace_stamp(p, 13);
+            trace_stamp(p, TRACE_FIRST_REMOTE);
         }
-        mbar_wait(&sched_empty[q], qphase ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_EMPTY, q);
-        ring[q] = ti;
-        mbar_arrive(&sched_full[q]);
-        if (++q == NSCHED) { q = 0; qphase ^= 1; }
+        bar_wait(p, smem, BAR_SCHED_EMPTY + q.i, q.phase ^ 1u);
+        ring[q.i] = ti;
+        mbar_arrive(bar(smem, BAR_SCHED_FULL + q.i));
+        q.next();
         ++n;
         if (ti.kind < 0) break;
     }
 }
 
 // warp 0: TMA producer
-__device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem, uint64_t* bars) {
-    uint64_t* full = bars + BAR_FULL;
-    uint64_t* empty = bars + BAR_EMPTY;
-    uint64_t* sched_full = bars + BAR_SCHED_FULL;
-    uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
-    uint64_t* prod_take = bars + BAR_PROD_TAKE;
+__device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem) {
     const TileInfo* ring = reinterpret_cast<const TileInfo*>(smem + OFF_RING);
     const int lane = threadIdx.x & 31;
-    int stage = 0, phase = 0, q = 0, qphase = 0;
+    Ring<STAGES> stage;
+    Ring<NSCHED> q;
     bool first = true, stamped = false;
     for (;;) {
         int kind = -1;
         TileInfo ti;
         if (lane == 0) {
-            mbar_wait(&sched_full[q], qphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, 300 + q);
-            ti = ring[q];
-            mbar_arrive(&sched_empty[q]);
+            bar_wait(p, smem, BAR_SCHED_FULL + q.i, q.phase);
+            ti = ring[q.i];
+            mbar_arrive(bar(smem, BAR_SCHED_EMPTY + q.i));
             kind = ti.kind;
         }
         kind = __shfl_sync(0xffffffffu, kind, 0);
@@ -1230,10 +1375,10 @@ __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem, u
         int nk = 0;
         if (lane == 0) {
             if (first)   // the stage area doubles as the dispatch staging buffer
-                mbar_wait(&bars[BAR_DISP_DONE], 0, p.dbg, p.timeout_ns, FM_TRAP_MBAR_EMPTY, 901);
+                bar_wait(p, smem, BAR_DISP_DONE, 0);
             first = false;
             fence_proxy_async_global();  // rows written by generic-proxy stores (peers / other SMs) -> TMA reads
-            nk = (kind == 0 ? p.H : p.P) / BLOCK_K;
+            nk = tile_kblocks(p, kind);
         }
         nk = __shfl_sync(0xffffffffu, nk, 0);
         const CUtensorMap* ta = kind == 0 ? &p.tm_a0 : &p.tm_a1;
@@ -1245,20 +1390,21 @@ __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem, u
             b_row = ti.b_row;
         }
         for (int kb = 0; kb < nk; ++kb) {
-            uint8_t* sa = smem + stage * STAGE_BYTES;
+            uint8_t* sa = smem + stage.i * STAGE_BYTES;
             const bool ld_a = (p.dbg_flags & 5) == 0, ld_b = (p.dbg_flags & 9) == 0;   // experiments only
             if (lane == 0) {
-                if (kb == take_at) mbar_arrive(&prod_take[q]);  // lets the scheduler claim the next tile
-                mbar_wait(&empty[stage], phase ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_EMPTY, stage);
+                if (kb == take_at) mbar_arrive(bar(smem, BAR_PROD_TAKE + q.i));  // lets the scheduler claim the next tile
+                bar_wait(p, smem, BAR_EMPTY + stage.i, stage.phase ^ 1u);
+                uint64_t* full = bar(smem, BAR_FULL + stage.i);
                 const uint32_t tx = (ld_a ? (uint32_t)A_STAGE_BYTES : 0u) + (ld_b ? (uint32_t)B_STAGE_BYTES : 0u);
-                if (tx) mbar_arrive_expect_tx(&full[stage], tx); else mbar_arrive(&full[stage]);
-                if (ld_a) tma_load_2d(sa, ta, kb * BLOCK_K, a_row, &full[stage]);
-                if (ld_b) tma_load_2d(sa + A_STAGE_BYTES, tb, kb * BLOCK_K, b_row, &full[stage]);
-                if (!stamped) { trace_stamp(p, 7); stamped = true; }   // first loads of the first tile issued
+                if (tx) mbar_arrive_expect_tx(full, tx); else mbar_arrive(full);
+                if (ld_a) tma_load_2d(sa, ta, kb * BLOCK_K, a_row, full);
+                if (ld_b) tma_load_2d(sa + A_STAGE_BYTES, tb, kb * BLOCK_K, b_row, full);
+                if (!stamped) { trace_stamp(p, TRACE_FIRST_TMA); stamped = true; }   // first loads of the first tile issued
             }
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            stage.next();
         }
-        if (++q == NSCHED) { q = 0; qphase ^= 1; }
+        q.next();
         __syncwarp();
     }
 }
@@ -1319,19 +1465,19 @@ __device__ __forceinline__ void chunk_to_smem(const float (&acc)[128], int c, ui
 // Rows at or beyond the block's valid rows are staged and stored too: they lie in the packet's pEC padding of h, and
 // GEMM1 multiplies them row-independently and drops their results.
 template <int MODE, bool HAS_BIAS>
-__device__ __forceinline__ void stage_h(const FmParams& p, uint8_t* smem, uint64_t* bars, const float (&acc)[128],
+__device__ __forceinline__ void stage_h(const FmParams& p, uint8_t* smem, const float (&acc)[128],
                                         const __nv_bfloat16* bias, int nchunks, int row0, int lane, uint32_t& chunk) {
     const float one[2] = {1.0f, 1.0f};
 #pragma unroll
     for (int c = 0; c < BLOCK_N / 64; ++c) {
         if (c >= nchunks) break;
         const int b = chunk & 1;
-        mbar_wait(&bars[BAR_STG_FREE + b], ((chunk >> 1) & 1) ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, 20 + b);
+        bar_wait(p, smem, BAR_STG_FREE + b, ((chunk >> 1) & 1) ^ 1);
         chunk_to_smem<MODE, HAS_BIAS>(acc, c, smem + OFF_EPI + b * EPI_CHUNK_BYTES + row0 * EPI_ROW_BYTES,
                                       HAS_BIAS ? bias + c * 64 : nullptr, lane, one, one);
         fence_proxy_async_smem();
         __syncwarp();
-        if (lane == 0) mbar_arrive(&bars[BAR_STG_FULL + b]);
+        if (lane == 0) mbar_arrive(bar(smem, BAR_STG_FULL + b));
         ++chunk;
     }
 }
@@ -1389,224 +1535,245 @@ __device__ __forceinline__ void drain_accumulator(const FmParams& p, const Drain
 // The consumers do not wait for their stores, nor fence or publish: a GEMM0 tile's h chunks are handed to the publisher
 // warp through the staging buffers (stage_h), and after a GEMM1 tile lane 0 of every consumer warp arrives on pub_full[];
 // the publisher warp takes over from there (ffn_publisher).
-__device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem, uint64_t* bars) {
-    uint64_t* full = bars + BAR_FULL;
-    uint64_t* empty = bars + BAR_EMPTY;
-    uint64_t* sched_full = bars + BAR_SCHED_FULL;
-    uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
-    uint64_t* pub_full = bars + BAR_PUB_FULL;
-    uint64_t* pub_empty = bars + BAR_PUB_EMPTY;
-    const TileInfo* ring = reinterpret_cast<const TileInfo*>(smem + OFF_RING);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int wg = (warp - EPI_WARP0) >> 2;
-    const int row0 = wg * 64 + (warp & 3) * 16;   // this warp's 16 rows of the tile
-    uint8_t* stg = smem + OFF_EPI + row0 * EPI_ROW_BYTES;   // GEMM1 transpose tile: this warp's rows of buffer 0
-    int q = 0, qphase = 0, stage = 0, phase = 0, ps = 0, pphase = 0, ntiles = 0;
+struct Consumer {         // one consumer warp's place in the rings it reads, kept across tiles
+    Ring<NSCHED> q;       // scheduler ring
+    Ring<STAGES> stage;   // pipeline stages
+    Ring<2> pub;          // GEMM1 tiles handed to the publisher (pub_full / pub_empty)
     uint32_t chunk = 0;   // GEMM0 h chunks this warp has staged so far (stage_h)
-    const bool stamper = tid == EPI_WARP0 * 32;
+    int ntiles = 0;
+    int lane;
+    int wg;               // warpgroup: A rows [64 wg, 64 wg + 64)
+    int row0;             // this warp's 16 rows of the tile
+    bool stamper;         // the thread that writes the consumers' trace stamps
+};
+
+// The k-block loop: one k-block's wgmma group in flight while the previous stage is handed back.  Returns with the last
+// k-block's group still in flight, and the stage it reads (-1 when there are no k-blocks).
+__device__ __forceinline__ int mainloop(const FmParams& p, uint8_t* smem, float (&acc)[128], int nk, Consumer& c) {
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.0f;
+    int prev = -1;
+    for (int kb = 0; kb < nk; ++kb) {
+        bar_wait(p, smem, BAR_FULL + c.stage.i, c.stage.phase);
+        if (kb == 0 && c.stamper) trace_tile(p, TRACE_TILE_FIRST_KB, c.ntiles);
+        if (!(p.dbg_flags & 2)) {   // (experiment: no MMA)
+            const uint32_t sa = smem_u32(smem + c.stage.i * STAGE_BYTES);
+            const uint64_t da = gmma_smem_desc_sw128(sa + c.wg * 64 * 128);
+            const uint64_t db = gmma_smem_desc_sw128(sa + A_STAGE_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < BLOCK_K / WGMMA_K; ++kk)
+                wgmma_m64n256k16_bf16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2));
+            wgmma_commit();
+        }
+        if (prev >= 0) {   // the previous k-block's MMAs have read their stage
+            wgmma_wait<1>();
+            __syncwarp();
+            if (c.lane == 0) mbar_arrive(bar(smem, BAR_EMPTY + prev));
+        }
+        prev = c.stage.i;
+        c.stage.next();
+    }
+    return prev;
+}
+
+// The start of both epilogues, once they have read the tile's fields from its ring slot: the last k-block's MMAs
+// complete, and its stage and the ring slot are handed back.
+__device__ __forceinline__ void mainloop_done(const FmParams& p, uint8_t* smem, float (&acc)[128], int prev, Consumer& c) {
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    __syncwarp();
+    if (c.lane == 0 && prev >= 0) mbar_arrive(bar(smem, BAR_EMPTY + prev));
+    if (c.stamper) trace_tile(p, TRACE_TILE_MMA_DONE, c.ntiles);
+    if (c.ntiles == 0 && p.W > 1)   // the staging area served as warp 2's window for the remote rows
+        named_sync<NAMED_BAR_WINDOW, DISP_THREADS>();
+    if (c.lane == 0) mbar_arrive(bar(smem, BAR_SCHED_EMPTY + c.q.i));   // every lane has read the slot (the __syncwarp above)
+    c.q.next();
+    if (c.stamper) trace_tile(p, TRACE_TILE_EPI_START, c.ntiles);
+}
+
+// f(std::true_type) with a bias, f(std::false_type) without: one specialised epilogue instantiation per (epilogue kind,
+// bias) pair, with no per-element or per-group branching
+template <class F>
+__device__ __forceinline__ void with_bias(const __nv_bfloat16* bias, F&& f) {
+    if (bias != nullptr) f(std::true_type{});
+    else f(std::false_type{});
+}
+
+// GEMM0 epilogue: h.  Every warp stages its 16 rows of each 64-column chunk (N is a multiple of 64, not necessarily of
+// the tile width) and goes straight on to the next tile; the publisher warp stores and publishes them.
+__device__ __forceinline__ void epilogue_h(const FmParams& p, uint8_t* smem, const TileInfo* ti, float (&acc)[128], int prev,
+                                           Consumer& c) {
+    const int n0 = ti->ntile * BLOCK_N, le = ti->le;
+    mainloop_done(p, smem, acc, prev, c);
+    const int nchunks = min(BLOCK_N / 64, (p.P - n0) / 64);
+    const __nv_bfloat16* bias = p.b_up ? p.b_up + (size_t)le * p.P + n0 : nullptr;
+    with_bias(bias, [&](auto has_bias) {
+        constexpr bool B = decltype(has_bias)::value;
+        if (p.act == 0) stage_h<EPI_G0_RELU, B>(p, smem, acc, bias, nchunks, c.row0, c.lane, c.chunk);
+        else stage_h<EPI_G0_GELU, B>(p, smem, acc, bias, nchunks, c.row0, c.lane, c.chunk);
+    });
+    if (c.stamper) trace_tile(p, TRACE_TILE_STORES, c.ntiles);
+}
+
+// GEMM1 epilogue: the destination rows are the SOURCE rank's return buffer (peer store), like the reference's GEMM1
+// epilogue writing into the peer heap (packet.cuh:338-340, processor.cuh:713-720), or with p.fused the tokens' output
+// rows there.  Then the tile is handed to the publisher.
+__device__ __forceinline__ void epilogue_out(const FmParams& p, uint8_t* smem, const TileInfo* ti, float (&acc)[128],
+                                             int prev, Consumer& c) {
+    const int lane = c.lane, row0 = c.row0;
+    // While the last k-block's MMAs run: the tile's fields from its ring slot and, for the fused epilogue, lane l < 16's
+    // routing record of tile row (row0 + l), so that nothing is fetched after the final wait.
+    const int ntile = ti->ntile, le = ti->le, pkt = ti->pkt, mblk = ti->mblk, my_rows = ti->rows, src = ti->src;
+    const bool fuse = p.fused != 0;
+    int my_tok = 0;
+    float my_pw = 0.0f, my_mcw = 1.0f;
+    if (fuse && p.dense) {
+        my_tok = mblk * BLOCK_M + row0 + lane;   // row i of the only packet IS token i
+    } else if (fuse && lane < 16 && row0 + lane < my_rows) {
+        const uint4 m = ld_global_v4(p.recv_meta + (size_t)pkt * p.pEC + (size_t)mblk * BLOCK_M + row0 + lane);
+        my_tok = (int)m.x;
+        my_pw = __uint_as_float(m.y);
+        my_mcw = __uint_as_float(m.z);
+    }
+    mainloop_done(p, smem, acc, prev, c);
+
+    const int N = p.H, n0 = ntile * BLOCK_N;
+    const int e_global = p.rank * p.nLx + le;
+    const int nchunks = row0 < my_rows ? min(BLOCK_N / 64, (N - n0) / 64) : 0;
+    // this warp's transpose tile is its rows of chunk buffer 0, which the TMA may still be reading for the last
+    // GEMM0 tile: wait as stage_h would before buffer 0's next use (chunk `next0`; the wait consumes nothing)
+    const uint32_t next0 = (c.chunk + 1) & ~1u;
+    bar_wait(p, smem, BAR_STG_FREE, ((next0 >> 1) & 1) ^ 1);
+    if (nchunks > 0) {
+        DrainArgs da;
+        da.stg = smem + OFF_EPI + row0 * EPI_ROW_BYTES; da.nchunks = nchunks; da.lane = lane; da.row0 = row0;
+        da.my_rows = my_rows; da.N = N; da.n0 = n0;
+        da.bias = p.b_down ? p.b_down + (size_t)le * p.H : nullptr;
+        da.out_rows = p.peer_ret_y[src] + ((size_t)e_global * p.pEC + (size_t)mblk * BLOCK_M) * p.H;
+        da.acc_base = fuse ? p.peer_out_acc[src] : nullptr;
+        da.my_tok = my_tok; da.my_pw = my_pw; da.my_mcw = my_mcw;
+        with_bias(da.bias, [&](auto has_bias) {
+            constexpr bool B = decltype(has_bias)::value;
+            if (!fuse) drain_accumulator<EPI_G1_STORE, B>(p, da, acc);
+            else if (p.k > 1) drain_accumulator<EPI_G1_FUSED_ADD, B>(p, da, acc);
+            else drain_accumulator<EPI_G1_FUSED_COPY, B>(p, da, acc);
+        });
+    }
+    if (c.stamper) trace_tile(p, TRACE_TILE_STORES, c.ntiles);
+
+    // hand the tile to the publisher: this warp's stores / REDs are issued
+    __syncwarp();
+    if (lane == 0) {
+        bar_wait(p, smem, BAR_PUB_EMPTY + c.pub.i, c.pub.phase ^ 1u);
+        mbar_arrive(bar(smem, BAR_PUB_FULL + c.pub.i));
+    }
+    c.pub.next();
+}
+
+__device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem) {
+    const TileInfo* ring = reinterpret_cast<const TileInfo*>(smem + OFF_RING);
+    const int tid = threadIdx.x, warp = tid >> 5;
+    Consumer c;
+    c.lane = tid & 31;
+    c.wg = (warp - EPI_WARP0) >> 2;
+    c.row0 = c.wg * 64 + (warp & 3) * 16;
+    // warp 4, lane 0, from values both epilogues keep in registers (a test of the thread index reloads the spilled index
+    // in each of them)
+    c.stamper = c.row0 == 0 && c.lane == 0;
     for (;;) {
-        mbar_wait(&sched_full[q], qphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, 100 + q);
-        // The tile's ring slot stays ours until its epilogue is set up (sched_empty is arrived on below): the per-tile
-        // fields are read from shared memory after the k-block loop instead of being kept live (spilled) across it.
-        const TileInfo* ti = ring + q;
+        bar_wait(p, smem, BAR_SCHED_FULL + c.q.i, c.q.phase);
+        // The tile's ring slot stays ours until its epilogue is set up (mainloop_done arrives on sched_empty): the
+        // per-tile fields are read from shared memory after the k-block loop instead of being kept live (spilled) across it.
+        const TileInfo* ti = ring + c.q.i;
         const int kind = ti->kind;
         if (kind < 0) break;
-
-        // ---- main loop: one k-block's wgmma group in flight while the previous stage is handed back
-        const int nk = (kind == 0 ? p.H : p.P) / BLOCK_K;
         float acc[128];
-#pragma unroll
-        for (int i = 0; i < 128; ++i) acc[i] = 0.0f;
-        int prev = -1;
-        for (int kb = 0; kb < nk; ++kb) {
-            mbar_wait(&full[stage], phase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_FULL, stage);
-            if (kb == 0 && ntiles < 16 && stamper) trace_stamp(p, 32 + ntiles);
-            if (!(p.dbg_flags & 2)) {   // (experiment: no MMA)
-                const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-                const uint64_t da = gmma_smem_desc_sw128(sa + wg * 64 * 128);
-                const uint64_t db = gmma_smem_desc_sw128(sa + A_STAGE_BYTES);
-                wgmma_fence();
-#pragma unroll
-                for (int kk = 0; kk < BLOCK_K / WGMMA_K; ++kk)
-                    wgmma_m64n256k16_bf16(acc, da + (uint64_t)(kk * 2), db + (uint64_t)(kk * 2));
-                wgmma_commit();
-            }
-            if (prev >= 0) {   // the previous k-block's MMAs have read their stage
-                wgmma_wait<1>();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty[prev]);
-            }
-            prev = stage;
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        // While the last k-block's MMAs run: the tile's fields from its ring slot and, for the fused GEMM1 epilogue,
-        // lane l < 16's routing record of tile row (row0 + l), so that nothing is fetched after the final wait.
-        const int ntile = ti->ntile, le = ti->le, pkt = ti->pkt, mblk = ti->mblk, my_rows = ti->rows, src = ti->src;
-        const bool fuse = p.fused != 0 && kind == 1;
-        int my_tok = 0;
-        float my_pw = 0.0f, my_mcw = 1.0f;
-        if (fuse && p.dense) {
-            my_tok = mblk * BLOCK_M + row0 + lane;   // row i of the only packet IS token i
-        } else if (fuse && lane < 16 && row0 + lane < my_rows) {
-            const uint4 m = ld_global_v4(p.recv_meta + (size_t)pkt * p.pEC + (size_t)mblk * BLOCK_M + row0 + lane);
-            my_tok = (int)m.x;
-            my_pw = __uint_as_float(m.y);
-            my_mcw = __uint_as_float(m.z);
-        }
-        wgmma_wait<0>();
-        wgmma_fence_regs(acc);
-        __syncwarp();
-        if (lane == 0 && prev >= 0) mbar_arrive(&empty[prev]);
-        if (ntiles < 16 && stamper) trace_stamp(p, 48 + ntiles);
-
-        if (ntiles == 0 && p.W > 1)   // the staging area served as warp 2's window for the remote rows
-            named_sync<NAMED_BAR_WINDOW, DISP_THREADS>();
-        if (lane == 0) mbar_arrive(&sched_empty[q]);   // every lane has read the slot (the __syncwarp above)
-        if (++q == NSCHED) { q = 0; qphase ^= 1; }
-        if (ntiles < 16 && stamper) trace_stamp(p, 64 + ntiles);
-
-        const int n0 = ntile * BLOCK_N;
-        if (kind == 0) {
-            // h: every warp stages its 16 rows of each 64-column chunk (N is a multiple of 64, not necessarily of the
-            // tile width) and goes straight on to the next tile; the publisher warp stores and publishes them
-            const int nchunks = min(BLOCK_N / 64, (p.P - n0) / 64);
-            const __nv_bfloat16* bias = p.b_up ? p.b_up + (size_t)le * p.P + n0 : nullptr;
-            if (bias == nullptr) {
-                if (p.act == 0) stage_h<EPI_G0_RELU, false>(p, smem, bars, acc, bias, nchunks, row0, lane, chunk);
-                else stage_h<EPI_G0_GELU, false>(p, smem, bars, acc, bias, nchunks, row0, lane, chunk);
-            } else {
-                if (p.act == 0) stage_h<EPI_G0_RELU, true>(p, smem, bars, acc, bias, nchunks, row0, lane, chunk);
-                else stage_h<EPI_G0_GELU, true>(p, smem, bars, acc, bias, nchunks, row0, lane, chunk);
-            }
-            if (ntiles < 16 && stamper) trace_stamp(p, 80 + ntiles);
-            ++ntiles;
-            continue;
-        }
-
-        // GEMM1: the destination rows are the SOURCE rank's return buffer (peer store), like the reference's GEMM1
-        // epilogue writing into the peer heap (packet.cuh:338-340, processor.cuh:713-720), or with `fuse` the tokens'
-        // output rows there
-        const int N = p.H;
-        const int e_global = p.rank * p.nLx + le;
-        __nv_bfloat16* out_rows = p.peer_ret_y[src] + ((size_t)e_global * p.pEC + (size_t)mblk * BLOCK_M) * p.H;
-        const __nv_bfloat16* bias = p.b_down ? p.b_down + (size_t)le * p.H : nullptr;
-        const int nchunks = row0 < my_rows ? min(BLOCK_N / 64, (N - n0) / 64) : 0;
-        // this warp's transpose tile is its rows of chunk buffer 0, which the TMA may still be reading for the last
-        // GEMM0 tile: wait as stage_h would before buffer 0's next use (chunk `next0`; the wait consumes nothing)
-        const uint32_t next0 = (chunk + 1) & ~1u;
-        mbar_wait(&bars[BAR_STG_FREE], ((next0 >> 1) & 1) ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, 22);
-        if (nchunks > 0) {
-            DrainArgs da;
-            da.stg = stg; da.nchunks = nchunks; da.lane = lane; da.row0 = row0; da.my_rows = my_rows; da.N = N; da.n0 = n0;
-            da.bias = bias; da.out_rows = out_rows; da.acc_base = fuse ? p.peer_out_acc[src] : nullptr;
-            da.my_tok = my_tok; da.my_pw = my_pw; da.my_mcw = my_mcw;
-            // one specialised instantiation per (epilogue kind, bias) pair: no per-element or per-group branching
-            const int mode = !fuse ? EPI_G1_STORE : (p.k > 1 ? EPI_G1_FUSED_ADD : EPI_G1_FUSED_COPY);
-            if (bias == nullptr) {
-                switch (mode) {
-                    case EPI_G1_STORE: drain_accumulator<EPI_G1_STORE, false>(p, da, acc); break;
-                    case EPI_G1_FUSED_ADD: drain_accumulator<EPI_G1_FUSED_ADD, false>(p, da, acc); break;
-                    default: drain_accumulator<EPI_G1_FUSED_COPY, false>(p, da, acc); break;
-                }
-            } else {
-                switch (mode) {
-                    case EPI_G1_STORE: drain_accumulator<EPI_G1_STORE, true>(p, da, acc); break;
-                    case EPI_G1_FUSED_ADD: drain_accumulator<EPI_G1_FUSED_ADD, true>(p, da, acc); break;
-                    default: drain_accumulator<EPI_G1_FUSED_COPY, true>(p, da, acc); break;
-                }
-            }
-        }
-        if (ntiles < 16 && stamper) trace_stamp(p, 80 + ntiles);
-
-        // hand the tile to the publisher: this warp's stores / REDs are issued
-        __syncwarp();
-        if (lane == 0) {
-            mbar_wait(&pub_empty[ps], pphase ^ 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, ps);
-            mbar_arrive(&pub_full[ps]);
-        }
-        if (++ps == 2) { ps = 0; pphase ^= 1; }
-        ++ntiles;
+        const int prev = mainloop(p, smem, acc, tile_kblocks(p, kind), c);
+        if (kind == 0) epilogue_h(p, smem, ti, acc, prev, c);
+        else epilogue_out(p, smem, ti, acc, prev, c);
+        ++c.ntiles;
     }
 }
 
-// warp 2: writes h and makes finished tiles visible.  For every tile of the ring:
-// GEMM0 -> one TMA tensor store per 64-column chunk the consumer warps have staged (stage_h), each buffer handed back as
-// soon as the TMA has read it; then, once the stores are complete, the release-add on the row block's h counter
-// (reference notifyNext's tSA counter, processor.cuh:490-615).
-// GEMM1 -> once all consumer warps have issued their stores / REDs: system-scope fence, then the packet / row-block
-// counter and, from the last tile, the flag on the source rank (reference processor.cuh:722-750).  The fences and the
+// warp 2, lane 0: writes h and makes finished tiles visible, for every tile of the ring in order.  The fences and the
 // store completion take 1-2 us (more over NVLink); here they overlap the next tile's MMA instead of delaying it.
-__device__ __forceinline__ void ffn_publisher(const FmParams& p, const Launch& L, uint8_t* smem, uint64_t* bars) {
-    uint64_t* sched_full = bars + BAR_SCHED_FULL;
-    uint64_t* sched_empty = bars + BAR_SCHED_EMPTY;
-    uint64_t* pub_full = bars + BAR_PUB_FULL;
-    uint64_t* pub_empty = bars + BAR_PUB_EMPTY;
-    uint64_t* stg_full = bars + BAR_STG_FULL;
-    uint64_t* stg_free = bars + BAR_STG_FREE;
+//
+// GEMM0: one TMA tensor store per 64-column chunk the consumer warps have staged (stage_h), each buffer handed back as
+// soon as the TMA has read it; then, once the stores are complete, the release-add on the row block's h counter
+// (reference notifyNext's tSA counter, processor.cuh:490-615).  `chunk` counts the chunks stored so far, in the
+// consumers' staging order.
+__device__ __forceinline__ void publish_h(const FmParams& p, uint8_t* smem, const TileInfo& ti, uint32_t& chunk) {
+    const int n0 = ti.ntile * BLOCK_N, nchunks = min(BLOCK_N / 64, (p.P - n0) / 64);
+    const int row = ti.pkt * p.pEC + ti.mblk * BLOCK_M;
+    // both buffers' stores in flight: chunk c is issued as soon as it is staged, and only then does the warp wait for
+    // the TMA to have read chunk c - 1, whose buffer the consumers refill with chunk c + 1
+    for (int c = 0; c < nchunks; ++c, ++chunk) {
+        const int b = chunk & 1;
+        bar_wait(p, smem, BAR_STG_FULL + b, (chunk >> 1) & 1);
+        tma_store_2d(&p.tm_a1, smem + OFF_EPI + b * EPI_CHUNK_BYTES, n0 + c * 64, row);
+        bulk_commit_group();
+        if (c > 0) {
+            bulk_wait_group_read<1>();   // chunk c - 1 has been read: its buffer may be refilled
+            mbar_arrive(bar(smem, BAR_STG_FREE + (b ^ 1)));
+        }
+    }
+    bulk_wait_group_read<0>();
+    mbar_arrive(bar(smem, BAR_STG_FREE + ((chunk - 1) & 1)));
+    bulk_wait_group0();            // the tile's h writes (async proxy) are complete ...
+    fence_proxy_async_global();    // ... and ordered before the generic-proxy release below
+    red_release_gpu_add_u32(p.g0_done + (size_t)ti.pkt * p.TCM + ti.mblk, 1u);
+}
+
+// GEMM1: once all consumer warps have issued their stores / REDs, a system-scope fence, then the packet or row-block
+// counter and, from the last tile, the flag on the source rank (reference processor.cuh:722-750).
+__device__ __forceinline__ void publish_out(const FmParams& p, const Launch& L, uint8_t* smem, const TileInfo& ti,
+                                            Ring<2>& pub) {
+    bar_wait(p, smem, BAR_PUB_FULL + pub.i, pub.phase);
+    mbar_arrive(bar(smem, BAR_PUB_EMPTY + pub.i));
+    pub.next();
+    if (p.fused) {
+        // local packet, output left in place: nobody waits for a flag (see finish_fused) -- no fence, no counter, no
+        // flag; kernel completion covers these adds
+        if (ti.src == p.rank && p.out_acc == p.out) return;
+        fence_acq_rel_sys();   // this tile's adds are performed before the packet counter moves
+        const unsigned int old = atom_acq_rel_gpu_add_u32(p.pkt_done + ti.pkt, 1u);
+        const unsigned int want = (unsigned int)(((ti.cnt + BLOCK_M - 1) / BLOCK_M) * p.TN1);
+        if (old + 1u == want)   // every GEMM1 tile of packet (src, le) has been added into src's output
+            st_release_sys_u64(p.peer_done_flag[ti.src] + (size_t)(p.rank * p.nLx + ti.le), (unsigned long long)L.epoch << 32);
+    } else {
+        fence_acq_rel_sys();
+        const unsigned int old = atom_acq_rel_gpu_add_u32(p.g1_done + (size_t)ti.pkt * p.TCM + ti.mblk, 1u);
+        if (old == (unsigned int)p.TN1 - 1u) {  // whole rows of this block are on the source rank
+            fence_acq_rel_sys();
+            const int e_global = p.rank * p.nLx + ti.le;
+            st_release_sys_u64(p.peer_ret_flag[ti.src] + (size_t)e_global * p.TCM + ti.mblk,
+                               ((unsigned long long)L.epoch << 32) | (unsigned int)ti.rows);
+        }
+    }
+}
+
+// warp 2: the publisher.  Lane 0 takes every tile of the ring in order and publishes it with publish_h or publish_out.
+__device__ __forceinline__ void ffn_publisher(const FmParams& p, const Launch& L, uint8_t* smem) {
     const TileInfo* ring = reinterpret_cast<const TileInfo*>(smem + OFF_RING);
     const int lane = threadIdx.x & 31;
-    int q = 0, qphase = 0, ps = 0, pphase = 0, ntiles = 0;
-    uint32_t chunk = 0;   // h chunks stored so far, in the consumers' staging order
+    Ring<NSCHED> q;
+    Ring<2> pub;
+    int ntiles = 0;
+    uint32_t chunk = 0;   // h chunks stored so far (publish_h)
     for (;;) {
         int kind = -1;
         if (lane == 0) {
-            mbar_wait(&sched_full[q], qphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_SCHED_FULL, 400 + q);
-            const TileInfo ti = ring[q];
-            mbar_arrive(&sched_empty[q]);
+            bar_wait(p, smem, BAR_SCHED_FULL + q.i, q.phase);
+            const TileInfo ti = ring[q.i];
+            mbar_arrive(bar(smem, BAR_SCHED_EMPTY + q.i));
             kind = ti.kind;
-            const int my_rows = ti.rows, my_mblk = ti.mblk, my_pkt = ti.pkt, my_src = ti.src;
-            if (kind == 0) {
-                const int n0 = ti.ntile * BLOCK_N, nchunks = min(BLOCK_N / 64, (p.P - n0) / 64);
-                const int row = my_pkt * p.pEC + my_mblk * BLOCK_M;
-                // both buffers' stores in flight: chunk c is issued as soon as it is staged, and only then does the
-                // warp wait for the TMA to have read chunk c - 1, whose buffer the consumers refill with chunk c + 1
-                for (int c = 0; c < nchunks; ++c, ++chunk) {
-                    const int b = chunk & 1;
-                    mbar_wait(&stg_full[b], (chunk >> 1) & 1, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, 30 + b);
-                    tma_store_2d(&p.tm_a1, smem + OFF_EPI + b * EPI_CHUNK_BYTES, n0 + c * 64, row);
-                    bulk_commit_group();
-                    if (c > 0) {
-                        bulk_wait_group_read<1>();   // chunk c - 1 has been read: its buffer may be refilled
-                        mbar_arrive(&stg_free[b ^ 1]);
-                    }
-                }
-                bulk_wait_group_read<0>();
-                mbar_arrive(&stg_free[(chunk - 1) & 1]);
-                bulk_wait_group0();            // the tile's h writes (async proxy) are complete ...
-                fence_proxy_async_global();    // ... and ordered before the generic-proxy release below
-                red_release_gpu_add_u32(p.g0_done + (size_t)my_pkt * p.TCM + my_mblk, 1u);
-            } else if (kind == 1) {
-                mbar_wait(&pub_full[ps], pphase, p.dbg, p.timeout_ns, FM_TRAP_MBAR_PUB, 10 + ps);
-                mbar_arrive(&pub_empty[ps]);
-                if (++ps == 2) { ps = 0; pphase ^= 1; }
-                if (p.fused) {
-                    if (my_src == p.rank && p.out_acc == p.out) {
-                        // local packet, output left in place: nobody waits for a flag (see finish_fused) -- no fence,
-                        // no counter, no flag; kernel completion covers these adds
-                    } else {
-                    fence_acq_rel_sys();   // this tile's adds are performed before the packet counter moves
-                    const unsigned int old = atom_acq_rel_gpu_add_u32(p.pkt_done + my_pkt, 1u);
-                    const unsigned int want = (unsigned int)(((ti.cnt + BLOCK_M - 1) / BLOCK_M) * p.TN1);
-                    if (old + 1u == want) {   // every GEMM1 tile of packet (src, le) has been added into src's output
-                        st_release_sys_u64(p.peer_done_flag[my_src] + (size_t)(p.rank * p.nLx + ti.le),
-                                           (unsigned long long)L.epoch << 32);
-                    }
-                    }
-                } else {
-                    fence_acq_rel_sys();
-                    const unsigned int old = atom_acq_rel_gpu_add_u32(p.g1_done + (size_t)my_pkt * p.TCM + my_mblk, 1u);
-                    if (old == (unsigned int)p.TN1 - 1u) {  // whole rows of this block are on the source rank
-                        fence_acq_rel_sys();
-                        const int e_global = p.rank * p.nLx + ti.le;
-                        st_release_sys_u64(p.peer_ret_flag[my_src] + (size_t)e_global * p.TCM + my_mblk,
-                                           ((unsigned long long)L.epoch << 32) | (unsigned int)my_rows);
-                    }
-                }
-            }
-            if (kind >= 0 && ntiles < 16) trace_stamp(p, 96 + ntiles);
+            if (kind == 0) publish_h(p, smem, ti, chunk);
+            else if (kind == 1) publish_out(p, L, smem, ti, pub);
+            if (kind >= 0) trace_tile(p, TRACE_TILE_PUBLISHED, ntiles);
         }
         kind = __shfl_sync(0xffffffffu, kind, 0);
-        if (++q == NSCHED) { q = 0; qphase ^= 1; }
+        q.next();
         ++ntiles;
         if (kind < 0) break;
         __syncwarp();
@@ -1616,31 +1783,12 @@ __device__ __forceinline__ void ffn_publisher(const FmParams& p, const Launch& L
 // kernel prologue: barriers of every later phase; runs before the router so it costs nothing on the critical path.
 // Warp 3's L2 warm-up needs this launch's work list, so it runs after the block sync that publishes the Launch record.
 __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BARS);
     const int tid = threadIdx.x, warp = tid >> 5;
     if (warp == 1 && (tid & 31) == 0) {
-        // arrival counts: full = the producer's expect_tx; empty = one lane per consumer warp; pub_full and stg_full =
-        // one lane per consumer warp; stg_free = the publisher; sched_empty = every ring reader (producer, publisher,
-        // consumer warps)
-        for (int i = 0; i < STAGES; ++i) { mbar_init(&bars[BAR_FULL + i], 1); mbar_init(&bars[BAR_EMPTY + i], NUM_EPI_WARPS); }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&bars[BAR_PUB_FULL + i], NUM_EPI_WARPS);
-            mbar_init(&bars[BAR_PUB_EMPTY + i], 1);
-        }
-        for (int i = 0; i < EPI_BUFS; ++i) {
-            mbar_init(&bars[BAR_STG_FULL + i], NUM_EPI_WARPS);
-            mbar_init(&bars[BAR_STG_FREE + i], 1);
-        }
-        for (int i = 0; i < NSCHED; ++i) {
-            mbar_init(&bars[BAR_SCHED_FULL + i], 1);
-            mbar_init(&bars[BAR_SCHED_EMPTY + i], 2 + NUM_EPI_WARPS);
-            mbar_init(&bars[BAR_PROD_TAKE + i], 1);
-        }
-        mbar_init(&bars[BAR_XROWS], 1);
-        mbar_init(&bars[BAR_DISP_DONE], 1);
-        mbar_init(&bars[BAR_WG], 1);
-        mbar_init(&bars[BAR_REMOTE], 1);
-        for (int i = 0; i < GATE_STAGES; ++i) { mbar_init(&bars[BAR_GFULL + i], 1); mbar_init(&bars[BAR_GEMPTY + i], NUM_EPI_WARPS); }
+#define FM_MBAR_INIT(ID, name, first, count, arrivals) \
+        for (int i = 0; i < (count); ++i) mbar_init(bar(smem, (first) + i), (arrivals));
+        FM_MBARRIERS(FM_MBAR_INIT)
+#undef FM_MBAR_INIT
         fence_mbar_init();
     }
     if (warp == 0 && (tid & 31) == 0) {
@@ -1657,15 +1805,12 @@ __device__ __forceinline__ void ffn_warm_l2(const FmParams& p, const Launch& L) 
         // then L2 hits.  A wrong guess costs nothing -- the tile is needed by some CTA of the first wave anyway.
         const int id = (int)blockIdx.x;
         if (id < L.total_items) {
-            int cur = 0;
-            while (id >= block_start(p, L, p.blocks[cur + 1])) ++cur;
-            const TileBlock blk = p.blocks[cur];
-            const int local = id - block_start(p, L, blk);
-            const int nt = local / L.tcm_items, le = blk.pkt % p.nLx;
-            const CUtensorMap* tb = blk.kind == 0 ? &p.tm_b0 : &p.tm_b1;
-            const int b0 = (blk.kind == 0 ? le * 2 * p.P : (le * 2 + 1) * p.H) + nt * BLOCK_N;
-            const int nk_w = (blk.kind == 0 ? p.H : p.P) / BLOCK_K;
-            for (int kb = 0; kb < min(nk_w, STAGES); ++kb) tma_prefetch_l2_2d(tb, kb * BLOCK_K, b0);
+            int cursor = 0;
+            const WorkItem w = decode_item(p, L, id, cursor);
+            const int kind = w.blk.kind;
+            const CUtensorMap* tb = kind == 0 ? &p.tm_b0 : &p.tm_b1;
+            const int b0 = b_tile_row(p, kind, w.le, w.nt);
+            for (int kb = 0; kb < min(tile_kblocks(p, kind), STAGES); ++kb) tma_prefetch_l2_2d(tb, kb * BLOCK_K, b0);
         }
     }
 }
@@ -1688,21 +1833,20 @@ static_assert(128 * REGS_PROD + 256 * REGS_CONS <= 65536, "register file of one 
 // split again: the consumers hand their registers back before the block sync, warps 0-3 take theirs back after it (an
 // increase waits for free registers, so it must not come before every consumer's decrease).
 __device__ __forceinline__ void ffn_roles(const FmParams& p, const Launch& L, uint8_t* smem) {
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BARS);
     const int tid = threadIdx.x, warp = tid >> 5;
     if (warp < EPI_WARP0) {
         setmaxnreg_dec<REGS_PROD>();
-        if (warp == 0) ffn_producer(p, smem, bars);
-        else if (warp == 2) ffn_publisher(p, L, smem, bars);
-        else if (warp == 3) { if ((tid & 31) == 0) ffn_scheduler(p, L, smem, bars); __syncwarp(); }
+        if (warp == 0) ffn_producer(p, smem);
+        else if (warp == 2) ffn_publisher(p, L, smem);
+        else if (warp == 3) { if ((tid & 31) == 0) ffn_scheduler(p, L, smem); __syncwarp(); }
     } else {
         setmaxnreg_inc<REGS_CONS>();
-        ffn_consumer(p, smem, bars);
+        ffn_consumer(p, smem);
         setmaxnreg_dec<REGS_ALL>();
     }
     __syncthreads();
     if (warp < EPI_WARP0) setmaxnreg_inc<REGS_ALL>();
-    if (tid == 0) trace_stamp(p, 5);
+    if (tid == 0) trace_stamp(p, TRACE_FFN_END);
 }
 
 // ============================================================================================================
@@ -1790,7 +1934,7 @@ __device__ __forceinline__ void finish_fused(const FmParams& p, const Launch& L,
             g.tick(p.dbg, p.timeout_ns, FM_TRAP_RET_FLAG, e, 0xD0E, 0);
     }
     __syncthreads();
-    if (tid == 0) trace_stamp(p, 14);   // every expert's contributions to this rank's tokens are in
+    if (tid == 0) trace_stamp(p, TRACE_DONE_FLAGS);   // every expert's contributions to this rank's tokens are in
     if (p.out_acc != p.out) {
         for (int ti = warp; ti < n_tok; ti += NUM_WARPS) {
             const __nv_bfloat16* src = p.out_acc + (size_t)(t0 + ti) * p.H;
@@ -1863,7 +2007,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
     const int tid = threadIdx.x, warp = tid >> 5;
     Launch* launch_s = reinterpret_cast<Launch*>(smem + OFF_LAUNCH);
 
-    if (tid == 0) trace_stamp(p, 0);
+    if (tid == 0) trace_stamp(p, TRACE_START);
     if (tid == 2 * 32) resolve_launch(p, launch_s);   // (warp 2 has no part in the prologue)
     ffn_setup(p, smem);   // mbarriers for the later phases (visible to everyone after the next block sync)
     __syncthreads();
@@ -1889,9 +2033,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
         if (tid == 0) *p.claim = 0u;
     }
     if (p.dense) gate_phase_dense(p, L, t0, n_tok); else gate_phase(p, L, smem, t0, n_tok);
-    if (tid == 0) trace_stamp(p, 1);
+    if (tid == 0) trace_stamp(p, TRACE_GATE_DONE);
     grid_barrier(p, L);
-    if (tid == 0) trace_stamp(p, 2);
+    if (tid == 0) trace_stamp(p, TRACE_BARRIER);
     // every CTA has read the launch counter (resolve_launch, before its arrival at the barrier): advance it for the next
     // launch on the stream, and record this launch's token count beside it (fm_last_launch)
     if (blockIdx.x == 0 && tid == 0) {
@@ -1907,16 +2051,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
         if (!p.dense) dispatch_phase(p, L, smem, t0, n_tok);
         else if (warp == 2 && (tid & 31) == 0)   // nothing to copy: GEMM0's TMA reads x in place; release the producer
             mbar_arrive(bar(smem, BAR_DISP_DONE));
-        if (warp == 2 && (tid & 31) == 0) trace_stamp(p, 3);
+        if (warp == 2 && (tid & 31) == 0) trace_stamp(p, TRACE_DISPATCH_END);
     }
-    if (tid == EPI_WARP0 * 32) trace_stamp(p, 4);
+    if (tid == EPI_WARP0 * 32) trace_stamp(p, TRACE_FFN_START);
     ffn_roles(p, L, smem);
 
     __syncthreads();
     if (p.fused) finish_fused(p, L, t0, n_tok);
     else combine_phase(p, L, smem, t0, n_tok);
     __syncthreads();
-    if (tid == 0) trace_stamp(p, 6);
+    if (tid == 0) trace_stamp(p, TRACE_KERNEL_END);
 }
 
 }  // namespace fm

@@ -24,17 +24,13 @@ struct DebugRecord {          // lives in pinned, device-mapped host memory (rea
 
 enum : unsigned int {
     FM_TRAP_NONE = 0,
-    FM_TRAP_MBAR_FULL = 1,
-    FM_TRAP_MBAR_EMPTY = 2,
-    // 3, 4: no longer used
-    FM_TRAP_MBAR_SCHED_FULL = 5,
-    FM_TRAP_MBAR_SCHED_EMPTY = 6,
+    FM_TRAP_MBAR = 1,   // info0 = the barrier's id in the kernel's mbarrier table (fm_kernel.cuh), info1 = the parity
+    // 2-6 and 12: no longer used
     FM_TRAP_GRID_BARRIER = 7,
     FM_TRAP_RECV_FLAG = 8,
     FM_TRAP_G0_DONE = 9,
     FM_TRAP_RET_FLAG = 10,
     FM_TRAP_RECV_ROWS = 11,
-    FM_TRAP_MBAR_PUB = 12,
     // not a trap: the launch read a token count outside [0, S] from device memory and ran on 0 tokens (info0 = the
     // count, info1 = S).  The host reports it once and clears the record; the context stays usable.
     FM_STATUS_BAD_COUNT = 13,
@@ -114,10 +110,11 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
+// `id` only names the barrier in a timeout record
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, DebugRecord* dbg,
-                                          unsigned long long timeout_ns, unsigned int code, unsigned int info) {
+                                          unsigned long long timeout_ns, unsigned int id) {
     SpinGuard g;
-    while (!mbar_try_wait(bar, parity)) g.tick(dbg, timeout_ns, code, info, parity, 0);
+    while (!mbar_try_wait(bar, parity)) g.tick(dbg, timeout_ns, FM_TRAP_MBAR, id, parity, 0);
 }
 
 // named CTA barriers (id 0 is __syncthreads): the N threads that take part, whole warps, either wait (sync) or only

@@ -14,7 +14,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, trace_slots
 from .config import MoEConfig
 
 _BUFFER_SPECS = {
@@ -373,7 +373,7 @@ class MoEContext:
         npk = d["world"] * d["num_local_experts"]
         shapes = {"topk_idx": (S, k), "topk_w": (S, k), "mcw": (S,), "slot": (S, k), "counts": (E,),
                   "recv_x": (npk, d["pEC"], H), "hidden": (npk, d["pEC"], P), "ret_y": (E, d["pEC"], H),
-                  "gate_out": (S, E), "recv_cnt": (npk,), "trace": (d["grid"], 128), "aux_loss": (2 * E + 1,)}
+                  "gate_out": (S, E), "recv_cnt": (npk,), "trace": (d["grid"], trace_slots.SLOTS), "aux_loss": (2 * E + 1,)}
         return arr.reshape(shapes[name])
 
     @property

@@ -10,6 +10,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."
 import numpy as np
 import torch
 
+from flashmoe_b200 import trace_slots as ts
 from flashmoe_b200.config import BASELINE_CONFIGS, MoEConfig
 from flashmoe_b200.runtime import MoEContext
 
@@ -19,10 +20,12 @@ CFGS["small"] = MoEConfig(num_experts=8, expert_top_k=2, sequence_len=512, hidde
 
 def analyse(tr, cfg, label=""):
     tr = tr.astype(np.int64)
-    t00 = tr[:, 0].min()
+    t00 = tr[:, ts.START].min()
     us = lambda a: (a - t00) / 1e3  # noqa: E731
-    names = {0: "start", 11: "gate_gemv", 10: "zero_issued", 15: "topk_warp0", 12: "gate_topk", 1: "gate_done", 2: "barrier", 8: "disp_prefix", 9: "disp_rows_done",
-             3: "dispatch_end", 7: "first_tma_issued", 4: "ffn_start", 5: "ffn_end", 6: "kernel_end"}
+    names = {ts.START: "start", ts.GATE_LOGITS: "gate_gemv", ts.ZERO_ISSUED: "zero_issued", ts.TOPK_WARP0: "topk_warp0",
+             ts.GATE_TOPK: "gate_topk", ts.GATE_DONE: "gate_done", ts.BARRIER: "barrier", ts.DISP_PREFIX: "disp_prefix",
+             ts.DISP_ROWS_DONE: "disp_rows_done", ts.DISPATCH_END: "dispatch_end", ts.FIRST_TMA: "first_tma_issued",
+             ts.FFN_START: "ffn_start", ts.FFN_END: "ffn_end", ts.KERNEL_END: "kernel_end"}
     print(f"--- {label} phases (us after the first CTA's start; min / median / max over CTAs)")
     for i, nm in names.items():
         v = us(tr[:, i][tr[:, i] > 0])
@@ -30,18 +33,20 @@ def analyse(tr, cfg, label=""):
             print(f"  {nm:14s} {v.min():8.1f} {np.median(v):8.1f} {v.max():8.1f}")
     rows = []
     for c in range(tr.shape[0]):   # every CTA runs its own scheduler, producer and consumer warpgroups
-        n = int((tr[c, 32:48] > 0).sum())
+        n = int((tr[c, ts.TILE_FIRST_KB:ts.TILE_FIRST_KB + ts.TILES] > 0).sum())
         for i in range(n):
-            rows.append(dict(c=c, i=i, claim=tr[c, 112 + i], ready=tr[c, 16 + i], first=tr[c, 32 + i], mma=tr[c, 48 + i],
-                             epi=tr[c, 64 + i], stores=tr[c, 80 + i], pub=tr[c, 96 + i],
-                             prev_mma=tr[c, 48 + i - 1] if i else tr[c, 4]))
+            rows.append(dict(c=c, i=i, claim=tr[c, ts.TILE_CLAIMED + i], ready=tr[c, ts.TILE_READY + i],
+                             first=tr[c, ts.TILE_FIRST_KB + i], mma=tr[c, ts.TILE_MMA_DONE + i],
+                             epi=tr[c, ts.TILE_EPI_START + i], stores=tr[c, ts.TILE_STORES + i],
+                             pub=tr[c, ts.TILE_PUBLISHED + i],
+                             prev_mma=tr[c, ts.TILE_MMA_DONE + i - 1] if i else tr[c, ts.FFN_START]))
     if not rows:
         print("  no tile stamps")
         return
     span = np.array([r["mma"] - r["first"] for r in rows]) / 1e3
     nk = {0: cfg.H // 64, 1: cfg.P // 64}
     kinds = np.array([1 if s > 0.6 * span.max() and span.max() > 1.8 * span.min() else 0 for s in span])
-    print(f"--- {label} tiles recorded (first 16 per CTA): {len(rows)}; GEMM0-like {int((kinds == 0).sum())}, GEMM1-like {int((kinds == 1).sum())}")
+    print(f"--- {label} tiles recorded (first {ts.TILES} per CTA): {len(rows)}; GEMM0-like {int((kinds == 0).sum())}, GEMM1-like {int((kinds == 1).sum())}")
     for kd in (0, 1):
         sel = [r for r, k in zip(rows, kinds) if k == kd]
         if not sel:
@@ -63,7 +68,7 @@ def analyse(tr, cfg, label=""):
     if t0rows:
         g = lambda key: np.median([(r[key] - t00) / 1e3 for r in t0rows])  # noqa: E731
         print(f"  per CTA, first tile: claimed {g('claim'):.1f}, rows ready {g('ready'):.1f}, first k-block landed {g('first'):.1f} us (medians)")
-    # tensor-busy time per CTA over the FFN phase (only the first 16 tiles of a CTA are stamped)
+    # tensor-busy time per CTA over the FFN phase (only the first ts.TILES tiles of a CTA are stamped)
     busy = {}
     for r in rows:
         busy[r["c"]] = busy.get(r["c"], 0) + (r["mma"] - r["first"])
@@ -72,7 +77,7 @@ def analyse(tr, cfg, label=""):
     t_last = np.array([max(r["mma"] for r in rows if r["c"] == c) for c in busy]) - t00
     print(f"  per CTA: mainloop-busy med {np.median(b):.1f} us; first k-block landed at med {np.median(t_first) / 1e3:.1f} "
           f"(min {t_first.min() / 1e3:.1f}, max {t_first.max() / 1e3:.1f}) us; last MMA complete med {np.median(t_last) / 1e3:.1f} max {t_last.max() / 1e3:.1f} us; "
-          f"kernel end {us(tr[:, 6].max()):.1f} us")
+          f"kernel end {us(tr[:, ts.KERNEL_END].max()):.1f} us")
 
 
 def main():

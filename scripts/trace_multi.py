@@ -10,6 +10,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from flashmoe_b200 import trace_slots as ts
 from flashmoe_b200.config import BASELINE_CONFIGS
 from flashmoe_b200.runtime import MoEContext, env_rank_world
 
@@ -51,22 +52,23 @@ def main():
         ctx.forward(x, wg, we, out=out)
     ctx.synchronize()
     tr = ctx.read("trace").astype(np.int64)
-    t00 = tr[:, 0].min()
+    t00 = tr[:, ts.START].min()
     us = lambda a: (a - t00) / 1e3  # noqa: E731
     rec = {}
-    for key, col, red in (("start_spread", 0, "max"), ("gate_done", 1, "med"), ("barrier", 2, "med"), ("disp_prefix", 8, "med"),
-                          ("disp_rows_done", 9, "med"), ("dispatch_end_max", 3, "max"), ("ffn_end_med", 5, "med"),
-                          ("done_flags_seen", 14, "med"), ("kernel_end", 6, "max")):
+    for key, col, red in (("start_spread", ts.START, "max"), ("gate_done", ts.GATE_DONE, "med"), ("barrier", ts.BARRIER, "med"),
+                          ("disp_prefix", ts.DISP_PREFIX, "med"), ("disp_rows_done", ts.DISP_ROWS_DONE, "med"),
+                          ("dispatch_end_max", ts.DISPATCH_END, "max"), ("ffn_end_med", ts.FFN_END, "med"),
+                          ("done_flags_seen", ts.DONE_FLAGS, "med"), ("kernel_end", ts.KERNEL_END, "max")):
         v = tr[:, col][tr[:, col] > 0]
         rec[key] = float(us(np.median(v) if red == "med" else v.max())) if len(v) else float("nan")
-    first_landed = tr[:, 32][tr[:, 32] > 0]
+    first_landed = tr[:, ts.TILE_FIRST_KB][tr[:, ts.TILE_FIRST_KB] > 0]
     rec["first_tile_kb0_landed_min"] = float(us(first_landed.min())) if len(first_landed) else float("nan")
     rec["first_tile_kb0_landed_med"] = float(us(np.median(first_landed))) if len(first_landed) else float("nan")
-    rem = tr[:, 13][tr[:, 13] > 0]
+    rem = tr[:, ts.FIRST_REMOTE][tr[:, ts.FIRST_REMOTE] > 0]
     rec["first_remote_tile_ready_min"] = float(us(rem.min())) if len(rem) else float("nan")
-    pub = tr[:, 96:112]
+    pub = tr[:, ts.TILE_PUBLISHED:ts.TILE_PUBLISHED + ts.TILES]
     rec["last_tile_published"] = float(us(pub.max())) if (pub > 0).any() else float("nan")
-    mma = tr[:, 48:64]   # MMA complete, per tile
+    mma = tr[:, ts.TILE_MMA_DONE:ts.TILE_MMA_DONE + ts.TILES]   # MMA complete, per tile
     rec["last_mma_complete"] = float(us(mma.max())) if (mma > 0).any() else float("nan")
     rec["abs_start_ns"] = int(t00)
     allr = [None] * world
