@@ -22,7 +22,7 @@ BUF_TOPK_IDX, BUF_TOPK_W, BUF_MCW, BUF_SLOT, BUF_COUNTS, BUF_RECV_X, BUF_HIDDEN,
 EXPORTED_SYMBOLS = (
     "fm_compiled_config", "fm_create", "fm_destroy", "fm_get_dims", "fm_num_local_experts", "fm_symm_size",
     "fm_symm_local_ptr", "fm_symm_export", "fm_symm_attach_ipc", "fm_symm_attach_ptrs", "fm_symm_use_external",
-    "fm_moe_forward", "fm_moe_forward_tokens", "fm_moe_forward_tokens_dev", "fm_last_launch", "fm_output_buffer", "fm_moe_forward_host", "fm_host_submit", "fm_host_wait", "fm_check", "fm_set_timeout_ms", "fm_set_trace", "fm_launch_count",
+    "fm_moe_forward", "fm_moe_forward_tokens", "fm_moe_forward_tokens_dev", "fm_moe_forward_routed", "fm_last_launch", "fm_output_buffer", "fm_moe_forward_host", "fm_host_submit", "fm_host_wait", "fm_check", "fm_set_timeout_ms", "fm_set_trace", "fm_launch_count",
     "fm_buffer_bytes",
     "fm_read_buffer", "fm_last_error", "fm_version",
 )
@@ -75,6 +75,7 @@ def load() -> ctypes.CDLL:
     L.fm_moe_forward.argtypes = [vp, cvp, cvp, cvp, cvp, cvp, vp, vp]
     L.fm_moe_forward_tokens.argtypes = [vp, cvp, ctypes.c_int, cvp, cvp, cvp, cvp, vp, vp]
     L.fm_moe_forward_tokens_dev.argtypes = [vp, cvp, cvp, cvp, cvp, cvp, cvp, vp, vp]
+    L.fm_moe_forward_routed.argtypes = [vp, cvp, ctypes.c_int, cvp, cvp, cvp, cvp, cvp, cvp, vp, vp]
     L.fm_last_launch.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_int32)]
     L.fm_moe_forward_host.argtypes = [vp, cvp, cvp, cvp, cvp, cvp, vp, vp]
     L.fm_output_buffer.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t)]

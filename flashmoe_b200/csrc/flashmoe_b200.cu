@@ -117,7 +117,8 @@ struct fm_ctx {
     int* counts = nullptr;
     __nv_bfloat16* gate_out = nullptr;
     int* chunk_counts = nullptr;
-    // [0] unused, [1] claim, [2..3] grid barrier (u64), [4..5] launch counter (u64), [6] token count of the last launch
+    // [0] unused, [1] claim, [2..3] grid barrier (u64), [4..5] launch counter (u64), [6] token count of the last launch,
+    // [7] epoch of the last routed launch that reported a bad expert index (FmParams::status_word)
     unsigned int* ctrl = nullptr;
     unsigned int* g0_done = nullptr;
     unsigned int* g1_done = nullptr;
@@ -240,6 +241,12 @@ int check_kernel_status(fm_ctx* c) {
         memset(c->dbg_host, 0, sizeof(fm::DebugRecord));
         return fail(FM_EINVAL, "device token count n_tokens = %d not in [0, S = %d]: that launch ran on 0 tokens", n, S);
     }
+    if (c->dbg_host != nullptr && c->dbg_host->code == fm::FM_STATUS_BAD_EXPERT) {   // (not a fault either)
+        const int t = (int)c->dbg_host->info0, j = (int)c->dbg_host->info1, e = (int)c->dbg_host->info2;
+        memset(c->dbg_host, 0, sizeof(fm::DebugRecord));
+        return fail(FM_EINVAL, "topk_idx[%d, %d] = %d not in [-1, E = %d): a routed launch treated that pick as -1", t, j, e,
+                    c->d.E);
+    }
     if (c->dbg_host != nullptr && c->dbg_host->code == fm::FM_TRAP_MBAR) {
         const fm::DebugRecord r = *c->dbg_host;
         const fm::MbarName b = fm::mbar_name((int)r.info0);
@@ -270,18 +277,32 @@ int check_kernel_status(fm_ctx* c) {
 // maps over x have n_tok rows.  The kernel derives everything that depends on n and on the launch's place in the
 // context's sequence of launches itself (fm_kernel.cuh, struct Launch), so the parameters built here are valid for
 // every replay of a captured launch, and this function issues nothing that stream capture forbids.
-int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* gate_w, const void* expert_w,
-           const void* bias_up, const void* bias_down, void* out, cudaStream_t stream) {
+// `routed`: caller routing (fm_moe_forward_routed) -- phase G reads the picks and weights from topk_idx / topk_w [n, k]
+// instead of running the router, and there are no gate weights (gate_w is NULL).
+int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* gate_w, bool routed, const int32_t* topk_idx,
+           const float* topk_w, const void* expert_w, const void* bias_up, const void* bias_down, void* out,
+           cudaStream_t stream) {
     if (c == nullptr) return fail(FM_EINVAL, "null context");
     if (n_tok < 0 || n_tok > c->d.S) return fail(FM_EINVAL, "n_tokens = %d not in [0, S = %d]", n_tok, c->d.S);
-    if (gate_w == nullptr || expert_w == nullptr || (n_tok > 0 && (x == nullptr || out == nullptr)))
+    if (routed) {
+        if (c->d.E == 1) return fail(FM_EINVAL, "caller routing needs num_experts > 1: an E = 1 context has no router to replace");
+        if (c->aux != nullptr)
+            return fail(FM_EINVAL, "caller routing is not available with is_training = 1: the auxiliary loss needs the "
+                                   "router's probabilities");
+        if (n_tok > 0 && (topk_idx == nullptr || topk_w == nullptr))
+            return fail(FM_EINVAL, "topk_idx and topk_w must be non-null device pointers");
+    } else if (gate_w == nullptr) {
         return fail(FM_EINVAL, "x, gate_w, expert_w and out must be non-null device pointers");
+    }
+    if (expert_w == nullptr || (n_tok > 0 && (x == nullptr || out == nullptr)))
+        return fail(FM_EINVAL, routed ? "x, expert_w and out must be non-null device pointers"
+                                      : "x, gate_w, expert_w and out must be non-null device pointers");
     if (reinterpret_cast<uintptr_t>(n_dev) % alignof(int))
         return fail(FM_EINVAL, "n_tokens_dev must be 4-byte aligned (got %p)", static_cast<const void*>(n_dev));
     {   // TMA tensor maps, cp.async.bulk row copies and the 16-byte vector accesses all need 16-byte aligned bases
-        const void* ptrs[] = {x, gate_w, expert_w, bias_up, bias_down, out};
-        const char* names[] = {"x", "gate_w", "expert_w", "bias_up", "bias_down", "out"};
-        for (int i = 0; i < 6; ++i)
+        const void* ptrs[] = {x, gate_w, expert_w, bias_up, bias_down, out, topk_idx, topk_w};
+        const char* names[] = {"x", "gate_w", "expert_w", "bias_up", "bias_down", "out", "topk_idx", "topk_w"};
+        for (int i = 0; i < 8; ++i)
             if (reinterpret_cast<uintptr_t>(ptrs[i]) % 16)
                 return fail(FM_EINVAL, "%s must be 16-byte aligned (got %p)", names[i], ptrs[i]);
     }
@@ -297,7 +318,7 @@ int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* ga
         c->cached_x = x;
         c->cached_x_rows = n_tok;
     }
-    if (c->tc_gate) {
+    if (c->tc_gate && !routed) {
         // router on tensor cores: x as [n_tok, H] in 32-row boxes, Wg_eff = the [H, E] tensor read flat as [E, H]
         // (python_bindings.cu:93-99, moe.cuh:107-109) in boxes of min(128, E rounded up to 64) rows; rows past E read as
         // zero
@@ -331,7 +352,7 @@ int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* ga
     fm::FmParams p;
     memset(&p, 0, sizeof(p));
     p.tm_a0 = c->tm_a0; p.tm_b0 = c->tm_b0; p.tm_a1 = c->tm_a1; p.tm_b1 = c->tm_b1;
-    if (c->tc_gate) { p.tm_gx = c->tm_gx; p.tm_gw = c->tm_gw; }
+    if (c->tc_gate && !routed) { p.tm_gx = c->tm_gx; p.tm_gw = c->tm_gw; }   // (a routed launch has no router maps)
     p.tc_gate = c->tc_gate ? 1 : 0;
     p.n_tokens = n_tok; p.n_tokens_dev = n_dev;
     p.H = d.H; p.P = d.P; p.E = d.E; p.k = d.k; p.W = d.world; p.rank = d.rank; p.nLx = nLx;
@@ -370,6 +391,10 @@ int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* ga
     if (d.world == 1) p.peer_out_acc[0] = p.out;
     p.aux = c->aux;
     p.dense = c->dense ? 1 : 0;
+    p.routed = routed ? 1 : 0;
+    p.routed_idx = topk_idx;
+    p.routed_w = topk_w;
+    p.status_word = c->ctrl + 7;
     p.dbg = c->dbg_dev;
     p.trace = c->trace_on ? c->trace : nullptr;
 
@@ -746,7 +771,8 @@ FM_API int fm_symm_attach_ptrs(fm_ctx_t* ctx, void* const* peer_bases) {
 
 FM_API int fm_moe_forward_tokens(fm_ctx_t* ctx, const void* x, int n_tokens, const void* gate_w, const void* expert_w,
                                  const void* bias_up, const void* bias_down, void* out, void* stream) {
-    return launch(ctx, x, n_tokens, nullptr, gate_w, expert_w, bias_up, bias_down, out, static_cast<cudaStream_t>(stream));
+    return launch(ctx, x, n_tokens, nullptr, gate_w, false, nullptr, nullptr, expert_w, bias_up, bias_down, out,
+                  static_cast<cudaStream_t>(stream));
 }
 
 FM_API int fm_moe_forward_tokens_dev(fm_ctx_t* ctx, const void* x, const int32_t* n_tokens_dev, const void* gate_w,
@@ -756,7 +782,18 @@ FM_API int fm_moe_forward_tokens_dev(fm_ctx_t* ctx, const void* x, const int32_t
     if (n_tokens_dev == nullptr) return fail(FM_EINVAL, "n_tokens_dev must be a device pointer to one int32");
     if (x == nullptr || out == nullptr)
         return fail(FM_EINVAL, "x and out must be non-null device pointers to S = %d rows", ctx->d.S);
-    return launch(ctx, x, ctx->d.S, n_tokens_dev, gate_w, expert_w, bias_up, bias_down, out,
+    return launch(ctx, x, ctx->d.S, n_tokens_dev, gate_w, false, nullptr, nullptr, expert_w, bias_up, bias_down, out,
+                  static_cast<cudaStream_t>(stream));
+}
+
+FM_API int fm_moe_forward_routed(fm_ctx_t* ctx, const void* x, int n_tokens, const int32_t* n_tokens_dev,
+                                 const int32_t* topk_idx, const float* topk_w, const void* expert_w,
+                                 const void* bias_up, const void* bias_down, void* out, void* stream) {
+    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
+    if (n_tokens_dev != nullptr && n_tokens != ctx->d.S)
+        return fail(FM_EINVAL, "with n_tokens_dev, n_tokens must be S = %d (the rows of x, out and the routing arrays); "
+                               "got %d", ctx->d.S, n_tokens);
+    return launch(ctx, x, n_tokens, n_tokens_dev, nullptr, true, topk_idx, topk_w, expert_w, bias_up, bias_down, out,
                   static_cast<cudaStream_t>(stream));
 }
 
@@ -806,7 +843,9 @@ FM_API int fm_host_submit(fm_ctx_t* ctx, const void* x_host, const void* gate_w,
     FM_CUDA(cudaMemcpyAsync(ctx->x_stage[slot], x_host, bytes, cudaMemcpyHostToDevice, ctx->s_h2d));
     FM_CUDA(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
     FM_CUDA(cudaStreamWaitEvent(s, ctx->ev_h2d[slot], 0));
-    if ((rc = launch(ctx, ctx->x_stage[slot], ctx->d.S, nullptr, gate_w, expert_w, bias_up, bias_down, ctx->out_stage[slot], s))) return rc;
+    if ((rc = launch(ctx, ctx->x_stage[slot], ctx->d.S, nullptr, gate_w, false, nullptr, nullptr, expert_w, bias_up,
+                     bias_down, ctx->out_stage[slot], s)))
+        return rc;
     FM_CUDA(cudaEventRecord(ctx->ev_kernel[slot], s));
     FM_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_kernel[slot], 0));
     FM_CUDA(cudaMemcpyAsync(out_host, ctx->out_stage[slot], bytes, cudaMemcpyDeviceToHost, ctx->s_d2h));

@@ -4,6 +4,7 @@
 //
 //   prologue  mbarriers for the later phases (off the critical path)
 //   phase G   router    x.Wg^T -> online softmax -> top-k -> capacity slots         (reference moe/gate.cuh:473-720)
+//             (or the caller's top-k ids and weights -> capacity slots: fm_moe_forward_routed)
 //             grid barrier (the only one, like the reference's gate.cuh:761)
 //   phase D   dispatch  token rows -> owner rank's receive buffer over NVLink (TMA bulk copies) + one flag per expert
 //                                                                                    (reference os/packet.cuh:21-286)
@@ -343,6 +344,13 @@ struct FmParams {
     // gMeC[E] mean routed fraction per expert, loss} (reference moe/gate.cuh:608-635,698-706,763-773); nullptr otherwise
     float* aux;
     int dense;          // E == 1: no router GEMV, no dispatch copy; GEMM0 reads x in place (reference moe/fffn.cuh:31-167)
+    // caller routing (fm_moe_forward_routed, routed != 0): phase G takes the picks and weights from these [n, k] arrays
+    // instead of the router; -1 = no expert.  status_word: the election of the one thread that reports an index outside
+    // [-1, E) in a launch (atomicExch of the epoch)
+    int routed;
+    const int* routed_idx;
+    const float* routed_w;
+    unsigned int* status_word;
     DebugRecord* dbg;
     unsigned long long* trace;  // optional [grid][TRACE_SLOTS] %globaltimer stamps (nullptr = off)
 };
@@ -807,7 +815,8 @@ __device__ __forceinline__ void softmax_topk(const FmParams& p, float* logit_s, 
 // Position of every (token, pick) among this chunk's selections of the same expert, ascending (token, pick) order, and
 // the chunk's per-expert counts.  One warp walks the entries 32 at a time: lanes holding the same expert find each other
 // with match.any, the rank inside the group is a popcount, the running per-expert count lives in shared memory (O(n)
-// instead of O(n^2); the 64k-token sweep point has 886 entries per CTA).
+// instead of O(n^2); the 64k-token sweep point has 886 entries per CTA).  A skipped pick of a routed launch (-1) takes no
+// rank and is not counted.
 __device__ __forceinline__ void slot_ranks(const FmParams& p, uint8_t* smem, int n_tok) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int E = p.E, k = p.k;
@@ -820,8 +829,9 @@ __device__ __forceinline__ void slot_ranks(const FmParams& p, uint8_t* smem, int
     if (warp == 0) {
         for (int i0 = 0; i0 < n_ent; i0 += 32) {
             const int i = i0 + lane;
-            const bool valid = i < n_ent;
-            const int e = valid ? (int)sel_e[i] : (E + lane);        // invalid lanes get unique keys
+            const int sel = i < n_ent ? (int)sel_e[i] : -1;
+            const bool valid = sel >= 0;
+            const int e = valid ? sel : (E + lane);                  // lanes without a pick get unique keys
             const unsigned int same = __match_any_sync(0xffffffffu, e);
             const unsigned int before = same & ((1u << lane) - 1u);
             if (valid) rank_s[i] = cnt_s[e] + __popc(before);
@@ -834,9 +844,25 @@ __device__ __forceinline__ void slot_ranks(const FmParams& p, uint8_t* smem, int
     for (int e = tid; e < E; e += NUM_THREADS) p.chunk_counts[(size_t)blockIdx.x * E + e] = cnt_s[e];
 }
 
+// The end of phase G once sel_e holds the chunk's picks (router and caller routing alike).  The Wg / logits scratch is
+// free from here on: start staging this chunk's token rows for the dispatch phase now (one bulk load, same barrier and
+// layout dispatch_phase expects for its first group), so the load runs under the slot ranks, the grid barrier and the
+// prefix pass instead of after them.
+__device__ __forceinline__ void gate_tail(const FmParams& p, uint8_t* smem, int t0, int n_tok) {
+    if (threadIdx.x == 32 && n_tok > 0) {   // (warp 1: warp 0 is about to compute the slot ranks)
+        const int row_bytes = p.H * 2;
+        const int rows0 = max(1, min(n_tok, D_XROWS_BYTES / row_bytes));
+        uint64_t* xbar = bar(smem, BAR_XROWS);
+        fence_proxy_async_smem();
+        mbar_arrive_expect_tx(xbar, (uint32_t)(rows0 * row_bytes));
+        bulk_load_1d(smem + D_OFF_XROWS, p.x + (size_t)t0 * p.H, (uint32_t)(rows0 * row_bytes), xbar);
+    }
+    slot_ranks(p, smem, n_tok);
+}
+
 __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int E = p.E, H = p.H;
+    const int E = p.E;
     float* logit_s = reinterpret_cast<float*>(smem + G_OFF_LOGIT);
     int16_t* sel_e = reinterpret_cast<int16_t*>(smem + G_OFF_SEL);
 
@@ -882,22 +908,62 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, u
         }
     }
     if (tid == 0) trace_stamp(p, TRACE_GATE_TOPK);
-    // The Wg / logits scratch is free from here on: start staging this chunk's token rows for the dispatch phase now
-    // (one bulk load, same barrier and layout dispatch_phase expects for its first group), so the load runs under the
-    // slot ranks, the grid barrier and the prefix pass instead of after them.
-    if (tid == 32 && n_tok > 0) {   // (warp 1: warp 0 is about to compute the slot ranks)
-        const int row_bytes = H * 2;
-        const int rows0 = max(1, min(n_tok, D_XROWS_BYTES / row_bytes));
-        uint64_t* xbar = bar(smem, BAR_XROWS);
-        fence_proxy_async_smem();
-        mbar_arrive_expect_tx(xbar, (uint32_t)(rows0 * row_bytes));
-        bulk_load_1d(smem + D_OFF_XROWS, p.x + (size_t)t0 * H, (uint32_t)(rows0 * row_bytes), xbar);
-    }
+    gate_tail(p, smem, t0, n_tok);
     if (p.aux != nullptr && L.S > 0) {   // gML[e] += (sum over this chunk) / S   (gate.cuh:628-634: atomicAdd(gML + e, colAgg / S))
         float* gml = p.aux + (size_t)(L.epoch & 1u) * (2 * E + 1);
         for (int e = tid; e < E; e += NUM_THREADS) atomicAdd(gml + e, __fdividef(aux_s[e], (float)L.S));
     }
-    slot_ranks(p, smem, n_tok);
+}
+
+// Entry gi of a routed launch's [n, k] arrays names expert e outside [-1, E).  The first thread of the launch to get here
+// (atomicExch of the epoch on a device word) writes the status record, so the message comes from one thread.
+__device__ __noinline__ void report_bad_expert(const FmParams& p, unsigned int epoch, int gi, int e) {
+    if (atomicExch(p.status_word, epoch) != epoch)
+        fm_record(p.dbg, FM_STATUS_BAD_EXPERT, (unsigned int)(gi / p.k), (unsigned int)(gi % p.k), (unsigned int)e, 0);
+}
+
+// Caller routing (fm_moe_forward_routed): the chunk's n_tok * k picks and weights come from routed_idx / routed_w
+// [n, k].  An index outside [-1, E) becomes -1 (no expert) and is reported once per launch -- it must not trap, every
+// rank takes part in the collective.  Writes topk_idx, topk_w = rne_bf16(w), mcw = 1 and sel_e; gate_out is not written.
+// With mcw = 1 the combine's term rne(w~ * rne(y / 1)) is rne(w~ * y) for every normal bf16 y.  Out of line on purpose:
+// inlined into the kernel it raised the kernel's spill loads from 544 to 596 B.
+__device__ __noinline__ void gate_phase_routed(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok) {
+    const int tid = threadIdx.x, warp = tid >> 5;
+    const int E = p.E, k = p.k;
+    int16_t* sel_e = reinterpret_cast<int16_t*>(smem + G_OFF_SEL);
+    // no gate-weight load to stay behind here: the output-row zero-fill goes first
+    if (p.fused && warp == NUM_WARPS - 1) zero_fill_out_rows(p, smem, t0, n_tok);
+    const int first = t0 * k, n_ent = n_tok * k;   // entries [first, first + n_ent) of the [n, k] arrays
+    auto route = [&](int i, int e, float w) {      // i: entry of the chunk
+        if (e < -1 || e >= E) {
+            report_bad_expert(p, L.epoch, first + i, e);
+            e = -1;
+        }
+        p.topk_idx[first + i] = e;
+        p.topk_w[first + i] = __float2bfloat16_rn(w);
+        sel_e[i] = (int16_t)e;
+    };
+    // 16-byte loads of the whole aligned quads of entries (the arrays start 16-byte aligned), single loads of the
+    // chunk's unaligned head and tail, so no entry outside the chunk is read
+    const int head = min(n_ent, (4 - (first & 3)) & 3);
+    const int nq = (n_ent - head) >> 2;
+    for (int q = tid; q < nq; q += NUM_THREADS) {
+        const int i = head + 4 * q;
+        const uint4 e4 = ld_global_nc_v4(p.routed_idx + first + i);
+        const uint4 w4 = ld_global_nc_v4(p.routed_w + first + i);
+        route(i, (int)e4.x, __uint_as_float(w4.x));
+        route(i + 1, (int)e4.y, __uint_as_float(w4.y));
+        route(i + 2, (int)e4.z, __uint_as_float(w4.z));
+        route(i + 3, (int)e4.w, __uint_as_float(w4.w));
+    }
+    const int tail0 = head + 4 * nq;
+    for (int i = tid; i < head + (n_ent - tail0); i += NUM_THREADS) {
+        const int j = i < head ? i : tail0 + (i - head);
+        route(j, p.routed_idx[first + j], p.routed_w[first + j]);
+    }
+    for (int i = tid; i < n_tok; i += NUM_THREADS) p.mcw[t0 + i] = 1.0f;
+    if (tid == 0) trace_stamp(p, TRACE_GATE_TOPK);
+    gate_tail(p, smem, t0, n_tok);   // (its first block sync orders the sel_e writes before the slot ranks)
 }
 
 // ============================================================================================================
@@ -1039,7 +1105,8 @@ __device__ __forceinline__ void dispatch_local_rows(const FmParams& p, const Lau
             const int tl = i / k, j = i - tl * k;
             const int ti = g0 + tl, t = t0 + ti;
             const int e = sel_e[ti * k + j];
-            const int s = base_s[e] + rank_s[ti * k + j];
+            // a skipped pick (-1, caller routing) gets slot INT32_MAX: every reader of p.slot takes slot >= EC as dropped
+            const int s = e < 0 ? INT32_MAX : base_s[e] + rank_s[ti * k + j];
             p.slot[(size_t)t * k + j] = s;
             if (s < EC) {
                 const int owner = e / p.nLx, le = e - owner * p.nLx;
@@ -1656,7 +1723,8 @@ __device__ __forceinline__ void epilogue_out(const FmParams& p, uint8_t* smem, c
         with_bias(da.bias, [&](auto has_bias) {
             constexpr bool B = decltype(has_bias)::value;
             if (!fuse) drain_accumulator<EPI_G1_STORE, B>(p, da, acc);
-            else if (p.k > 1) drain_accumulator<EPI_G1_FUSED_ADD, B>(p, da, acc);
+            // (caller routing scales k = 1 too: one add of rne(w~ * y) onto the zero-filled row is exact)
+            else if (p.k > 1 || p.routed) drain_accumulator<EPI_G1_FUSED_ADD, B>(p, da, acc);
             else drain_accumulator<EPI_G1_FUSED_COPY, B>(p, da, acc);
         });
     }
@@ -1854,6 +1922,7 @@ __device__ __forceinline__ void ffn_roles(const FmParams& p, const Launch& L, ui
 // finish_fused below).  For token t with picks (e_j, slot_j):
 //   k > 1: out[t,c] = bf16-accumulate over kept j of rne( p~_j * rne( y_j[c] / mCw ) )   (processor.cuh:110-169)
 //   k = 1: out[t,:] = y_0 (no scaling), zeros if dropped                                  (processor.cuh:170-203)
+//          (caller routing scales k = 1 like k > 1, with mCw = 1)
 // Deterministic gather (no atomics, no zero-fill pass); for k == 2 it equals the reference's atomicAdd result
 // exactly because bf16 addition commutes and 0 + a is exact.
 // ============================================================================================================
@@ -1982,7 +2051,7 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, const Launch& L
     }
     for (int i = tid; i < n_tok; i += NUM_THREADS) c_m[i] = p.mcw[t0 + i];
     __syncthreads();
-    if (k == 1) {
+    if (k == 1 && !p.routed) {
         for (int ti = warp; ti < n_tok; ti += NUM_WARPS) {
             const bool keep = c_s[ti] < EC;
             const __nv_bfloat16* yrow = p.ret_y + ((size_t)c_e[ti] * p.pEC + (keep ? c_s[ti] : 0)) * H;
@@ -1993,7 +2062,7 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, const Launch& L
                 st_global_v4(orow + h, v);
             }
         }
-    } else if (k == 2) {
+    } else if (k <= 2) {   // (k = 1 with caller routing: the scaled term rne(w~ * y))
         combine_rows<2, 4>(p, EC, t0, n_tok, c_e, c_s, c_w, c_m);
     } else {
         combine_rows<8, 1>(p, EC, t0, n_tok, c_e, c_s, c_w, c_m);
@@ -2032,7 +2101,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
         }
         if (tid == 0) *p.claim = 0u;
     }
-    if (p.dense) gate_phase_dense(p, L, t0, n_tok); else gate_phase(p, L, smem, t0, n_tok);
+    if (p.dense) gate_phase_dense(p, L, t0, n_tok);
+    else if (p.routed) gate_phase_routed(p, L, smem, t0, n_tok);
+    else gate_phase(p, L, smem, t0, n_tok);
     if (tid == 0) trace_stamp(p, TRACE_GATE_DONE);
     grid_barrier(p, L);
     if (tid == 0) trace_stamp(p, TRACE_BARRIER);

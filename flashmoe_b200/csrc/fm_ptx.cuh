@@ -34,6 +34,9 @@ enum : unsigned int {
     // not a trap: the launch read a token count outside [0, S] from device memory and ran on 0 tokens (info0 = the
     // count, info1 = S).  The host reports it once and clears the record; the context stays usable.
     FM_STATUS_BAD_COUNT = 13,
+    // not a trap: a routed launch read an expert index outside [-1, E) and treated that pick as -1 (info0 = the token,
+    // info1 = the pick, info2 = the index).  Reported once like FM_STATUS_BAD_COUNT.
+    FM_STATUS_BAD_EXPERT = 14,
 };
 
 // plain stores to pinned host memory (no PCIe atomics needed); first writer wins loosely

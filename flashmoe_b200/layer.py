@@ -15,8 +15,10 @@ from .runtime import MoEContext
 class MoEOutput(NamedTuple):
     out: torch.Tensor                 # [B, T, H] bf16
     topk_idx: torch.Tensor            # [B*T, k] int32   expert picked per token, in pick order
-    topk_weight: torch.Tensor         # [B*T, k] bf16    gateOut[t, e_j] (bf16-rounded softmax probability)
+    topk_weight: torch.Tensor         # [B*T, k] bf16    gateOut[t, e_j] (bf16-rounded softmax probability); after a
+                                      #                  routed call the caller's weights rounded to bf16
     slot: torch.Tensor                # [B*T, k] int32   slot in the (rank, expert) packet; >= capacity means dropped
+                                      #                  (INT32_MAX for a -1 pick of a routed call)
     aux_loss: Optional[torch.Tensor] = None   # is_training = 1: f32 [2E+1] = gML[E] | gMeC[E] | load-balancing loss
 
 
@@ -48,16 +50,31 @@ class FlashMoELayer(torch.nn.Module):
             self.bias_down = None
 
     @torch.no_grad()
-    def forward(self, x: torch.Tensor, return_routing: bool = False, n_tokens: Optional[torch.Tensor] = None):
+    def forward(self, x: torch.Tensor, return_routing: bool = False, n_tokens: Optional[torch.Tensor] = None,
+                topk_idx: Optional[torch.Tensor] = None, topk_weight: Optional[torch.Tensor] = None):
         """x [B, T, H] bf16 on this layer's device with B*T <= S (the capacity is that of B*T tokens,
         `cfg.EC_of(B*T)`).  Asynchronous on torch's current stream unless `return_routing` (reading the routing tables
         synchronises).  `n_tokens`: a one-element int32 tensor on the device with the token count n; x then holds
         B*T = S rows of which the first n are the tokens (see `MoEContext.forward_tokens`), and the call can be captured
-        once in a CUDA graph and replayed for any n.  The routing tables then hold the n rows of the last launch."""
+        once in a CUDA graph and replayed for any n.  The routing tables then hold the n rows of the last launch.
+
+        `topk_idx` / `topk_weight` [B*T, k] (both or neither): the caller's routing instead of this layer's gate
+        (`MoEContext.forward_routed`; -1 = no expert, k = 1 is scaled by its weight too).  The indices may be any
+        integer type (int64 from `torch.topk` is converted to int32), the weights any floating type (converted to
+        float32); `gate_weight` is not used."""
         if x.dim() != 3:
             raise RuntimeError("Input must be 3D [batch, seq, H]")
-        out = self.ctx.forward_tokens(x, self.gate_weight, self.expert_weight, bias_up=self.bias_up,
-                                      bias_down=self.bias_down, n_tokens=n_tokens)
+        if (topk_idx is None) != (topk_weight is None):
+            raise RuntimeError("pass both topk_idx and topk_weight, or neither")
+        if topk_idx is not None:
+            if topk_idx.is_floating_point() or not topk_weight.is_floating_point():
+                raise RuntimeError("topk_idx must be an integer tensor and topk_weight a floating-point one")
+            out = self.ctx.forward_routed(x, topk_idx.to(torch.int32).contiguous(),
+                                          topk_weight.to(torch.float32).contiguous(), self.expert_weight,
+                                          bias_up=self.bias_up, bias_down=self.bias_down, n_tokens=n_tokens)
+        else:
+            out = self.ctx.forward_tokens(x, self.gate_weight, self.expert_weight, bias_up=self.bias_up,
+                                          bias_down=self.bias_down, n_tokens=n_tokens)
         if not return_routing:
             return out
         return self.routing(out)

@@ -159,12 +159,14 @@ class MoEContext:
     def num_local_experts(self) -> int:
         return self.dims["num_local_experts"]
 
-    def _validate_weights(self, gate_weights: torch.Tensor, expert_weights: torch.Tensor) -> None:
+    def _validate_weights(self, gate_weights: Optional[torch.Tensor], expert_weights: torch.Tensor) -> None:
+        """`gate_weights` None: a routed call, which has none."""
         d = self.dims
-        _check_tensor("Gate weights", gate_weights, self.device)
+        if gate_weights is not None:
+            _check_tensor("Gate weights", gate_weights, self.device)
+            if gate_weights.dim() != 2 or gate_weights.size(0) != d["H"] or gate_weights.size(1) != d["E"]:
+                raise RuntimeError(f"Gate weights must be [H={d['H']}, E={d['E']}]. Got {list(gate_weights.shape)}")
         _check_tensor("Expert weights", expert_weights, self.device)
-        if gate_weights.dim() != 2 or gate_weights.size(0) != d["H"] or gate_weights.size(1) != d["E"]:
-            raise RuntimeError(f"Gate weights must be [H={d['H']}, E={d['E']}]. Got {list(gate_weights.shape)}")
         nlx = d["num_local_experts"]
         if expert_weights.dim() != 4 or expert_weights.size(0) != nlx:
             raise RuntimeError(f"Expert count mismatch. Expected {nlx} local experts, got {expert_weights.size(0)}")
@@ -174,7 +176,7 @@ class MoEContext:
             raise RuntimeError(f"Expert weights must be [*, 2, P={d['P']}, H={d['H']}]. Got [*, 2, "
                                f"{expert_weights.size(2)}, {expert_weights.size(3)}]")
 
-    def _validate(self, input: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor,
+    def _validate(self, input: torch.Tensor, gate_weights: Optional[torch.Tensor], expert_weights: torch.Tensor,
                   exact_s: bool = True) -> int:
         """Same conditions as the reference's TORCH_CHECKs (python_bindings.cu:22-65) plus dtype and alignment checks.
         `exact_s`: the input is [batch, seq, H] with batch*seq == S (forward); otherwise any [..., H] holding at most S
@@ -260,6 +262,52 @@ class MoEContext:
         _lib.check(self._L.fm_moe_forward_tokens(self._ctx, x.data_ptr() if n else None, n, gate_weights.data_ptr(),
                                                  expert_weights.data_ptr(), bu, bd, out.data_ptr() if n else None,
                                                  stream))
+        self.last_tokens = n
+        return out
+
+    def forward_routed(self, x: torch.Tensor, topk_idx: torch.Tensor, topk_weight: torch.Tensor,
+                       expert_weights: torch.Tensor, bias_up: Optional[torch.Tensor] = None,
+                       bias_down: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                       n_tokens: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`forward_tokens` on the caller's routing instead of the built-in router (fm_moe_forward_routed): `topk_idx`
+        int32 [n, k] names each token's experts (global ids; -1 = no expert) and `topk_weight` float32 [n, k] their
+        weights, both contiguous CUDA tensors on this context's device (no conversions are made here; see
+        `FlashMoELayer.forward` for one that converts).  out[t] is the bf16 accumulation, in pick order, of
+        rne(rne_bf16(w_j) * y_j) over the kept picks -- for k = 1 too (the router path copies y unscaled there).
+        Capacity and slots are the router path's.  An index outside [-1, E) is treated as -1 and makes the next
+        `check` / `synchronize` raise once.  Not available on E = 1 or is_training = 1 contexts.
+
+        `n_tokens` (one-element int32 CUDA tensor): as in `forward_tokens`; x, out and the routing tensors then hold S
+        rows, of which the kernel reads the first n when it starts."""
+        n = self._validate(x, None, expert_weights, exact_s=False)
+        k = self.dims["k"]
+        for name, t, dt in (("topk_idx", topk_idx, torch.int32), ("topk_weight", topk_weight, torch.float32)):
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != self.device:
+                raise RuntimeError(f"{name} must be a CUDA tensor on {self.device}")
+            if t.dtype != dt:
+                raise RuntimeError(f"{name} must be {dt}, got {t.dtype}")
+            if not t.is_contiguous():
+                raise RuntimeError(f"{name} must be contiguous")
+            if tuple(t.shape) != (n, k):
+                raise RuntimeError(f"{name} must be [n={n}, k={k}] like x's tokens, got {list(t.shape)}")
+            if n and t.data_ptr() % 16:
+                raise RuntimeError(f"{name} must start on a 16-byte boundary; got storage offset {t.storage_offset()}")
+        bu, bd = self._bias_ptrs(bias_up, bias_down)
+        out = self._output(x, out)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        if n_tokens is not None:
+            self._check_count_tensor(n_tokens)
+            if n != self.dims["S"]:
+                raise RuntimeError(f"with a device-side n_tokens, x must hold exactly S={self.dims['S']} tokens (got {n})")
+            _lib.check(self._L.fm_moe_forward_routed(self._ctx, x.data_ptr(), n, n_tokens.data_ptr(),
+                                                     topk_idx.data_ptr(), topk_weight.data_ptr(),
+                                                     expert_weights.data_ptr(), bu, bd, out.data_ptr(), stream))
+            self.last_tokens = None
+            return out
+        _lib.check(self._L.fm_moe_forward_routed(self._ctx, x.data_ptr() if n else None, n, None,
+                                                 topk_idx.data_ptr() if n else None,
+                                                 topk_weight.data_ptr() if n else None, expert_weights.data_ptr(),
+                                                 bu, bd, out.data_ptr() if n else None, stream))
         self.last_tokens = n
         return out
 

@@ -137,8 +137,31 @@ FM_API int fm_moe_forward_tokens_dev(fm_ctx_t* ctx, const void* x, const int32_t
                                      const void* expert_w, const void* bias_up, const void* bias_down, void* out,
                                      void* stream);
 
+/* Same, on the caller's routing instead of the built-in router (no gate weights): topk_idx int32 [n, k] and topk_w fp32
+ * [n, k], DEVICE memory, contiguous and 16-byte aligned, name the experts of each token's k picks and their weights;
+ * -1 means "no expert" (the pick takes no capacity, is not counted and moves no row).  The token count follows
+ * fm_moe_forward_tokens (n_tokens_dev == NULL: x, out and the routing arrays hold n_tokens rows) or
+ * fm_moe_forward_tokens_dev (n_tokens_dev != NULL: n is read from the device when the kernel starts, the arrays hold S
+ * rows and n_tokens must be S); rows at or past n are never read, rows of out at or past n are never written.
+ * Capacity EC(n) and slots (ascending (token, pick) order among the picks of one expert; kept = slot < EC) are the
+ * router path's.  Result: out[t] = bf16 accumulation, in ascending pick order from +0, of rne(w~_j * y_j) over the kept
+ * picks j, with w~_j = rne_bf16(topk_w[t, j]) and y_j the bf16 output of expert topk_idx[t, j] on row t (bias
+ * included) -- the router path's combine with p~ = w~ and mCw = 1.  k = 1 is scaled too (the router path copies y
+ * unscaled; pass w = 1 for that).  A token may name one expert twice (each pick is its own row); weights are not checked
+ * (a NaN propagates).  An index outside [-1, E) does not fault: it is treated as -1 and the next fm_check /
+ * fm_read_buffer / fm_host_wait returns FM_EINVAL once, naming the token, the pick and the value; the context stays
+ * usable.  FM_EINVAL for an E = 1 context (no router to replace) and an is_training = 1 context (the auxiliary loss
+ * needs router probabilities).  With world > 1 each rank passes its own routing, in global expert ids, and its own
+ * count; the kind of call (routed or not) may differ between ranks, the number of calls may not.  May be captured in a
+ * CUDA graph like the other entry points: the pointers are fixed at capture, the arrays' contents (and *n_tokens_dev)
+ * are read when the launch starts. */
+FM_API int fm_moe_forward_routed(fm_ctx_t* ctx, const void* x, int n_tokens, const int32_t* n_tokens_dev,
+                                 const int32_t* topk_idx, const float* topk_w, const void* expert_w,
+                                 const void* bias_up, const void* bias_down, void* out, void* stream);
+
 /* ---- CUDA graphs ----
- * Every forward entry point on device buffers (fm_moe_forward, fm_moe_forward_tokens, fm_moe_forward_tokens_dev) may
+ * Every forward entry point on device buffers (fm_moe_forward, fm_moe_forward_tokens, fm_moe_forward_tokens_dev,
+ * fm_moe_forward_routed) may
  * be captured into a CUDA graph and the graph replayed any number of times, interleaved with eager calls on the same
  * context.  A launch keeps no per-launch state in its parameters: the kernel takes its epoch, grid-barrier target and
  * token-dependent sizes from the context's device-side launch counter (and the device-side count) when it starts.
@@ -184,15 +207,18 @@ FM_API int fm_set_trace(fm_ctx_t* ctx, int enable);
 
 /* ---- inspection (tests / debugging): copy an internal device buffer to host memory after synchronising ---- */
 enum fm_buffer {
-    FM_BUF_TOPK_IDX = 0, /* int32 [S,k]   expert index per pick (bit-exact parity target) */
-    FM_BUF_TOPK_W = 1,   /* bf16  [S,k]   gateOut[t, e_j] (bf16-rounded probability) */
-    FM_BUF_MCW = 2,      /* f32   [S]     sum of the k selected fp32 probabilities */
-    FM_BUF_SLOT = 3,     /* int32 [S,k]   slot in the (this rank, expert) packet; >= EC means dropped */
+    FM_BUF_TOPK_IDX = 0, /* int32 [S,k]   expert index per pick (bit-exact parity target); routed: the caller's, invalid
+                            ones replaced by -1 */
+    FM_BUF_TOPK_W = 1,   /* bf16  [S,k]   gateOut[t, e_j] (bf16-rounded probability); routed: rne_bf16(topk_w) */
+    FM_BUF_MCW = 2,      /* f32   [S]     sum of the k selected fp32 probabilities; routed: 1.0 */
+    FM_BUF_SLOT = 3,     /* int32 [S,k]   slot in the (this rank, expert) packet; >= EC means dropped; routed: INT32_MAX
+                            for a -1 pick */
     FM_BUF_COUNTS = 4,   /* int32 [E]     selections per expert on this rank (incl. dropped) */
     FM_BUF_RECV_X = 5,   /* bf16  [W, nLx, pEC, H]  dispatched rows received by this rank */
     FM_BUF_HIDDEN = 6,   /* bf16  [W, nLx, pEC, P]  h = act(x W_up^T + b) staging */
     FM_BUF_RET_Y = 7,    /* bf16  [E, pEC, H]       expert outputs returned to this rank */
-    FM_BUF_GATE_OUT = 8, /* bf16  [S, E]  full softmax row (reference gateOut[S,PX] without the padding columns) */
+    FM_BUF_GATE_OUT = 8, /* bf16  [S, E]  full softmax row (reference gateOut[S,PX] without the padding columns); not
+                            written by a routed launch */
     FM_BUF_RECV_CNT = 9, /* int32 [W, nLx] rows received per (source rank, local expert) in the last forward */
     FM_BUF_TRACE = 10,   /* u64   [grid, 128] %globaltimer stamps of the last forward (fm_set_trace) */
     FM_BUF_AUX_LOSS = 11 /* f32   [2E+1] is_training = 1 only: gML[E] (mean gate probability per expert), gMeC[E] (mean
