@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -277,13 +278,22 @@ int check_kernel_status(fm_ctx* c) {
 // maps over x have n_tok rows.  The kernel derives everything that depends on n and on the launch's place in the
 // context's sequence of launches itself (fm_kernel.cuh, struct Launch), so the parameters built here are valid for
 // every replay of a captured launch, and this function issues nothing that stream capture forbids.
-// `routed`: caller routing (fm_moe_forward_routed) -- phase G reads the picks and weights from topk_idx / topk_w [n, k]
-// instead of running the router, and there are no gate weights (gate_w is NULL).
-int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* gate_w, bool routed, const int32_t* topk_idx,
+// `route` (fm::RouteMode): ROUTE_CALLER is caller routing (fm_moe_forward_routed) -- phase G reads the picks and weights
+// from topk_idx / topk_w [n, k] instead of running the router, and there are no gate weights (gate_w is NULL).
+// ROUTE_GATED (fm_moe_forward_gated) runs the router's logits with the rule `router` (checked by the caller) and the
+// optional score_bias [E].
+int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* gate_w, int route, const int32_t* topk_idx,
            const float* topk_w, const void* expert_w, const void* bias_up, const void* bias_down, void* out,
-           cudaStream_t stream) {
+           cudaStream_t stream, const fm_router_t* router = nullptr, const float* score_bias = nullptr) {
     if (c == nullptr) return fail(FM_EINVAL, "null context");
     if (n_tok < 0 || n_tok > c->d.S) return fail(FM_EINVAL, "n_tokens = %d not in [0, S = %d]", n_tok, c->d.S);
+    const bool routed = route == fm::ROUTE_CALLER;
+    if (route == fm::ROUTE_GATED) {
+        if (c->d.E == 1) return fail(FM_EINVAL, "a gated call needs num_experts > 1: an E = 1 context has no router");
+        if (c->aux != nullptr)
+            return fail(FM_EINVAL, "a gated call is not available with is_training = 1: the auxiliary loss is defined on "
+                                   "softmax probabilities");
+    }
     if (routed) {
         if (c->d.E == 1) return fail(FM_EINVAL, "caller routing needs num_experts > 1: an E = 1 context has no router to replace");
         if (c->aux != nullptr)
@@ -391,10 +401,15 @@ int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* ga
     if (d.world == 1) p.peer_out_acc[0] = p.out;
     p.aux = c->aux;
     p.dense = c->dense ? 1 : 0;
-    p.routed = routed ? 1 : 0;
+    p.route = route;
     p.routed_idx = topk_idx;
     p.routed_w = topk_w;
     p.status_word = c->ctrl + 7;
+    if (route == fm::ROUTE_GATED) {
+        p.scoring = router->scoring; p.n_group = router->n_group; p.topk_group = router->topk_group;
+        p.group_top = router->group_top; p.renormalize = router->renormalize; p.route_scale = router->scale;
+        p.score_bias = score_bias;
+    }
     p.dbg = c->dbg_dev;
     p.trace = c->trace_on ? c->trace : nullptr;
 
@@ -771,8 +786,8 @@ FM_API int fm_symm_attach_ptrs(fm_ctx_t* ctx, void* const* peer_bases) {
 
 FM_API int fm_moe_forward_tokens(fm_ctx_t* ctx, const void* x, int n_tokens, const void* gate_w, const void* expert_w,
                                  const void* bias_up, const void* bias_down, void* out, void* stream) {
-    return launch(ctx, x, n_tokens, nullptr, gate_w, false, nullptr, nullptr, expert_w, bias_up, bias_down, out,
-                  static_cast<cudaStream_t>(stream));
+    return launch(ctx, x, n_tokens, nullptr, gate_w, fm::ROUTE_ROUTER, nullptr, nullptr, expert_w, bias_up, bias_down,
+                  out, static_cast<cudaStream_t>(stream));
 }
 
 FM_API int fm_moe_forward_tokens_dev(fm_ctx_t* ctx, const void* x, const int32_t* n_tokens_dev, const void* gate_w,
@@ -782,8 +797,8 @@ FM_API int fm_moe_forward_tokens_dev(fm_ctx_t* ctx, const void* x, const int32_t
     if (n_tokens_dev == nullptr) return fail(FM_EINVAL, "n_tokens_dev must be a device pointer to one int32");
     if (x == nullptr || out == nullptr)
         return fail(FM_EINVAL, "x and out must be non-null device pointers to S = %d rows", ctx->d.S);
-    return launch(ctx, x, ctx->d.S, n_tokens_dev, gate_w, false, nullptr, nullptr, expert_w, bias_up, bias_down, out,
-                  static_cast<cudaStream_t>(stream));
+    return launch(ctx, x, ctx->d.S, n_tokens_dev, gate_w, fm::ROUTE_ROUTER, nullptr, nullptr, expert_w, bias_up,
+                  bias_down, out, static_cast<cudaStream_t>(stream));
 }
 
 FM_API int fm_moe_forward_routed(fm_ctx_t* ctx, const void* x, int n_tokens, const int32_t* n_tokens_dev,
@@ -793,8 +808,41 @@ FM_API int fm_moe_forward_routed(fm_ctx_t* ctx, const void* x, int n_tokens, con
     if (n_tokens_dev != nullptr && n_tokens != ctx->d.S)
         return fail(FM_EINVAL, "with n_tokens_dev, n_tokens must be S = %d (the rows of x, out and the routing arrays); "
                                "got %d", ctx->d.S, n_tokens);
-    return launch(ctx, x, n_tokens, n_tokens_dev, nullptr, true, topk_idx, topk_w, expert_w, bias_up, bias_down, out,
-                  static_cast<cudaStream_t>(stream));
+    return launch(ctx, x, n_tokens, n_tokens_dev, nullptr, fm::ROUTE_CALLER, topk_idx, topk_w, expert_w, bias_up,
+                  bias_down, out, static_cast<cudaStream_t>(stream));
+}
+
+FM_API int fm_moe_forward_gated(fm_ctx_t* ctx, const void* x, int n_tokens, const int32_t* n_tokens_dev,
+                                const void* gate_w, const fm_router_t* router, const float* score_bias,
+                                const void* expert_w, const void* bias_up, const void* bias_down, void* out,
+                                void* stream) {
+    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
+    if (router == nullptr) return fail(FM_EINVAL, "router must point to an fm_router_t");
+    const fm_router_t& r = *router;
+    const int E = ctx->d.E, k = ctx->d.k;
+    if (r.scoring != 0 && r.scoring != 1)
+        return fail(FM_EINVAL, "router.scoring = %d: 0 (softmax) or 1 (sigmoid)", r.scoring);
+    if (r.n_group < 1 || r.n_group > fm::MAX_GROUPS || E % r.n_group != 0)
+        return fail(FM_EINVAL, "router.n_group = %d: must be in [1, %d] and divide E = %d", r.n_group, fm::MAX_GROUPS, E);
+    if (r.topk_group < 1 || r.topk_group > r.n_group)
+        return fail(FM_EINVAL, "router.topk_group = %d not in [1, n_group = %d]", r.topk_group, r.n_group);
+    if (r.n_group > 1 && ((r.group_top != 1 && r.group_top != 2) || r.group_top > E / r.n_group))
+        return fail(FM_EINVAL, "router.group_top = %d: 1 or 2, and at most the group size E / n_group = %d",
+                    r.group_top, E / r.n_group);
+    if (k > r.topk_group * (E / r.n_group))
+        return fail(FM_EINVAL, "k = %d picks need at least k experts in the topk_group = %d kept groups of %d", k,
+                    r.topk_group, E / r.n_group);
+    if (r.renormalize != 0 && r.renormalize != 1)
+        return fail(FM_EINVAL, "router.renormalize = %d: 0 or 1", r.renormalize);
+    if (!std::isfinite(r.scale) || !(r.scale > 0.0f))
+        return fail(FM_EINVAL, "router.scale = %g: must be finite and > 0", (double)r.scale);
+    if (reinterpret_cast<uintptr_t>(score_bias) % 16)
+        return fail(FM_EINVAL, "score_bias must be 16-byte aligned (got %p)", static_cast<const void*>(score_bias));
+    if (n_tokens_dev != nullptr && n_tokens != ctx->d.S)
+        return fail(FM_EINVAL, "with n_tokens_dev, n_tokens must be S = %d (the rows of x and out); got %d", ctx->d.S,
+                    n_tokens);
+    return launch(ctx, x, n_tokens, n_tokens_dev, gate_w, fm::ROUTE_GATED, nullptr, nullptr, expert_w, bias_up,
+                  bias_down, out, static_cast<cudaStream_t>(stream), router, score_bias);
 }
 
 FM_API int fm_last_launch(fm_ctx_t* ctx, uint64_t* launches, int32_t* n_tokens) {
@@ -843,8 +891,8 @@ FM_API int fm_host_submit(fm_ctx_t* ctx, const void* x_host, const void* gate_w,
     FM_CUDA(cudaMemcpyAsync(ctx->x_stage[slot], x_host, bytes, cudaMemcpyHostToDevice, ctx->s_h2d));
     FM_CUDA(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
     FM_CUDA(cudaStreamWaitEvent(s, ctx->ev_h2d[slot], 0));
-    if ((rc = launch(ctx, ctx->x_stage[slot], ctx->d.S, nullptr, gate_w, false, nullptr, nullptr, expert_w, bias_up,
-                     bias_down, ctx->out_stage[slot], s)))
+    if ((rc = launch(ctx, ctx->x_stage[slot], ctx->d.S, nullptr, gate_w, fm::ROUTE_ROUTER, nullptr, nullptr, expert_w,
+                     bias_up, bias_down, ctx->out_stage[slot], s)))
         return rc;
     FM_CUDA(cudaEventRecord(ctx->ev_kernel[slot], s));
     FM_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_kernel[slot], 0));

@@ -4,7 +4,8 @@
 //
 //   prologue  mbarriers for the later phases (off the critical path)
 //   phase G   router    x.Wg^T -> online softmax -> top-k -> capacity slots         (reference moe/gate.cuh:473-720)
-//             (or the caller's top-k ids and weights -> capacity slots: fm_moe_forward_routed)
+//             (or the caller's top-k ids and weights -> capacity slots: fm_moe_forward_routed;
+//              or x.Wg^T -> softmax / sigmoid scores, bias, group limit, top-k, scaled weights: fm_moe_forward_gated)
 //             grid barrier (the only one, like the reference's gate.cuh:761)
 //   phase D   dispatch  token rows -> owner rank's receive buffer over NVLink (TMA bulk copies) + one flag per expert
 //                                                                                    (reference os/packet.cuh:21-286)
@@ -112,8 +113,9 @@ constexpr int MAX_EXPERTS = 1024;   // validate_config rejects more; sizes the p
 //   [128K, 176K)      | sel_e i16 + rank i32,    | read                      | (stages)             |
 //                     | G_SEL_MAX each           |                           |                      |
 //   [176K, 188K)      | slot_ranks counts (on    | base / total / own,       | (stages)             |
-//                     | base), training column   | MAX_EXPERTS each          |                      |
-//                     | sums (on own)            |                           |                      |
+//                     | base), gated score bias  | MAX_EXPERTS each          |                      |
+//                     | (on total), training     |                           |                      |
+//                     | column sums (on own)     |                           |                      |
 //   epilogue [0, 8K)  | zero source of the       | read by the fill's bulk   | chunk buffers        |
 //                     | output-row fill (warp 11)| stores until warps 4-11's |                      |
 //                     |                          | wait_group.read           |                      |
@@ -132,6 +134,7 @@ constexpr int D_OFF_OWN = D_OFF_TOTAL + MAX_EXPERTS * 4;   // int32 own[E]: by t
 constexpr int D_PREFIX_END = D_OFF_OWN + MAX_EXPERTS * 4;
 constexpr int G_OFF_CNT = D_OFF_BASE;                      // int32 [E] slot_ranks' running counts
 constexpr int G_OFF_COLSUM = D_OFF_OWN;                    // f32 [E] training: this chunk's sum_t p[t,e]
+constexpr int G_OFF_BIAS = D_OFF_TOTAL;                    // f32 [E] gated launch: score_bias (0 without one)
 constexpr int D_OFF_XROWS = 0;                             // staged token rows of this chunk
 constexpr int D_XROWS_BYTES = 128 * 1024;
 constexpr int C_OFF_E = 0;                                 // int32 [tpc * k] expert
@@ -150,6 +153,8 @@ static_assert(C_RECORDS_END <= PIPE_BYTES, "combine records within the stage are
 static_assert(D_WIN_BYTES > 0 && EPI_ZERO_BYTES + D_WIN_BYTES <= EPI_BYTES,
               "zero source and remote-row window within the epilogue staging area");
 static_assert(G_OFF_COLSUM + MAX_EXPERTS * (int)sizeof(float) <= D_PREFIX_END, "a column sum per expert");
+static_assert(G_OFF_BIAS >= G_OFF_CNT + MAX_EXPERTS * 4 && G_OFF_BIAS + MAX_EXPERTS * (int)sizeof(float) <= D_PREFIX_END,
+              "a score bias per expert, clear of slot_ranks' counts");
 
 // mbarriers (mbar_init / mbar_arrive / bar_wait on bar(smem, id)).  FM_MBARRIERS below declares every group once:
 // X(ID, name, first id, count, arrival count); BAR_<ID> is the group's first id, ffn_setup initialises every barrier
@@ -280,6 +285,16 @@ struct TileBlock {  // one contiguous run of work items: all tiles of one GEMM o
     int g0, g1;     // GEMM0 / GEMM1 blocks before this one in the work list (block_start)
 };
 
+// Where phase G takes a launch's routing from.  A caller-routed and a gated launch both store mcw = 1 and take the
+// scaling combine for every k (k = 1 included); only the router launch copies y unscaled at k = 1.
+enum RouteMode : int {
+    ROUTE_ROUTER = 0,   // the built-in router: softmax, top-k, renormalise (fm_moe_forward, fm_moe_forward_tokens[_dev])
+    ROUTE_CALLER = 1,   // the caller's top-k ids and weights (fm_moe_forward_routed)
+    ROUTE_GATED = 2,    // the router's logits, scored and selected by the call's fm_router_t (fm_moe_forward_gated)
+};
+enum : int { SCORE_SOFTMAX = 0, SCORE_SIGMOID = 1 };   // FmParams::scoring (fm_router_t.scoring)
+constexpr int MAX_GROUPS = 32;                        // n_group bound: a token's kept groups are one 32-bit mask
+
 struct FmParams {
     CUtensorMap tm_a0;  // recv_x  as [W*nLx*pEC, H]  box {64, 128}
     CUtensorMap tm_b0;  // expert_weights as [nLx*2*P, H]  box {64, 128}  (W_up rows)
@@ -344,13 +359,18 @@ struct FmParams {
     // gMeC[E] mean routed fraction per expert, loss} (reference moe/gate.cuh:608-635,698-706,763-773); nullptr otherwise
     float* aux;
     int dense;          // E == 1: no router GEMV, no dispatch copy; GEMM0 reads x in place (reference moe/fffn.cuh:31-167)
-    // caller routing (fm_moe_forward_routed, routed != 0): phase G takes the picks and weights from these [n, k] arrays
-    // instead of the router; -1 = no expert.  status_word: the election of the one thread that reports an index outside
-    // [-1, E) in a launch (atomicExch of the epoch)
-    int routed;
+    // where phase G takes the routing from (RouteMode).  ROUTE_CALLER (fm_moe_forward_routed): the picks and weights
+    // come from these [n, k] arrays instead of the router; -1 = no expert.  status_word: the election of the one thread
+    // that reports an index outside [-1, E) in a launch (atomicExch of the epoch)
+    int route;
     const int* routed_idx;
     const float* routed_w;
     unsigned int* status_word;
+    // ROUTE_GATED (fm_moe_forward_gated): the router's logits, then scored_topk with this rule (fm_router_t, checked by
+    // the host); score_bias [E] or nullptr, read when the launch starts
+    int scoring, n_group, topk_group, group_top, renormalize;
+    float route_scale;
+    const float* score_bias;
     DebugRecord* dbg;
     unsigned long long* trace;  // optional [grid][TRACE_SLOTS] %globaltimer stamps (nullptr = off)
 };
@@ -751,6 +771,31 @@ __device__ __forceinline__ int softmax_topk_lanes(int E) {
 // expert compares greater than -inf (a token with NaN logits) picks expert 0, like the reference's scan.  Writes
 // gate_out, topk_idx, topk_w, mcw and sel_e, and leaves the probabilities in the logits scratch (the training-mode
 // column sums read them).
+// The probabilities of one token (row l of the logits scratch, gate_out row go) for a group of LPT lanes: every lane of
+// the group runs the reference's recurrence over the whole row, then lane `sub` replaces its experts' logits by p and
+// writes them to gate_out (idle groups, !valid, only compute).  softmax_topk and scored_topk share it, so a gated
+// launch's softmax scores are the router's bits.  (No FmParams argument: out of line, in scored_topk, every field read
+// through the reference would be reloaded after each store.)
+__device__ __forceinline__ void softmax_row(float* l, __nv_bfloat16* go, int E, int sub, int LPT, bool valid) {
+    float dI = 0.0f, mI = -INFINITY;
+    // (unrolled so that the loads, the running maxima and the exponentials of 8 steps are in flight together;
+    // the dependent chain is then one max and one fma per step -- same operations in the same order)
+#pragma unroll 8
+    for (int e = 0; e < E; ++e) {
+        const float pM = mI;
+        mI = fmaxf(mI, l[e]);
+        dI = fmaf(dI, fast_expf(pM - mI), fast_expf(l[e] - mI));
+    }
+    __syncwarp();   // every lane of the group has read the logits before they are replaced by probabilities
+    if (valid)
+#pragma unroll 4
+        for (int e = sub; e < E; e += LPT) {
+            const float pe = __fdividef(fast_expf(l[e] - mI), dI);
+            l[e] = pe;
+            go[e] = __float2bfloat16_rn(pe);
+        }
+}
+
 __device__ __forceinline__ void softmax_topk(const FmParams& p, float* logit_s, int ldl, int16_t* sel_e, int t0, int s0,
                                              int n_sub) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -763,23 +808,7 @@ __device__ __forceinline__ void softmax_topk(const FmParams& p, float* logit_s, 
         const int ti = valid ? ti_raw : n_sub - 1;   // (idle groups compute on a copy of the last row, write nothing)
         float* l = logit_s + ti * ldl;
         const int t = t0 + s0 + ti;
-        float dI = 0.0f, mI = -INFINITY;
-        // (unrolled so that the loads, the running maxima and the exponentials of 8 steps are in flight together;
-        // the dependent chain is then one max and one fma per step -- same operations in the same order)
-#pragma unroll 8
-        for (int e = 0; e < E; ++e) {
-            const float pM = mI;
-            mI = fmaxf(mI, l[e]);
-            dI = fmaf(dI, fast_expf(pM - mI), fast_expf(l[e] - mI));
-        }
-        __syncwarp();   // every lane of the group has read the logits before they are replaced by probabilities
-        if (valid)
-#pragma unroll 4
-            for (int e = sub; e < E; e += LPT) {
-                const float pe = __fdividef(fast_expf(l[e] - mI), dI);
-                l[e] = pe;
-                p.gate_out[(size_t)t * E + e] = __float2bfloat16_rn(pe);
-            }
+        softmax_row(l, p.gate_out + (size_t)t * E, E, sub, LPT, valid);
         unsigned int taken = 0u;
         float sum = 0.0f;
         for (int i = 0; i < k; ++i) {
@@ -808,6 +837,146 @@ __device__ __forceinline__ void softmax_topk(const FmParams& p, float* logit_s, 
             }
         }
         if (sub == 0 && valid) p.mcw[t] = sum;
+        __syncwarp();
+    }
+}
+
+// Sigmoid score of a gated launch: 1 / (1 + 2^fl(-l * log2e)), the power by ex2.approx.ftz (fast_expf), the sum and
+// the reciprocal rounded to nearest.  Relative error against 1 / (1 + e^-l): at most 2^-21 (ex2) + 2^-24 * |l| (the
+// rounded argument) + 2 * 2^-24 (sum, reciprocal), to first order; l = -inf or below about -88 gives +0, +inf gives 1.
+__device__ __forceinline__ float sigmoid_score(float l) { return __frcp_rn(__fadd_rn(1.0f, fast_expf(-l))); }
+
+// Best candidate of a group of LPT lanes: the larger value, on equal values the lower index (every lane ends with the
+// group's winner).  Index 0x7fffffff = nothing compared greater than -inf.
+__device__ __forceinline__ void group_argmax(float& bv, int& bi, int LPT) {
+    for (int off = LPT >> 1; off >= 1; off >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
+        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+    }
+}
+
+// Scores and top-k of one sub-chunk of a gated launch (fm_moe_forward_gated), for every E in [2, 1024], on
+// softmax_topk's lane groups (lane `sub` owns experts sub, sub + LPT, ...):
+//   s_e = the router's softmax probability (softmax_row) or sigmoid_score(l_e), left in the logits scratch and
+//         written to gate_out;
+//   c_e = fl(s_e + b_e) with b = the staged score bias (zeros without one: s + 0 = s), for selection only;
+//   n_group > 1: lane `sub` scores its groups sub, sub + LPT, ... (G_g = the largest c of the group, or fl(largest +
+//         second largest)); topk_group argmax rounds give the kept-group mask, and the experts of the other groups
+//         start out in `taken`, so the k rounds below never pick them;
+//   k rounds of softmax_topk's scan on c (strict '>', lower index on equal values, NaN never greater, a round with
+//         nothing greater than -inf takes index 0 -- groups and experts alike);
+//   w_j = s_{e_j}; renormalize: W = sum of the w_j in pick order from +0, w_j = W > 0 ? w_j / W : 0 (rounded
+//         division); then w_j = fl(w_j * scale).
+// Writes gate_out, topk_idx, topk_w = rne_bf16(w), mcw = 1 and sel_e.  Called by every thread of the CTA.  Out of line
+// on purpose, like gate_phase_routed, and with few arguments: the kernel keeps the router path's registers, stack and
+// spills.  (Inlined, the kernel's spills rose from 156 / 544 B to 184 / 584 B; out of line with the scratch pointers
+// as arguments to 164 / 572 B; a whole gated gate_phase out of line grew the kernel's stack from 256 to 432 B.)
+__device__ __noinline__ void scored_topk(const FmParams& p, uint8_t* smem, int t0, int s0, int n_sub) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    // every field this stage uses, read once: p is a reference here (out of line), and a field read through it in a
+    // loop is reloaded after every store
+    const int E = p.E, k = p.k;
+    const int scoring = p.scoring, NG = p.n_group, topk_group = p.topk_group, group_top = p.group_top;
+    const bool renormalize = p.renormalize != 0;
+    const float scale = p.route_scale;
+    __nv_bfloat16* const gate_out = p.gate_out;
+    int* const topk_idx = p.topk_idx;
+    __nv_bfloat16* const topk_w = p.topk_w;
+    float* const mcw = p.mcw;
+    float* logit_s = reinterpret_cast<float*>(smem + G_OFF_LOGIT);
+    int16_t* sel_e = reinterpret_cast<int16_t*>(smem + G_OFF_SEL);
+    const int ldl = E + 1;
+    float* bias_s = reinterpret_cast<float*>(smem + G_OFF_BIAS);
+    if (s0 == 0) {   // the launch's first sub-chunk: stage the bias (read once per launch, so a captured graph follows
+                     // in-place updates of it)
+        const float* score_bias = p.score_bias;
+        for (int e = threadIdx.x; e < E; e += NUM_THREADS) bias_s[e] = score_bias != nullptr ? score_bias[e] : 0.0f;
+        __syncthreads();
+    }
+    const int LPT = softmax_topk_lanes(E), lg = __ffs(LPT) - 1;
+    const int TPW = 32 >> lg, sub = lane & (LPT - 1);
+    const int GS = E / NG;
+    // groups per lane: NG <= 32, and LPT >= 4 for E > 8, LPT >= E >= NG below -- at most 8
+    constexpr int GPL = MAX_GROUPS / 4;
+    for (int tb = warp * TPW; tb < n_sub; tb += NUM_WARPS * TPW) {
+        const int ti_raw = tb + (lane >> lg);
+        const bool valid = ti_raw < n_sub;
+        const int ti = valid ? ti_raw : n_sub - 1;   // (idle groups compute on a copy of the last row, write nothing)
+        float* l = logit_s + ti * ldl;
+        const int t = t0 + s0 + ti;
+        __nv_bfloat16* const go = gate_out + (size_t)t * E;
+        if (scoring == SCORE_SOFTMAX) {
+            softmax_row(l, go, E, sub, LPT, valid);
+        } else if (valid) {
+            for (int e = sub; e < E; e += LPT) {
+                const float s = sigmoid_score(l[e]);
+                l[e] = s;
+                go[e] = __float2bfloat16_rn(s);
+            }
+        }
+        __syncwarp();   // every score of the row is in place before lanes read each other's experts
+        unsigned int taken = 0u;   // bit c: expert sub + c * LPT is excluded (outside the kept groups) or picked
+        if (NG > 1) {
+            float gs[GPL];
+#pragma unroll
+            for (int q = 0; q < GPL; ++q) {
+                const int g = sub + q * LPT;
+                float m1 = -INFINITY, m2 = -INFINITY;
+                if (g < NG)
+                    for (int e = g * GS; e < (g + 1) * GS; ++e) {
+                        const float v = l[e] + bias_s[e];
+                        if (v > m1) { m2 = m1; m1 = v; }
+                        else if (v > m2) m2 = v;
+                    }
+                gs[q] = group_top == 2 ? m1 + m2 : m1;
+            }
+            unsigned int kept = 0u;
+            for (int r = 0; r < topk_group; ++r) {
+                float bv = -INFINITY;
+                int bg = 0x7fffffff;
+#pragma unroll
+                for (int q = 0; q < GPL; ++q) {
+                    const int g = sub + q * LPT;
+                    if (g < NG && gs[q] > bv && !((kept >> g) & 1u)) { bv = gs[q]; bg = g; }
+                }
+                group_argmax(bv, bg, LPT);
+                if (bg == 0x7fffffff) bg = 0;
+                kept |= 1u << bg;
+            }
+            int c = 0;
+            for (int e = sub; e < E; e += LPT, ++c)
+                if (!((kept >> (e / GS)) & 1u)) taken |= 1u << c;
+        }
+        float W = 0.0f;
+        for (int i = 0; i < k; ++i) {
+            float bv = -INFINITY;
+            int bi = 0x7fffffff;
+            if (valid) {
+                int c = 0;
+#pragma unroll 4
+                for (int e = sub; e < E; e += LPT, ++c) {
+                    const float v = l[e] + bias_s[e];
+                    if (v > bv && !((taken >> c) & 1u)) { bv = v; bi = e; }
+                }
+            }
+            group_argmax(bv, bi, LPT);
+            if (bi == 0x7fffffff) { bi = 0; }   // nothing comparable left (NaN scores): index 0, as softmax_topk
+            if ((bi & (LPT - 1)) == sub) taken |= 1u << (bi >> lg);
+            if (sub == 0 && valid) {
+                W = __fadd_rn(W, l[bi]);
+                topk_idx[(size_t)t * k + i] = bi;
+                sel_e[(s0 + ti) * k + i] = (int16_t)bi;
+            }
+        }
+        if (sub == 0 && valid) {
+            for (int i = 0; i < k; ++i) {
+                float w = l[sel_e[(s0 + ti) * k + i]];
+                if (renormalize) w = W > 0.0f ? __fdiv_rn(w, W) : 0.0f;
+                topk_w[(size_t)t * k + i] = __float2bfloat16_rn(__fmul_rn(w, scale));
+            }
+            mcw[t] = 1.0f;
+        }
         __syncwarp();
     }
 }
@@ -860,6 +1029,8 @@ __device__ __forceinline__ void gate_tail(const FmParams& p, uint8_t* smem, int 
     slot_ranks(p, smem, n_tok);
 }
 
+// The router launch's phase G, and a gated launch's (p.route == ROUTE_GATED): the same logits, then scored_topk
+// instead of softmax_topk.
 __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int E = p.E;
@@ -891,7 +1062,8 @@ __device__ __forceinline__ void gate_phase(const FmParams& p, const Launch& L, u
         __syncthreads();
         if (tid == 0) trace_stamp(p, TRACE_GATE_LOGITS);
         if (p.fused && s0 == 0 && warp == NUM_WARPS - 1) zero_fill_out_rows(p, smem, t0, n_tok);
-        softmax_topk(p, logit_s, ldl, sel_e, t0, s0, n_sub);
+        if (p.route == ROUTE_GATED) scored_topk(p, smem, t0, s0, n_sub);
+        else softmax_topk(p, logit_s, ldl, sel_e, t0, s0, n_sub);
         if (tid == 0) trace_stamp(p, TRACE_TOPK_WARP0);
         __syncthreads();
         if (p.aux != nullptr) {
@@ -1723,8 +1895,8 @@ __device__ __forceinline__ void epilogue_out(const FmParams& p, uint8_t* smem, c
         with_bias(da.bias, [&](auto has_bias) {
             constexpr bool B = decltype(has_bias)::value;
             if (!fuse) drain_accumulator<EPI_G1_STORE, B>(p, da, acc);
-            // (caller routing scales k = 1 too: one add of rne(w~ * y) onto the zero-filled row is exact)
-            else if (p.k > 1 || p.routed) drain_accumulator<EPI_G1_FUSED_ADD, B>(p, da, acc);
+            // (caller and gated routing scale k = 1 too: one add of rne(w~ * y) onto the zero-filled row is exact)
+            else if (p.k > 1 || p.route != ROUTE_ROUTER) drain_accumulator<EPI_G1_FUSED_ADD, B>(p, da, acc);
             else drain_accumulator<EPI_G1_FUSED_COPY, B>(p, da, acc);
         });
     }
@@ -1922,7 +2094,7 @@ __device__ __forceinline__ void ffn_roles(const FmParams& p, const Launch& L, ui
 // finish_fused below).  For token t with picks (e_j, slot_j):
 //   k > 1: out[t,c] = bf16-accumulate over kept j of rne( p~_j * rne( y_j[c] / mCw ) )   (processor.cuh:110-169)
 //   k = 1: out[t,:] = y_0 (no scaling), zeros if dropped                                  (processor.cuh:170-203)
-//          (caller routing scales k = 1 like k > 1, with mCw = 1)
+//          (caller and gated routing scale k = 1 like k > 1, with mCw = 1)
 // Deterministic gather (no atomics, no zero-fill pass); for k == 2 it equals the reference's atomicAdd result
 // exactly because bf16 addition commutes and 0 + a is exact.
 // ============================================================================================================
@@ -2051,7 +2223,7 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, const Launch& L
     }
     for (int i = tid; i < n_tok; i += NUM_THREADS) c_m[i] = p.mcw[t0 + i];
     __syncthreads();
-    if (k == 1 && !p.routed) {
+    if (k == 1 && p.route == ROUTE_ROUTER) {
         for (int ti = warp; ti < n_tok; ti += NUM_WARPS) {
             const bool keep = c_s[ti] < EC;
             const __nv_bfloat16* yrow = p.ret_y + ((size_t)c_e[ti] * p.pEC + (keep ? c_s[ti] : 0)) * H;
@@ -2062,7 +2234,7 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, const Launch& L
                 st_global_v4(orow + h, v);
             }
         }
-    } else if (k <= 2) {   // (k = 1 with caller routing: the scaled term rne(w~ * y))
+    } else if (k <= 2) {   // (k = 1 with caller or gated routing: the scaled term rne(w~ * y))
         combine_rows<2, 4>(p, EC, t0, n_tok, c_e, c_s, c_w, c_m);
     } else {
         combine_rows<8, 1>(p, EC, t0, n_tok, c_e, c_s, c_w, c_m);
@@ -2102,8 +2274,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
         if (tid == 0) *p.claim = 0u;
     }
     if (p.dense) gate_phase_dense(p, L, t0, n_tok);
-    else if (p.routed) gate_phase_routed(p, L, smem, t0, n_tok);
-    else gate_phase(p, L, smem, t0, n_tok);
+    else if (p.route == ROUTE_CALLER) gate_phase_routed(p, L, smem, t0, n_tok);
+    else gate_phase(p, L, smem, t0, n_tok);   // (the router, and a gated launch's logits)
     if (tid == 0) trace_stamp(p, TRACE_GATE_DONE);
     grid_barrier(p, L);
     if (tid == 0) trace_stamp(p, TRACE_BARRIER);

@@ -9,6 +9,7 @@ from typing import NamedTuple, Optional
 import torch
 
 from .config import MoEConfig
+from .router import RouterSpec
 from .runtime import MoEContext
 
 
@@ -16,7 +17,8 @@ class MoEOutput(NamedTuple):
     out: torch.Tensor                 # [B, T, H] bf16
     topk_idx: torch.Tensor            # [B*T, k] int32   expert picked per token, in pick order
     topk_weight: torch.Tensor         # [B*T, k] bf16    gateOut[t, e_j] (bf16-rounded softmax probability); after a
-                                      #                  routed call the caller's weights rounded to bf16
+                                      #                  routed call the caller's weights rounded to bf16; with a
+                                      #                  `router` rule the rule's weights w rounded to bf16
     slot: torch.Tensor                # [B*T, k] int32   slot in the (rank, expert) packet; >= capacity means dropped
                                       #                  (INT32_MAX for a -1 pick of a routed call)
     aux_loss: Optional[torch.Tensor] = None   # is_training = 1: f32 [2E+1] = gML[E] | gMeC[E] | load-balancing loss
@@ -27,13 +29,25 @@ class FlashMoELayer(torch.nn.Module):
 
     Parameters are held in the reference's layouts: `gate_weight` [H, E] (consumed flat as [E, H]),
     `expert_weight` [nLx, 2, P, H] (this rank's experts), optional `bias_up` [nLx, P] / `bias_down` [nLx, H].
+
+    `router`: a `RouterSpec` (sigmoid scores, group-limited top-k, no renormalisation, a route scale, ...) the kernel
+    applies to the gate's logits instead of the built-in softmax / top-k / renormalise (`MoEContext.forward_gated`).
+    `score_bias` (with a `router` only): hold an fp32 [E] selection bias, `score_bias` (Hugging Face's
+    `e_score_correction_bias`), zero-initialised; the caller updates it in place, e.g. from the `counts` buffer.
     """
 
     def __init__(self, cfg: MoEConfig, rank: int = 0, world: int = 1, device: Optional[int] = None, group=None,
-                 bias: bool = False):
+                 bias: bool = False, router: Optional[RouterSpec] = None, score_bias: bool = False):
         super().__init__()
         cfg.check_hot_path()
+        if router is not None:
+            if not isinstance(router, RouterSpec):
+                raise TypeError(f"router must be a RouterSpec, got {type(router).__name__}")
+            router.check(cfg.E, cfg.k)
+        elif score_bias:
+            raise ValueError("score_bias needs a router rule (router=RouterSpec(...))")
         self.cfg = cfg
+        self.router = router
         self.ctx = MoEContext(cfg, rank=rank, world=world, device=device, group=group)
         dev = self.ctx.device
         nlx = self.ctx.num_local_experts
@@ -48,6 +62,8 @@ class FlashMoELayer(torch.nn.Module):
         else:
             self.bias_up = None
             self.bias_down = None
+        self.score_bias = (torch.nn.Parameter(torch.zeros(cfg.E, device=dev, dtype=torch.float32), requires_grad=False)
+                           if score_bias else None)
 
     @torch.no_grad()
     def forward(self, x: torch.Tensor, return_routing: bool = False, n_tokens: Optional[torch.Tensor] = None,
@@ -61,7 +77,7 @@ class FlashMoELayer(torch.nn.Module):
         `topk_idx` / `topk_weight` [B*T, k] (both or neither): the caller's routing instead of this layer's gate
         (`MoEContext.forward_routed`; -1 = no expert, k = 1 is scaled by its weight too).  The indices may be any
         integer type (int64 from `torch.topk` is converted to int32), the weights any floating type (converted to
-        float32); `gate_weight` is not used."""
+        float32); `gate_weight` is not used.  Otherwise, with a `router` rule, the gated forward runs."""
         if x.dim() != 3:
             raise RuntimeError("Input must be 3D [batch, seq, H]")
         if (topk_idx is None) != (topk_weight is None):
@@ -72,6 +88,10 @@ class FlashMoELayer(torch.nn.Module):
             out = self.ctx.forward_routed(x, topk_idx.to(torch.int32).contiguous(),
                                           topk_weight.to(torch.float32).contiguous(), self.expert_weight,
                                           bias_up=self.bias_up, bias_down=self.bias_down, n_tokens=n_tokens)
+        elif self.router is not None:
+            out = self.ctx.forward_gated(x, self.gate_weight, self.expert_weight, self.router,
+                                         score_bias=self.score_bias, bias_up=self.bias_up, bias_down=self.bias_down,
+                                         n_tokens=n_tokens)
         else:
             out = self.ctx.forward_tokens(x, self.gate_weight, self.expert_weight, bias_up=self.bias_up,
                                           bias_down=self.bias_down, n_tokens=n_tokens)

@@ -16,6 +16,7 @@ import torch
 
 from . import _lib, trace_slots
 from .config import MoEConfig
+from .router import RouterSpec
 
 _BUFFER_SPECS = {
     "topk_idx": (_lib.BUF_TOPK_IDX, np.int32),
@@ -308,6 +309,54 @@ class MoEContext:
                                                  topk_idx.data_ptr() if n else None,
                                                  topk_weight.data_ptr() if n else None, expert_weights.data_ptr(),
                                                  bu, bd, out.data_ptr() if n else None, stream))
+        self.last_tokens = n
+        return out
+
+    def forward_gated(self, x: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor,
+                      router: RouterSpec, score_bias: Optional[torch.Tensor] = None,
+                      bias_up: Optional[torch.Tensor] = None, bias_down: Optional[torch.Tensor] = None,
+                      out: Optional[torch.Tensor] = None, n_tokens: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`forward_tokens` with the routing rule `router` (a `RouterSpec`) applied in the kernel to the router's logits
+        (fm_moe_forward_gated): softmax or sigmoid scores, an optional `score_bias` added for selection only, a group
+        limit, top-k, renormalisation and a route scale.  From the routing on, the launch runs exactly as
+        `forward_routed` on its own topk_idx and weights: the weights are `rne_bf16(w)`, k = 1 is scaled, mcw = 1,
+        gate_out holds the unbiased scores.  `score_bias`: contiguous float32 [E] CUDA tensor on this device (global
+        expert ids), read when each launch starts (a captured graph follows in-place updates).  `n_tokens` as in
+        `forward_tokens`.  Not available on E = 1 or is_training = 1 contexts."""
+        if not isinstance(router, RouterSpec):
+            raise TypeError(f"router must be a RouterSpec, got {type(router).__name__}")
+        d = self.dims
+        router.check(d["E"], d["k"])
+        n = self._validate(x, gate_weights, expert_weights, exact_s=False)
+        if score_bias is not None:
+            if not isinstance(score_bias, torch.Tensor) or not score_bias.is_cuda or score_bias.device != self.device:
+                raise RuntimeError(f"score_bias must be a CUDA tensor on {self.device}")
+            if score_bias.dtype != torch.float32:
+                raise RuntimeError(f"score_bias must be torch.float32, got {score_bias.dtype}")
+            if not score_bias.is_contiguous():
+                raise RuntimeError("score_bias must be contiguous")
+            if tuple(score_bias.shape) != (d["E"],):
+                raise RuntimeError(f"score_bias must be [E={d['E']}], got {list(score_bias.shape)}")
+            if score_bias.data_ptr() % 16:
+                raise RuntimeError("score_bias must start on a 16-byte boundary; got storage offset "
+                                   f"{score_bias.storage_offset()}")
+        bu, bd = self._bias_ptrs(bias_up, bias_down)
+        out = self._output(x, out)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        rt = ctypes.byref(router.to_c())
+        sb = score_bias.data_ptr() if score_bias is not None else None
+        if n_tokens is not None:
+            self._check_count_tensor(n_tokens)
+            if n != d["S"]:
+                raise RuntimeError(f"with a device-side n_tokens, x must hold exactly S={d['S']} tokens (got {n})")
+            _lib.check(self._L.fm_moe_forward_gated(self._ctx, x.data_ptr(), n, n_tokens.data_ptr(),
+                                                    gate_weights.data_ptr(), rt, sb, expert_weights.data_ptr(), bu,
+                                                    bd, out.data_ptr(), stream))
+            self.last_tokens = None
+            return out
+        _lib.check(self._L.fm_moe_forward_gated(self._ctx, x.data_ptr() if n else None, n, None,
+                                                gate_weights.data_ptr(), rt, sb, expert_weights.data_ptr(), bu, bd,
+                                                out.data_ptr() if n else None, stream))
         self.last_tokens = n
         return out
 

@@ -159,14 +159,51 @@ FM_API int fm_moe_forward_routed(fm_ctx_t* ctx, const void* x, int n_tokens, con
                                  const int32_t* topk_idx, const float* topk_w, const void* expert_w,
                                  const void* bias_up, const void* bias_down, void* out, void* stream);
 
+/* A router rule for fm_moe_forward_gated (DeepSeek-V2/V3, Kimi K2, GLM-4.5, Qwen-MoE, OLMoE and Llama 4 style routers). */
+typedef struct fm_router {
+    int32_t scoring;      /* 0 softmax (the router's own recurrence), 1 sigmoid */
+    int32_t n_group;      /* experts split into n_group contiguous groups of E / n_group; 1 = no group limit */
+    int32_t topk_group;   /* groups kept per token */
+    int32_t group_top;    /* group score = sum of the group's 1 (max) or 2 largest biased scores */
+    int32_t renormalize;  /* 0 / 1 */
+    float scale;          /* route scale applied to every weight */
+} fm_router_t;
+
+/* Same as fm_moe_forward_routed, but the routing is computed in the kernel from the gate weights by the rule *router:
+ * the router's logits l (the same GEMV / tensor-core product as fm_moe_forward_tokens), then per token t
+ *   1. scores s_e: scoring 0 = the router's softmax probability (the bits of gate_out of an fm_moe_forward_tokens
+ *      launch); scoring 1 = sigmoid, computed as __frcp_rn(1 + ex2.approx.ftz(fl(-l * log2e))), relative error at most
+ *      2^-21 + 2^-24 * (|l| + 2) against 1 / (1 + e^-l);
+ *   2. choice values c_e = fl(s_e + score_bias[e]) (c = s without a bias); the bias steers selection only;
+ *   3. n_group > 1: group score G_g = the largest c of the group (group_top 1) or fl(largest + second largest)
+ *      (group_top 2); the topk_group groups with the largest G are kept, the experts of the others cannot be picked
+ *      (DeepSeek's own Gate.forward; not the 0.0 mask of the Hugging Face DeepseekV3TopkRouter);
+ *   4. k picks by c among the allowed experts, k rounds of a strict '>': an equal value goes to the lower index, NaN
+ *      never compares greater, a round in which nothing compares greater than -inf takes index 0 (groups likewise);
+ *   5. weights w_j = s_{e_j} (unbiased); renormalize: W = fp32 sum of the w_j in pick order from +0,
+ *      w_j = W > 0 ? w_j / W (rounded) : 0 (capacity-dropped picks count in W); then w_j = fl(w_j * scale).
+ * The launch stores topk_idx, topk_w = rne_bf16(w), mcw = 1 and gate_out = rne_bf16(s) (the unbiased scores), and from
+ * there runs exactly as fm_moe_forward_routed on that routing: capacity, slots, the mCw = 1 combine, k = 1 scaled.
+ * The token count follows fm_moe_forward_routed.  score_bias: fp32 [E] device memory, 16-byte aligned, or NULL; its
+ * contents are read when each launch starts.  FM_EINVAL for router == NULL, scoring not 0 / 1, n_group not in [1, 32]
+ * or not dividing E, topk_group not in [1, n_group], n_group > 1 with group_top not 1 / 2 or above E / n_group,
+ * k > topk_group * E / n_group, renormalize not 0 / 1, scale not finite or <= 0, a misaligned score_bias, an E = 1
+ * context and an is_training = 1 context.  With world > 1 each rank passes its own gate weights and bias (global expert
+ * ids). */
+FM_API int fm_moe_forward_gated(fm_ctx_t* ctx, const void* x, int n_tokens, const int32_t* n_tokens_dev,
+                                const void* gate_w, const fm_router_t* router, const float* score_bias /* [E] or NULL */,
+                                const void* expert_w, const void* bias_up, const void* bias_down, void* out,
+                                void* stream);
+
 /* ---- CUDA graphs ----
  * Every forward entry point on device buffers (fm_moe_forward, fm_moe_forward_tokens, fm_moe_forward_tokens_dev,
- * fm_moe_forward_routed) may
+ * fm_moe_forward_routed, fm_moe_forward_gated) may
  * be captured into a CUDA graph and the graph replayed any number of times, interleaved with eager calls on the same
  * context.  A launch keeps no per-launch state in its parameters: the kernel takes its epoch, grid-barrier target and
  * token-dependent sizes from the context's device-side launch counter (and the device-side count) when it starts.
- * What is fixed at capture: the pointers (x, out, weights, biases, n_tokens_dev), a host-side n_tokens, and the
- * fm_set_trace and fm_set_timeout_ms settings.  Replays of launches on one context must run in stream order, one at a
+ * What is fixed at capture: the pointers (x, out, weights, biases, score_bias, n_tokens_dev), a host-side n_tokens, a
+ * gated call's fm_router_t values, and the fm_set_trace and fm_set_timeout_ms settings (the contents of score_bias are
+ * read at every replay, so a graph follows in-place bias updates).  Replays of launches on one context must run in stream order, one at a
  * time, like eager calls.  With world > 1 every rank issues the same number of launches, eager calls and replays
  * together, in the same order.  The host-buffer entry points (fm_moe_forward_host, fm_host_submit) cannot be captured.
  *
@@ -209,8 +246,9 @@ FM_API int fm_set_trace(fm_ctx_t* ctx, int enable);
 enum fm_buffer {
     FM_BUF_TOPK_IDX = 0, /* int32 [S,k]   expert index per pick (bit-exact parity target); routed: the caller's, invalid
                             ones replaced by -1 */
-    FM_BUF_TOPK_W = 1,   /* bf16  [S,k]   gateOut[t, e_j] (bf16-rounded probability); routed: rne_bf16(topk_w) */
-    FM_BUF_MCW = 2,      /* f32   [S]     sum of the k selected fp32 probabilities; routed: 1.0 */
+    FM_BUF_TOPK_W = 1,   /* bf16  [S,k]   gateOut[t, e_j] (bf16-rounded probability); routed: rne_bf16(topk_w); gated:
+                            rne_bf16(w_j), the renormalised and scaled weight */
+    FM_BUF_MCW = 2,      /* f32   [S]     sum of the k selected fp32 probabilities; routed and gated: 1.0 */
     FM_BUF_SLOT = 3,     /* int32 [S,k]   slot in the (this rank, expert) packet; >= EC means dropped; routed: INT32_MAX
                             for a -1 pick */
     FM_BUF_COUNTS = 4,   /* int32 [E]     selections per expert on this rank (incl. dropped) */
@@ -218,7 +256,7 @@ enum fm_buffer {
     FM_BUF_HIDDEN = 6,   /* bf16  [W, nLx, pEC, P]  h = act(x W_up^T + b) staging */
     FM_BUF_RET_Y = 7,    /* bf16  [E, pEC, H]       expert outputs returned to this rank */
     FM_BUF_GATE_OUT = 8, /* bf16  [S, E]  full softmax row (reference gateOut[S,PX] without the padding columns); not
-                            written by a routed launch */
+                            written by a routed launch; gated: rne_bf16(s), the full unbiased score row */
     FM_BUF_RECV_CNT = 9, /* int32 [W, nLx] rows received per (source rank, local expert) in the last forward */
     FM_BUF_TRACE = 10,   /* u64   [grid, 128] %globaltimer stamps of the last forward (fm_set_trace) */
     FM_BUF_AUX_LOSS = 11 /* f32   [2E+1] is_training = 1 only: gML[E] (mean gate probability per expert), gMeC[E] (mean
