@@ -77,21 +77,32 @@ EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
+// A tensor map and the base and row count it was encoded for (its other parameters are fixed per context).
+struct TmapCache {
+    const void* base = nullptr;
+    uint64_t rows = 0;
+    CUtensorMap map = {};
+};
+
 // 2-D row-major bf16 tensor [rows, cols], tile box [box_rows, 64 cols], 128-byte swizzle (matches the wgmma smem
-// descriptors built in fm_ptx.cuh), out-of-bounds elements read as zero.
-int make_tmap(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+// descriptors built in fm_ptx.cuh), out-of-bounds elements read as zero.  Re-encoded only when the base or the row count
+// differs from the cached map's; a failed encode leaves the cache as it was.
+int cached_tmap(TmapCache* tc, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+    if (tc->base == base && tc->rows == rows) return FM_OK;
     EncodeTiledFn fn = get_encode_fn();
     if (fn == nullptr) return fail(FM_ECUDA, "cuTensorMapEncodeTiled entry point not available");
     const cuuint64_t dims[2] = {cols, rows};
     const cuuint64_t strides[1] = {cols * 2};
     const cuuint32_t box[2] = {(cuuint32_t)fm::BLOCK_K, box_rows};
     const cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+    CUtensorMap m;
+    CUresult r = fn(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS)
         return fail(FM_ECUDA, "cuTensorMapEncodeTiled failed with CUresult %d (base=%p rows=%llu cols=%llu)", (int)r,
                     base, (unsigned long long)rows, (unsigned long long)cols);
+    *tc = {base, rows, m};
     return FM_OK;
 }
 
@@ -142,13 +153,7 @@ struct fm_ctx {
     bool fused = false;   // GEMM1 epilogue adds straight into the source rank's output (no return buffer / gather)
     bool dense = false;   // E == 1: GEMM0 reads x in place, no router GEMV, no dispatch copy (reference fffn.cuh:31-167)
     float* aux = nullptr; // is_training: [2][2E+1] {gML, gMeC, loss} by epoch parity
-    const void* cached_x = nullptr;     // the maps over the caller's x (tm_a0 when dense, tm_gx) are keyed on pointer AND
-    int cached_x_rows = 0;              // row count: a map with more rows than this call's x would read past it
     bool tc_gate = false;               // router logits on the tensor cores (E <= 256)
-    const void* cached_gx = nullptr;
-    int cached_gx_rows = 0;
-    const void* cached_gw = nullptr;
-    CUtensorMap tm_gx, tm_gw;
     unsigned int* pkt_done = nullptr;
     void* peer_base[FM_MAX_WORLD] = {};
     bool peer_opened[FM_MAX_WORLD] = {};
@@ -157,10 +162,7 @@ struct fm_ctx {
     fm::DebugRecord* dbg_dev = nullptr;
     unsigned long long* trace = nullptr;
     bool trace_on = false;
-    // tensor-map cache (re-encoded only when the caller's weight pointer changes)
-    const void* cached_expert_w = nullptr;
-    CUtensorMap tm_a0, tm_b0, tm_a1, tm_b1;
-    bool tm_static_ready = false;
+    TmapCache tm_a0, tm_b0, tm_a1, tm_b1, tm_gx, tm_gw;   // FmParams::tm_* (fm_symm_use_external moves recv_x's base)
 };
 
 namespace {
@@ -272,99 +274,119 @@ int check_kernel_status(fm_ctx* c) {
     return FM_OK;
 }
 
+// What a forward entry point received.  n_tok is the host count; with n_dev the kernel reads the count from *n_dev when
+// it starts, and n_tok is then S (the rows of x, out and the routing arrays).  A routed call (fm::ROUTE_CALLER) has
+// topk_idx / topk_w [n, k] and no gate weights; a gated one (ROUTE_GATED) has the rule `router` and score_bias [E].
+struct ForwardCall {
+    const void* x;
+    int n_tok;
+    const int32_t* n_dev;
+    const void *gate_w, *expert_w, *bias_up, *bias_down;
+    void *out, *stream;   // stream: a cudaStream_t
+    bool count_on_device = false;   // fm_moe_forward_tokens_dev: the count exists only in device memory, n_dev is required
+    int route = fm::ROUTE_ROUTER;
+    const int32_t* topk_idx = nullptr;
+    const float* topk_w = nullptr;
+    const fm_router_t* router = nullptr;
+    const float* score_bias = nullptr;
+};
+
+// The conditions on a gated call's rule that the header lists (flashmoe_b200.router.RouterSpec mirrors them).
+int check_router(const fm_dims_t& d, const fm_router_t& r) {
+    const int E = d.E;
+    if (r.scoring != 0 && r.scoring != 1)
+        return fail(FM_EINVAL, "router.scoring = %d: 0 (softmax) or 1 (sigmoid)", r.scoring);
+    if (r.n_group < 1 || r.n_group > fm::MAX_GROUPS || E % r.n_group != 0)
+        return fail(FM_EINVAL, "router.n_group = %d: must be in [1, %d] and divide E = %d", r.n_group, fm::MAX_GROUPS, E);
+    if (r.topk_group < 1 || r.topk_group > r.n_group)
+        return fail(FM_EINVAL, "router.topk_group = %d not in [1, n_group = %d]", r.topk_group, r.n_group);
+    if (r.n_group > 1 && ((r.group_top != 1 && r.group_top != 2) || r.group_top > E / r.n_group))
+        return fail(FM_EINVAL, "router.group_top = %d: 1 or 2, and at most the group size E / n_group = %d",
+                    r.group_top, E / r.n_group);
+    if (d.k > r.topk_group * (E / r.n_group))
+        return fail(FM_EINVAL, "k = %d picks need at least k experts in the topk_group = %d kept groups of %d", d.k,
+                    r.topk_group, E / r.n_group);
+    if (r.renormalize != 0 && r.renormalize != 1)
+        return fail(FM_EINVAL, "router.renormalize = %d: 0 or 1", r.renormalize);
+    if (!std::isfinite(r.scale) || !(r.scale > 0.0f))
+        return fail(FM_EINVAL, "router.scale = %g: must be finite and > 0", (double)r.scale);
+    return FM_OK;
+}
+
+// Every argument check of a forward call; issues no CUDA call.  The pointers only some entry points take are checked
+// before any field of the context is read.
+int check_call(const fm_ctx* c, const ForwardCall& f) {
+    if (f.count_on_device && f.n_dev == nullptr) return fail(FM_EINVAL, "n_tokens_dev must point to an int32");
+    if (f.route == fm::ROUTE_GATED && f.router == nullptr) return fail(FM_EINVAL, "router must point to an fm_router_t");
+    const fm_dims_t& d = c->d;
+    if (f.n_tok < 0 || f.n_tok > d.S) return fail(FM_EINVAL, "n_tokens = %d not in [0, S = %d]", f.n_tok, d.S);
+    if (f.n_dev != nullptr && f.n_tok != d.S)
+        return fail(FM_EINVAL, "with n_tokens_dev, n_tokens must be S = %d (the rows of x, out and the routing arrays); "
+                               "got %d", d.S, f.n_tok);
+    // both replace the router's softmax top-k: an E = 1 context has no router, and the auxiliary loss of a training one
+    // is defined on the router's probabilities
+    if (f.route != fm::ROUTE_ROUTER && (d.E == 1 || c->aux != nullptr))
+        return fail(FM_EINVAL, "%s needs num_experts > 1 and is_training = 0; this context has E = %d, is_training = %d",
+                    f.route == fm::ROUTE_CALLER ? "caller routing" : "a gated call", d.E, c->cfg.is_training);
+    int rc;
+    if (f.route == fm::ROUTE_GATED && (rc = check_router(d, *f.router))) return rc;
+    // Nothing reads the per-token rows of a call on no tokens.  TMA tensor maps, cp.async.bulk row copies and the
+    // 16-byte vector accesses all need 16-byte aligned bases.
+    const bool rows = f.n_tok > 0, routed = f.route == fm::ROUTE_CALLER;
+    const struct { const void* ptr; const char* name; bool required; } args[] = {
+        {f.x, "x", rows}, {f.gate_w, "gate_w", !routed}, {f.expert_w, "expert_w", true}, {f.bias_up, "bias_up", false},
+        {f.bias_down, "bias_down", false}, {f.out, "out", rows}, {f.topk_idx, "topk_idx", routed && rows},
+        {f.topk_w, "topk_w", routed && rows}, {f.score_bias, "score_bias", false}};
+    for (const auto& a : args)
+        if (a.required && a.ptr == nullptr) return fail(FM_EINVAL, "%s must be a non-null device pointer", a.name);
+    for (const auto& a : args)
+        if (reinterpret_cast<uintptr_t>(a.ptr) % 16)
+            return fail(FM_EINVAL, "%s must be 16-byte aligned (got %p)", a.name, a.ptr);
+    if (reinterpret_cast<uintptr_t>(f.n_dev) % alignof(int32_t))
+        return fail(FM_EINVAL, "n_tokens_dev must be 4-byte aligned (got %p)", static_cast<const void*>(f.n_dev));
+    if (!c->attached) return fail(FM_ESTATE, "peers not attached: call fm_symm_attach_ipc/ptrs before fm_moe_forward");
+    return FM_OK;
+}
+
 // One forward of n tokens (0 <= n <= S): the call computes exactly what a context created for n tokens would --
 // capacity EC(n), tokens per CTA ceil(n / grid) -- while every buffer keeps its create-time (maximum) size and stride.
-// n is n_tok, or with n_dev != nullptr the count the kernel reads from *n_dev when it starts (n_tok is then S).  The
-// maps over x have n_tok rows.  The kernel derives everything that depends on n and on the launch's place in the
-// context's sequence of launches itself (fm_kernel.cuh, struct Launch), so the parameters built here are valid for
-// every replay of a captured launch, and this function issues nothing that stream capture forbids.
-// `route` (fm::RouteMode): ROUTE_CALLER is caller routing (fm_moe_forward_routed) -- phase G reads the picks and weights
-// from topk_idx / topk_w [n, k] instead of running the router, and there are no gate weights (gate_w is NULL).
-// ROUTE_GATED (fm_moe_forward_gated) runs the router's logits with the rule `router` (checked by the caller) and the
-// optional score_bias [E].
-int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* gate_w, int route, const int32_t* topk_idx,
-           const float* topk_w, const void* expert_w, const void* bias_up, const void* bias_down, void* out,
-           cudaStream_t stream, const fm_router_t* router = nullptr, const float* score_bias = nullptr) {
-    if (c == nullptr) return fail(FM_EINVAL, "null context");
-    if (n_tok < 0 || n_tok > c->d.S) return fail(FM_EINVAL, "n_tokens = %d not in [0, S = %d]", n_tok, c->d.S);
-    const bool routed = route == fm::ROUTE_CALLER;
-    if (route == fm::ROUTE_GATED) {
-        if (c->d.E == 1) return fail(FM_EINVAL, "a gated call needs num_experts > 1: an E = 1 context has no router");
-        if (c->aux != nullptr)
-            return fail(FM_EINVAL, "a gated call is not available with is_training = 1: the auxiliary loss is defined on "
-                                   "softmax probabilities");
-    }
-    if (routed) {
-        if (c->d.E == 1) return fail(FM_EINVAL, "caller routing needs num_experts > 1: an E = 1 context has no router to replace");
-        if (c->aux != nullptr)
-            return fail(FM_EINVAL, "caller routing is not available with is_training = 1: the auxiliary loss needs the "
-                                   "router's probabilities");
-        if (n_tok > 0 && (topk_idx == nullptr || topk_w == nullptr))
-            return fail(FM_EINVAL, "topk_idx and topk_w must be non-null device pointers");
-    } else if (gate_w == nullptr) {
-        return fail(FM_EINVAL, "x, gate_w, expert_w and out must be non-null device pointers");
-    }
-    if (expert_w == nullptr || (n_tok > 0 && (x == nullptr || out == nullptr)))
-        return fail(FM_EINVAL, routed ? "x, expert_w and out must be non-null device pointers"
-                                      : "x, gate_w, expert_w and out must be non-null device pointers");
-    if (reinterpret_cast<uintptr_t>(n_dev) % alignof(int))
-        return fail(FM_EINVAL, "n_tokens_dev must be 4-byte aligned (got %p)", static_cast<const void*>(n_dev));
-    {   // TMA tensor maps, cp.async.bulk row copies and the 16-byte vector accesses all need 16-byte aligned bases
-        const void* ptrs[] = {x, gate_w, expert_w, bias_up, bias_down, out, topk_idx, topk_w};
-        const char* names[] = {"x", "gate_w", "expert_w", "bias_up", "bias_down", "out", "topk_idx", "topk_w"};
-        for (int i = 0; i < 8; ++i)
-            if (reinterpret_cast<uintptr_t>(ptrs[i]) % 16)
-                return fail(FM_EINVAL, "%s must be 16-byte aligned (got %p)", names[i], ptrs[i]);
-    }
-    if (!c->attached) return fail(FM_ESTATE, "peers not attached: call fm_symm_attach_ipc/ptrs before fm_moe_forward");
+// The kernel derives everything that depends on n and on the launch's place in the context's sequence of launches
+// itself (fm_kernel.cuh, struct Launch), so the parameters built here are valid for every replay of a captured launch,
+// and this function issues nothing that stream capture forbids.
+int launch(fm_ctx* c, const ForwardCall& f) {
+    int rc;
+    if ((rc = check_call(c, f))) return rc;
     FM_CUDA(cudaSetDevice(c->device));
     const fm_dims_t& d = c->d;
     const int nLx = d.num_local_experts;
-    int rc;
-    // The maps over the caller's x have exactly n_tok rows (a box taller than that reads the missing rows as zero).  With
-    // no tokens nothing reads x, and no map is encoded.
-    if (c->dense && n_tok > 0 && (c->cached_x != x || c->cached_x_rows != n_tok)) {   // E == 1: GEMM0's A operand is x
-        if ((rc = make_tmap(&c->tm_a0, x, (uint64_t)n_tok, d.H, fm::BLOCK_M))) return rc;
-        c->cached_x = x;
-        c->cached_x_rows = n_tok;
-    }
-    if (c->tc_gate && !routed) {
-        // router on tensor cores: x as [n_tok, H] in 32-row boxes, Wg_eff = the [H, E] tensor read flat as [E, H]
-        // (python_bindings.cu:93-99, moe.cuh:107-109) in boxes of min(128, E rounded up to 64) rows; rows past E read as
-        // zero
-        if (n_tok > 0 && (c->cached_gx != x || c->cached_gx_rows != n_tok)) {
-            if ((rc = make_tmap(&c->tm_gx, x, (uint64_t)n_tok, d.H, 32))) return rc;
-            c->cached_gx = x;
-            c->cached_gx_rows = n_tok;
-        }
-        if (c->cached_gw != gate_w) {
-            const uint32_t e64 = (uint32_t)((d.E + 63) / 64 * 64);
-            if ((rc = make_tmap(&c->tm_gw, gate_w, (uint64_t)d.E, d.H, std::min(128u, e64)))) return rc;
-            c->cached_gw = gate_w;
-        }
-    }
-    if (!c->tm_static_ready) {
-        if (!c->dense && (rc = make_tmap(&c->tm_a0, static_cast<char*>(c->symm) + c->off_recv_x, (uint64_t)c->num_pkts * d.pEC, d.H,
-                                         fm::BLOCK_M)))
-            return rc;
-        if ((rc = make_tmap(&c->tm_a1, c->hidden, (uint64_t)c->num_pkts * d.pEC, d.P, fm::BLOCK_M))) return rc;
-        c->tm_static_ready = true;
-    }
-    if (c->cached_expert_w != expert_w) {
-        // expert_weights [nLx, 2, P, H]: [i,0] is W_up [P,H]; [i,1] is the same P*H block viewed as W_down [H,P]
-        // (python_bindings.cu:104-119).  One tensor map per GEMM over the whole tensor with a per-expert row stride
-        // of 2*P (resp. 2*H) rows is not expressible in 2-D, so rows are addressed as [nLx*2*P, H] / [nLx*2*H, P]:
-        // expert i's W_up starts at row i*2*P, its W_down at row (i*2+1)*H of the [.,P] view.
-        if ((rc = make_tmap(&c->tm_b0, expert_w, (uint64_t)nLx * 2 * d.P, d.H, fm::BLOCK_N))) return rc;
-        if ((rc = make_tmap(&c->tm_b1, expert_w, (uint64_t)nLx * 2 * d.H, d.P, fm::BLOCK_N))) return rc;
-        c->cached_expert_w = expert_w;
-    }
+    // The maps over x have exactly n_tok rows (a box taller than that reads the missing rows as zero); with no tokens
+    // nothing reads x, and no map over it is encoded.  GEMM0's A operand is x itself when dense (E == 1), otherwise the
+    // rows dispatched into recv_x.
+    const uint64_t n = (uint64_t)f.n_tok, pkt_rows = (uint64_t)c->num_pkts * d.pEC;
+    const void* a0 = c->dense ? f.x : static_cast<const char*>(c->symm) + c->off_recv_x;
+    const uint64_t a0_rows = c->dense ? n : pkt_rows;
+    if (a0_rows > 0 && (rc = cached_tmap(&c->tm_a0, a0, a0_rows, d.H, fm::BLOCK_M))) return rc;
+    if ((rc = cached_tmap(&c->tm_a1, c->hidden, pkt_rows, d.P, fm::BLOCK_M))) return rc;
+    // expert_weights [nLx, 2, P, H]: [i,0] is W_up [P,H]; [i,1] is the same P*H block viewed as W_down [H,P]
+    // (python_bindings.cu:104-119).  One tensor map per GEMM over the whole tensor with a per-expert row stride
+    // of 2*P (resp. 2*H) rows is not expressible in 2-D, so rows are addressed as [nLx*2*P, H] / [nLx*2*H, P]:
+    // expert i's W_up starts at row i*2*P, its W_down at row (i*2+1)*H of the [.,P] view.
+    if ((rc = cached_tmap(&c->tm_b0, f.expert_w, (uint64_t)nLx * 2 * d.P, d.H, fm::BLOCK_N))) return rc;
+    if ((rc = cached_tmap(&c->tm_b1, f.expert_w, (uint64_t)nLx * 2 * d.H, d.P, fm::BLOCK_N))) return rc;
+    // router on tensor cores: x as [n_tok, H] in 32-row boxes, Wg_eff = the [H, E] tensor read flat as [E, H]
+    // (python_bindings.cu:93-99, moe.cuh:107-109) in boxes of min(128, E rounded up to 64) rows; rows past E read as
+    // zero.  A routed launch has no router maps.
+    const bool gate_maps = c->tc_gate && f.route != fm::ROUTE_CALLER;
+    const uint32_t e64 = (uint32_t)((d.E + 63) / 64 * 64);
+    if (gate_maps && n > 0 && (rc = cached_tmap(&c->tm_gx, f.x, n, d.H, 32))) return rc;
+    if (gate_maps && (rc = cached_tmap(&c->tm_gw, f.gate_w, (uint64_t)d.E, d.H, std::min(128u, e64)))) return rc;
+
     fm::FmParams p;
     memset(&p, 0, sizeof(p));
-    p.tm_a0 = c->tm_a0; p.tm_b0 = c->tm_b0; p.tm_a1 = c->tm_a1; p.tm_b1 = c->tm_b1;
-    if (c->tc_gate && !routed) { p.tm_gx = c->tm_gx; p.tm_gw = c->tm_gw; }   // (a routed launch has no router maps)
+    p.tm_a0 = c->tm_a0.map; p.tm_b0 = c->tm_b0.map; p.tm_a1 = c->tm_a1.map; p.tm_b1 = c->tm_b1.map;
+    if (gate_maps) { p.tm_gx = c->tm_gx.map; p.tm_gw = c->tm_gw.map; }
     p.tc_gate = c->tc_gate ? 1 : 0;
-    p.n_tokens = n_tok; p.n_tokens_dev = n_dev;
+    p.n_tokens = f.n_tok; p.n_tokens_dev = f.n_dev;
     p.H = d.H; p.P = d.P; p.E = d.E; p.k = d.k; p.W = d.world; p.rank = d.rank; p.nLx = nLx;
     p.pEC = d.pEC; p.TCM = d.TCM; p.act = c->cfg.hidden_act;
     p.TN0 = c->TN0; p.TN1 = c->TN1; p.num_pkts = c->num_pkts; p.num_blocks = c->num_blocks;
@@ -374,11 +396,11 @@ int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* ga
     p.timeout_ns = c->timeout_ns;
     p.launch_ctr = reinterpret_cast<unsigned long long*>(c->ctrl + 4);
     p.launch_tokens = reinterpret_cast<int*>(c->ctrl + 6);
-    p.x = static_cast<const __nv_bfloat16*>(x);
-    p.wg = static_cast<const __nv_bfloat16*>(gate_w);
-    p.b_up = static_cast<const __nv_bfloat16*>(bias_up);
-    p.b_down = static_cast<const __nv_bfloat16*>(bias_down);
-    p.out = static_cast<__nv_bfloat16*>(out);
+    p.x = static_cast<const __nv_bfloat16*>(f.x);
+    p.wg = static_cast<const __nv_bfloat16*>(f.gate_w);
+    p.b_up = static_cast<const __nv_bfloat16*>(f.bias_up);
+    p.b_down = static_cast<const __nv_bfloat16*>(f.bias_down);
+    p.out = static_cast<__nv_bfloat16*>(f.out);
     p.topk_idx = c->topk_idx; p.topk_w = c->topk_w; p.mcw = c->mcw; p.slot = c->slot; p.counts = c->counts;
     p.gate_out = c->gate_out; p.chunk_counts = c->chunk_counts;
     p.claim = c->ctrl + 1;
@@ -401,14 +423,14 @@ int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* ga
     if (d.world == 1) p.peer_out_acc[0] = p.out;
     p.aux = c->aux;
     p.dense = c->dense ? 1 : 0;
-    p.route = route;
-    p.routed_idx = topk_idx;
-    p.routed_w = topk_w;
+    p.route = f.route;
+    p.routed_idx = f.topk_idx;
+    p.routed_w = f.topk_w;
     p.status_word = c->ctrl + 7;
-    if (route == fm::ROUTE_GATED) {
-        p.scoring = router->scoring; p.n_group = router->n_group; p.topk_group = router->topk_group;
-        p.group_top = router->group_top; p.renormalize = router->renormalize; p.route_scale = router->scale;
-        p.score_bias = score_bias;
+    if (f.route == fm::ROUTE_GATED) {
+        p.scoring = f.router->scoring; p.n_group = f.router->n_group; p.topk_group = f.router->topk_group;
+        p.group_top = f.router->group_top; p.renormalize = f.router->renormalize; p.route_scale = f.router->scale;
+        p.score_bias = f.score_bias;
     }
     p.dbg = c->dbg_dev;
     p.trace = c->trace_on ? c->trace : nullptr;
@@ -417,7 +439,7 @@ int launch(fm_ctx* c, const void* x, int n_tok, const int* n_dev, const void* ga
     lc.gridDim = dim3(c->grid);
     lc.blockDim = dim3(fm::NUM_THREADS);
     lc.dynamicSmemBytes = (size_t)fm::SMEM_BYTES;
-    lc.stream = stream;
+    lc.stream = static_cast<cudaStream_t>(f.stream);
     // The persistent grid spins on flags, counters and one grid barrier, so every CTA must be resident: the launch is
     // cooperative (the driver then refuses to start it unless the whole grid fits, also next to other work on the GPU).
     cudaLaunchAttribute attr;
@@ -738,7 +760,6 @@ FM_API int fm_symm_use_external(fm_ctx_t* ctx, void* base, size_t bytes) {
     if (ctx->symm != nullptr && !ctx->symm_external) FM_CUDA(cudaFree(ctx->symm));
     ctx->symm = base;
     ctx->symm_external = true;
-    ctx->tm_static_ready = false;
     if (ctx->d.world == 1) ctx->peer_base[0] = base;
     return FM_OK;
 }
@@ -786,30 +807,30 @@ FM_API int fm_symm_attach_ptrs(fm_ctx_t* ctx, void* const* peer_bases) {
 
 FM_API int fm_moe_forward_tokens(fm_ctx_t* ctx, const void* x, int n_tokens, const void* gate_w, const void* expert_w,
                                  const void* bias_up, const void* bias_down, void* out, void* stream) {
-    return launch(ctx, x, n_tokens, nullptr, gate_w, fm::ROUTE_ROUTER, nullptr, nullptr, expert_w, bias_up, bias_down,
-                  out, static_cast<cudaStream_t>(stream));
+    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
+    return launch(ctx, {x, n_tokens, nullptr, gate_w, expert_w, bias_up, bias_down, out, stream});
 }
 
 FM_API int fm_moe_forward_tokens_dev(fm_ctx_t* ctx, const void* x, const int32_t* n_tokens_dev, const void* gate_w,
                                      const void* expert_w, const void* bias_up, const void* bias_down, void* out,
                                      void* stream) {
     if (ctx == nullptr) return fail(FM_EINVAL, "null context");
-    if (n_tokens_dev == nullptr) return fail(FM_EINVAL, "n_tokens_dev must be a device pointer to one int32");
-    if (x == nullptr || out == nullptr)
-        return fail(FM_EINVAL, "x and out must be non-null device pointers to S = %d rows", ctx->d.S);
-    return launch(ctx, x, ctx->d.S, n_tokens_dev, gate_w, fm::ROUTE_ROUTER, nullptr, nullptr, expert_w, bias_up,
-                  bias_down, out, static_cast<cudaStream_t>(stream));
+    // x and out hold S rows; a null count pointer is rejected before the context is read
+    const int rows = n_tokens_dev != nullptr ? ctx->d.S : 0;
+    ForwardCall f = {x, rows, n_tokens_dev, gate_w, expert_w, bias_up, bias_down, out, stream};
+    f.count_on_device = true;
+    return launch(ctx, f);
 }
 
 FM_API int fm_moe_forward_routed(fm_ctx_t* ctx, const void* x, int n_tokens, const int32_t* n_tokens_dev,
                                  const int32_t* topk_idx, const float* topk_w, const void* expert_w,
                                  const void* bias_up, const void* bias_down, void* out, void* stream) {
     if (ctx == nullptr) return fail(FM_EINVAL, "null context");
-    if (n_tokens_dev != nullptr && n_tokens != ctx->d.S)
-        return fail(FM_EINVAL, "with n_tokens_dev, n_tokens must be S = %d (the rows of x, out and the routing arrays); "
-                               "got %d", ctx->d.S, n_tokens);
-    return launch(ctx, x, n_tokens, n_tokens_dev, nullptr, fm::ROUTE_CALLER, topk_idx, topk_w, expert_w, bias_up,
-                  bias_down, out, static_cast<cudaStream_t>(stream));
+    ForwardCall f = {x, n_tokens, n_tokens_dev, nullptr /* no gate weights */, expert_w, bias_up, bias_down, out, stream};
+    f.route = fm::ROUTE_CALLER;
+    f.topk_idx = topk_idx;
+    f.topk_w = topk_w;
+    return launch(ctx, f);
 }
 
 FM_API int fm_moe_forward_gated(fm_ctx_t* ctx, const void* x, int n_tokens, const int32_t* n_tokens_dev,
@@ -817,32 +838,11 @@ FM_API int fm_moe_forward_gated(fm_ctx_t* ctx, const void* x, int n_tokens, cons
                                 const void* expert_w, const void* bias_up, const void* bias_down, void* out,
                                 void* stream) {
     if (ctx == nullptr) return fail(FM_EINVAL, "null context");
-    if (router == nullptr) return fail(FM_EINVAL, "router must point to an fm_router_t");
-    const fm_router_t& r = *router;
-    const int E = ctx->d.E, k = ctx->d.k;
-    if (r.scoring != 0 && r.scoring != 1)
-        return fail(FM_EINVAL, "router.scoring = %d: 0 (softmax) or 1 (sigmoid)", r.scoring);
-    if (r.n_group < 1 || r.n_group > fm::MAX_GROUPS || E % r.n_group != 0)
-        return fail(FM_EINVAL, "router.n_group = %d: must be in [1, %d] and divide E = %d", r.n_group, fm::MAX_GROUPS, E);
-    if (r.topk_group < 1 || r.topk_group > r.n_group)
-        return fail(FM_EINVAL, "router.topk_group = %d not in [1, n_group = %d]", r.topk_group, r.n_group);
-    if (r.n_group > 1 && ((r.group_top != 1 && r.group_top != 2) || r.group_top > E / r.n_group))
-        return fail(FM_EINVAL, "router.group_top = %d: 1 or 2, and at most the group size E / n_group = %d",
-                    r.group_top, E / r.n_group);
-    if (k > r.topk_group * (E / r.n_group))
-        return fail(FM_EINVAL, "k = %d picks need at least k experts in the topk_group = %d kept groups of %d", k,
-                    r.topk_group, E / r.n_group);
-    if (r.renormalize != 0 && r.renormalize != 1)
-        return fail(FM_EINVAL, "router.renormalize = %d: 0 or 1", r.renormalize);
-    if (!std::isfinite(r.scale) || !(r.scale > 0.0f))
-        return fail(FM_EINVAL, "router.scale = %g: must be finite and > 0", (double)r.scale);
-    if (reinterpret_cast<uintptr_t>(score_bias) % 16)
-        return fail(FM_EINVAL, "score_bias must be 16-byte aligned (got %p)", static_cast<const void*>(score_bias));
-    if (n_tokens_dev != nullptr && n_tokens != ctx->d.S)
-        return fail(FM_EINVAL, "with n_tokens_dev, n_tokens must be S = %d (the rows of x and out); got %d", ctx->d.S,
-                    n_tokens);
-    return launch(ctx, x, n_tokens, n_tokens_dev, gate_w, fm::ROUTE_GATED, nullptr, nullptr, expert_w, bias_up,
-                  bias_down, out, static_cast<cudaStream_t>(stream), router, score_bias);
+    ForwardCall f = {x, n_tokens, n_tokens_dev, gate_w, expert_w, bias_up, bias_down, out, stream};
+    f.route = fm::ROUTE_GATED;
+    f.router = router;
+    f.score_bias = score_bias;
+    return launch(ctx, f);
 }
 
 FM_API int fm_last_launch(fm_ctx_t* ctx, uint64_t* launches, int32_t* n_tokens) {
@@ -853,7 +853,7 @@ FM_API int fm_last_launch(fm_ctx_t* ctx, uint64_t* launches, int32_t* n_tokens) 
 FM_API int fm_moe_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, const void* expert_w, const void* bias_up,
                           const void* bias_down, void* out, void* stream) {
     if (ctx == nullptr) return fail(FM_EINVAL, "null context");
-    return fm_moe_forward_tokens(ctx, x, ctx->d.S, gate_w, expert_w, bias_up, bias_down, out, stream);
+    return launch(ctx, {x, ctx->d.S, nullptr, gate_w, expert_w, bias_up, bias_down, out, stream});
 }
 
 // ---- host-buffer entry points -----------------------------------------------------------------------------------
@@ -891,9 +891,8 @@ FM_API int fm_host_submit(fm_ctx_t* ctx, const void* x_host, const void* gate_w,
     FM_CUDA(cudaMemcpyAsync(ctx->x_stage[slot], x_host, bytes, cudaMemcpyHostToDevice, ctx->s_h2d));
     FM_CUDA(cudaEventRecord(ctx->ev_h2d[slot], ctx->s_h2d));
     FM_CUDA(cudaStreamWaitEvent(s, ctx->ev_h2d[slot], 0));
-    if ((rc = launch(ctx, ctx->x_stage[slot], ctx->d.S, nullptr, gate_w, fm::ROUTE_ROUTER, nullptr, nullptr, expert_w,
-                     bias_up, bias_down, ctx->out_stage[slot], s)))
-        return rc;
+    if ((rc = launch(ctx, {ctx->x_stage[slot], ctx->d.S, nullptr, gate_w, expert_w, bias_up, bias_down,
+                           ctx->out_stage[slot], stream}))) return rc;
     FM_CUDA(cudaEventRecord(ctx->ev_kernel[slot], s));
     FM_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_kernel[slot], 0));
     FM_CUDA(cudaMemcpyAsync(out_host, ctx->out_stage[slot], bytes, cudaMemcpyDeviceToHost, ctx->s_d2h));

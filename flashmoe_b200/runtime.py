@@ -63,16 +63,21 @@ def exchange_blobs(mine: bytes, world: int, group=None) -> bytes:
     return b"".join(gathered)
 
 
-def _check_tensor(name: str, t: torch.Tensor, device: torch.device) -> None:
-    if not t.is_cuda:
-        raise RuntimeError(f"{name} must be CUDA tensor")
-    if t.device != device:
-        raise RuntimeError(f"{name} is on {t.device}, context is on {device}")
+def _check_tensor(name: str, t: torch.Tensor, device: torch.device, dtype: torch.dtype = torch.bfloat16,
+                  shape: Optional[Dict[str, int]] = None, aligned: bool = True) -> None:
+    """A tensor argument of a C call: a contiguous CUDA tensor on `device` of `dtype`, shaped `shape` when given (named
+    dimensions: {"n": 5, "k": 2} is [n=5, k=2]), starting on a 16-byte boundary when `aligned`.  Reads metadata only (no
+    .item()): a check must not synchronise, and may run under stream capture."""
+    if not isinstance(t, torch.Tensor) or t.device != device:
+        raise RuntimeError(f"{name} must be a CUDA tensor on {device}, got {getattr(t, 'device', type(t).__name__)}")
     if not t.is_contiguous():
         raise RuntimeError(f"{name} must be contiguous")
-    if t.dtype != torch.bfloat16:
-        raise RuntimeError(f"{name} must be torch.bfloat16 (compiled Element), got {t.dtype}")
-    if t.data_ptr() % 16:
+    if t.dtype != dtype:
+        raise RuntimeError(f"{name} must be {dtype}, got {t.dtype}")
+    if shape is not None and t.shape != tuple(shape.values()):
+        dims = ", ".join(f"{k}={v}" for k, v in shape.items())
+        raise RuntimeError(f"{name} must be [{dims}], got {list(t.shape)}")
+    if aligned and t.data_ptr() % 16:
         raise RuntimeError(f"{name} must start on a 16-byte boundary (TMA tensor maps, bulk row copies and the vector "
                            f"accesses need it); got storage offset {t.storage_offset()}")
 
@@ -164,18 +169,16 @@ class MoEContext:
         """`gate_weights` None: a routed call, which has none."""
         d = self.dims
         if gate_weights is not None:
-            _check_tensor("Gate weights", gate_weights, self.device)
-            if gate_weights.dim() != 2 or gate_weights.size(0) != d["H"] or gate_weights.size(1) != d["E"]:
-                raise RuntimeError(f"Gate weights must be [H={d['H']}, E={d['E']}]. Got {list(gate_weights.shape)}")
+            _check_tensor("Gate weights", gate_weights, self.device, shape={"H": d["H"], "E": d["E"]})
         _check_tensor("Expert weights", expert_weights, self.device)
         nlx = d["num_local_experts"]
-        if expert_weights.dim() != 4 or expert_weights.size(0) != nlx:
-            raise RuntimeError(f"Expert count mismatch. Expected {nlx} local experts, got {expert_weights.size(0)}")
-        if expert_weights.size(1) != 2:
+        s = expert_weights.shape
+        if len(s) != 4 or s[0] != nlx:
+            raise RuntimeError(f"Expert count mismatch. Expected {nlx} local experts, got {s[0]}")
+        if s[1] != 2:
             raise RuntimeError("Expert weights must have up and down projections [nLx, 2, P, H]")
-        if expert_weights.size(2) != d["P"] or expert_weights.size(3) != d["H"]:
-            raise RuntimeError(f"Expert weights must be [*, 2, P={d['P']}, H={d['H']}]. Got [*, 2, "
-                               f"{expert_weights.size(2)}, {expert_weights.size(3)}]")
+        if s[2] != d["P"] or s[3] != d["H"]:
+            raise RuntimeError(f"Expert weights must be [*, 2, P={d['P']}, H={d['H']}]. Got [*, 2, {s[2]}, {s[3]}]")
 
     def _validate(self, input: torch.Tensor, gate_weights: Optional[torch.Tensor], expert_weights: torch.Tensor,
                   exact_s: bool = True) -> int:
@@ -184,16 +187,17 @@ class MoEContext:
         tokens (forward_tokens).  Returns the number of tokens."""
         d = self.dims
         _check_tensor("Input", input, self.device)
+        s = input.shape
         if exact_s:
-            if input.dim() != 3:
+            if len(s) != 3:
                 raise RuntimeError("Input must be 3D [batch, seq, H]")
-            if input.size(0) * input.size(1) != d["S"]:
-                raise RuntimeError(f"Input batch*seq must equal compiled S={d['S']}. Got batch={input.size(0)}, "
-                                   f"seq={input.size(1)} (product={input.size(0) * input.size(1)})")
-        elif input.dim() < 1:
+            if s[0] * s[1] != d["S"]:
+                raise RuntimeError(f"Input batch*seq must equal compiled S={d['S']}. Got batch={s[0]}, seq={s[1]} "
+                                   f"(product={s[0] * s[1]})")
+        elif len(s) < 1:
             raise RuntimeError("Input must be [..., H]")
-        if input.size(-1) != d["H"]:
-            raise RuntimeError(f"Input hidden_size must equal compiled H={d['H']}. Got {input.size(-1)}")
+        if s[-1] != d["H"]:
+            raise RuntimeError(f"Input hidden_size must equal compiled H={d['H']}. Got {s[-1]}")
         n = input.numel() // d["H"]
         if n > d["S"]:
             raise RuntimeError(f"Input holds {n} tokens, more than the context's S={d['S']}")
@@ -211,11 +215,9 @@ class MoEContext:
     def _bias_ptrs(self, bias_up, bias_down):
         d = self.dims
         nlx = d["num_local_experts"]
-        for name, b, n in (("bias_up", bias_up, d["P"]), ("bias_down", bias_down, d["H"])):
+        for name, b, dim in (("bias_up", bias_up, "P"), ("bias_down", bias_down, "H")):
             if b is not None:
-                _check_tensor(name, b, self.device)
-                if tuple(b.shape) != (nlx, n):
-                    raise RuntimeError(f"{name} must be [{nlx}, {n}], got {list(b.shape)}")
+                _check_tensor(name, b, self.device, shape={"nLx": nlx, dim: d[dim]})
         return (bias_up.data_ptr() if bias_up is not None else None,
                 bias_down.data_ptr() if bias_down is not None else None)
 
@@ -250,20 +252,12 @@ class MoEContext:
         n = self._validate(x, gate_weights, expert_weights, exact_s=False)
         bu, bd = self._bias_ptrs(bias_up, bias_down)
         out = self._output(x, out)
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        if n_tokens is not None:
-            self._check_count_tensor(n_tokens)
-            if n != self.dims["S"]:
-                raise RuntimeError(f"with a device-side n_tokens, x must hold exactly S={self.dims['S']} tokens (got {n})")
-            _lib.check(self._L.fm_moe_forward_tokens_dev(self._ctx, x.data_ptr(), n_tokens.data_ptr(),
-                                                         gate_weights.data_ptr(), expert_weights.data_ptr(), bu, bd,
-                                                         out.data_ptr(), stream))
-            self.last_tokens = None
-            return out
-        _lib.check(self._L.fm_moe_forward_tokens(self._ctx, x.data_ptr() if n else None, n, gate_weights.data_ptr(),
-                                                 expert_weights.data_ptr(), bu, bd, out.data_ptr() if n else None,
-                                                 stream))
-        self.last_tokens = n
+        L, c, stream = self._L, self._ctx, torch.cuda.current_stream(self.device).cuda_stream
+        gw, we = gate_weights.data_ptr(), expert_weights.data_ptr()
+        # the two C calls differ in their third argument only: the count, or the pointer to it
+        fn = L.fm_moe_forward_tokens if n_tokens is None else L.fm_moe_forward_tokens_dev
+        self._launch(lambda nd, xp, op: fn(c, xp, n if nd is None else nd, gw, we, bu, bd, op, stream),
+                     n, n_tokens, x, out)
         return out
 
     def forward_routed(self, x: torch.Tensor, topk_idx: torch.Tensor, topk_weight: torch.Tensor,
@@ -281,35 +275,15 @@ class MoEContext:
         `n_tokens` (one-element int32 CUDA tensor): as in `forward_tokens`; x, out and the routing tensors then hold S
         rows, of which the kernel reads the first n when it starts."""
         n = self._validate(x, None, expert_weights, exact_s=False)
-        k = self.dims["k"]
-        for name, t, dt in (("topk_idx", topk_idx, torch.int32), ("topk_weight", topk_weight, torch.float32)):
-            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != self.device:
-                raise RuntimeError(f"{name} must be a CUDA tensor on {self.device}")
-            if t.dtype != dt:
-                raise RuntimeError(f"{name} must be {dt}, got {t.dtype}")
-            if not t.is_contiguous():
-                raise RuntimeError(f"{name} must be contiguous")
-            if tuple(t.shape) != (n, k):
-                raise RuntimeError(f"{name} must be [n={n}, k={k}] like x's tokens, got {list(t.shape)}")
-            if n and t.data_ptr() % 16:
-                raise RuntimeError(f"{name} must start on a 16-byte boundary; got storage offset {t.storage_offset()}")
+        routing = {"n": n, "k": self.dims["k"]}
+        _check_tensor("topk_idx", topk_idx, self.device, torch.int32, shape=routing, aligned=n > 0)
+        _check_tensor("topk_weight", topk_weight, self.device, torch.float32, shape=routing, aligned=n > 0)
         bu, bd = self._bias_ptrs(bias_up, bias_down)
         out = self._output(x, out)
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        if n_tokens is not None:
-            self._check_count_tensor(n_tokens)
-            if n != self.dims["S"]:
-                raise RuntimeError(f"with a device-side n_tokens, x must hold exactly S={self.dims['S']} tokens (got {n})")
-            _lib.check(self._L.fm_moe_forward_routed(self._ctx, x.data_ptr(), n, n_tokens.data_ptr(),
-                                                     topk_idx.data_ptr(), topk_weight.data_ptr(),
-                                                     expert_weights.data_ptr(), bu, bd, out.data_ptr(), stream))
-            self.last_tokens = None
-            return out
-        _lib.check(self._L.fm_moe_forward_routed(self._ctx, x.data_ptr() if n else None, n, None,
-                                                 topk_idx.data_ptr() if n else None,
-                                                 topk_weight.data_ptr() if n else None, expert_weights.data_ptr(),
-                                                 bu, bd, out.data_ptr() if n else None, stream))
-        self.last_tokens = n
+        L, c, stream = self._L, self._ctx, torch.cuda.current_stream(self.device).cuda_stream
+        we = expert_weights.data_ptr()
+        self._launch(lambda nd, xp, op, ip, wp: L.fm_moe_forward_routed(c, xp, n, nd, ip, wp, we, bu, bd, op, stream),
+                     n, n_tokens, x, out, topk_idx, topk_weight)
         return out
 
     def forward_gated(self, x: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor,
@@ -329,43 +303,33 @@ class MoEContext:
         router.check(d["E"], d["k"])
         n = self._validate(x, gate_weights, expert_weights, exact_s=False)
         if score_bias is not None:
-            if not isinstance(score_bias, torch.Tensor) or not score_bias.is_cuda or score_bias.device != self.device:
-                raise RuntimeError(f"score_bias must be a CUDA tensor on {self.device}")
-            if score_bias.dtype != torch.float32:
-                raise RuntimeError(f"score_bias must be torch.float32, got {score_bias.dtype}")
-            if not score_bias.is_contiguous():
-                raise RuntimeError("score_bias must be contiguous")
-            if tuple(score_bias.shape) != (d["E"],):
-                raise RuntimeError(f"score_bias must be [E={d['E']}], got {list(score_bias.shape)}")
-            if score_bias.data_ptr() % 16:
-                raise RuntimeError("score_bias must start on a 16-byte boundary; got storage offset "
-                                   f"{score_bias.storage_offset()}")
+            _check_tensor("score_bias", score_bias, self.device, torch.float32, shape={"E": d["E"]})
         bu, bd = self._bias_ptrs(bias_up, bias_down)
         out = self._output(x, out)
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        rt = ctypes.byref(router.to_c())
+        L, c, stream = self._L, self._ctx, torch.cuda.current_stream(self.device).cuda_stream
+        gw, rt, we = gate_weights.data_ptr(), ctypes.byref(router.to_c()), expert_weights.data_ptr()
         sb = score_bias.data_ptr() if score_bias is not None else None
-        if n_tokens is not None:
-            self._check_count_tensor(n_tokens)
-            if n != d["S"]:
-                raise RuntimeError(f"with a device-side n_tokens, x must hold exactly S={d['S']} tokens (got {n})")
-            _lib.check(self._L.fm_moe_forward_gated(self._ctx, x.data_ptr(), n, n_tokens.data_ptr(),
-                                                    gate_weights.data_ptr(), rt, sb, expert_weights.data_ptr(), bu,
-                                                    bd, out.data_ptr(), stream))
-            self.last_tokens = None
-            return out
-        _lib.check(self._L.fm_moe_forward_gated(self._ctx, x.data_ptr() if n else None, n, None,
-                                                gate_weights.data_ptr(), rt, sb, expert_weights.data_ptr(), bu, bd,
-                                                out.data_ptr() if n else None, stream))
-        self.last_tokens = n
+        self._launch(lambda nd, xp, op: L.fm_moe_forward_gated(c, xp, n, nd, gw, rt, sb, we, bu, bd, op, stream),
+                     n, n_tokens, x, out)
         return out
 
-    def _check_count_tensor(self, t: torch.Tensor) -> None:
-        """Metadata only (no .item(): a check must not synchronise, and may run under stream capture)."""
-        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != self.device:
-            raise RuntimeError(f"n_tokens must be a CUDA tensor on {self.device}")
-        if t.dtype != torch.int32 or t.numel() != 1:
-            raise RuntimeError(f"n_tokens must be a one-element torch.int32 tensor, got {t.dtype} with {t.numel()} elements")
+    def _launch(self, call, n: int, n_tokens: Optional[torch.Tensor], *rows: torch.Tensor) -> None:
+        """The token-count convention of the forward calls: run `call(n_tokens_dev, *row pointers)`, where `rows` are
+        the tensors with one row per token (x, out, the routing arrays), then set `last_tokens`.  A host count (n_tokens
+        None) passes no count pointer, and no row pointers at n = 0 (nothing reads them).  A device count is a
+        one-element int32 CUDA tensor the kernel reads when it starts; the rows are then S, and `last_tokens` is None
+        (`launch_record()` has the count)."""
+        if n_tokens is None:
+            _lib.check(call(None, *[t.data_ptr() for t in rows]) if n else call(None, *[None] * len(rows)))
+            self.last_tokens = n
+            return
+        _check_tensor("n_tokens", n_tokens, self.device, torch.int32, aligned=False)   # the C side asks for 4 bytes
+        if n_tokens.numel() != 1:
+            raise RuntimeError(f"n_tokens must be a one-element torch.int32 tensor, got {n_tokens.numel()} elements")
+        if n != self.dims["S"]:
+            raise RuntimeError(f"with a device-side n_tokens, x must hold exactly S={self.dims['S']} tokens (got {n})")
+        _lib.check(call(n_tokens.data_ptr(), *[t.data_ptr() for t in rows]))
+        self.last_tokens = None
 
     def launch_record(self) -> Tuple[int, int]:
         """(launches, n_tokens): how many launches this context has run on the device -- graph replays included, unlike
