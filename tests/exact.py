@@ -95,20 +95,29 @@ def order_key(bits: np.ndarray) -> np.ndarray:
 
 def grid_log2(a: np.ndarray) -> int:
     """Largest q such that every element of `a` (bf16 values as float64) is a multiple of 2^q (0 for an all-zero array)."""
-    v = np.abs(np.asarray(a, dtype=np.float64))
-    v = v[v != 0]
-    if v.size == 0:
+    v = np.abs(np.asarray(a, dtype=np.float64)).ravel()
+    hi = float(v.max(initial=0.0))
+    if hi == 0:
         return 0
-    m, e = np.frexp(v)                       # v = m 2^e, m in [0.5, 1); bf16 has 8 significant bits
-    mi = np.rint(m * 256).astype(np.int64)
-    assert np.array_equal(mi.astype(np.float64) / 256, m), "not a bf16 value"
-    tz = np.zeros_like(mi)
-    r = mi.copy()
-    for _ in range(8):
-        even = (r & 1) == 0
-        tz += even
-        r = np.where(even, r >> 1, r)
-    return int((e - 8 + tz).min())
+    lo = float(v.min(where=v > 0, initial=np.inf))
+    if 2.0 ** -126 <= lo and hi < 2.0 ** 127 and hi < lo * 2.0 ** 50:
+        # fast path (a weight matrix of a model-sized layer): every element is a multiple of 2^Q, Q = the exponent of
+        # the smallest one less bf16's 7 fraction bits; the lowest set bit of the OR of all of them in units of 2^Q
+        # is the grid
+        f = v.astype(np.float32)
+        assert np.array_equal(f, v) and not (f.view(np.uint32) & 0xFFFF).any(), "not a bf16 value"
+        Q = int(np.frexp(lo)[1]) - 8
+        acc = int(np.bitwise_or.reduce((v * 2.0 ** -Q).astype(np.int64)))
+        return Q + (acc & -acc).bit_length() - 1
+    v = v[v != 0]
+    # from the float64 bits: the significand (implicit bit included for normals) over its lowest set bit is the odd
+    # part, which has at most bf16's 8 significant bits; the lowest set bit gives the element's grid
+    u = v.view(np.uint64)
+    e = (u >> np.uint64(52)).astype(np.int64)
+    m = (u & np.uint64((1 << 52) - 1)) | np.where(e > 0, 1 << 52, 0).astype(np.uint64)
+    low = m & (~m + np.uint64(1))
+    assert (m < (low << np.uint64(8))).all(), "not a bf16 value"
+    return int((np.maximum(e, 1) - 1075 + np.log2(low).astype(np.int64)).min())
 
 
 def _fmt(bits) -> str:

@@ -1,0 +1,365 @@
+"""The exact-input reference (tests/exact.py) for gated forwards (fm_moe_forward_gated), and the router's sub-chunk
+arithmetic.
+
+A CTA's ceil(n / grid) tokens go through the router in sub-chunks of TS tokens, as many as fit one padded fp32 logits
+row each in the logits scratch (gate_phase in fm_kernel.cuh); the tensor-core router caps TS at one 128-row tile.
+`regime` states that arithmetic, and tests/test_subchunk_cases.py pins its constants to the kernel's source.
+
+`check_gated_routing` checks a gated launch's gate_out, picks and weights against intervals: the scores are those of the
+softmax reference (exact.router_reference) or of the kernel's sigmoid, the selection value adds the fp32 score bias, the
+kept groups and the picks are decided from the intervals, and a token whose picks the intervals cannot decide is counted
+as ambiguous instead of checked.  The rest of a gated launch is a routed launch on its own routing
+(exact_routed.check_routed_forward).  No pytest in here.
+"""
+from __future__ import annotations
+
+import dataclasses
+import os
+from typing import List, Optional
+
+import numpy as np
+import torch
+
+from tests import exact as ex
+from tests import exact_routed as er
+
+# ----------------------------------------------------------------------------- sub-chunk arithmetic (fm_kernel.cuh)
+G_LOGIT_BYTES = 64 * 1024   # the logits scratch
+G_SEL_MAX = 8192            # tokens per CTA * k: sel_e / rank scratch, the largest the host accepts
+TC_ROWS = 128               # BLOCK_M: the tensor-core router's sub-chunk cap (two wgmma warpgroups of 64 rows)
+H100_SMS = 132              # the grid of an H100 SXM (one CTA per SM); GPU tests use the context's own grid
+
+
+def softmax_topk_lanes(E: int) -> int:
+    """Lanes per token of the router's softmax / top-k (fm_kernel.cuh softmax_topk_lanes)."""
+    if E > 8:
+        return 4 if E <= 128 else 8 if E <= 256 else 16 if E <= 512 else 32
+    p = 1
+    while p < E:
+        p <<= 1
+    return p
+
+
+def tc_router(E: int, env=None) -> bool:
+    """The router path fm_create picks: tensor cores for 17 <= E <= 256 unless FM_TC_GATE says otherwise (E = 1
+    takes the dense path and no router)."""
+    v = (os.environ if env is None else env).get("FM_TC_GATE", "")
+    want = int(v) != 0 if v else E > 16
+    return E != 1 and E <= 256 and want
+
+
+@dataclasses.dataclass(frozen=True)
+class Regime:
+    grid: int
+    tpc: int                 # tokens per CTA, ceil(n / grid)
+    TS: int                  # tokens per sub-chunk
+    sub_chunks: List[int]    # sub-chunk sizes of the fullest CTA
+    sel_entries: int         # tpc * k: entries of the sel_e / rank scratch
+    s_max: int               # the largest S, a multiple of 128, with ceil(S / grid) * k <= G_SEL_MAX
+
+    def position(self, n: int) -> np.ndarray:
+        """Sub-chunk index of each of the first n tokens inside its CTA."""
+        return (np.arange(n) % self.tpc) // self.TS if self.tpc else np.zeros(0, np.int64)
+
+
+def regime(E: int, k: int, n: int, grid: int, tc: bool) -> Regime:
+    tpc = -(-n // grid)
+    ts = G_LOGIT_BYTES // (4 * (E + 1))
+    if tc:
+        ts = min(ts, TC_ROWS)
+    elif tpc:
+        ts = min(ts, tpc)   # (the GEMV path trims TS to the CTA's tokens; the sizes are the same)
+    subs = [min(ts, tpc - s0) for s0 in range(0, tpc, ts)]
+    s_max = (grid * (G_SEL_MAX // k)) // 128 * 128
+    return Regime(grid, tpc, ts, subs, tpc * k, s_max)
+
+
+# ----------------------------------------------------------------------------- inputs at a model's layer size
+class _PerExpert:
+    """w[e] computed on demand: the reference reads one expert's weights at a time."""
+
+    def __init__(self, fn):
+        self.fn = fn
+
+    def __getitem__(self, e):
+        return self.fn(int(e))
+
+
+class LayerInputs:
+    """Exact inputs at a model's layer size (e.g. DeepSeek-V3: H = 7168, P = 2048, E = 256), in the role of
+    exact.ExactInputs: the expert weights are drawn one expert at a time from a seed per (expert, block), uploaded to
+    the device expert by expert and converted to float64 one expert at a time for the reference, so neither side
+    holds all E experts in float64 (60 GB at DeepSeek-V3's size).  x: integers in [-x_range, x_range]; Wg_eff: sparse
+    (density `wg_density`) entries +-2^-6, so the logits of H-term sums stay near unit scale; W_up: integers in
+    [-up_range, up_range] * 2^-3; W_down: integers in [-down_range, down_range] * 2^-5.  No biases."""
+
+    bu = bd = None
+
+    def __init__(self, cfg, seed: int, *, x_range: int = 4, wg_density: float = 1 / 16, up_range: int = 2,
+                 down_range: int = 2):
+        self.cfg, self.seed, self.up_range, self.down_range = cfg, seed, up_range, down_range
+        S, H, E = cfg.S, cfg.H, cfg.E
+        g = np.random.default_rng(seed)
+        x = g.integers(-x_range, x_range + 1, size=(S, H), dtype=np.int8)
+        wg = (g.integers(0, 2, size=(E, H), dtype=np.int8) * 2 - 1) * (g.random((E, H)) < wg_density)
+        self.x = torch.from_numpy(x).bfloat16().reshape(cfg.mini_batch, cfg.sequence_len, H)
+        self.wg = (torch.from_numpy(wg.astype(np.float32)) * 2.0 ** ex.WG_GRID).bfloat16().reshape(-1).reshape(H, E)
+        self.x64 = x.reshape(S, H).astype(np.float64)
+        self.wg_eff64 = wg.astype(np.float64) * 2.0 ** ex.WG_GRID
+        self.w_up64 = _PerExpert(lambda e: self._ints(e, 0).astype(np.float64) * 2.0 ** ex.WUP_GRID)       # [P, H]
+        self.w_down64 = _PerExpert(lambda e: self._ints(e, 1).astype(np.float64) * 2.0 ** ex.WDOWN_GRID)   # [H, P]
+        self.underflow_tokens = self.zero_tokens = np.zeros(0, np.int64)
+
+    def _ints(self, e: int, block: int) -> np.ndarray:
+        """int8 [P, H] of W_up (block 0) or [H, P] of W_down_eff (block 1) of expert e."""
+        P, H = self.cfg.P, self.cfg.H
+        r = self.up_range if block == 0 else self.down_range
+        g = np.random.default_rng((self.seed, e, block))
+        return g.integers(-r, r + 1, size=(P, H) if block == 0 else (H, P), dtype=np.int8)
+
+    def bias64(self, which):
+        return None
+
+    def device(self, dev):
+        """(x, gate weights, expert weights [E, 2, P, H], None, None) on `dev`; the down block is W_down_eff [H, P]
+        viewed flat as [P, H]."""
+        E, P, H = self.cfg.E, self.cfg.P, self.cfg.H
+        we = torch.empty((E, 2, P, H), dtype=torch.bfloat16, device=dev)
+        for e in range(E):
+            for block, grid in ((0, ex.WUP_GRID), (1, ex.WDOWN_GRID)):
+                w = torch.from_numpy(self._ints(e, block)).to(dev).bfloat16() * 2.0 ** grid
+                we[e, block] = w.reshape(P, H)
+        return self.x.to(dev), self.wg.to(dev), we, None, None
+
+
+# ----------------------------------------------------------------------------- gated routing reference
+def sigmoid_bounds(logits):
+    """Interval of the kernel's sigmoid (flashmoe_b200.h): relative 2^-21 + 2^-24 (|l| + 2), with a margin."""
+    s = 1.0 / (1.0 + np.exp(-logits))
+    eps = 2.0 ** -21 + 2.0 ** -24 * (np.abs(logits) * 1.01 + 3)
+    return s * (1 - eps), s * (1 + eps), s
+
+
+@dataclasses.dataclass
+class Scores:
+    s_lo: np.ndarray       # [n, E] bounds of the device's fp32 score
+    s_hi: np.ndarray
+    s_mid: np.ndarray
+    go_lo: np.ndarray      # bf16 bits [n, E] bounds of gate_out
+    go_hi: np.ndarray
+
+
+def scores(router, k, x, wg_eff) -> Scores:
+    if router.scoring == "softmax":
+        ref = ex.router_reference(x, wg_eff, k)
+        return Scores(ref.p_lo, ref.p_hi, 0.5 * (ref.p_lo + ref.p_hi), ref.go_lo, ref.go_hi)
+    ex.assert_exact_sums(x, wg_eff, None, "router logits")
+    lo, hi, mid = sigmoid_bounds(x @ wg_eff.T)
+    return Scores(lo, hi, mid, ex.f64_to_bf16(lo), ex.f64_to_bf16(hi))
+
+
+def _group_scores(c, router):
+    """[n, n_group] group scores of the selection values c [n, E]: the largest, or the sum of the two largest."""
+    n, E = c.shape
+    g = -np.sort(-c.reshape(n, router.n_group, E // router.n_group), axis=2)
+    return g[:, :, 0] if router.group_top == 1 else g[:, :, 0] + g[:, :, 1]
+
+
+def kept_groups(c, router):
+    """bool [n, n_group]: the topk_group groups of the largest group score, the lower group on equal scores."""
+    G = _group_scores(np.atleast_2d(c), router)
+    rows = np.arange(G.shape[0])
+    kept = np.zeros(G.shape, bool)
+    for _ in range(router.topk_group):
+        kept[rows, np.argmax(np.where(kept, -np.inf, G), axis=1)] = True
+    return kept
+
+
+def route_mid(c, router, k):
+    """The reference's picks [n, k] on the selection values c [n, E] (interval midpoints): larger c first, the lower
+    index on equal values, only experts of the kept groups."""
+    c = np.atleast_2d(c)
+    if router.n_group > 1:
+        allowed = np.repeat(kept_groups(c, router), c.shape[1] // router.n_group, axis=1)
+        c = np.where(allowed, c, -np.inf)
+    return np.argsort(-c, axis=1, kind="stable")[:, :k].astype(np.int32)
+
+
+def weights_bounds(sc: Scores, picks, router):
+    """Bounds [n, k] of the device's fp32 weight before its bf16 rounding."""
+    rows = np.arange(picks.shape[0])[:, None]
+    k = picks.shape[1]
+    w_lo, w_hi = sc.s_lo[rows, picks], sc.s_hi[rows, picks]
+    if router.renormalize:
+        W_lo = w_lo.sum(1, keepdims=True) * (1 - k * 2.0 ** -24)
+        W_hi = w_hi.sum(1, keepdims=True) * (1 + k * 2.0 ** -24)
+        w_lo, w_hi = w_lo / W_hi, w_hi / W_lo
+    return w_lo * router.scale * (1 - 3 * 2.0 ** -24), w_hi * router.scale * (1 + 3 * 2.0 ** -24)
+
+
+def check_gated_routing(logits, bias, router, k, dev_idx, dev_go, dev_w, wg_x):
+    """`logits` [n, E] are the exact logits x . Wg_eff^T of wg_x = (x, Wg_eff); they serve only to recognise exact ties
+    (equal logits and equal bias give identical device values), the score intervals come from wg_x.
+    gate_out inside its interval; every decided token's picks equal the reference's and its weights lie inside
+    their interval; returns the number of ambiguous tokens.  A failure names the stage (gate_out, topk_idx or topk_w),
+    the first failing token and pick, and the experts involved."""
+    n, E = logits.shape
+    if n == 0:
+        return 0
+    sc = scores(router, k, *wg_x)
+    g = ex.order_key(dev_go)
+    ok = (g >= ex.order_key(sc.go_lo)) & (g <= ex.order_key(sc.go_hi))
+    if not ok.all():
+        t, e = (int(v) for v in np.argwhere(~ok)[0])
+        raise AssertionError(f"gate_out (gated): {int((~ok).sum())} elements outside their interval; first at token "
+                             f"{t}, expert {e}: device {ex._fmt(dev_go[t, e])}, reference "
+                             f"[{ex._fmt(sc.go_lo[t, e])}, {ex._fmt(sc.go_hi[t, e])}]")
+    bv = np.zeros(E) if bias is None else np.asarray(bias, dtype=np.float64)
+    m = 2.0 ** -23 * (np.abs(sc.s_hi) + np.abs(bv)) + 1e-300        # the fp32 rounding of s + b
+    c_lo, c_hi, c_mid = sc.s_lo + bv - m, sc.s_hi + bv + m, sc.s_mid + bv
+    picks = route_mid(c_mid, router, k)
+    rows = np.arange(n)
+    decided = np.ones(n, bool)
+    allowed = np.ones((n, E), bool)
+    if router.n_group > 1:   # the kept groups must be certain: every kept group's score above every other group's
+        kept = kept_groups(c_mid, router)
+        G_lo, G_hi = _group_scores(c_lo, router), _group_scores(c_hi, router)
+        G_lo, G_hi = G_lo - 2.0 ** -23 * np.abs(G_lo), G_hi + 2.0 ** -23 * np.abs(G_hi)   # (the sum's rounding)
+        lo_kept = np.where(kept, G_lo, np.inf).min(1)
+        hi_other = np.where(kept, -np.inf, G_hi).max(1)
+        decided &= lo_kept > hi_other
+        allowed = np.repeat(kept, E // router.n_group, axis=1)
+
+    def precedes(r, a, b):   # the device's c[r, a] certainly ranks before c[r, b]: disjoint intervals, or identical
+        same = (logits[r, a] == logits[r, b]) & (bv[a] == bv[b])   # inputs (identical device values) with a < b
+        return (c_lo[r, a] > c_hi[r, b]) | (same & (a < b))
+
+    for j in range(k - 1):
+        decided &= precedes(rows, picks[:, j], picks[:, j + 1])
+    rest = allowed.copy()
+    rest[rows[:, None], picks] = False
+    decided &= (precedes(rows[:, None], picks[:, -1:], np.arange(E)[None, :]) | ~rest).all(1)
+    ambiguous = int((~decided).sum())
+    bad = decided & (np.asarray(dev_idx) != picks).any(1)
+    if bad.any():
+        t = int(np.flatnonzero(bad)[0])
+        j = int(np.flatnonzero(dev_idx[t] != picks[t])[0])
+        raise AssertionError(f"topk_idx (gated): {int(bad.sum())} decided tokens differ; first token {t} pick {j}: "
+                             f"device {list(map(int, dev_idx[t]))}, reference {picks[t].tolist()} (selection values "
+                             f"of those experts: {c_mid[t, dev_idx[t]].tolist()} vs {c_mid[t, picks[t]].tolist()})")
+    w_lo, w_hi = weights_bounds(sc, picks, router)
+    kk = ex.order_key(dev_w)
+    wok = (kk >= ex.order_key(ex.f64_to_bf16(w_lo))) & (kk <= ex.order_key(ex.f64_to_bf16(w_hi)))
+    wbad = decided[:, None] & ~wok
+    if wbad.any():
+        t, j = (int(v) for v in np.argwhere(wbad)[0])
+        raise AssertionError(f"topk_w (gated): {int(wbad.any(1).sum())} tokens with a weight outside its interval; "
+                             f"first token {t} pick {j} (expert {int(picks[t, j])}): device {ex._fmt(dev_w[t, j])}, "
+                             f"reference [{w_lo[t, j]!r}, {w_hi[t, j]!r}]")
+    return ambiguous
+
+
+# ----------------------------------------------------------------------------- device records from the reference
+def routed_device(inp: ex.ExactInputs, topk: np.ndarray, w: np.ndarray, EC: int, stats: Optional[ex.Stats] = None):
+    """A Device record of a routed launch on (topk, w) computed by the reference (ReLU: exact, GELU: the interval's
+    lower end), with recv_x, hidden and ret_y.  `stats` gets the h and out elements whose exact value needed
+    rounding."""
+    cfg = inp.cfg
+    E, H, P = cfg.E, cfg.H, cfg.P
+    n = topk.shape[0]
+    x = inp.x64[:n]
+    run = er.sanitize(topk, E)
+    w_bits = ex.f32_to_bf16(np.asarray(w, dtype=np.float32))
+    slot, counts, recv_cnt, kept = er.slots_from_routing(run, E, EC)
+    toks = ex.packet_tokens(run, slot, E, EC)
+    rmax = max(1, int(recv_cnt.max(initial=0)))
+    recv_x = np.zeros((E, rmax, H), np.uint16)
+    hidden = np.zeros((E, rmax, P), np.uint16)
+    ret_y = np.zeros((E, rmax, H), np.uint16)
+    for e in range(E):
+        c = len(toks[e])
+        if c == 0:
+            continue
+        recv_x[e, :c] = ex.f64_to_bf16(x[toks[e]])
+        h = ex.gemm0_reference(x[toks[e]], inp.w_up64[e], None if inp.bu is None else inp.bias64("up")[e],
+                               cfg.hidden_act, f"GEMM0 of expert {e}")
+        hidden[e, :c] = h.lo
+        y = ex.gemm1_reference(h.lo, inp.w_down64[e], None if inp.bd is None else inp.bias64("down")[e],
+                               f"GEMM1 of expert {e}")
+        ret_y[e, :c] = y.lo
+        if stats is not None:
+            stats.add("hidden", h.lo.size, ex.rounded_count(h))
+    y_of = ret_y[np.where(kept, run, 0), np.where(kept, slot, 0)]
+    out = er.combine_routed(y_of, kept, w_bits)
+    if stats is not None:   # the combine in real arithmetic against its bf16 result
+        real = (np.where(kept, ex.bits_to_f64(w_bits), 0.0)[:, :, None] * ex.bits_to_f64(y_of)).sum(1)
+        stats.add("out", out.size, int((ex.bits_to_f64(out) != real).sum()))
+    return ex.Device(out, run.copy(), w_bits, np.ones(n, np.float32), None, slot, counts, recv_cnt, recv_x, hidden,
+                     ret_y)
+
+
+def reference_device_gated(inp: ex.ExactInputs, router, bias, EC: int, n: Optional[int] = None,
+                           stats: Optional[ex.Stats] = None) -> ex.Device:
+    """The gated counterpart of exact.reference_device: a Device record computed from the interval midpoints (scores,
+    selection values, picks, weights), what a correct kernel could have produced.  The planted-fault tests start from
+    it."""
+    cfg = inp.cfg
+    x = inp.x64[: (cfg.S if n is None else n)]
+    sc = scores(router, cfg.k, x, inp.wg_eff64)
+    b = np.zeros(cfg.E) if bias is None else np.asarray(bias, dtype=np.float64)
+    picks = route_mid(sc.s_mid + b, router, cfg.k) if x.shape[0] else np.zeros((0, cfg.k), np.int32)
+    w_lo, w_hi = weights_bounds(sc, picks, router)
+    dev = routed_device(inp, picks, (0.5 * (w_lo + w_hi)).astype(np.float32), EC, stats)
+    dev.gate_out = ex.f64_to_bf16(sc.s_mid)
+    return dev
+
+
+def weights_f32(w_bits: np.ndarray) -> np.ndarray:
+    """bf16 bits as the fp32 weights a routed replay takes (the same bits after rne_bf16)."""
+    return (np.asarray(w_bits, dtype=np.uint16).astype(np.uint32) << 16).view(np.float32)
+
+
+def check_gated_forward(inp: ex.ExactInputs, dev: ex.Device, router, bias, EC: int,
+                        stats: Optional[ex.Stats] = None) -> int:
+    """A gated launch over the first n = len(dev.topk_idx) tokens: check_gated_routing, then every later stage as a
+    routed launch on the device's own routing.  Returns the number of ambiguous tokens."""
+    n = dev.topk_idx.shape[0]
+    x = inp.x64[:n]
+    amb = check_gated_routing(x @ inp.wg_eff64.T, bias, router, inp.cfg.k, dev.topk_idx, dev.gate_out, dev.topk_w,
+                              (x, inp.wg_eff64))
+    er.check_routed_forward(inp, dev, dev.topk_idx, weights_f32(dev.topk_w), EC, stats)
+    return amb
+
+
+# ----------------------------------------------------------------------------- training-mode auxiliary loss
+def check_aux(aux: np.ndarray, ref: ex.RouterRef, counts: np.ndarray, n: int, rg: Regime) -> None:
+    """gML, gMeC and the loss of a training launch over n tokens (aux = [gML E | gMeC E | loss]).
+    gML[e] = sum_t p[t, e] / n: an interval from p_lo / p_hi, widened by a first-order bound of the kernel's fp32
+    sums (a term passes at most ceil(TS / 32) lane adds, 5 shuffle adds, one add per sub-chunk, the division and one
+    atomic add per CTA).  gMeC[e] = __fdividef(counts[e], n): within the division's bound of counts / n, and equal to it
+    when n is a power of two.  The loss sum_e gML gMeC / E: an interval from those of gML and gMeC."""
+    E = counts.shape[0]
+    gml, gmec, loss = aux[:E].astype(np.float64), aux[E:2 * E].astype(np.float64), float(aux[2 * E])
+    if n == 0:
+        ex.check_equal(aux, np.zeros_like(aux), "aux (no tokens: all zero)", ("entry",))
+        return
+    depth = -(-rg.TS // 32) + 5 + len(rg.sub_chunks) + rg.grid + 4
+    tot_hi = ref.p_hi.sum(0)
+    slack = depth * ex.U32 * tot_hi / n + ex.EPS_DIV * tot_hi / n
+    lo, hi = ref.p_lo.sum(0) / n - slack, tot_hi / n + slack
+    bad = (gml < lo) | (gml > hi)
+    if bad.any():
+        e = int(np.flatnonzero(bad)[0])
+        raise AssertionError(f"gML: {int(bad.sum())} of {E} experts outside the interval; first expert {e}: device "
+                             f"{gml[e]!r}, reference [{lo[e]!r}, {hi[e]!r}]")
+    ce = counts.astype(np.float64) / n
+    if n & (n - 1) == 0:
+        ex.check_equal(aux[E:2 * E], ce.astype(np.float32), "gMeC = counts / n", ("expert",))
+    else:
+        bad = np.abs(gmec - ce) > ex.EPS_DIV * ce
+        assert not bad.any(), (f"gMeC: expert {int(np.flatnonzero(bad)[0])}: device "
+                               f"{gmec[bad][0]!r}, counts / n {ce[bad][0]!r}")
+    t_lo, t_hi = np.maximum(lo, 0) * gmec / E, hi * gmec / E
+    l_lo = t_lo.sum() * (1 - (E + 6) * ex.U32)   # per term: the product, __fdividef (4 roundings' worth), E adds
+    l_hi = t_hi.sum() * (1 + (E + 6) * ex.U32)
+    assert l_lo <= loss <= l_hi, f"aux loss: device {loss!r} outside [{l_lo!r}, {l_hi!r}]"

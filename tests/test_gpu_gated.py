@@ -14,6 +14,7 @@ from flashmoe_b200.config import MoEConfig
 from flashmoe_b200.router import RouterSpec
 from tests import exact as ex
 from tests import exact_routed as er
+from tests.exact_gated import check_gated_routing
 from tests.test_gated_api import gated_routing_f64
 from tests.torch_gated import moe_forward_gated_cpu
 from tests.torch_routed import moe_forward_routed_cpu
@@ -108,94 +109,6 @@ def test_softmax_scoring_is_the_routers(E, k):
 
 
 # ----------------------------------------------------------------------------- exact inputs
-def _sigmoid_bounds(logits):
-    """Interval of the kernel's sigmoid (flashmoe_b200.h): relative 2^-21 + 2^-24 (|l| + 2), with a margin."""
-    s = 1.0 / (1.0 + np.exp(-logits))
-    eps = 2.0 ** -21 + 2.0 ** -24 * (np.abs(logits) * 1.01 + 3)
-    return s * (1 - eps), s * (1 + eps), s
-
-
-def _precedes(a, b, c_lo, c_hi, key):
-    """The device's c[a] certainly ranks before c[b]: disjoint intervals, or identical inputs (identical device
-    values) with a < b."""
-    return c_lo[a] > c_hi[b] or (key[a] == key[b] and a < b)
-
-
-def check_gated_routing(logits, bias, router, k, dev_idx, dev_go, dev_w, wg_x):
-    """gate_out inside its interval; every decided token's picks equal the reference's and its weights lie inside
-    their interval; returns the number of ambiguous tokens."""
-    n, E = logits.shape
-    if router.scoring == "softmax":
-        ref = ex.router_reference(*wg_x, k)
-        s_lo, s_hi = ref.p_lo, ref.p_hi
-        s_mid = 0.5 * (s_lo + s_hi)
-        go_lo, go_hi = ref.go_lo, ref.go_hi
-    else:
-        s_lo, s_hi, s_mid = _sigmoid_bounds(logits)
-        go_lo, go_hi = ex.f64_to_bf16(s_lo), ex.f64_to_bf16(s_hi)
-    ok = (ex.order_key(dev_go) >= ex.order_key(go_lo)) & (ex.order_key(dev_go) <= ex.order_key(go_hi))
-    assert ok.all(), f"gate_out outside its interval at {np.argwhere(~ok)[0]}"
-    b = np.zeros(E) if bias is None else bias.astype(np.float64)
-    m = 2.0 ** -23 * (np.abs(s_hi) + np.abs(b)) + 1e-300        # the fp32 rounding of s + b
-    c_lo, c_hi = s_lo + b - m, s_hi + b + m
-    ambiguous = 0
-    GS = E // router.n_group
-    for t in range(n):
-        key = [(logits[t, e], b[e]) for e in range(E)]
-        r_idx = _route_mid(s_mid[t] + b, router, k)
-        decided = True
-        allowed = np.ones(E, bool)
-        if router.n_group > 1:   # the kept groups must be certain: every kept G above every other G
-            lo = np.sort(c_lo[t].reshape(-1, GS), axis=1)[:, ::-1]
-            hi = np.sort(c_hi[t].reshape(-1, GS), axis=1)[:, ::-1]
-            G_lo = lo[:, 0] if router.group_top == 1 else lo[:, 0] + lo[:, 1]
-            G_hi = hi[:, 0] if router.group_top == 1 else hi[:, 0] + hi[:, 1]
-            G_lo, G_hi = G_lo - 2.0 ** -23 * np.abs(G_lo), G_hi + 2.0 ** -23 * np.abs(G_hi)   # (the sum's rounding)
-            kept = _kept_groups(s_mid[t] + b, router)
-            if (~kept).any() and not G_lo[kept].min() > G_hi[~kept].max():
-                decided = False
-            allowed = np.repeat(kept, GS)
-        picks = list(r_idx)
-        for j in range(k - 1):
-            if not _precedes(picks[j], picks[j + 1], c_lo[t], c_hi[t], key):
-                decided = False
-        rest = [e for e in range(E) if allowed[e] and e not in picks]
-        if any(not _precedes(picks[-1], e, c_lo[t], c_hi[t], key) for e in rest):
-            decided = False
-        if not decided:
-            ambiguous += 1
-            continue
-        assert dev_idx[t].tolist() == picks, f"token {t}: picks {dev_idx[t].tolist()}, reference {picks}"
-        w_lo, w_hi = s_lo[t, picks], s_hi[t, picks]
-        if router.renormalize:
-            W_lo, W_hi = w_lo.sum() * (1 - k * 2.0 ** -24), w_hi.sum() * (1 + k * 2.0 ** -24)
-            w_lo, w_hi = w_lo / W_hi, w_hi / W_lo
-        w_lo = w_lo * router.scale * (1 - 3 * 2.0 ** -24)
-        w_hi = w_hi * router.scale * (1 + 3 * 2.0 ** -24)
-        kk = ex.order_key(dev_w[t])
-        assert (kk >= ex.order_key(ex.f64_to_bf16(w_lo))).all() and (kk <= ex.order_key(ex.f64_to_bf16(w_hi))).all(), \
-            f"token {t}: topk_w outside its interval"
-    return ambiguous
-
-
-def _kept_groups(c, router):
-    GS = c.size // router.n_group
-    g = np.sort(c.reshape(-1, GS), axis=1)[:, ::-1]
-    G = g[:, 0] if router.group_top == 1 else g[:, 0] + g[:, 1]
-    kept = np.zeros(router.n_group, bool)
-    for _ in range(router.topk_group):
-        cand = np.where(kept, -np.inf, G)
-        kept[int(np.argmax(cand))] = True
-    return kept
-
-
-def _route_mid(c, router, k):
-    """The reference's picks on the interval midpoints (larger c first, the lower index on equal values)."""
-    allowed = np.repeat(_kept_groups(c, router), c.size // router.n_group) if router.n_group > 1 else \
-        np.ones(c.size, bool)
-    return [int(e) for e in np.argsort(-np.where(allowed, c, -np.inf), kind="stable")[:k]]
-
-
 EXACT = {
     "E8_k2_sigmoid_groups_bias": (8, 2, RouterSpec("sigmoid", 4, 2, 2, True, 2.0), True, {}),
     "E8_k1_llama4_gather": (8, 1, RouterSpec("sigmoid", renormalize=False), False, {"FM_FUSED_COMBINE": "0"}),
