@@ -17,12 +17,13 @@ FM_HOST_SLOTS = 3
 
 # enum fm_buffer
 BUF_TOPK_IDX, BUF_TOPK_W, BUF_MCW, BUF_SLOT, BUF_COUNTS, BUF_RECV_X, BUF_HIDDEN, BUF_RET_Y, BUF_GATE_OUT, BUF_RECV_CNT, BUF_TRACE, BUF_AUX_LOSS = range(12)
+BUF_SHARED_Y = 12
 
 # every symbol include/flashmoe_b200.h declares (tests check the library exports all of them)
 EXPORTED_SYMBOLS = (
     "fm_compiled_config", "fm_create", "fm_destroy", "fm_get_dims", "fm_num_local_experts", "fm_symm_size",
     "fm_symm_local_ptr", "fm_symm_export", "fm_symm_attach_ipc", "fm_symm_attach_ptrs", "fm_symm_use_external",
-    "fm_moe_forward", "fm_moe_forward_tokens", "fm_moe_forward_tokens_dev", "fm_moe_forward_routed", "fm_moe_forward_gated", "fm_last_launch", "fm_output_buffer", "fm_moe_forward_host", "fm_host_submit", "fm_host_wait", "fm_check", "fm_set_timeout_ms", "fm_set_trace", "fm_launch_count",
+    "fm_moe_forward", "fm_moe_forward_tokens", "fm_moe_forward_tokens_dev", "fm_moe_forward_routed", "fm_moe_forward_gated", "fm_shared_reserve", "fm_moe_forward_shared", "fm_last_launch", "fm_output_buffer", "fm_moe_forward_host", "fm_host_submit", "fm_host_wait", "fm_check", "fm_set_timeout_ms", "fm_set_trace", "fm_launch_count",
     "fm_buffer_bytes",
     "fm_read_buffer", "fm_last_error", "fm_version",
 )
@@ -49,6 +50,12 @@ class FmRouter(ctypes.Structure):
     """fm_router_t: the router rule of fm_moe_forward_gated (flashmoe_b200.router.RouterSpec builds one)."""
     _fields_ = [("scoring", ctypes.c_int32), ("n_group", ctypes.c_int32), ("topk_group", ctypes.c_int32),
                 ("group_top", ctypes.c_int32), ("renormalize", ctypes.c_int32), ("scale", ctypes.c_float)]
+
+
+class FmSharedExpert(ctypes.Structure):
+    """fm_shared_expert_t: the shared expert of fm_moe_forward_shared (device pointers and its intermediate size Ps)."""
+    _fields_ = [("w", ctypes.c_void_p), ("bias_up", ctypes.c_void_p), ("bias_down", ctypes.c_void_p),
+                ("inter", ctypes.c_int32)]
 
 
 _lib: Optional[ctypes.CDLL] = None
@@ -84,6 +91,9 @@ def load() -> ctypes.CDLL:
     L.fm_moe_forward_routed.argtypes = [vp, cvp, ctypes.c_int, cvp, cvp, cvp, cvp, cvp, cvp, vp, vp]
     L.fm_moe_forward_gated.argtypes = [vp, cvp, ctypes.c_int, cvp, cvp, ctypes.POINTER(FmRouter), cvp, cvp, cvp, cvp,
                                        vp, vp]
+    L.fm_shared_reserve.argtypes = [vp, ctypes.c_int32]
+    L.fm_moe_forward_shared.argtypes = [vp, cvp, ctypes.c_int, cvp, cvp, ctypes.POINTER(FmRouter), cvp, cvp, cvp, cvp,
+                                        cvp, cvp, ctypes.POINTER(FmSharedExpert), vp, vp]
     L.fm_last_launch.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_int32)]
     L.fm_moe_forward_host.argtypes = [vp, cvp, cvp, cvp, cvp, cvp, vp, vp]
     L.fm_output_buffer.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t)]

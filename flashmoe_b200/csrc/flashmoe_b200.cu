@@ -77,18 +77,18 @@ EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
-// A tensor map and the base and row count it was encoded for (its other parameters are fixed per context).
+// A tensor map and the base and shape it was encoded for (its box is fixed per cache).
 struct TmapCache {
     const void* base = nullptr;
-    uint64_t rows = 0;
+    uint64_t rows = 0, cols = 0;
     CUtensorMap map = {};
 };
 
 // 2-D row-major bf16 tensor [rows, cols], tile box [box_rows, 64 cols], 128-byte swizzle (matches the wgmma smem
-// descriptors built in fm_ptx.cuh), out-of-bounds elements read as zero.  Re-encoded only when the base or the row count
+// descriptors built in fm_ptx.cuh), out-of-bounds elements read as zero.  Re-encoded only when the base or the shape
 // differs from the cached map's; a failed encode leaves the cache as it was.
 int cached_tmap(TmapCache* tc, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
-    if (tc->base == base && tc->rows == rows) return FM_OK;
+    if (tc->base == base && tc->rows == rows && tc->cols == cols) return FM_OK;
     EncodeTiledFn fn = get_encode_fn();
     if (fn == nullptr) return fail(FM_ECUDA, "cuTensorMapEncodeTiled entry point not available");
     const cuuint64_t dims[2] = {cols, rows};
@@ -102,7 +102,7 @@ int cached_tmap(TmapCache* tc, const void* base, uint64_t rows, uint64_t cols, u
     if (r != CUDA_SUCCESS)
         return fail(FM_ECUDA, "cuTensorMapEncodeTiled failed with CUresult %d (base=%p rows=%llu cols=%llu)", (int)r,
                     base, (unsigned long long)rows, (unsigned long long)cols);
-    *tc = {base, rows, m};
+    *tc = {base, rows, cols, m};
     return FM_OK;
 }
 
@@ -116,6 +116,7 @@ struct fm_ctx {
     int tpc = 0;
     int TN0 = 0, TN1 = 0, num_pkts = 0, num_blocks = 0;
     int g0_blocks = 0, g1_blocks = 0;   // GEMM0 / GEMM1 blocks of the work list (items = their tiles x row blocks per packet)
+    int split_blk = 0;                  // leading local GEMM0 blocks of the work list (the shared expert's GEMM1 follows them)
     int dbg_flags = 0;
     // in-kernel waits give up after this long (fm_set_timeout_ms): generous by default so that ordinary rank skew (a peer
     // still loading data, compiling, paused in a debugger) is not turned into a trap -- see fm_ptx.cuh SpinGuard
@@ -163,6 +164,13 @@ struct fm_ctx {
     unsigned long long* trace = nullptr;
     bool trace_on = false;
     TmapCache tm_a0, tm_b0, tm_a1, tm_b1, tm_gx, tm_gw;   // FmParams::tm_* (fm_symm_use_external moves recv_x's base)
+    // shared expert (fm_shared_reserve): staging h_s [S, shared_max] and y_s [S, H], row-block counters [S / 128]
+    int shared_max = 0;
+    __nv_bfloat16* h_s = nullptr;
+    __nv_bfloat16* y_s = nullptr;
+    unsigned int* s0_done = nullptr;
+    unsigned int* s1_done = nullptr;
+    TmapCache tm_xs, tm_ws0, tm_ws1, tm_hs;
 };
 
 namespace {
@@ -289,6 +297,8 @@ struct ForwardCall {
     const float* topk_w = nullptr;
     const fm_router_t* router = nullptr;
     const float* score_bias = nullptr;
+    bool with_shared = false;   // fm_moe_forward_shared: `shared` is required
+    const fm_shared_expert_t* shared = nullptr;
 };
 
 // The conditions on a gated call's rule that the header lists (flashmoe_b200.router.RouterSpec mirrors them).
@@ -318,6 +328,14 @@ int check_router(const fm_dims_t& d, const fm_router_t& r) {
 int check_call(const fm_ctx* c, const ForwardCall& f) {
     if (f.count_on_device && f.n_dev == nullptr) return fail(FM_EINVAL, "n_tokens_dev must point to an int32");
     if (f.route == fm::ROUTE_GATED && f.router == nullptr) return fail(FM_EINVAL, "router must point to an fm_router_t");
+    if (f.with_shared && f.shared == nullptr) return fail(FM_EINVAL, "shared must point to an fm_shared_expert_t");
+    // fm_moe_forward_shared picks the route from gate_w and router: the other route's arguments must be absent
+    if (f.route != fm::ROUTE_CALLER && (f.topk_idx != nullptr || f.topk_w != nullptr))
+        return fail(FM_EINVAL, "topk_idx / topk_w are the caller's routing: gate_w must be NULL with them");
+    if (f.route == fm::ROUTE_CALLER && f.router != nullptr)
+        return fail(FM_EINVAL, "router needs gate_w (a rule applies to the router's logits)");
+    if (f.route != fm::ROUTE_GATED && f.score_bias != nullptr)
+        return fail(FM_EINVAL, "score_bias needs gate_w and router (it steers a rule's selection)");
     const fm_dims_t& d = c->d;
     if (f.n_tok < 0 || f.n_tok > d.S) return fail(FM_EINVAL, "n_tokens = %d not in [0, S = %d]", f.n_tok, d.S);
     if (f.n_dev != nullptr && f.n_tok != d.S)
@@ -330,13 +348,28 @@ int check_call(const fm_ctx* c, const ForwardCall& f) {
                     f.route == fm::ROUTE_CALLER ? "caller routing" : "a gated call", d.E, c->cfg.is_training);
     int rc;
     if (f.route == fm::ROUTE_GATED && (rc = check_router(d, *f.router))) return rc;
+    const fm_shared_expert_t none = {};
+    const fm_shared_expert_t& sh = f.shared != nullptr ? *f.shared : none;
+    if (f.with_shared) {
+        if (d.E == 1)
+            return fail(FM_EINVAL, "a shared expert needs num_experts > 1 (an E = 1 context is one dense expert already)");
+        if (sh.inter <= 0 || sh.inter % 64)
+            return fail(FM_EINVAL, "shared->inter = %d must be a positive multiple of 64", sh.inter);
+        if (c->shared_max == 0)
+            return fail(FM_ESTATE, "no shared-expert staging: call fm_shared_reserve on this context first");
+        if (sh.inter > c->shared_max)
+            return fail(FM_EINVAL, "shared->inter = %d is above the reserved %d (fm_shared_reserve)", sh.inter,
+                        c->shared_max);
+    }
     // Nothing reads the per-token rows of a call on no tokens.  TMA tensor maps, cp.async.bulk row copies and the
     // 16-byte vector accesses all need 16-byte aligned bases.
     const bool rows = f.n_tok > 0, routed = f.route == fm::ROUTE_CALLER;
     const struct { const void* ptr; const char* name; bool required; } args[] = {
         {f.x, "x", rows}, {f.gate_w, "gate_w", !routed}, {f.expert_w, "expert_w", true}, {f.bias_up, "bias_up", false},
         {f.bias_down, "bias_down", false}, {f.out, "out", rows}, {f.topk_idx, "topk_idx", routed && rows},
-        {f.topk_w, "topk_w", routed && rows}, {f.score_bias, "score_bias", false}};
+        {f.topk_w, "topk_w", routed && rows}, {f.score_bias, "score_bias", false},
+        {sh.w, "shared->w", f.with_shared}, {sh.bias_up, "shared->bias_up", false},
+        {sh.bias_down, "shared->bias_down", false}};
     for (const auto& a : args)
         if (a.required && a.ptr == nullptr) return fail(FM_EINVAL, "%s must be a non-null device pointer", a.name);
     for (const auto& a : args)
@@ -380,6 +413,16 @@ int launch(fm_ctx* c, const ForwardCall& f) {
     const uint32_t e64 = (uint32_t)((d.E + 63) / 64 * 64);
     if (gate_maps && n > 0 && (rc = cached_tmap(&c->tm_gx, f.x, n, d.H, 32))) return rc;
     if (gate_maps && (rc = cached_tmap(&c->tm_gw, f.gate_w, (uint64_t)d.E, d.H, std::min(128u, e64)))) return rc;
+    // shared expert: x in 128-row boxes (its GEMM0's A), w [2, Ps, H] as W_up [Ps, H] and W_down [H, Ps], h_s as [S, Ps]
+    const fm_shared_expert_t* sh = f.shared;
+    const uint64_t Ps = sh != nullptr ? (uint64_t)sh->inter : 0;
+    if (sh != nullptr) {
+        const void* w_down = static_cast<const char*>(sh->w) + Ps * d.H * 2;
+        if (n > 0 && (rc = cached_tmap(&c->tm_xs, f.x, n, d.H, fm::BLOCK_M))) return rc;
+        if ((rc = cached_tmap(&c->tm_ws0, sh->w, Ps, d.H, fm::BLOCK_N))) return rc;
+        if ((rc = cached_tmap(&c->tm_ws1, w_down, d.H, Ps, fm::BLOCK_N))) return rc;
+        if ((rc = cached_tmap(&c->tm_hs, c->h_s, d.S, Ps, fm::BLOCK_M))) return rc;
+    }
 
     fm::FmParams p;
     memset(&p, 0, sizeof(p));
@@ -431,6 +474,14 @@ int launch(fm_ctx* c, const ForwardCall& f) {
         p.scoring = f.router->scoring; p.n_group = f.router->n_group; p.topk_group = f.router->topk_group;
         p.group_top = f.router->group_top; p.renormalize = f.router->renormalize; p.route_scale = f.router->scale;
         p.score_bias = f.score_bias;
+    }
+    if (sh != nullptr) {
+        if (n > 0) p.tm_xs = c->tm_xs.map;
+        p.tm_ws0 = c->tm_ws0.map; p.tm_ws1 = c->tm_ws1.map; p.tm_hs = c->tm_hs.map;
+        p.shared = 1; p.Ps = (int)Ps; p.TN0s = ceil_div((int)Ps, fm::BLOCK_N); p.split_blk = c->split_blk;
+        p.s_b_up = static_cast<const __nv_bfloat16*>(sh->bias_up);
+        p.s_b_down = static_cast<const __nv_bfloat16*>(sh->bias_down);
+        p.h_s = c->h_s; p.y_s = c->y_s; p.s0_done = c->s0_done; p.s1_done = c->s1_done;
     }
     p.dbg = c->dbg_dev;
     p.trace = c->trace_on ? c->trace : nullptr;
@@ -616,6 +667,9 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
         for (const Unit& u : g1_units) push(1, u);
     }
     ctx->num_blocks = (int)blocks.size();
+    while (ctx->split_blk < ctx->num_blocks && blocks[ctx->split_blk].kind == 0 &&
+           blocks[ctx->split_blk].pkt / nLx == rank)
+        ++ctx->split_blk;
     ctx->g0_blocks = n_g[0];
     ctx->g1_blocks = n_g[1];
     fm::TileBlock sentinel;
@@ -702,7 +756,7 @@ FM_API int fm_destroy(fm_ctx_t* ctx) {
         if (ctx->peer_opened[r] && ctx->peer_base[r] != nullptr) cudaIpcCloseMemHandle(ctx->peer_base[r]);
     void* bufs[] = {ctx->topk_idx, ctx->topk_w, ctx->mcw, ctx->slot, ctx->counts, ctx->gate_out, ctx->chunk_counts,
                     ctx->ctrl, ctx->g0_done, ctx->g1_done, ctx->pkt_done, ctx->recv_cnt, ctx->blocks, ctx->hidden, ctx->trace,
-                    ctx->aux};
+                    ctx->aux, ctx->h_s, ctx->y_s, ctx->s0_done, ctx->s1_done};
     for (void* b : bufs)
         if (b != nullptr) cudaFree(b);
     for (int i = 0; i < FM_HOST_SLOTS; ++i) {
@@ -845,6 +899,47 @@ FM_API int fm_moe_forward_gated(fm_ctx_t* ctx, const void* x, int n_tokens, cons
     return launch(ctx, f);
 }
 
+FM_API int fm_shared_reserve(fm_ctx_t* ctx, int32_t max_inter) {
+    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
+    if (max_inter <= 0 || max_inter % 64)
+        return fail(FM_EINVAL, "max_inter = %d must be a positive multiple of 64", max_inter);
+    if (ctx->d.E == 1)
+        return fail(FM_EINVAL, "a shared expert needs num_experts > 1 (an E = 1 context is one dense expert already)");
+    if (ctx->shared_max != 0)
+        return fail(FM_ESTATE, "the shared-expert staging is already reserved (max_inter = %d)", ctx->shared_max);
+    FM_CUDA(cudaSetDevice(ctx->device));
+    const size_t S = (size_t)ctx->d.S;
+    int rc;
+    if ((rc = dev_alloc(&ctx->h_s, S * max_inter)) || (rc = dev_alloc(&ctx->y_s, S * ctx->d.H)) ||
+        (rc = dev_alloc(&ctx->s0_done, S / fm::BLOCK_M)) || (rc = dev_alloc(&ctx->s1_done, S / fm::BLOCK_M))) {
+        void* bufs[] = {ctx->h_s, ctx->y_s, ctx->s0_done, ctx->s1_done};
+        for (void* b : bufs)
+            if (b != nullptr) cudaFree(b);
+        ctx->h_s = ctx->y_s = nullptr;
+        ctx->s0_done = ctx->s1_done = nullptr;
+        return rc;
+    }
+    ctx->shared_max = max_inter;
+    return FM_OK;
+}
+
+FM_API int fm_moe_forward_shared(fm_ctx_t* ctx, const void* x, int n_tokens, const int32_t* n_tokens_dev,
+                                 const void* gate_w, const fm_router_t* router, const float* score_bias,
+                                 const int32_t* topk_idx, const float* topk_w,
+                                 const void* expert_w, const void* bias_up, const void* bias_down,
+                                 const fm_shared_expert_t* shared, void* out, void* stream) {
+    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
+    ForwardCall f = {x, n_tokens, n_tokens_dev, gate_w, expert_w, bias_up, bias_down, out, stream};
+    f.route = gate_w == nullptr ? fm::ROUTE_CALLER : router == nullptr ? fm::ROUTE_ROUTER : fm::ROUTE_GATED;
+    f.topk_idx = topk_idx;
+    f.topk_w = topk_w;
+    f.router = router;
+    f.score_bias = score_bias;
+    f.with_shared = true;
+    f.shared = shared;
+    return launch(ctx, f);
+}
+
 FM_API int fm_last_launch(fm_ctx_t* ctx, uint64_t* launches, int32_t* n_tokens) {
     if (ctx == nullptr) return fail(FM_EINVAL, "null context");
     return read_launch_record(ctx, launches, n_tokens);
@@ -967,6 +1062,9 @@ static int buffer_desc(const fm_ctx_t* c, int which, const void** ptr, size_t* b
             if (c->aux == nullptr) return fail(FM_EINVAL, "the auxiliary loss exists only with is_training = 1");
             // the last launch's half of the [2][2E+1] buffer: fm_read_buffer adds its offset from the device's launch count
             *ptr = c->aux; *bytes = (size_t)(2 * d.E + 1) * 4; break;
+        case FM_BUF_SHARED_Y:
+            if (c->y_s == nullptr) return fail(FM_EINVAL, "the shared expert's outputs exist only after fm_shared_reserve");
+            *ptr = c->y_s; *bytes = (size_t)d.S * d.H * 2; break;
         default: return fail(FM_EINVAL, "unknown buffer id %d", which);
     }
     return FM_OK;

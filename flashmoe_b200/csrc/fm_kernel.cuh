@@ -302,6 +302,11 @@ struct FmParams {
     CUtensorMap tm_b1;  // expert_weights as [nLx*2*H, P]  box {64, 128}  (W_down rows)
     CUtensorMap tm_gx;  // router on tensor cores: x as [n_tokens, H], box {64, 32}
     CUtensorMap tm_gw;  // router on tensor cores: Wg_eff [E, H], box {64, min(128, E rounded up to 64)}
+    // shared expert (shared != 0, fm_moe_forward_shared): a dense FFN of intermediate size Ps on the call's own tokens
+    CUtensorMap tm_xs;   // x as [n_tokens, H], box {64, 128}: its GEMM0's A
+    CUtensorMap tm_ws0;  // W_up_s as [Ps, H], box {64, 256}
+    CUtensorMap tm_ws1;  // W_down_s (the same Ps*H block) as [H, Ps], box {64, 256}
+    CUtensorMap tm_hs;   // h_s as [S, Ps], box {64, 128}: its GEMM0's h stores and GEMM1's A
     int tc_gate;        // 1 = logits by wgmma (E <= 256); 0 = register-blocked CUDA-core GEMV
     // The call's token count and everything derived from it are resolved on the device (resolve_launch, struct Launch).
     // n_tokens: the count itself, or with n_tokens_dev the context's S -- the rows of the maps over x and the bound of
@@ -371,9 +376,17 @@ struct FmParams {
     int scoring, n_group, topk_group, group_top, renormalize;
     float route_scale;
     const float* score_bias;
+    // shared expert: TN0s = ceil(Ps / 256) GEMM0 column tiles; its GEMM1 items follow the first split_blk blocks of the
+    // work list (the local routed GEMM0 blocks).  s_b_up [Ps] / s_b_down [H] or nullptr; h_s [S, Ps] and y_s [S, H]
+    // staging; s0_done / s1_done [S / 128]: its GEMM0 / GEMM1 tiles finished per row block of tokens
+    int shared, Ps, TN0s, split_blk;
+    const __nv_bfloat16 *s_b_up, *s_b_down;
+    __nv_bfloat16 *h_s, *y_s;
+    unsigned int *s0_done, *s1_done;
     DebugRecord* dbg;
     unsigned long long* trace;  // optional [grid][TRACE_SLOTS] %globaltimer stamps (nullptr = off)
 };
+static_assert(sizeof(FmParams) <= 4096, "kernel parameters within the 4 KiB every launch path accepts");
 
 // Launch state.  Nothing that changes from launch to launch is a kernel parameter, so a launch captured in a CUDA graph
 // computes the right values on every replay: every CTA reads the context's launch counter (and, for a device-side count,
@@ -389,6 +402,9 @@ struct Launch {
     int tpc;                         // tokens per CTA, ceil(S / grid)
     int tcm_items;                   // row blocks per packet in the work list: TCM of EC at W == 1, the maximum TCM at W > 1
     int total_items;                 // work items of the launch
+    // the shared expert's items (all 0 without one): s_rb = ceil(S / 128) row blocks of tokens; its GEMM0 items are
+    // ids [0, s0_items), its GEMM1 items follow the first s_split routed items (see split_item)
+    int s_rb, s0_items, s_split, s1_items;
 };
 static_assert(sizeof(Launch) <= SMEM_USED - OFF_LAUNCH, "the Launch record's shared-memory slot");
 
@@ -415,12 +431,36 @@ __device__ __forceinline__ void resolve_launch(const FmParams& p, Launch* L) {
     // does not know their token counts and keeps the maximum (the empty row blocks are skipped by the scheduler)
     L->tcm_items = p.W == 1 ? (ec + BLOCK_M - 1) / BLOCK_M : p.TCM;
     L->total_items = p.items_per_rb * L->tcm_items;
+    L->s_rb = L->s0_items = L->s_split = L->s1_items = 0;
+    if (p.shared) {
+        const TileBlock& b = p.blocks[p.split_blk];
+        L->s_rb = (n + BLOCK_M - 1) / BLOCK_M;
+        L->s0_items = L->s_rb * p.TN0s;
+        L->s1_items = L->s_rb * p.TN1;
+        L->s_split = (b.g0 * p.TN0 + b.g1 * p.TN1) * L->tcm_items;   // block_start of block split_blk
+        L->total_items += L->s0_items + L->s1_items;
+    }
 }
 
 // first work item of block b: every earlier block holds tcm_items row blocks times its GEMM's column tiles, so the item
 // space follows the call's row-block count without rebuilding the table
 __device__ __forceinline__ int block_start(const FmParams& p, const Launch& L, const TileBlock& b) {
     return (b.g0 * p.TN0 + b.g1 * p.TN1) * L.tcm_items;
+}
+
+// Item `id` of the launch -> the shared expert's GEMM (0 or 1), with `id` made its index among that GEMM's items, or -1,
+// with `id` made the routed item's id.  The shared GEMM0 items come first (they need nothing but x, which is in memory
+// when the kernel starts, so they fill the time the routed packets' rows take to land); its GEMM1 items follow the local
+// routed GEMM0 blocks (by then their h rows are complete, and they fill the time until the routed GEMM1 dependencies
+// resolve).  Without a shared expert both ranges are empty and every id is its routed id.
+__device__ __forceinline__ int split_item(const Launch& L, int& id) {
+    if (id < L.s0_items) return 0;
+    id -= L.s0_items;
+    if (id < L.s_split) return -1;
+    id -= L.s_split;
+    if (id < L.s1_items) return 1;
+    id += L.s_split - L.s1_items;
+    return -1;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1475,7 +1515,8 @@ struct TileInfo {     // written by the scheduler warp, read by the producer / c
     int rows;         // valid rows of that block
     int src;          // source rank of the packet
     int cnt;          // rows of the whole packet
-    int pad[3];
+    int shared;       // 1: a tile of the shared expert (mblk = row block of tokens, rows = its tokens; no packet)
+    int pad[2];
 };
 static_assert(sizeof(TileInfo) <= 64, "a ring slot is 64 bytes");
 
@@ -1500,8 +1541,23 @@ __device__ __forceinline__ WorkItem decode_item(const FmParams& p, const Launch&
     return w;
 }
 
-// k-blocks of a tile: GEMM0 reduces over H, GEMM1 over P
-__device__ __forceinline__ int tile_kblocks(const FmParams& p, int kind) { return (kind == 0 ? p.H : p.P) / BLOCK_K; }
+// k-blocks of a tile: GEMM0 reduces over H, GEMM1 over P (the shared expert's over Ps)
+__device__ __forceinline__ int tile_kblocks(const FmParams& p, int kind, int shared = 0) {
+    return (kind == 0 ? p.H : shared ? p.Ps : p.P) / BLOCK_K;
+}
+
+// A shared-expert item: GEMM `kind` of row block mb of the call's tokens, column tile nt.  GEMM0 reads x in place and
+// waits for nothing; GEMM1 waits until every GEMM0 tile of its row block has stored its h rows.
+__device__ __forceinline__ void shared_tile(const FmParams& p, const Launch& L, int kind, int id, TileInfo& ti) {
+    const int mb = id % L.s_rb, nt = id / L.s_rb;
+    if (kind == 1) {
+        const unsigned int* ctr = p.s0_done + mb;
+        SpinGuard g;
+        while (ld_acquire_gpu_u32(ctr) < (unsigned int)p.TN0s) g.tick(p.dbg, p.timeout_ns, FM_TRAP_G0_DONE, 0x5E, mb, 0);
+    }
+    ti.kind = kind; ti.shared = 1; ti.ntile = nt; ti.mblk = mb; ti.rows = min(BLOCK_M, L.S - mb * BLOCK_M);
+    ti.src = p.rank; ti.cnt = L.S; ti.b_row = nt * BLOCK_N;
+}
 
 // TMA row of column tile nt's B operand.  expert_weights [nLx,2,P,H]: W_up(le) starts at row le*2*P of the [.,H] view;
 // W_down(le) (the [P,H] block flat-viewed as [H,P]) starts at row (le*2+1)*H of the [.,P] view.
@@ -1525,11 +1581,16 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L
         }
         TileInfo ti;
         ti.kind = -1; ti.ntile = 0; ti.le = 0; ti.b_row = 0; ti.pkt = 0; ti.mblk = 0; ti.rows = 0;
-        ti.src = 0; ti.cnt = 0; ti.pad[0] = ti.pad[1] = ti.pad[2] = 0;
+        ti.src = 0; ti.cnt = 0; ti.shared = 0; ti.pad[0] = ti.pad[1] = 0;
         for (;;) {
-            const int id = (int)atomicAdd(p.claim, 1u);
+            int id = (int)atomicAdd(p.claim, 1u);
             if (id >= L.total_items) break;
             trace_tile(p, TRACE_TILE_CLAIMED, n);
+            const int sk = p.shared ? split_item(L, id) : -1;
+            if (sk >= 0) {
+                shared_tile(p, L, sk, id, ti);
+                break;
+            }
             const WorkItem w = decode_item(p, L, id, cursor);
             const TileBlock& blk = w.blk;
             const int mb = w.mb, nt = w.nt, pkt = blk.pkt, le = w.le, src = w.src;
@@ -1601,31 +1662,33 @@ __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem) {
     Ring<NSCHED> q;
     bool first = true, stamped = false;
     for (;;) {
-        int kind = -1;
+        int kind = -1, shared = 0;
         TileInfo ti;
         if (lane == 0) {
             bar_wait(p, smem, BAR_SCHED_FULL + q.i, q.phase);
             ti = ring[q.i];
             mbar_arrive(bar(smem, BAR_SCHED_EMPTY + q.i));
             kind = ti.kind;
+            shared = ti.shared;
         }
         kind = __shfl_sync(0xffffffffu, kind, 0);
         if (kind < 0) break;
+        shared = __shfl_sync(0xffffffffu, shared, 0);
         int nk = 0;
         if (lane == 0) {
             if (first)   // the stage area doubles as the dispatch staging buffer
                 bar_wait(p, smem, BAR_DISP_DONE, 0);
             first = false;
             fence_proxy_async_global();  // rows written by generic-proxy stores (peers / other SMs) -> TMA reads
-            nk = tile_kblocks(p, kind);
+            nk = tile_kblocks(p, kind, shared);
         }
         nk = __shfl_sync(0xffffffffu, nk, 0);
-        const CUtensorMap* ta = kind == 0 ? &p.tm_a0 : &p.tm_a1;
-        const CUtensorMap* tb = kind == 0 ? &p.tm_b0 : &p.tm_b1;
+        const CUtensorMap* ta = shared ? (kind == 0 ? &p.tm_xs : &p.tm_hs) : (kind == 0 ? &p.tm_a0 : &p.tm_a1);
+        const CUtensorMap* tb = shared ? (kind == 0 ? &p.tm_ws0 : &p.tm_ws1) : (kind == 0 ? &p.tm_b0 : &p.tm_b1);
         const int take_at = min(nk - 1, max(0, nk - CLAIM_AHEAD_KB));
         int a_row = 0, b_row = 0;
         if (lane == 0) {
-            a_row = ti.pkt * p.pEC + ti.mblk * BLOCK_M;
+            a_row = (shared ? 0 : ti.pkt * p.pEC) + ti.mblk * BLOCK_M;   // (the shared expert's rows are the tokens)
             b_row = ti.b_row;
         }
         for (int kb = 0; kb < nk; ++kb) {
@@ -1844,9 +1907,11 @@ __device__ __forceinline__ void with_bias(const __nv_bfloat16* bias, F&& f) {
 __device__ __forceinline__ void epilogue_h(const FmParams& p, uint8_t* smem, const TileInfo* ti, float (&acc)[128], int prev,
                                            Consumer& c) {
     const int n0 = ti->ntile * BLOCK_N, le = ti->le;
+    const bool shared = ti->shared != 0;
     mainloop_done(p, smem, acc, prev, c);
-    const int nchunks = min(BLOCK_N / 64, (p.P - n0) / 64);
-    const __nv_bfloat16* bias = p.b_up ? p.b_up + (size_t)le * p.P + n0 : nullptr;
+    const int nchunks = min(BLOCK_N / 64, ((shared ? p.Ps : p.P) - n0) / 64);
+    const __nv_bfloat16* bias = shared ? (p.s_b_up ? p.s_b_up + n0 : nullptr)
+                                       : (p.b_up ? p.b_up + (size_t)le * p.P + n0 : nullptr);
     with_bias(bias, [&](auto has_bias) {
         constexpr bool B = decltype(has_bias)::value;
         if (p.act == 0) stage_h<EPI_G0_RELU, B>(p, smem, acc, bias, nchunks, c.row0, c.lane, c.chunk);
@@ -1864,7 +1929,8 @@ __device__ __forceinline__ void epilogue_out(const FmParams& p, uint8_t* smem, c
     // While the last k-block's MMAs run: the tile's fields from its ring slot and, for the fused epilogue, lane l < 16's
     // routing record of tile row (row0 + l), so that nothing is fetched after the final wait.
     const int ntile = ti->ntile, le = ti->le, pkt = ti->pkt, mblk = ti->mblk, my_rows = ti->rows, src = ti->src;
-    const bool fuse = p.fused != 0;
+    const bool shared = ti->shared != 0;   // the shared expert's s rows: stored into y_s, by token, like EPI_G1_STORE
+    const bool fuse = p.fused != 0 && !shared;
     int my_tok = 0;
     float my_pw = 0.0f, my_mcw = 1.0f;
     if (fuse && p.dense) {
@@ -1888,8 +1954,9 @@ __device__ __forceinline__ void epilogue_out(const FmParams& p, uint8_t* smem, c
         DrainArgs da;
         da.stg = smem + OFF_EPI + row0 * EPI_ROW_BYTES; da.nchunks = nchunks; da.lane = lane; da.row0 = row0;
         da.my_rows = my_rows; da.N = N; da.n0 = n0;
-        da.bias = p.b_down ? p.b_down + (size_t)le * p.H : nullptr;
-        da.out_rows = p.peer_ret_y[src] + ((size_t)e_global * p.pEC + (size_t)mblk * BLOCK_M) * p.H;
+        da.bias = shared ? p.s_b_down : p.b_down ? p.b_down + (size_t)le * p.H : nullptr;
+        da.out_rows = shared ? p.y_s + (size_t)mblk * BLOCK_M * p.H
+                             : p.peer_ret_y[src] + ((size_t)e_global * p.pEC + (size_t)mblk * BLOCK_M) * p.H;
         da.acc_base = fuse ? p.peer_out_acc[src] : nullptr;
         da.my_tok = my_tok; da.my_pw = my_pw; da.my_mcw = my_mcw;
         with_bias(da.bias, [&](auto has_bias) {
@@ -1929,7 +1996,7 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem) {
         const int kind = ti->kind;
         if (kind < 0) break;
         float acc[128];
-        const int prev = mainloop(p, smem, acc, tile_kblocks(p, kind), c);
+        const int prev = mainloop(p, smem, acc, tile_kblocks(p, kind, ti->shared), c);
         if (kind == 0) epilogue_h(p, smem, ti, acc, prev, c);
         else epilogue_out(p, smem, ti, acc, prev, c);
         ++c.ntiles;
@@ -1944,14 +2011,17 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem) {
 // (reference notifyNext's tSA counter, processor.cuh:490-615).  `chunk` counts the chunks stored so far, in the
 // consumers' staging order.
 __device__ __forceinline__ void publish_h(const FmParams& p, uint8_t* smem, const TileInfo& ti, uint32_t& chunk) {
-    const int n0 = ti.ntile * BLOCK_N, nchunks = min(BLOCK_N / 64, (p.P - n0) / 64);
-    const int row = ti.pkt * p.pEC + ti.mblk * BLOCK_M;
+    // the shared expert's h: its own map and counters, rows = tokens
+    const int n0 = ti.ntile * BLOCK_N, nchunks = min(BLOCK_N / 64, ((ti.shared ? p.Ps : p.P) - n0) / 64);
+    const int row = (ti.shared ? 0 : ti.pkt * p.pEC) + ti.mblk * BLOCK_M;
+    const CUtensorMap* map = ti.shared ? &p.tm_hs : &p.tm_a1;
+    unsigned int* ctr = ti.shared ? p.s0_done + ti.mblk : p.g0_done + (size_t)ti.pkt * p.TCM + ti.mblk;
     // both buffers' stores in flight: chunk c is issued as soon as it is staged, and only then does the warp wait for
     // the TMA to have read chunk c - 1, whose buffer the consumers refill with chunk c + 1
     for (int c = 0; c < nchunks; ++c, ++chunk) {
         const int b = chunk & 1;
         bar_wait(p, smem, BAR_STG_FULL + b, (chunk >> 1) & 1);
-        tma_store_2d(&p.tm_a1, smem + OFF_EPI + b * EPI_CHUNK_BYTES, n0 + c * 64, row);
+        tma_store_2d(map, smem + OFF_EPI + b * EPI_CHUNK_BYTES, n0 + c * 64, row);
         bulk_commit_group();
         if (c > 0) {
             bulk_wait_group_read<1>();   // chunk c - 1 has been read: its buffer may be refilled
@@ -1962,7 +2032,7 @@ __device__ __forceinline__ void publish_h(const FmParams& p, uint8_t* smem, cons
     mbar_arrive(bar(smem, BAR_STG_FREE + ((chunk - 1) & 1)));
     bulk_wait_group0();            // the tile's h writes (async proxy) are complete ...
     fence_proxy_async_global();    // ... and ordered before the generic-proxy release below
-    red_release_gpu_add_u32(p.g0_done + (size_t)ti.pkt * p.TCM + ti.mblk, 1u);
+    red_release_gpu_add_u32(ctr, 1u);
 }
 
 // GEMM1: once all consumer warps have issued their stores / REDs, a system-scope fence, then the packet or row-block
@@ -1972,10 +2042,16 @@ __device__ __forceinline__ void publish_out(const FmParams& p, const Launch& L, 
     bar_wait(p, smem, BAR_PUB_FULL + pub.i, pub.phase);
     mbar_arrive(bar(smem, BAR_PUB_EMPTY + pub.i));
     pub.next();
+    if (ti.shared) {   // the shared expert's s rows, read on this GPU by the completion phase
+        fence_acq_rel_gpu();
+        red_release_gpu_add_u32(p.s1_done + ti.mblk, 1u);
+        return;
+    }
     if (p.fused) {
         // local packet, output left in place: nobody waits for a flag (see finish_fused) -- no fence, no counter, no
-        // flag; kernel completion covers these adds
-        if (ti.src == p.rank && p.out_acc == p.out) return;
+        // flag; kernel completion covers these adds.  With a shared expert the completion phase adds s to the finished
+        // rows, so it waits for the local experts too.
+        if (ti.src == p.rank && p.out_acc == p.out && !p.shared) return;
         fence_acq_rel_sys();   // this tile's adds are performed before the packet counter moves
         const unsigned int old = atom_acq_rel_gpu_add_u32(p.pkt_done + ti.pkt, 1u);
         const unsigned int want = (unsigned int)(((ti.cnt + BLOCK_M - 1) / BLOCK_M) * p.TN1);
@@ -2043,8 +2119,13 @@ __device__ __forceinline__ void ffn_warm_l2(const FmParams& p, const Launch& L) 
         // Warm L2 with the 256-row weight tile this CTA will most likely claim first (item id = CTA index: the first wave is
         // claimed in arrival order), pipeline depth only: HBM is idle during the router and the first tile's loads are
         // then L2 hits.  A wrong guess costs nothing -- the tile is needed by some CTA of the first wave anyway.
-        const int id = (int)blockIdx.x;
-        if (id < L.total_items) {
+        int id = (int)blockIdx.x;
+        const int sk = p.shared && id < L.total_items ? split_item(L, id) : -1;
+        if (sk >= 0) {   // a shared-expert tile: its weights' column tile
+            const CUtensorMap* tb = sk == 0 ? &p.tm_ws0 : &p.tm_ws1;
+            for (int kb = 0; kb < min(tile_kblocks(p, sk, 1), STAGES); ++kb)
+                tma_prefetch_l2_2d(tb, kb * BLOCK_K, (id / L.s_rb) * BLOCK_N);
+        } else if (id < L.total_items) {
             int cursor = 0;
             const WorkItem w = decode_item(p, L, id, cursor);
             const int kind = w.blk.kind;
@@ -2098,9 +2179,31 @@ __device__ __forceinline__ void ffn_roles(const FmParams& p, const Launch& L, ui
 // Deterministic gather (no atomics, no zero-fill pass); for k == 2 it equals the reference's atomicAdd result
 // exactly because bf16 addition commutes and 0 + a is exact.
 // ============================================================================================================
+// The shared expert's term: rne(fl32(r) + fl32(s)) per element, for 8 bf16 routed results r and shared outputs s
+__device__ __forceinline__ uint4 add_shared_bf16x8(const uint4& r, const uint4& s) {
+    float a[8], b[8];
+    unpack8(r, a);
+    unpack8(s, b);
+    uint4 o;
+    o.x = pack_bf16x2(a[0] + b[0], a[1] + b[1]); o.y = pack_bf16x2(a[2] + b[2], a[3] + b[3]);
+    o.z = pack_bf16x2(a[4] + b[4], a[5] + b[5]); o.w = pack_bf16x2(a[6] + b[6], a[7] + b[7]);
+    return o;
+}
+
+// every shared-expert GEMM1 tile of the row blocks holding this CTA's tokens has stored its s rows into y_s
+__device__ __noinline__ void wait_shared_rows(const FmParams& p, int t0, int n_tok) {
+    if (n_tok == 0) return;
+    for (int rb = t0 / BLOCK_M + (int)threadIdx.x; rb <= (t0 + n_tok - 1) / BLOCK_M; rb += NUM_THREADS) {
+        SpinGuard g;
+        while (ld_acquire_gpu_u32(p.s1_done + rb) < (unsigned int)p.TN1)
+            g.tick(p.dbg, p.timeout_ns, FM_TRAP_RET_FLAG, 0x5E, rb, 0);
+    }
+}
+
+// ys: the shared expert's outputs y_s (added after the k terms) or nullptr
 template <int KMAX, int PIECES>
 __device__ __forceinline__ void combine_rows(const FmParams& p, int EC, int t0, int n_tok, const int* c_e, const int* c_s,
-                                             const float* c_w, const float* c_m) {
+                                             const float* c_w, const float* c_m, const __nv_bfloat16* ys) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int H = p.H, k = p.k;
     for (int ti = warp; ti < n_tok; ti += NUM_WARPS) {
@@ -2153,6 +2256,7 @@ __device__ __forceinline__ void combine_rows(const FmParams& p, int EC, int t0, 
                 uint4 o;
                 o.x = pack_bf16x2(acc[0], acc[1]); o.y = pack_bf16x2(acc[2], acc[3]);
                 o.z = pack_bf16x2(acc[4], acc[5]); o.w = pack_bf16x2(acc[6], acc[7]);
+                if (ys != nullptr) o = add_shared_bf16x8(o, ld_global_v4(ys + (size_t)(t0 + ti) * H + h));
                 st_global_v4(orow + h, o);
             }
         }
@@ -2160,37 +2264,44 @@ __device__ __forceinline__ void combine_rows(const FmParams& p, int EC, int t0, 
 }
 
 // fused path: the output rows were accumulated by the GEMM1 epilogues; wait until every expert (local or remote) has
-// reported all of its contributions, then (W > 1) move my rows from the symmetric accumulator to the caller's tensor
+// reported all of its contributions, then (W > 1) move my rows from the symmetric accumulator to the caller's tensor.
+// With a shared expert, out[t] = rne(r[t] + s[t]) once r[t] is complete (the routed terms were added onto +0, which keeps
+// k <= 2 order-independent; a third add in arrival order would not be): in place at W = 1, in the copy at W > 1.
 __device__ __forceinline__ void finish_fused(const FmParams& p, const Launch& L, int t0, int n_tok) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     // Contributions of experts on THIS GPU need no flag when the rows are left where they were accumulated (out == the
     // accumulation target): they are complete when the kernel is, and nobody reads them before.  Only the experts on other
     // ranks -- whose adds arrive over NVLink at their own pace -- must have reported; with a separate caller tensor (the
-    // copy below) the local ones must have, too.
-    const bool need_local = p.out_acc != p.out;
+    // copy below), or a shared expert's term to add to the finished rows, the local ones must have, too (a CTA without
+    // tokens has no rows to read).
+    const bool need_local = p.out_acc != p.out || (p.shared && n_tok > 0);
     for (int e = tid; e < p.E; e += NUM_THREADS) {
         if (!need_local && e / p.nLx == p.rank) continue;
         SpinGuard g;
         while ((ld_acquire_sys_u64(p.done_flag + e) >> 32) != L.epoch)
             g.tick(p.dbg, p.timeout_ns, FM_TRAP_RET_FLAG, e, 0xD0E, 0);
     }
+    if (p.shared) wait_shared_rows(p, t0, n_tok);
     __syncthreads();
     if (tid == 0) trace_stamp(p, TRACE_DONE_FLAGS);   // every expert's contributions to this rank's tokens are in
-    if (p.out_acc != p.out) {
+    if (p.out_acc != p.out || p.shared) {
+        const __nv_bfloat16* ys = p.shared ? p.y_s : nullptr;
         for (int ti = warp; ti < n_tok; ti += NUM_WARPS) {
-            const __nv_bfloat16* src = p.out_acc + (size_t)(t0 + ti) * p.H;
-            __nv_bfloat16* dst = p.out + (size_t)(t0 + ti) * p.H;
+            const size_t row = (size_t)(t0 + ti) * p.H;
+            const __nv_bfloat16* src = p.out_acc + row;
+            __nv_bfloat16* dst = p.out + row;
             for (int hg = 0; hg < p.H; hg += 1024) {
-                uint4 v[4];
+                uint4 v[4], s[4];
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int h = hg + i * 256 + lane * 8;
                     if (h < p.H) v[i] = ld_global_v4(src + h);
+                    if (h < p.H && ys != nullptr) s[i] = ld_global_v4(ys + row + h);
                 }
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int h = hg + i * 256 + lane * 8;
-                    if (h < p.H) st_global_v4(dst + h, v[i]);
+                    if (h < p.H) st_global_v4(dst + h, ys != nullptr ? add_shared_bf16x8(v[i], s[i]) : v[i]);
                 }
             }
         }
@@ -2222,7 +2333,9 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, const Launch& L
         }
     }
     for (int i = tid; i < n_tok; i += NUM_THREADS) c_m[i] = p.mcw[t0 + i];
+    if (p.shared) wait_shared_rows(p, t0, n_tok);
     __syncthreads();
+    const __nv_bfloat16* ys = p.shared ? p.y_s : nullptr;   // the shared expert's term, added after the k terms
     if (k == 1 && p.route == ROUTE_ROUTER) {
         for (int ti = warp; ti < n_tok; ti += NUM_WARPS) {
             const bool keep = c_s[ti] < EC;
@@ -2231,13 +2344,14 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, const Launch& L
             for (int h = lane * 8; h < H; h += 256) {
                 uint4 v = make_uint4(0u, 0u, 0u, 0u);
                 if (keep) v = ld_global_v4(yrow + h);
+                if (ys != nullptr) v = add_shared_bf16x8(v, ld_global_v4(ys + (size_t)(t0 + ti) * H + h));
                 st_global_v4(orow + h, v);
             }
         }
     } else if (k <= 2) {   // (k = 1 with caller or gated routing: the scaled term rne(w~ * y))
-        combine_rows<2, 4>(p, EC, t0, n_tok, c_e, c_s, c_w, c_m);
+        combine_rows<2, 4>(p, EC, t0, n_tok, c_e, c_s, c_w, c_m, ys);
     } else {
-        combine_rows<8, 1>(p, EC, t0, n_tok, c_e, c_s, c_w, c_m);
+        combine_rows<8, 1>(p, EC, t0, n_tok, c_e, c_s, c_w, c_m, ys);
     }
 }
 
@@ -2263,6 +2377,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) fm_moe_forward_kernel(const __
             p.g1_done[i] = 0u;
         }
         for (int i = tid; i < p.num_pkts; i += NUM_THREADS) p.pkt_done[i] = 0u;
+        if (p.shared)   // the shared expert's row-block counters (every row block this launch can have)
+            for (int i = tid; i < L.s_rb; i += NUM_THREADS) p.s0_done[i] = p.s1_done[i] = 0u;
         // the arrival counters of the NEXT epoch's parity: nobody reads them any more (launch epoch-1 is over) and no
         // peer can write them yet (a rank starts forward epoch+1 only after this launch has returned all its rows)
         unsigned int* next_rows = p.recv_rows + (size_t)((L.epoch + 1u) & 1u) * p.num_pkts * p.TCM;

@@ -10,7 +10,7 @@ import torch
 
 from .config import MoEConfig
 from .router import RouterSpec
-from .runtime import MoEContext
+from .runtime import MoEContext, SharedExpert
 
 
 class MoEOutput(NamedTuple):
@@ -34,10 +34,14 @@ class FlashMoELayer(torch.nn.Module):
     applies to the gate's logits instead of the built-in softmax / top-k / renormalise (`MoEContext.forward_gated`).
     `score_bias` (with a `router` only): hold an fp32 [E] selection bias, `score_bias` (Hugging Face's
     `e_score_correction_bias`), zero-initialised; the caller updates it in place, e.g. from the `counts` buffer.
+    `shared_inter`: hold a shared expert of that intermediate size Ps, `shared_weight` [2, Ps, H] (one routed expert's
+    layout; plus `shared_bias_up` [Ps] / `shared_bias_down` [H] with `bias`), which every token passes through on every
+    route: out[t] = rne_bf16(routed[t] + s[t]) (`MoEContext.forward_tokens`'s `shared_expert`).
     """
 
     def __init__(self, cfg: MoEConfig, rank: int = 0, world: int = 1, device: Optional[int] = None, group=None,
-                 bias: bool = False, router: Optional[RouterSpec] = None, score_bias: bool = False):
+                 bias: bool = False, router: Optional[RouterSpec] = None, score_bias: bool = False,
+                 shared_inter: Optional[int] = None):
         super().__init__()
         cfg.check_hot_path()
         if router is not None:
@@ -48,7 +52,7 @@ class FlashMoELayer(torch.nn.Module):
             raise ValueError("score_bias needs a router rule (router=RouterSpec(...))")
         self.cfg = cfg
         self.router = router
-        self.ctx = MoEContext(cfg, rank=rank, world=world, device=device, group=group)
+        self.ctx = MoEContext(cfg, rank=rank, world=world, device=device, group=group, shared_inter=shared_inter)
         dev = self.ctx.device
         nlx = self.ctx.num_local_experts
         scale = cfg.H ** -0.5
@@ -64,6 +68,16 @@ class FlashMoELayer(torch.nn.Module):
             self.bias_down = None
         self.score_bias = (torch.nn.Parameter(torch.zeros(cfg.E, device=dev, dtype=torch.float32), requires_grad=False)
                            if score_bias else None)
+        self.shared_inter = shared_inter
+        self.shared_weight = self.shared_bias_up = self.shared_bias_down = None
+        if shared_inter is not None:
+            self.shared_weight = torch.nn.Parameter(torch.randn(2, shared_inter, cfg.H, device=dev).mul_(scale).bfloat16(),
+                                                    requires_grad=False)
+            if bias:
+                self.shared_bias_up = torch.nn.Parameter(torch.zeros(shared_inter, device=dev, dtype=torch.bfloat16),
+                                                         requires_grad=False)
+                self.shared_bias_down = torch.nn.Parameter(torch.zeros(cfg.H, device=dev, dtype=torch.bfloat16),
+                                                           requires_grad=False)
 
     @torch.no_grad()
     def forward(self, x: torch.Tensor, return_routing: bool = False, n_tokens: Optional[torch.Tensor] = None,
@@ -82,19 +96,22 @@ class FlashMoELayer(torch.nn.Module):
             raise RuntimeError("Input must be 3D [batch, seq, H]")
         if (topk_idx is None) != (topk_weight is None):
             raise RuntimeError("pass both topk_idx and topk_weight, or neither")
+        shared = (SharedExpert(self.shared_weight, self.shared_bias_up, self.shared_bias_down)
+                  if self.shared_weight is not None else None)
         if topk_idx is not None:
             if topk_idx.is_floating_point() or not topk_weight.is_floating_point():
                 raise RuntimeError("topk_idx must be an integer tensor and topk_weight a floating-point one")
             out = self.ctx.forward_routed(x, topk_idx.to(torch.int32).contiguous(),
                                           topk_weight.to(torch.float32).contiguous(), self.expert_weight,
-                                          bias_up=self.bias_up, bias_down=self.bias_down, n_tokens=n_tokens)
+                                          bias_up=self.bias_up, bias_down=self.bias_down, n_tokens=n_tokens,
+                                          shared_expert=shared)
         elif self.router is not None:
             out = self.ctx.forward_gated(x, self.gate_weight, self.expert_weight, self.router,
                                          score_bias=self.score_bias, bias_up=self.bias_up, bias_down=self.bias_down,
-                                         n_tokens=n_tokens)
+                                         n_tokens=n_tokens, shared_expert=shared)
         else:
             out = self.ctx.forward_tokens(x, self.gate_weight, self.expert_weight, bias_up=self.bias_up,
-                                          bias_down=self.bias_down, n_tokens=n_tokens)
+                                          bias_down=self.bias_down, n_tokens=n_tokens, shared_expert=shared)
         if not return_routing:
             return out
         return self.routing(out)
@@ -113,4 +130,5 @@ class FlashMoELayer(torch.nn.Module):
     def extra_repr(self) -> str:
         c = self.cfg
         return (f"S={c.S}, H={c.H}, P={c.P}, E={c.E}, k={c.k}, act={'gelu' if c.hidden_act else 'relu'}, "
-                f"rank={self.ctx.rank}/{self.ctx.world}")
+                f"rank={self.ctx.rank}/{self.ctx.world}"
+                + (f", shared_inter={self.shared_inter}" if self.shared_inter is not None else ""))

@@ -9,7 +9,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from typing import Dict, Optional, Tuple
+from typing import Dict, NamedTuple, Optional, Tuple
 
 import numpy as np
 import torch
@@ -31,6 +31,7 @@ _BUFFER_SPECS = {
     "recv_cnt": (_lib.BUF_RECV_CNT, np.int32),
     "trace": (_lib.BUF_TRACE, np.uint64),
     "aux_loss": (_lib.BUF_AUX_LOSS, np.float32),
+    "shared_y": (_lib.BUF_SHARED_Y, np.uint16),
 }
 
 
@@ -82,17 +83,52 @@ def _check_tensor(name: str, t: torch.Tensor, device: torch.device, dtype: torch
                            f"accesses need it); got storage offset {t.storage_offset()}")
 
 
+class SharedExpert(NamedTuple):
+    """A shared expert (fm_moe_forward_shared): a dense FFN every token passes through, its output added to the routed
+    combine.  `w` bf16 [2, Ps, H] is one routed expert's layout ([0] = W_up [Ps, H], [1] flat-viewed as W_down [H, Ps]);
+    `bias_up` bf16 [Ps] and `bias_down` bf16 [H] are optional.  Ps is a multiple of 64.  Several shared experts of size P
+    are one of size n_shared * P: concatenate their W_up rows and their W_down columns."""
+    w: torch.Tensor
+    bias_up: Optional[torch.Tensor] = None
+    bias_down: Optional[torch.Tensor] = None
+
+
+def shared_expert_struct(se: SharedExpert, device: torch.device, H: int, reserved: Optional[int]) -> _lib.FmSharedExpert:
+    """Check a `SharedExpert` against a context on `device` with hidden size H and reserved intermediate size `reserved`
+    (None: not reserved), and return its fm_shared_expert_t.  The caller keeps the tensors alive."""
+    if not isinstance(se, SharedExpert):
+        raise TypeError(f"shared_expert must be a SharedExpert, got {type(se).__name__}")
+    if reserved is None:
+        raise RuntimeError("this context has no shared-expert staging: create it with shared_inter=")
+    if not isinstance(se.w, torch.Tensor) or se.w.dim() != 3:
+        raise RuntimeError(f"shared_expert.w must be a 3-D tensor [2, Ps, H], got {getattr(se.w, 'shape', se.w)}")
+    ps = int(se.w.shape[1])
+    _check_tensor("shared_expert.w", se.w, device, shape={"up/down": 2, "Ps": ps, "H": H})
+    if ps <= 0 or ps % 64:
+        raise RuntimeError(f"shared_expert.w: Ps = {ps} must be a positive multiple of 64")
+    if ps > reserved:
+        raise RuntimeError(f"shared_expert.w: Ps = {ps} is above the context's shared_inter = {reserved}")
+    for name, b, dims in (("bias_up", se.bias_up, {"Ps": ps}), ("bias_down", se.bias_down, {"H": H})):
+        if b is not None:
+            _check_tensor(f"shared_expert.{name}", b, device, shape=dims)
+    return _lib.FmSharedExpert(se.w.data_ptr(), se.bias_up.data_ptr() if se.bias_up is not None else None,
+                               se.bias_down.data_ptr() if se.bias_down is not None else None, ps)
+
+
 class MoEContext:
     """Owns the native context (workspaces, symmetric slab, peer mappings) for one rank."""
 
     def __init__(self, cfg: Optional[MoEConfig] = None, rank: int = 0, world: int = 1,
                  device: Optional[int] = None, group=None, timeout_ms: Optional[int] = None,
-                 symmetric: Optional[str] = None):
+                 symmetric: Optional[str] = None, shared_inter: Optional[int] = None):
         """`symmetric` selects how the peers' slabs are mapped when world > 1: "ipc" (default; cudaMalloc + CUDA IPC
         handles over torch.distributed) or "torch" (the slab is allocated with torch.distributed._symmetric_memory --
         the allocator PyTorch backs with CUDA VMM / NVSHMEM -- and the peer pointers come from its rendezvous; this is
         the hook for externally managed symmetric heaps, reference bootstrap.cuh:359-360,442-443).  Environment
-        override: FM_SYMM=ipc|torch."""
+        override: FM_SYMM=ipc|torch.
+
+        `shared_inter`: reserve the staging of a shared expert of intermediate size up to this (a multiple of 64;
+        fm_shared_reserve), so that the forward calls accept `shared_expert=`."""
         self._L = _lib.load()
         self._ctx = ctypes.c_void_p()
         if device is None:
@@ -108,6 +144,10 @@ class MoEContext:
         self.cfg = cfg if cfg is not None else _lib.compiled_config()
         if timeout_ms is not None:
             _lib.check(self._L.fm_set_timeout_ms(self._ctx, int(timeout_ms)))
+        self.shared_inter: Optional[int] = None
+        if shared_inter is not None:
+            _lib.check(self._L.fm_shared_reserve(self._ctx, int(shared_inter)))
+            self.shared_inter = int(shared_inter)
         # tokens of the last forward (valid rows of the routing tables `read` returns); None after a call with a
         # device-side count (launch_record() has it)
         self.last_tokens: Optional[int] = 0
@@ -236,7 +276,8 @@ class MoEContext:
 
     def forward_tokens(self, x: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor,
                        bias_up: Optional[torch.Tensor] = None, bias_down: Optional[torch.Tensor] = None,
-                       out: Optional[torch.Tensor] = None, n_tokens: Optional[torch.Tensor] = None) -> torch.Tensor:
+                       out: Optional[torch.Tensor] = None, n_tokens: Optional[torch.Tensor] = None,
+                       shared_expert: Optional[SharedExpert] = None) -> torch.Tensor:
         """Enqueue one fused forward over the n = x.numel() // H tokens of `x` (contiguous bf16 [..., H], 0 <= n <= S)
         on torch's current stream; returns `out` (default: a tensor like `x`), async.  The result is exactly what a
         context created for S = n computes: routing, capacity `cfg.EC_of(n)`, drops, outputs and, in training mode, the
@@ -248,12 +289,22 @@ class MoEContext:
         (fm_moe_forward_tokens_dev): no host synchronisation, and one captured CUDA graph serves every n.  `x` must then
         hold exactly S tokens; its rows n and above may hold anything and affect no result, and rows n and above of
         `out` are not written.  `last_tokens` is then None -- `launch_record()` returns the count the launch ran with.
-        A count outside [0, S] runs the launch on 0 tokens and makes the next `check` / `synchronize` raise."""
+        A count outside [0, S] runs the launch on 0 tokens and makes the next `check` / `synchronize` raise.
+
+        `shared_expert`: a `SharedExpert` whose output s[t] every token adds to its routed result r[t] (the row this call
+        writes without one): out[t] = rne_bf16(r[t] + s[t]); everything else is unchanged.  Needs a context created with
+        `shared_inter` >= its Ps; `read("shared_y")` returns the s rows.  The same keyword works on `forward_routed` and
+        `forward_gated`."""
         n = self._validate(x, gate_weights, expert_weights, exact_s=False)
         bu, bd = self._bias_ptrs(bias_up, bias_down)
         out = self._output(x, out)
         L, c, stream = self._L, self._ctx, torch.cuda.current_stream(self.device).cuda_stream
         gw, we = gate_weights.data_ptr(), expert_weights.data_ptr()
+        if shared_expert is not None:
+            se = self._shared(shared_expert)
+            self._launch(lambda nd, xp, op: L.fm_moe_forward_shared(c, xp, n, nd, gw, None, None, None, None, we, bu, bd,
+                                                                    se, op, stream), n, n_tokens, x, out)
+            return out
         # the two C calls differ in their third argument only: the count, or the pointer to it
         fn = L.fm_moe_forward_tokens if n_tokens is None else L.fm_moe_forward_tokens_dev
         self._launch(lambda nd, xp, op: fn(c, xp, n if nd is None else nd, gw, we, bu, bd, op, stream),
@@ -263,7 +314,8 @@ class MoEContext:
     def forward_routed(self, x: torch.Tensor, topk_idx: torch.Tensor, topk_weight: torch.Tensor,
                        expert_weights: torch.Tensor, bias_up: Optional[torch.Tensor] = None,
                        bias_down: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
-                       n_tokens: Optional[torch.Tensor] = None) -> torch.Tensor:
+                       n_tokens: Optional[torch.Tensor] = None,
+                       shared_expert: Optional[SharedExpert] = None) -> torch.Tensor:
         """`forward_tokens` on the caller's routing instead of the built-in router (fm_moe_forward_routed): `topk_idx`
         int32 [n, k] names each token's experts (global ids; -1 = no expert) and `topk_weight` float32 [n, k] their
         weights, both contiguous CUDA tensors on this context's device (no conversions are made here; see
@@ -282,6 +334,12 @@ class MoEContext:
         out = self._output(x, out)
         L, c, stream = self._L, self._ctx, torch.cuda.current_stream(self.device).cuda_stream
         we = expert_weights.data_ptr()
+        if shared_expert is not None:
+            se = self._shared(shared_expert)
+            self._launch(lambda nd, xp, op, ip, wp: L.fm_moe_forward_shared(c, xp, n, nd, None, None, None, ip, wp, we, bu,
+                                                                            bd, se, op, stream),
+                         n, n_tokens, x, out, topk_idx, topk_weight)
+            return out
         self._launch(lambda nd, xp, op, ip, wp: L.fm_moe_forward_routed(c, xp, n, nd, ip, wp, we, bu, bd, op, stream),
                      n, n_tokens, x, out, topk_idx, topk_weight)
         return out
@@ -289,7 +347,8 @@ class MoEContext:
     def forward_gated(self, x: torch.Tensor, gate_weights: torch.Tensor, expert_weights: torch.Tensor,
                       router: RouterSpec, score_bias: Optional[torch.Tensor] = None,
                       bias_up: Optional[torch.Tensor] = None, bias_down: Optional[torch.Tensor] = None,
-                      out: Optional[torch.Tensor] = None, n_tokens: Optional[torch.Tensor] = None) -> torch.Tensor:
+                      out: Optional[torch.Tensor] = None, n_tokens: Optional[torch.Tensor] = None,
+                      shared_expert: Optional[SharedExpert] = None) -> torch.Tensor:
         """`forward_tokens` with the routing rule `router` (a `RouterSpec`) applied in the kernel to the router's logits
         (fm_moe_forward_gated): softmax or sigmoid scores, an optional `score_bias` added for selection only, a group
         limit, top-k, renormalisation and a route scale.  From the routing on, the launch runs exactly as
@@ -309,9 +368,17 @@ class MoEContext:
         L, c, stream = self._L, self._ctx, torch.cuda.current_stream(self.device).cuda_stream
         gw, rt, we = gate_weights.data_ptr(), ctypes.byref(router.to_c()), expert_weights.data_ptr()
         sb = score_bias.data_ptr() if score_bias is not None else None
+        if shared_expert is not None:
+            se = self._shared(shared_expert)
+            self._launch(lambda nd, xp, op: L.fm_moe_forward_shared(c, xp, n, nd, gw, rt, sb, None, None, we, bu, bd, se,
+                                                                    op, stream), n, n_tokens, x, out)
+            return out
         self._launch(lambda nd, xp, op: L.fm_moe_forward_gated(c, xp, n, nd, gw, rt, sb, we, bu, bd, op, stream),
                      n, n_tokens, x, out)
         return out
+
+    def _shared(self, se: SharedExpert):
+        return ctypes.byref(shared_expert_struct(se, self.device, self.dims["H"], self.shared_inter))
 
     def _launch(self, call, n: int, n_tokens: Optional[torch.Tensor], *rows: torch.Tensor) -> None:
         """The token-count convention of the forward calls: run `call(n_tokens_dev, *row pointers)`, where `rows` are
@@ -434,7 +501,8 @@ class MoEContext:
         npk = d["world"] * d["num_local_experts"]
         shapes = {"topk_idx": (S, k), "topk_w": (S, k), "mcw": (S,), "slot": (S, k), "counts": (E,),
                   "recv_x": (npk, d["pEC"], H), "hidden": (npk, d["pEC"], P), "ret_y": (E, d["pEC"], H),
-                  "gate_out": (S, E), "recv_cnt": (npk,), "trace": (d["grid"], trace_slots.SLOTS), "aux_loss": (2 * E + 1,)}
+                  "gate_out": (S, E), "recv_cnt": (npk,), "trace": (d["grid"], trace_slots.SLOTS), "aux_loss": (2 * E + 1,),
+                  "shared_y": (S, H)}
         return arr.reshape(shapes[name])
 
     @property

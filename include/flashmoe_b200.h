@@ -195,9 +195,56 @@ FM_API int fm_moe_forward_gated(fm_ctx_t* ctx, const void* x, int n_tokens, cons
                                 const void* expert_w, const void* bias_up, const void* bias_down, void* out,
                                 void* stream);
 
+/* ---- shared expert (DeepSeek-V2/V3 and Kimi K2 n_shared_experts, Qwen-MoE shared_expert_intermediate_size, Llama 4,
+ * GLM-4.5, DeepSpeed Residual-MoE) ----
+ * A dense FFN every token passes through, its output added to the routed combine:
+ *   w          bf16 [2, Ps, H], contiguous: exactly one routed expert's slice of expert_w -- [0] is W_up [Ps, H], [1] is the
+ *              same Ps*H block flat-viewed as W_down [H, Ps]
+ *   bias_up    bf16 [Ps] or NULL (zero)     bias_down  bf16 [H] or NULL (zero)
+ *   inter      Ps, a positive multiple of 64, at most the context's reserved size (fm_shared_reserve)
+ * For every token t < n: s[t] = the bf16 output of that FFN on x[t], with a routed expert's arithmetic (GEMM0 + bias_up ->
+ * the context's hidden_act -> bf16 h -> GEMM1 + bias_down -> one bf16 RNE), and
+ *   out[t] = rne_bf16(fl32(r[t]) + fl32(s[t]))   (the sum in fp32, then one RNE)
+ * where r[t] is, bit for bit, the row the same call without a shared expert writes -- on every route (router, caller,
+ * gated), for every k, on both the fused and the gather combine, the router path's unscaled k = 1 copy included.  s is
+ * not added into the output row beside the routed terms (with k <= 2 the fused combine is order-independent only because
+ * it adds two bf16 terms onto +0; a third add would depend on arrival order): it is staged and added once, after the
+ * row's routed contributions are complete.  Everything else -- topk_idx, topk_w, mcw, slot, counts, recv_cnt, gate_out
+ * and, with is_training = 1, FM_BUF_AUX_LOSS -- is exactly the call without a shared expert.  The shared tiles run in the
+ * same persistent kernel as the routed ones: they need only x, so they fill the time the routed rows take to arrive. */
+typedef struct fm_shared_expert {
+    const void* w;          /* bf16 [2, Ps, H] */
+    const void* bias_up;    /* bf16 [Ps] or NULL */
+    const void* bias_down;  /* bf16 [H] or NULL */
+    int32_t inter;          /* Ps */
+} fm_shared_expert_t;
+
+/* Allocate the shared expert's staging (h_s [S, max_inter], y_s [S, H], row-block counters); once per context,
+ * before any forward that passes a shared expert (and before any capture).  FM_EINVAL for max_inter not a positive
+ * multiple of 64, or an E = 1 context; FM_ESTATE on a second call. */
+FM_API int fm_shared_reserve(fm_ctx_t* ctx, int32_t max_inter);
+
+/* One forward with a shared expert, on any of the three routes:
+ *   gate_w == NULL            caller routing: topk_idx / topk_w as fm_moe_forward_routed (router must be NULL)
+ *   gate_w, router == NULL    the built-in router, as fm_moe_forward_tokens (topk_idx, topk_w and score_bias NULL)
+ *   gate_w and router         the rule *router with score_bias, as fm_moe_forward_gated (topk_idx and topk_w NULL)
+ * The token count follows fm_moe_forward_routed: a host n_tokens, or n_tokens_dev with n_tokens = S (rows n and above of
+ * x may then hold anything, NaN included, and affect no result).  Every condition of the chosen route applies, and
+ * FM_EINVAL for shared == NULL, shared->w == NULL, inter not a positive multiple of 64 or above the reserved size, a
+ * misaligned (not 16-byte) w, bias_up or bias_down, an E = 1 context, gate_w with topk_idx / topk_w, router without
+ * gate_w, and score_bias without router; FM_ESTATE without fm_shared_reserve.  Training contexts are accepted on the
+ * router route.  May be captured in a CUDA graph like the other entry points (the shared expert's pointers and inter
+ * are fixed at capture, the weights' contents are read at every replay).  With world > 1 each rank passes its own
+ * shared expert, or calls an entry point without one: the kind of call may differ between ranks. */
+FM_API int fm_moe_forward_shared(fm_ctx_t* ctx, const void* x, int n_tokens, const int32_t* n_tokens_dev,
+                                 const void* gate_w, const fm_router_t* router, const float* score_bias,
+                                 const int32_t* topk_idx, const float* topk_w,
+                                 const void* expert_w, const void* bias_up, const void* bias_down,
+                                 const fm_shared_expert_t* shared, void* out, void* stream);
+
 /* ---- CUDA graphs ----
  * Every forward entry point on device buffers (fm_moe_forward, fm_moe_forward_tokens, fm_moe_forward_tokens_dev,
- * fm_moe_forward_routed, fm_moe_forward_gated) may
+ * fm_moe_forward_routed, fm_moe_forward_gated, fm_moe_forward_shared) may
  * be captured into a CUDA graph and the graph replayed any number of times, interleaved with eager calls on the same
  * context.  A launch keeps no per-launch state in its parameters: the kernel takes its epoch, grid-barrier target and
  * token-dependent sizes from the context's device-side launch counter (and the device-side count) when it starts.
@@ -259,8 +306,10 @@ enum fm_buffer {
                             written by a routed launch; gated: rne_bf16(s), the full unbiased score row */
     FM_BUF_RECV_CNT = 9, /* int32 [W, nLx] rows received per (source rank, local expert) in the last forward */
     FM_BUF_TRACE = 10,   /* u64   [grid, 128] %globaltimer stamps of the last forward (fm_set_trace) */
-    FM_BUF_AUX_LOSS = 11 /* f32   [2E+1] is_training = 1 only: gML[E] (mean gate probability per expert), gMeC[E] (mean
+    FM_BUF_AUX_LOSS = 11, /* f32  [2E+1] is_training = 1 only: gML[E] (mean gate probability per expert), gMeC[E] (mean
                             routed fraction per expert), loss = sum_e gML*gMeC / E  (moe/gate.cuh:608-635,698-706,763-773) */
+    FM_BUF_SHARED_Y = 12 /* bf16  [S,H]   the shared expert's s rows of the last launch that had one (rows < n valid);
+                            after fm_shared_reserve only */
 };
 FM_API int fm_buffer_bytes(const fm_ctx_t* ctx, int which, size_t* bytes);
 FM_API int fm_read_buffer(fm_ctx_t* ctx, int which, void* host_dst, size_t bytes);
