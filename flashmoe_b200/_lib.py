@@ -18,6 +18,7 @@ FM_HOST_SLOTS = 3
 # enum fm_buffer
 BUF_TOPK_IDX, BUF_TOPK_W, BUF_MCW, BUF_SLOT, BUF_COUNTS, BUF_RECV_X, BUF_HIDDEN, BUF_RET_Y, BUF_GATE_OUT, BUF_RECV_CNT, BUF_TRACE, BUF_AUX_LOSS = range(12)
 BUF_SHARED_Y = 12
+BUF_SHARED_HIDDEN = 13
 
 # every symbol include/flashmoe_b200.h declares (tests check the library exports all of them)
 EXPORTED_SYMBOLS = (

@@ -166,6 +166,7 @@ struct fm_ctx {
     TmapCache tm_a0, tm_b0, tm_a1, tm_b1, tm_gx, tm_gw;   // FmParams::tm_* (fm_symm_use_external moves recv_x's base)
     // shared expert (fm_shared_reserve): staging h_s [S, shared_max] and y_s [S, H], row-block counters [S / 128]
     int shared_max = 0;
+    int shared_ps = 0;   // Ps of the last launch enqueued (or captured) with a shared expert: h_s's row stride
     __nv_bfloat16* h_s = nullptr;
     __nv_bfloat16* y_s = nullptr;
     unsigned int* s0_done = nullptr;
@@ -500,6 +501,7 @@ int launch(fm_ctx* c, const ForwardCall& f) {
     lc.numAttrs = 1;
     FM_CUDA(cudaLaunchKernelEx(&lc, fm::fm_moe_forward_kernel, p));
     c->launches += 1;
+    if (sh != nullptr) c->shared_ps = (int)Ps;
     return FM_OK;
 }
 
@@ -1065,6 +1067,9 @@ static int buffer_desc(const fm_ctx_t* c, int which, const void** ptr, size_t* b
         case FM_BUF_SHARED_Y:
             if (c->y_s == nullptr) return fail(FM_EINVAL, "the shared expert's outputs exist only after fm_shared_reserve");
             *ptr = c->y_s; *bytes = (size_t)d.S * d.H * 2; break;
+        case FM_BUF_SHARED_HIDDEN:   // [S, Ps] at the stride of the last shared launch's tensor map (tm_hs)
+            if (c->shared_ps == 0) return fail(FM_EINVAL, "the shared expert's h_s exists only after a launch with one");
+            *ptr = c->h_s; *bytes = (size_t)d.S * c->shared_ps * 2; break;
         default: return fail(FM_EINVAL, "unknown buffer id %d", which);
     }
     return FM_OK;

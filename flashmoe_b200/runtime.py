@@ -32,6 +32,7 @@ _BUFFER_SPECS = {
     "trace": (_lib.BUF_TRACE, np.uint64),
     "aux_loss": (_lib.BUF_AUX_LOSS, np.float32),
     "shared_y": (_lib.BUF_SHARED_Y, np.uint16),
+    "shared_hidden": (_lib.BUF_SHARED_HIDDEN, np.uint16),
 }
 
 
@@ -293,8 +294,8 @@ class MoEContext:
 
         `shared_expert`: a `SharedExpert` whose output s[t] every token adds to its routed result r[t] (the row this call
         writes without one): out[t] = rne_bf16(r[t] + s[t]); everything else is unchanged.  Needs a context created with
-        `shared_inter` >= its Ps; `read("shared_y")` returns the s rows.  The same keyword works on `forward_routed` and
-        `forward_gated`."""
+        `shared_inter` >= its Ps; `read("shared_y")` returns the s rows and `read("shared_hidden")` their h_s [S, Ps].
+        The same keyword works on `forward_routed` and `forward_gated`."""
         n = self._validate(x, gate_weights, expert_weights, exact_s=False)
         bu, bd = self._bias_ptrs(bias_up, bias_down)
         out = self._output(x, out)
@@ -502,7 +503,7 @@ class MoEContext:
         shapes = {"topk_idx": (S, k), "topk_w": (S, k), "mcw": (S,), "slot": (S, k), "counts": (E,),
                   "recv_x": (npk, d["pEC"], H), "hidden": (npk, d["pEC"], P), "ret_y": (E, d["pEC"], H),
                   "gate_out": (S, E), "recv_cnt": (npk,), "trace": (d["grid"], trace_slots.SLOTS), "aux_loss": (2 * E + 1,),
-                  "shared_y": (S, H)}
+                  "shared_y": (S, H), "shared_hidden": (S, arr.size // S)}   # (Ps of the last shared launch)
         return arr.reshape(shapes[name])
 
     @property

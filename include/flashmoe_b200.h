@@ -308,8 +308,10 @@ enum fm_buffer {
     FM_BUF_TRACE = 10,   /* u64   [grid, 128] %globaltimer stamps of the last forward (fm_set_trace) */
     FM_BUF_AUX_LOSS = 11, /* f32  [2E+1] is_training = 1 only: gML[E] (mean gate probability per expert), gMeC[E] (mean
                             routed fraction per expert), loss = sum_e gML*gMeC / E  (moe/gate.cuh:608-635,698-706,763-773) */
-    FM_BUF_SHARED_Y = 12 /* bf16  [S,H]   the shared expert's s rows of the last launch that had one (rows < n valid);
+    FM_BUF_SHARED_Y = 12, /* bf16 [S,H]   the shared expert's s rows of the last launch that had one (rows < n valid);
                             after fm_shared_reserve only */
+    FM_BUF_SHARED_HIDDEN = 13 /* bf16 [S,Ps] the shared expert's h_s rows of the last launch that had one (rows < n
+                            valid), Ps that launch's (a captured launch's, recorded at capture); FM_EINVAL before any */
 };
 FM_API int fm_buffer_bytes(const fm_ctx_t* ctx, int which, size_t* bytes);
 FM_API int fm_read_buffer(fm_ctx_t* ctx, int which, void* host_dst, size_t bytes);

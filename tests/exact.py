@@ -399,6 +399,16 @@ def combine_tokens(y_of: np.ndarray, kept: np.ndarray, pw_bits: np.ndarray, mcw:
     return Rounded(f64_to_bf16(acc_lo), f64_to_bf16(acc_hi), real)
 
 
+def add_shared(r: Rounded, s_bits: np.ndarray) -> Rounded:
+    """out = rne_bf16(fl32(r) + fl32(s)): a shared expert's s rows (bf16 bits [n, H]) added to the routed result r after
+    r is rounded.  The sum of two bf16 numbers is exact in float64 and rounds once to fp32, then to bf16; the map is
+    monotone in r, so the ends of r's interval map to the ends of out's.  `exact` is the sum before those roundings (at
+    r's lower end), so rounded_count counts the elements that round in this step."""
+    s = bits_to_f64(s_bits)
+    lo = bits_to_f64(r.lo) + s
+    return Rounded(f64_to_bf16(lo), f64_to_bf16(bits_to_f64(r.hi) + s), lo)
+
+
 # ----------------------------------------------------------------------------- statistics
 class Stats:
     """Per stage: elements checked, elements whose exact value needed rounding, intervals of nonzero width."""
@@ -487,9 +497,12 @@ class Device:
     ret_y: Optional[np.ndarray]    # [E, pEC, H] (gather path) or None
 
 
-def check_forward(inp: ExactInputs, dev: Device, EC: int, n: Optional[int] = None, stats: Optional[Stats] = None):
+def check_forward(inp: ExactInputs, dev: Device, EC: int, n: Optional[int] = None, stats: Optional[Stats] = None,
+                  shared_s: Optional[np.ndarray] = None):
     """Every stage of one launch over the first n tokens of `inp` (default all), in pipeline order; GEMM1 and the
-    combine are referenced from the device's own hidden, topk_w and mcw, so a failure names the stage that broke."""
+    combine are referenced from the device's own hidden, topk_w and mcw, so a failure names the stage that broke.
+    `shared_s`: a shared expert's s rows (bf16 bits [n, H]); out is then rne(r + s) of the routed result r (add_shared),
+    rows whose picks were all dropped rne(+0 + s)."""
     cfg = inp.cfg
     E, k, H = cfg.E, cfg.k, cfg.H
     st = stats if stats is not None else Stats()
@@ -547,12 +560,17 @@ def check_forward(inp: ExactInputs, dev: Device, EC: int, n: Optional[int] = Non
 
     y_of = y_dev_ref[dev.topk_idx, np.where(kept, slot, 0)]          # [n, k, H]
     out_ref = combine_tokens(y_of, kept, dev.topk_w, dev.mcw)
-    w = _interval_check(dev.out, out_ref, "out", ("token", "column"), max_width=None)
-    st.add("out", dev.out.size, rounded_count(out_ref) if k > 1 else 0, w)
     dropped = ~kept.any(axis=1)
+    empty, what = np.zeros((int(dropped.sum()), H), np.uint16), "out"
+    if shared_s is not None:
+        st.add("out (routed)", 0, rounded_count(out_ref) if k > 1 else 0)
+        out_ref, what = add_shared(out_ref, shared_s), "out = rne(r + s)"
+        empty = add_shared(Rounded(empty, empty, 0), shared_s[dropped]).lo
+    w = _interval_check(dev.out, out_ref, what, ("token", "column"), max_width=None)
+    st.add(what, dev.out.size, rounded_count(out_ref) if k > 1 or shared_s is not None else 0, w)
     if dropped.any():
-        check_equal(dev.out[dropped], np.zeros((int(dropped.sum()), H), np.uint16),
-                    "out rows of tokens whose picks were all dropped (+0)", ("row", "column"))
+        check_equal(dev.out[dropped], empty, f"{what} rows of tokens whose picks were all dropped (r = +0)",
+                    ("row", "column"), signed_zero=shared_s is None)
         st.add("all-dropped rows", int(dropped.sum()) * H)
     return st
 

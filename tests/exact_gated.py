@@ -320,14 +320,15 @@ def weights_f32(w_bits: np.ndarray) -> np.ndarray:
 
 
 def check_gated_forward(inp: ex.ExactInputs, dev: ex.Device, router, bias, EC: int,
-                        stats: Optional[ex.Stats] = None) -> int:
+                        stats: Optional[ex.Stats] = None, shared_s: Optional[np.ndarray] = None) -> int:
     """A gated launch over the first n = len(dev.topk_idx) tokens: check_gated_routing, then every later stage as a
-    routed launch on the device's own routing.  Returns the number of ambiguous tokens."""
+    routed launch on the device's own routing (with a shared expert's s rows `shared_s`, out = rne(r + s)).  Returns
+    the number of ambiguous tokens."""
     n = dev.topk_idx.shape[0]
     x = inp.x64[:n]
     amb = check_gated_routing(x @ inp.wg_eff64.T, bias, router, inp.cfg.k, dev.topk_idx, dev.gate_out, dev.topk_w,
                               (x, inp.wg_eff64))
-    er.check_routed_forward(inp, dev, dev.topk_idx, weights_f32(dev.topk_w), EC, stats)
+    er.check_routed_forward(inp, dev, dev.topk_idx, weights_f32(dev.topk_w), EC, stats, shared_s)
     return amb
 
 

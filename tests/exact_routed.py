@@ -72,11 +72,12 @@ def sanitize(topk: np.ndarray, E: int) -> np.ndarray:
 
 
 def check_routed_forward(inp: ex.ExactInputs, dev: ex.Device, topk: np.ndarray, w: np.ndarray, EC: int,
-                         stats: Optional[ex.Stats] = None) -> ex.Stats:
+                         stats: Optional[ex.Stats] = None, shared_s: Optional[np.ndarray] = None) -> ex.Stats:
     """Every stage of one routed launch over the first n = len(topk) tokens of `inp`: the routing tables, slots,
     counts, recv_cnt, the dispatched rows, h, y (ret_y on the gather path) and out, bit for bit (GELU's h within its
     interval); rows whose picks were all skipped or dropped must be +0.  GEMM1 and the combine are referenced from
-    the device's own hidden, so a failure names the stage that broke."""
+    the device's own hidden, so a failure names the stage that broke.  `shared_s`: a shared expert's s rows (bf16 bits
+    [n, H]); out is then rne(r + s) (exact.add_shared), and the rows without a kept pick rne(+0 + s)."""
     cfg = inp.cfg
     E, H = cfg.E, cfg.H
     st = stats if stats is not None else ex.Stats()
@@ -119,12 +120,17 @@ def check_routed_forward(inp: ex.ExactInputs, dev: ex.Device, topk: np.ndarray, 
             st.add("ret_y", c * H)
     y_of = y_ref[np.where(kept, run, 0), np.where(kept, slot, 0)]
     out = combine_routed(y_of, kept, w_bits)
-    ex.check_equal(dev.out, out, "out", ("token", "column"), signed_zero=False)
-    st.add("out", dev.out.size)
     none = ~kept.any(axis=1)
+    empty, what, rounded = np.zeros((int(none.sum()), H), np.uint16), "out", 0
+    if shared_s is not None:
+        r = ex.add_shared(ex.Rounded(out, out, 0), shared_s)
+        out, what, rounded = r.lo, "out = rne(r + s)", ex.rounded_count(r)
+        empty = ex.add_shared(ex.Rounded(empty, empty, 0), shared_s[none]).lo
+    ex.check_equal(dev.out, out, what, ("token", "column"), signed_zero=False)
+    st.add(what, dev.out.size, rounded)
     if none.any():
-        ex.check_equal(dev.out[none], np.zeros((int(none.sum()), H), np.uint16),
-                       "out rows of tokens whose picks were all skipped or dropped (+0)", ("row", "column"))
+        ex.check_equal(dev.out[none], empty, f"{what} rows of tokens whose picks were all skipped or dropped (r = +0)",
+                       ("row", "column"), signed_zero=shared_s is None)
         st.add("rows without a kept pick", int(none.sum()) * H)
     return st
 

@@ -30,6 +30,7 @@ def test_header_declares_and_binding_exports():
         assert re.search(rf"FM_API\s+int\s+{name}\s*\(", HEADER), name
         assert name in _lib.EXPORTED_SYMBOLS
     assert re.search(r"FM_BUF_SHARED_Y\s*=\s*12\b", HEADER) and _lib.BUF_SHARED_Y == 12
+    assert re.search(r"FM_BUF_SHARED_HIDDEN\s*=\s*13\b", HEADER) and _lib.BUF_SHARED_HIDDEN == 13
 
 
 def test_struct_matches_header():
