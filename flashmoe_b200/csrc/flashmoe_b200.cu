@@ -114,9 +114,7 @@ struct fm_ctx {
     int device = 0;
     int grid = 0;
     int tpc = 0;
-    int TN0 = 0, TN1 = 0, num_pkts = 0, num_blocks = 0;
-    int g0_blocks = 0, g1_blocks = 0;   // GEMM0 / GEMM1 blocks of the work list (items = their tiles x row blocks per packet)
-    int split_blk = 0;                  // leading local GEMM0 blocks of the work list (the shared expert's GEMM1 follows them)
+    int TN1 = 0, num_pkts = 0, num_blocks = 0;
     int dbg_flags = 0;
     // in-kernel waits give up after this long (fm_set_timeout_ms): generous by default so that ordinary rank skew (a peer
     // still loading data, compiling, paused in a debugger) is not turned into a trap -- see fm_ptx.cuh SpinGuard
@@ -163,7 +161,7 @@ struct fm_ctx {
     fm::DebugRecord* dbg_dev = nullptr;
     unsigned long long* trace = nullptr;
     bool trace_on = false;
-    TmapCache tm_a0, tm_b0, tm_a1, tm_b1, tm_gx, tm_gw;   // FmParams::tm_* (fm_symm_use_external moves recv_x's base)
+    TmapCache tm[fm::NUM_TMAPS];   // FmParams::tm (fm_symm_use_external moves recv_x's base)
     // shared expert (fm_shared_reserve): staging h_s [S, shared_max] and y_s [S, H], row-block counters [S / 128]
     int shared_max = 0;
     int shared_ps = 0;   // Ps of the last launch enqueued (or captured) with a shared expert: h_s's row stride
@@ -171,7 +169,6 @@ struct fm_ctx {
     __nv_bfloat16* y_s = nullptr;
     unsigned int* s0_done = nullptr;
     unsigned int* s1_done = nullptr;
-    TmapCache tm_xs, tm_ws0, tm_ws1, tm_hs;
 };
 
 namespace {
@@ -399,51 +396,71 @@ int launch(fm_ctx* c, const ForwardCall& f) {
     const uint64_t n = (uint64_t)f.n_tok, pkt_rows = (uint64_t)c->num_pkts * d.pEC;
     const void* a0 = c->dense ? f.x : static_cast<const char*>(c->symm) + c->off_recv_x;
     const uint64_t a0_rows = c->dense ? n : pkt_rows;
-    if (a0_rows > 0 && (rc = cached_tmap(&c->tm_a0, a0, a0_rows, d.H, fm::BLOCK_M))) return rc;
-    if ((rc = cached_tmap(&c->tm_a1, c->hidden, pkt_rows, d.P, fm::BLOCK_M))) return rc;
-    // expert_weights [nLx, 2, P, H]: [i,0] is W_up [P,H]; [i,1] is the same P*H block viewed as W_down [H,P]
-    // (python_bindings.cu:104-119).  One tensor map per GEMM over the whole tensor with a per-expert row stride
-    // of 2*P (resp. 2*H) rows is not expressible in 2-D, so rows are addressed as [nLx*2*P, H] / [nLx*2*H, P]:
-    // expert i's W_up starts at row i*2*P, its W_down at row (i*2+1)*H of the [.,P] view.
-    if ((rc = cached_tmap(&c->tm_b0, f.expert_w, (uint64_t)nLx * 2 * d.P, d.H, fm::BLOCK_N))) return rc;
-    if ((rc = cached_tmap(&c->tm_b1, f.expert_w, (uint64_t)nLx * 2 * d.H, d.P, fm::BLOCK_N))) return rc;
     // router on tensor cores: x as [n_tok, H] in 32-row boxes, Wg_eff = the [H, E] tensor read flat as [E, H]
     // (python_bindings.cu:93-99, moe.cuh:107-109) in boxes of min(128, E rounded up to 64) rows; rows past E read as
     // zero.  A routed launch has no router maps.
     const bool gate_maps = c->tc_gate && f.route != fm::ROUTE_CALLER;
     const uint32_t e64 = (uint32_t)((d.E + 63) / 64 * 64);
-    if (gate_maps && n > 0 && (rc = cached_tmap(&c->tm_gx, f.x, n, d.H, 32))) return rc;
-    if (gate_maps && (rc = cached_tmap(&c->tm_gw, f.gate_w, (uint64_t)d.E, d.H, std::min(128u, e64)))) return rc;
-    // shared expert: x in 128-row boxes (its GEMM0's A), w [2, Ps, H] as W_up [Ps, H] and W_down [H, Ps], h_s as [S, Ps]
     const fm_shared_expert_t* sh = f.shared;
     const uint64_t Ps = sh != nullptr ? (uint64_t)sh->inter : 0;
-    if (sh != nullptr) {
-        const void* w_down = static_cast<const char*>(sh->w) + Ps * d.H * 2;
-        if (n > 0 && (rc = cached_tmap(&c->tm_xs, f.x, n, d.H, fm::BLOCK_M))) return rc;
-        if ((rc = cached_tmap(&c->tm_ws0, sh->w, Ps, d.H, fm::BLOCK_N))) return rc;
-        if ((rc = cached_tmap(&c->tm_ws1, w_down, d.H, Ps, fm::BLOCK_N))) return rc;
-        if ((rc = cached_tmap(&c->tm_hs, c->h_s, d.S, Ps, fm::BLOCK_M))) return rc;
-    }
+    const char* ws = sh != nullptr ? static_cast<const char*>(sh->w) : nullptr;
+    // expert_weights [nLx, 2, P, H]: [i,0] is W_up [P,H]; [i,1] is the same P*H block viewed as W_down [H,P]
+    // (python_bindings.cu:104-119).  One tensor map per GEMM over the whole tensor with a per-expert row stride
+    // of 2*P (resp. 2*H) rows is not expressible in 2-D, so rows are addressed as [nLx*2*P, H] / [nLx*2*H, P]:
+    // expert i's W_up starts at row i*2*P, its W_down at row (i*2+1)*H of the [.,P] view.  The shared expert's
+    // w [2, Ps, H] is one such expert: W_up_s [Ps, H] and W_down_s [H, Ps].
+    struct MapSpec { const void* base; uint64_t rows, cols; uint32_t box_rows; bool needed; };
+    const MapSpec maps[fm::NUM_TMAPS] = {
+        {a0, a0_rows, (uint64_t)d.H, fm::BLOCK_M, a0_rows > 0},                            // TM_A0
+        {f.expert_w, (uint64_t)nLx * 2 * d.P, (uint64_t)d.H, fm::BLOCK_N, true},           // TM_B0
+        {c->hidden, pkt_rows, (uint64_t)d.P, fm::BLOCK_M, true},                           // TM_A1
+        {f.expert_w, (uint64_t)nLx * 2 * d.H, (uint64_t)d.P, fm::BLOCK_N, true},           // TM_B1
+        {f.x, n, (uint64_t)d.H, 32, gate_maps && n > 0},                                   // TM_GX
+        {f.gate_w, (uint64_t)d.E, (uint64_t)d.H, std::min(128u, e64), gate_maps},          // TM_GW
+        {f.x, n, (uint64_t)d.H, fm::BLOCK_M, sh != nullptr && n > 0},                      // TM_XS
+        {ws, Ps, (uint64_t)d.H, fm::BLOCK_N, sh != nullptr},                               // TM_WS0
+        {ws + Ps * d.H * 2, (uint64_t)d.H, Ps, fm::BLOCK_N, sh != nullptr},                // TM_WS1
+        {c->h_s, (uint64_t)d.S, Ps, fm::BLOCK_M, sh != nullptr},                           // TM_HS
+    };
 
     fm::FmParams p;
     memset(&p, 0, sizeof(p));
-    p.tm_a0 = c->tm_a0.map; p.tm_b0 = c->tm_b0.map; p.tm_a1 = c->tm_a1.map; p.tm_b1 = c->tm_b1.map;
-    if (gate_maps) { p.tm_gx = c->tm_gx.map; p.tm_gw = c->tm_gw.map; }
+    for (int i = 0; i < fm::NUM_TMAPS; ++i) {
+        const MapSpec& m = maps[i];
+        if (!m.needed) continue;
+        if ((rc = cached_tmap(&c->tm[i], m.base, m.rows, m.cols, m.box_rows))) return rc;
+        p.tm[i] = c->tm[i].map;
+    }
+    // the GEMMs' operands, fields in fm::GemmOp's order: {A map, B map, A rows per packet, B row of expert 0,
+    // B rows per expert, k-blocks, output columns, column tiles, rows from a packet, bias per expert, done counters per
+    // packet, destination, bias, done counters}
+    const int from_packet = c->dense ? 0 : 1;
+    using bf16p = const __nv_bfloat16*;
+    p.gemm[fm::GEMM_UP] = {fm::TM_A0, fm::TM_B0, d.pEC, 0, 2 * d.P, d.H / fm::BLOCK_K, d.P, ceil_div(d.P, fm::BLOCK_N),
+                           from_packet, d.P, d.TCM, 0, static_cast<bf16p>(f.bias_up), c->g0_done};
+    p.gemm[fm::GEMM_DOWN] = {fm::TM_A1, fm::TM_B1, d.pEC, d.H, 2 * d.H, d.P / fm::BLOCK_K, d.H, c->TN1, from_packet, d.H,
+                             0, c->fused ? fm::DEST_FUSED : fm::DEST_RETURN, static_cast<bf16p>(f.bias_down), nullptr};
+    if (sh != nullptr) {   // rows are the call's tokens
+        p.shared = 1;
+        p.y_s = c->y_s; p.s0_done = c->s0_done; p.s1_done = c->s1_done;
+        const int ps = (int)Ps;
+        p.gemm[fm::GEMM_S_UP] = {fm::TM_XS, fm::TM_WS0, 0, 0, 0, d.H / fm::BLOCK_K, ps, ceil_div(ps, fm::BLOCK_N), 0, 0,
+                                 0, 0, static_cast<bf16p>(sh->bias_up), c->s0_done};
+        p.gemm[fm::GEMM_S_DOWN] = {fm::TM_HS, fm::TM_WS1, 0, 0, 0, ps / fm::BLOCK_K, d.H, c->TN1, 0, 0, 0, fm::DEST_Y_S,
+                                   static_cast<bf16p>(sh->bias_down), nullptr};
+    }
     p.tc_gate = c->tc_gate ? 1 : 0;
     p.n_tokens = f.n_tok; p.n_tokens_dev = f.n_dev;
     p.H = d.H; p.P = d.P; p.E = d.E; p.k = d.k; p.W = d.world; p.rank = d.rank; p.nLx = nLx;
     p.pEC = d.pEC; p.TCM = d.TCM; p.act = c->cfg.hidden_act;
-    p.TN0 = c->TN0; p.TN1 = c->TN1; p.num_pkts = c->num_pkts; p.num_blocks = c->num_blocks;
+    p.TN1 = c->TN1; p.num_pkts = c->num_pkts; p.num_blocks = c->num_blocks;
     p.drop_tokens = c->cfg.drop_tokens; p.ec_mult = c->cfg.capacity_factor * d.k;   // EC(n), as expert_capacity
-    p.items_per_rb = c->g0_blocks * c->TN0 + c->g1_blocks * c->TN1;
     p.dbg_flags = c->dbg_flags;
     p.timeout_ns = c->timeout_ns;
     p.launch_ctr = reinterpret_cast<unsigned long long*>(c->ctrl + 4);
     p.launch_tokens = reinterpret_cast<int*>(c->ctrl + 6);
     p.x = static_cast<const __nv_bfloat16*>(f.x);
     p.wg = static_cast<const __nv_bfloat16*>(f.gate_w);
-    p.b_up = static_cast<const __nv_bfloat16*>(f.bias_up);
-    p.b_down = static_cast<const __nv_bfloat16*>(f.bias_down);
     p.out = static_cast<__nv_bfloat16*>(f.out);
     p.topk_idx = c->topk_idx; p.topk_w = c->topk_w; p.mcw = c->mcw; p.slot = c->slot; p.counts = c->counts;
     p.gate_out = c->gate_out; p.chunk_counts = c->chunk_counts;
@@ -475,14 +492,6 @@ int launch(fm_ctx* c, const ForwardCall& f) {
         p.scoring = f.router->scoring; p.n_group = f.router->n_group; p.topk_group = f.router->topk_group;
         p.group_top = f.router->group_top; p.renormalize = f.router->renormalize; p.route_scale = f.router->scale;
         p.score_bias = f.score_bias;
-    }
-    if (sh != nullptr) {
-        if (n > 0) p.tm_xs = c->tm_xs.map;
-        p.tm_ws0 = c->tm_ws0.map; p.tm_ws1 = c->tm_ws1.map; p.tm_hs = c->tm_hs.map;
-        p.shared = 1; p.Ps = (int)Ps; p.TN0s = ceil_div((int)Ps, fm::BLOCK_N); p.split_blk = c->split_blk;
-        p.s_b_up = static_cast<const __nv_bfloat16*>(sh->bias_up);
-        p.s_b_down = static_cast<const __nv_bfloat16*>(sh->bias_down);
-        p.h_s = c->h_s; p.y_s = c->y_s; p.s0_done = c->s0_done; p.s1_done = c->s1_done;
     }
     p.dbg = c->dbg_dev;
     p.trace = c->trace_on ? c->trace : nullptr;
@@ -610,25 +619,18 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
     }
     const int nLx = d.num_local_experts;
     ctx->dbg_flags = env_int("FM_DBG_FLAGS", 0);
-    ctx->TN0 = ceil_div(d.P, fm::BLOCK_N);
     ctx->TN1 = ceil_div(d.H, fm::BLOCK_N);
     ctx->num_pkts = world * nLx;
 
     // Work list.  Sources in the order own rank, rank+1, ... (local rows need no NVLink hop, so they are ready first).
-    // A work item is one 128 x 256 output tile of one packet.  The table stores, per block, how many GEMM0 and GEMM1 blocks
+    // A work item is one 128 x 256 output tile of one packet.  The table stores, per block, how many blocks of each GEMM
     // precede it; the kernel derives the block's first item from the call's row blocks per packet (fm::block_start).
     struct Unit { int pkt; bool local; };
     std::vector<Unit> units;
     for (int j = 0; j < world; ++j)
         for (int le = 0; le < nLx; ++le) units.push_back({((rank + j) % world) * nLx + le, j == 0});
     std::vector<fm::TileBlock> blocks;
-    int n_g[2] = {0, 0};
-    auto push = [&](int kind, const Unit& u) {
-        fm::TileBlock b;
-        b.kind = kind; b.pkt = u.pkt; b.g0 = n_g[0]; b.g1 = n_g[1];
-        blocks.push_back(b);
-        ++n_g[kind];
-    };
+    auto push = [&](int gemm, const Unit& u) { blocks.push_back({{}, gemm, u.pkt}); };
     // GEMM0: local sources first (their rows are acknowledged first), then rank+1, rank+2, ...  GEMM1: REMOTE sources
     // first, local last -- the outputs of remote packets cross NVLink as reductions and their done flags have a link round
     // trip ahead of them, so they should not be what every rank finishes with; the local packets' adds are cheap and
@@ -668,15 +670,21 @@ FM_API int fm_create(const fm_config_t* cfg, int rank, int world, int device, fm
         for (const Unit& u : units) push(0, u);
         for (const Unit& u : g1_units) push(1, u);
     }
+    // The shared expert's blocks, empty in a launch without one.  Its GEMM0 comes first: it needs nothing but x, which is
+    // in memory when the kernel starts, so it fills the time the routed packets' rows take to land.  Its GEMM1 follows
+    // the leading local routed GEMM0 blocks: by then its h rows are complete, and it fills the time until the routed
+    // GEMM1 dependencies resolve.
+    size_t split = 0;
+    while (split < blocks.size() && blocks[split].gemm == fm::GEMM_UP && blocks[split].pkt / nLx == rank) ++split;
+    blocks.insert(blocks.begin() + split, {{}, fm::GEMM_S_DOWN, rank * nLx});
+    blocks.insert(blocks.begin(), {{}, fm::GEMM_S_UP, rank * nLx});
     ctx->num_blocks = (int)blocks.size();
-    while (ctx->split_blk < ctx->num_blocks && blocks[ctx->split_blk].kind == 0 &&
-           blocks[ctx->split_blk].pkt / nLx == rank)
-        ++ctx->split_blk;
-    ctx->g0_blocks = n_g[0];
-    ctx->g1_blocks = n_g[1];
-    fm::TileBlock sentinel;
-    sentinel.kind = -1; sentinel.pkt = 0; sentinel.g0 = n_g[0]; sentinel.g1 = n_g[1];
-    blocks.push_back(sentinel);
+    blocks.push_back({{}, -1, 0});   // the sentinel: its block_start is the launch's item count
+    int n_g[fm::NUM_GEMMS] = {};
+    for (fm::TileBlock& b : blocks) {
+        std::copy(n_g, n_g + fm::NUM_GEMMS, b.g);
+        if (b.gemm >= 0) ++n_g[b.gemm];
+    }
 
 #define FM_TRY(expr)          \
     do {                      \
@@ -1067,7 +1075,7 @@ static int buffer_desc(const fm_ctx_t* c, int which, const void** ptr, size_t* b
         case FM_BUF_SHARED_Y:
             if (c->y_s == nullptr) return fail(FM_EINVAL, "the shared expert's outputs exist only after fm_shared_reserve");
             *ptr = c->y_s; *bytes = (size_t)d.S * d.H * 2; break;
-        case FM_BUF_SHARED_HIDDEN:   // [S, Ps] at the stride of the last shared launch's tensor map (tm_hs)
+        case FM_BUF_SHARED_HIDDEN:   // [S, Ps] at the stride of the last shared launch's tensor map (TM_HS)
             if (c->shared_ps == 0) return fail(FM_EINVAL, "the shared expert's h_s exists only after a launch with one");
             *ptr = c->h_s; *bytes = (size_t)d.S * c->shared_ps * 2; break;
         default: return fail(FM_EINVAL, "unknown buffer id %d", which);

@@ -279,10 +279,55 @@ constexpr int NAMED_BAR_LOCAL_DONE = 6;
 constexpr int NAMED_BAR_WINDOW = 7;
 constexpr int NAMED_BAR_GATE_MMA = 8;
 
-struct TileBlock {  // one contiguous run of work items: all tiles of one GEMM of one packet (or of a packet pair)
-    int kind;       // 0 = GEMM0 (x.W_up^T), 1 = GEMM1 (h.W_down^T)
-    int pkt;        // local packet index = src * nLx + le
-    int g0, g1;     // GEMM0 / GEMM1 blocks before this one in the work list (block_start)
+// The GEMMs of the expert FFN, FmParams::gemm[] ids.  GEMM0 (x.W_up^T) is even, its GEMM1 (h.W_down^T) the next id:
+// kind = id & 1.  The shared expert's GEMMs run on the call's tokens, in row blocks of Launch::s_rb.
+enum : int { GEMM_UP = 0, GEMM_DOWN = 1, GEMM_S_UP = 2, GEMM_S_DOWN = 3, NUM_GEMMS = 4 };
+
+// One contiguous run of work items: all tiles of one GEMM of one packet.  16 bytes: the scheduler reads two of them for
+// every item it claims, skipped items included, and a larger block measured slower on lists of many empty items.
+struct __align__(16) TileBlock {
+    unsigned short g[NUM_GEMMS];   // blocks of each GEMM before this one in the work list (block_start)
+    int gemm;                      // GEMM_* (the sentinel: -1)
+    int pkt;   // local packet index = src * nLx + le (the shared expert's: rank * nLx, its tokens are this rank's)
+};
+static_assert(sizeof(TileBlock) == 16 && 2 * MAX_EXPERTS + NUM_GEMMS <= 0xffff, "16-byte blocks, counts in 16 bits");
+
+// Tensor maps of a launch, FmParams::tm[] ids (encoded by the host from one table in launch()).
+enum : int {
+    TM_A0,    // GEMM_UP's A: recv_x as [W*nLx*pEC, H] (dense: x as [n_tokens, H]), box {64, 128}
+    TM_B0,    // expert_weights as [nLx*2*P, H], box {64, 256} (W_up rows)
+    TM_A1,    // hidden as [W*nLx*pEC, P], box {64, 128}: GEMM_DOWN's A loads and GEMM_UP's h stores
+    TM_B1,    // expert_weights as [nLx*2*H, P], box {64, 256} (W_down rows)
+    TM_GX,    // router on tensor cores: x as [n_tokens, H], box {64, 32}
+    TM_GW,    // router on tensor cores: Wg_eff [E, H], box {64, min(128, E rounded up to 64)}
+    TM_XS,    // shared expert: x as [n_tokens, H], box {64, 128}: GEMM_S_UP's A
+    TM_WS0,   // W_up_s as [Ps, H], box {64, 256}
+    TM_WS1,   // W_down_s (the same Ps*H block) as [H, Ps], box {64, 256}
+    TM_HS,    // h_s as [S, Ps], box {64, 128}: GEMM_S_DOWN's A loads and GEMM_S_UP's h stores
+    NUM_TMAPS
+};
+
+// Where a GEMM1 epilogue writes its rows, and how the publisher announces them (GemmOp::dest)
+enum : int {
+    DEST_RETURN = 0,   // the source rank's return buffer ret_y; g1_done, then the row block's return flag
+    DEST_FUSED = 1,    // scaled into the tokens' output rows on the source rank; pkt_done, then the done flag
+    DEST_Y_S = 2,      // y_s by token (the shared expert's s rows); s1_done
+};
+
+// Everything the FFN's warp roles need about one GEMM's operands, filled by the host per launch.  Tile (mblk, ntile) of
+// packet pkt = src * nLx + le reads A rows pkt * a_pkt_rows + 128 mblk and B rows b_row0 + le * b_le_rows + 256 ntile.
+struct GemmOp {
+    int a, b;               // FmParams::tm ids of the A and B operands (a GEMM0 stores h through its GEMM1's A map)
+    int a_pkt_rows;         // A rows per packet: pEC, or 0 where the rows are the call's tokens
+    int b_row0, b_le_rows;
+    int kblocks;            // K / BLOCK_K
+    int n, tn;              // output columns and column tiles, ceil(n / BLOCK_N)
+    int from_packet;        // 1: the rows are a dispatched packet's (packet flag and row acks); 0: the call's tokens
+    int bias_le;            // bias elements per local expert
+    int done_pkt;           // GEMM0: done counters per packet (its row block's counter: done[pkt * done_pkt + mblk])
+    int dest;               // GEMM1: DEST_*
+    const __nv_bfloat16* bias;   // [n] per local expert, or nullptr
+    unsigned int* done;     // GEMM0: its tiles finished per row block (g0_done, s0_done)
 };
 
 // Where phase G takes a launch's routing from.  A caller-routed and a gated launch both store mcw = 1 and take the
@@ -296,17 +341,8 @@ enum : int { SCORE_SOFTMAX = 0, SCORE_SIGMOID = 1 };   // FmParams::scoring (fm_
 constexpr int MAX_GROUPS = 32;                        // n_group bound: a token's kept groups are one 32-bit mask
 
 struct FmParams {
-    CUtensorMap tm_a0;  // recv_x  as [W*nLx*pEC, H]  box {64, 128}
-    CUtensorMap tm_b0;  // expert_weights as [nLx*2*P, H]  box {64, 128}  (W_up rows)
-    CUtensorMap tm_a1;  // hidden  as [W*nLx*pEC, P]  box {64, 128}: GEMM1's A loads and GEMM0's h stores
-    CUtensorMap tm_b1;  // expert_weights as [nLx*2*H, P]  box {64, 128}  (W_down rows)
-    CUtensorMap tm_gx;  // router on tensor cores: x as [n_tokens, H], box {64, 32}
-    CUtensorMap tm_gw;  // router on tensor cores: Wg_eff [E, H], box {64, min(128, E rounded up to 64)}
-    // shared expert (shared != 0, fm_moe_forward_shared): a dense FFN of intermediate size Ps on the call's own tokens
-    CUtensorMap tm_xs;   // x as [n_tokens, H], box {64, 128}: its GEMM0's A
-    CUtensorMap tm_ws0;  // W_up_s as [Ps, H], box {64, 256}
-    CUtensorMap tm_ws1;  // W_down_s (the same Ps*H block) as [H, Ps], box {64, 256}
-    CUtensorMap tm_hs;   // h_s as [S, Ps], box {64, 128}: its GEMM0's h stores and GEMM1's A
+    CUtensorMap tm[NUM_TMAPS];   // TM_*; a map the launch does not use is zero
+    GemmOp gemm[NUM_GEMMS];      // GEMM_*; the shared expert's are zero without one
     int tc_gate;        // 1 = logits by wgmma (E <= 256); 0 = register-blocked CUDA-core GEMV
     // The call's token count and everything derived from it are resolved on the device (resolve_launch, struct Launch).
     // n_tokens: the count itself, or with n_tokens_dev the context's S -- the rows of the maps over x and the bound of
@@ -315,15 +351,14 @@ struct FmParams {
     int n_tokens;
     const int* n_tokens_dev;
     int H, P, E, k, W, rank, nLx, pEC, TCM, act;
-    int TN0, TN1, num_pkts, num_blocks;
+    int TN1, num_pkts, num_blocks;
     int drop_tokens, ec_mult;   // capacity EC(n) = (drop_tokens ? ceil(n / E) : n) * ec_mult, ec_mult = capacity_factor * k
-    int items_per_rb;   // work items per row block of every packet: GEMM0 blocks * TN0 + GEMM1 blocks * TN1
     int dbg_flags;      // experiments only (results are garbage): bit0 = skip all TMA loads, bit1 = skip MMA issue,
                         // bit2 = skip the A loads, bit3 = skip the B loads
     unsigned long long timeout_ns;
     unsigned long long* launch_ctr;   // [1] launches this context has run (CTA 0 advances it after the grid barrier)
     int* launch_tokens;               // [1] the token count the last launch ran with
-    const __nv_bfloat16 *x, *wg, *b_up, *b_down;
+    const __nv_bfloat16 *x, *wg;
     __nv_bfloat16* out;
     int* topk_idx;             // [S,k]
     __nv_bfloat16* topk_w;     // [S,k]
@@ -376,12 +411,10 @@ struct FmParams {
     int scoring, n_group, topk_group, group_top, renormalize;
     float route_scale;
     const float* score_bias;
-    // shared expert: TN0s = ceil(Ps / 256) GEMM0 column tiles; its GEMM1 items follow the first split_blk blocks of the
-    // work list (the local routed GEMM0 blocks).  s_b_up [Ps] / s_b_down [H] or nullptr; h_s [S, Ps] and y_s [S, H]
-    // staging; s0_done / s1_done [S / 128]: its GEMM0 / GEMM1 tiles finished per row block of tokens
-    int shared, Ps, TN0s, split_blk;
-    const __nv_bfloat16 *s_b_up, *s_b_down;
-    __nv_bfloat16 *h_s, *y_s;
+    // shared expert (fm_moe_forward_shared; its GEMMs are gemm[GEMM_S_UP], gemm[GEMM_S_DOWN]): y_s [S, H] staging;
+    // s0_done / s1_done [S / 128]: its GEMM0 / GEMM1 tiles finished per row block of tokens
+    int shared;
+    __nv_bfloat16* y_s;
     unsigned int *s0_done, *s1_done;
     DebugRecord* dbg;
     unsigned long long* trace;  // optional [grid][TRACE_SLOTS] %globaltimer stamps (nullptr = off)
@@ -402,11 +435,24 @@ struct Launch {
     int tpc;                         // tokens per CTA, ceil(S / grid)
     int tcm_items;                   // row blocks per packet in the work list: TCM of EC at W == 1, the maximum TCM at W > 1
     int total_items;                 // work items of the launch
-    // the shared expert's items (all 0 without one): s_rb = ceil(S / 128) row blocks of tokens; its GEMM0 items are
-    // ids [0, s0_items), its GEMM1 items follow the first s_split routed items (see split_item)
-    int s_rb, s0_items, s_split, s1_items;
+    int s_rb;                        // the shared expert's row blocks of tokens, ceil(S / 128) (0 without one)
 };
 static_assert(sizeof(Launch) <= SMEM_USED - OFF_LAUNCH, "the Launch record's shared-memory slot");
+
+// row blocks of each block of GEMM g in this launch: a packet's tcm_items, or the shared expert's s_rb
+__device__ __forceinline__ int gemm_row_blocks(const Launch& L, int g) {
+    return g < GEMM_S_UP ? L.tcm_items : L.s_rb;
+}
+
+// first work item of block b: every earlier block of GEMM g holds its row blocks times its column tiles, so the item
+// space follows the call's row-block counts without rebuilding the table (the shared expert's blocks are empty without
+// one: s_rb = 0, and every item id is the routed list's)
+__device__ __forceinline__ int block_start(const FmParams& p, const Launch& L, const TileBlock& b) {
+    int start = 0;
+#pragma unroll
+    for (int g = 0; g < NUM_GEMMS; ++g) start += b.g[g] * p.gemm[g].tn * gemm_row_blocks(L, g);
+    return start;
+}
 
 // one thread per CTA, before the prologue's block sync
 __device__ __forceinline__ void resolve_launch(const FmParams& p, Launch* L) {
@@ -430,37 +476,8 @@ __device__ __forceinline__ void resolve_launch(const FmParams& p, Launch* L) {
     // one rank knows every packet's capacity, so the work list shrinks to this call's row blocks; a receiver with peers
     // does not know their token counts and keeps the maximum (the empty row blocks are skipped by the scheduler)
     L->tcm_items = p.W == 1 ? (ec + BLOCK_M - 1) / BLOCK_M : p.TCM;
-    L->total_items = p.items_per_rb * L->tcm_items;
-    L->s_rb = L->s0_items = L->s_split = L->s1_items = 0;
-    if (p.shared) {
-        const TileBlock& b = p.blocks[p.split_blk];
-        L->s_rb = (n + BLOCK_M - 1) / BLOCK_M;
-        L->s0_items = L->s_rb * p.TN0s;
-        L->s1_items = L->s_rb * p.TN1;
-        L->s_split = (b.g0 * p.TN0 + b.g1 * p.TN1) * L->tcm_items;   // block_start of block split_blk
-        L->total_items += L->s0_items + L->s1_items;
-    }
-}
-
-// first work item of block b: every earlier block holds tcm_items row blocks times its GEMM's column tiles, so the item
-// space follows the call's row-block count without rebuilding the table
-__device__ __forceinline__ int block_start(const FmParams& p, const Launch& L, const TileBlock& b) {
-    return (b.g0 * p.TN0 + b.g1 * p.TN1) * L.tcm_items;
-}
-
-// Item `id` of the launch -> the shared expert's GEMM (0 or 1), with `id` made its index among that GEMM's items, or -1,
-// with `id` made the routed item's id.  The shared GEMM0 items come first (they need nothing but x, which is in memory
-// when the kernel starts, so they fill the time the routed packets' rows take to land); its GEMM1 items follow the local
-// routed GEMM0 blocks (by then their h rows are complete, and they fill the time until the routed GEMM1 dependencies
-// resolve).  Without a shared expert both ranges are empty and every id is its routed id.
-__device__ __forceinline__ int split_item(const Launch& L, int& id) {
-    if (id < L.s0_items) return 0;
-    id -= L.s0_items;
-    if (id < L.s_split) return -1;
-    id -= L.s_split;
-    if (id < L.s1_items) return 1;
-    id += L.s_split - L.s1_items;
-    return -1;
+    L->s_rb = p.shared ? (n + BLOCK_M - 1) / BLOCK_M : 0;
+    L->total_items = block_start(p, *L, p.blocks[p.num_blocks]);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -568,8 +585,8 @@ __device__ __forceinline__ void gate_logits_tc(const FmParams& p, uint8_t* smem,
                 uint8_t* sa = smem + G_OFF_WG + s * stage_bytes;
                 uint64_t* full = bar(smem, BAR_GFULL + s);
                 mbar_arrive_expect_tx(full, tx);
-                for (int j = 0; j < nb32; ++j) tma_load_2d(sa + j * 4096, &p.tm_gx, kb * BLOCK_K, t0 + s0 + j * 32, full);
-                tma_load_2d(sa + a_cap, &p.tm_gw, kb * BLOCK_K, e0, full);
+                for (int j = 0; j < nb32; ++j) tma_load_2d(sa + j * 4096, &p.tm[TM_GX], kb * BLOCK_K, t0 + s0 + j * 32, full);
+                tma_load_2d(sa + a_cap, &p.tm[TM_GW], kb * BLOCK_K, e0, full);
             }
         } else if (warp >= EPI_WARP0) {        // consumer warpgroups
             const int wg = (warp - EPI_WARP0) >> 2;
@@ -1503,19 +1520,21 @@ __device__ __forceinline__ void dispatch_phase(const FmParams& p, const Launch& 
 //   interleaves them with a lag instead).  item -> (row block m fastest, column tile n).  Every packet holds tcm_items row
 //   blocks per column tile: on one rank the TCM of this call's capacity, with several ranks (where a receiver does not
 //   know its peers' token counts) the context's maximum.  Either way the list is a superset: row blocks beyond the
-//   packet's row count are skipped once the packet flag is known.  A GEMM1 tile waits for g0_done[pkt][m] == TN0.
+//   packet's row count are skipped once the packet flag is known.  A GEMM1 tile waits until its GEMM0's done counter
+//   of its row block (g0_done[pkt][m], or s0_done[m] for the shared expert) reaches that GEMM0's column tiles.  The
+//   shared expert's blocks are placed by the host (fm_create) and hold s_rb row blocks of the call's tokens.
 // ============================================================================================================
 struct TileInfo {     // written by the scheduler warp, read by the producer / consumer / publisher warps
-    int kind;         // 0 GEMM0, 1 GEMM1, -1 stop
+    int gemm;         // GEMM_* (kind = gemm & 1), -1 stop
     int ntile;
     int le;           // local expert
-    int b_row;        // TMA row coordinate of the B tile
+    int a_row;        // TMA row coordinates of the A and B tiles (GemmOp); a GEMM0's h rows are its A rows
+    int b_row;
     int pkt;          // local packet index src * nLx + le
-    int mblk;         // 128-row block of that packet
+    int mblk;         // 128-row block of that packet (the shared expert's: of the call's tokens)
     int rows;         // valid rows of that block
     int src;          // source rank of the packet
     int cnt;          // rows of the whole packet
-    int shared;       // 1: a tile of the shared expert (mblk = row block of tokens, rows = its tokens; no packet)
     int pad[2];
 };
 static_assert(sizeof(TileInfo) <= 64, "a ring slot is 64 bytes");
@@ -1525,6 +1544,7 @@ struct WorkItem {     // a work item id, decoded
     int mb;           // row block of the packet
     int nt;           // column tile
     int le, src;      // the packet's local expert and source rank
+    int b_row;        // TMA row of the tile's B operand
 };
 
 // Item `id` of this launch's work list.  `cursor` is the index of a block at or before the item's; the scheduler keeps it
@@ -1533,36 +1553,14 @@ __device__ __forceinline__ WorkItem decode_item(const FmParams& p, const Launch&
     while (id >= block_start(p, L, p.blocks[cursor + 1])) ++cursor;
     WorkItem w;
     w.blk = p.blocks[cursor];
-    const int local = id - block_start(p, L, w.blk);
-    w.mb = local % L.tcm_items;   // row blocks fastest
-    w.nt = local / L.tcm_items;
+    const GemmOp& op = p.gemm[w.blk.gemm];
+    const int local = id - block_start(p, L, w.blk), rbs = gemm_row_blocks(L, w.blk.gemm);
+    w.mb = local % rbs;   // row blocks fastest
+    w.nt = local / rbs;
     w.le = w.blk.pkt % p.nLx;
     w.src = w.blk.pkt / p.nLx;
+    w.b_row = op.b_row0 + w.le * op.b_le_rows + w.nt * BLOCK_N;
     return w;
-}
-
-// k-blocks of a tile: GEMM0 reduces over H, GEMM1 over P (the shared expert's over Ps)
-__device__ __forceinline__ int tile_kblocks(const FmParams& p, int kind, int shared = 0) {
-    return (kind == 0 ? p.H : shared ? p.Ps : p.P) / BLOCK_K;
-}
-
-// A shared-expert item: GEMM `kind` of row block mb of the call's tokens, column tile nt.  GEMM0 reads x in place and
-// waits for nothing; GEMM1 waits until every GEMM0 tile of its row block has stored its h rows.
-__device__ __forceinline__ void shared_tile(const FmParams& p, const Launch& L, int kind, int id, TileInfo& ti) {
-    const int mb = id % L.s_rb, nt = id / L.s_rb;
-    if (kind == 1) {
-        const unsigned int* ctr = p.s0_done + mb;
-        SpinGuard g;
-        while (ld_acquire_gpu_u32(ctr) < (unsigned int)p.TN0s) g.tick(p.dbg, p.timeout_ns, FM_TRAP_G0_DONE, 0x5E, mb, 0);
-    }
-    ti.kind = kind; ti.shared = 1; ti.ntile = nt; ti.mblk = mb; ti.rows = min(BLOCK_M, L.S - mb * BLOCK_M);
-    ti.src = p.rank; ti.cnt = L.S; ti.b_row = nt * BLOCK_N;
-}
-
-// TMA row of column tile nt's B operand.  expert_weights [nLx,2,P,H]: W_up(le) starts at row le*2*P of the [.,H] view;
-// W_down(le) (the [P,H] block flat-viewed as [H,P]) starts at row (le*2+1)*H of the [.,P] view.
-__device__ __forceinline__ int b_tile_row(const FmParams& p, int kind, int le, int nt) {
-    return (kind == 0 ? le * 2 * p.P : (le * 2 + 1) * p.H) + nt * BLOCK_N;
 }
 
 // warp 3, lane 0: claims work items and resolves their dependencies AHEAD of the TMA producer, so the atomic, the
@@ -1580,29 +1578,27 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L
             prev.next();
         }
         TileInfo ti;
-        ti.kind = -1; ti.ntile = 0; ti.le = 0; ti.b_row = 0; ti.pkt = 0; ti.mblk = 0; ti.rows = 0;
-        ti.src = 0; ti.cnt = 0; ti.shared = 0; ti.pad[0] = ti.pad[1] = 0;
+        ti.gemm = -1; ti.ntile = 0; ti.le = 0; ti.a_row = 0; ti.b_row = 0; ti.pkt = 0; ti.mblk = 0; ti.rows = 0;
+        ti.src = 0; ti.cnt = 0; ti.pad[0] = ti.pad[1] = 0;
         for (;;) {
-            int id = (int)atomicAdd(p.claim, 1u);
+            const int id = (int)atomicAdd(p.claim, 1u);
             if (id >= L.total_items) break;
             trace_tile(p, TRACE_TILE_CLAIMED, n);
-            const int sk = p.shared ? split_item(L, id) : -1;
-            if (sk >= 0) {
-                shared_tile(p, L, sk, id, ti);
-                break;
-            }
             const WorkItem w = decode_item(p, L, id, cursor);
             const TileBlock& blk = w.blk;
+            const GemmOp& op = p.gemm[blk.gemm];
+            const int kind = blk.gemm & 1;
             const int mb = w.mb, nt = w.nt, pkt = blk.pkt, le = w.le, src = w.src;
             const bool first_item = mb == 0 && nt == 0;   // the packet's first item of this GEMM
             const bool same_gpu = src == p.rank;   // flag and counters written from this GPU: gpu scope suffices
             const unsigned int epoch = L.epoch;
             // wait for the packet (src, le): flag = {epoch, rows}  (reference subscriber.cuh:52-185)
-            // dense: all of the call's rows, in x (the map over x may have more rows -- a device-side count reads S rows --
-            // and the rows past the call's count only reach h's padding rows, which GEMM1's epilogue drops: rows below)
+            // the call's tokens (dense, shared expert): all of the call's rows, in x (the map over x may have more rows --
+            // a device-side count reads S rows -- and the rows past the call's count only reach h's padding rows, which
+            // GEMM1's epilogue drops: rows below)
             unsigned long long f = ((unsigned long long)epoch << 32) | (unsigned int)L.S;
             bool stale = false;
-            if (!p.dense) {
+            if (op.from_packet) {
                 SpinGuard g;
                 for (;;) {
                     f = same_gpu ? ld_acquire_gpu_u64(p.recv_flag + pkt) : ld_acquire_sys_u64(p.recv_flag + pkt);
@@ -1618,16 +1614,18 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L
             if (stale) continue;
             const int cnt = (int)(f & 0xffffffffull);
             // once per packet and GEMM (its first item): bookkeeping that needs the count
-            if (first_item && blk.kind == 0 && !p.dense) p.recv_cnt[pkt] = cnt;
-            if (p.fused && first_item && blk.kind == 1 && cnt == 0)   // nothing to contribute: tell the source now
+            if (first_item && kind == 0 && op.from_packet) p.recv_cnt[pkt] = cnt;
+            if (p.fused && first_item && kind == 1 && cnt == 0)   // nothing to contribute: tell the source now
                 st_release_sys_u64(p.peer_done_flag[src] + (size_t)(p.rank * p.nLx + le), (unsigned long long)epoch << 32);
             const int rows = max(0, min(BLOCK_M, cnt - mb * BLOCK_M));
             if (rows == 0) continue;   // an empty row block of the static superset
             SpinGuard g;
-            if (blk.kind == 1) {  // GEMM1 needs the whole h row block (reference notifyNext, processor.cuh:490-615)
-                const unsigned int* ctr = p.g0_done + (size_t)pkt * p.TCM + mb;
-                while (ld_acquire_gpu_u32(ctr) < (unsigned int)p.TN0) g.tick(p.dbg, p.timeout_ns, FM_TRAP_G0_DONE, pkt, mb, 0);
-            } else if (!p.dense) {  // GEMM0 needs the rows of this block to have landed (dispatch acks)
+            if (kind == 1) {  // GEMM1 needs the whole h row block (reference notifyNext, processor.cuh:490-615)
+                const GemmOp& op0 = p.gemm[blk.gemm - 1];
+                const unsigned int* ctr = op0.done + (size_t)pkt * op0.done_pkt + mb;
+                while (ld_acquire_gpu_u32(ctr) < (unsigned int)op0.tn)
+                    g.tick(p.dbg, p.timeout_ns, FM_TRAP_G0_DONE, pkt, mb, (unsigned int)blk.gemm);
+            } else if (op.from_packet) {  // GEMM0 needs the rows of this block to have landed (dispatch acks)
                 const unsigned int* rctr = p.recv_rows + ((size_t)(epoch & 1u) * p.num_pkts + pkt) * p.TCM + mb;
                 for (;;) {
                     const unsigned int got = same_gpu ? ld_acquire_gpu_u32(rctr) : ld_acquire_sys_u32(rctr);
@@ -1635,13 +1633,14 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L
                     g.tick(p.dbg, p.timeout_ns, FM_TRAP_RECV_ROWS, pkt, mb, rows);
                 }
             }
-            ti.kind = blk.kind; ti.ntile = nt; ti.le = le; ti.pkt = pkt; ti.mblk = mb; ti.rows = rows;
+            ti.gemm = blk.gemm; ti.ntile = nt; ti.le = le; ti.pkt = pkt; ti.mblk = mb; ti.rows = rows;
             ti.src = src; ti.cnt = cnt;
-            ti.b_row = b_tile_row(p, blk.kind, le, nt);
+            ti.a_row = pkt * op.a_pkt_rows + mb * BLOCK_M;
+            ti.b_row = w.b_row;
             break;
         }
-        if (ti.kind >= 0) trace_tile(p, TRACE_TILE_READY, n);
-        if (ti.kind >= 0 && ti.src != p.rank && !seen_remote) {
+        if (ti.gemm >= 0) trace_tile(p, TRACE_TILE_READY, n);
+        if (ti.gemm >= 0 && ti.src != p.rank && !seen_remote) {
             seen_remote = true;
             trace_stamp(p, TRACE_FIRST_REMOTE);
         }
@@ -1650,7 +1649,7 @@ __device__ __forceinline__ void ffn_scheduler(const FmParams& p, const Launch& L
         mbar_arrive(bar(smem, BAR_SCHED_FULL + q.i));
         q.next();
         ++n;
-        if (ti.kind < 0) break;
+        if (ti.gemm < 0) break;
     }
 }
 
@@ -1662,33 +1661,32 @@ __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem) {
     Ring<NSCHED> q;
     bool first = true, stamped = false;
     for (;;) {
-        int kind = -1, shared = 0;
+        int gemm = -1;
         TileInfo ti;
         if (lane == 0) {
             bar_wait(p, smem, BAR_SCHED_FULL + q.i, q.phase);
             ti = ring[q.i];
             mbar_arrive(bar(smem, BAR_SCHED_EMPTY + q.i));
-            kind = ti.kind;
-            shared = ti.shared;
+            gemm = ti.gemm;
         }
-        kind = __shfl_sync(0xffffffffu, kind, 0);
-        if (kind < 0) break;
-        shared = __shfl_sync(0xffffffffu, shared, 0);
+        gemm = __shfl_sync(0xffffffffu, gemm, 0);
+        if (gemm < 0) break;
+        const GemmOp& op = p.gemm[gemm];
         int nk = 0;
         if (lane == 0) {
             if (first)   // the stage area doubles as the dispatch staging buffer
                 bar_wait(p, smem, BAR_DISP_DONE, 0);
             first = false;
             fence_proxy_async_global();  // rows written by generic-proxy stores (peers / other SMs) -> TMA reads
-            nk = tile_kblocks(p, kind, shared);
+            nk = op.kblocks;
         }
         nk = __shfl_sync(0xffffffffu, nk, 0);
-        const CUtensorMap* ta = shared ? (kind == 0 ? &p.tm_xs : &p.tm_hs) : (kind == 0 ? &p.tm_a0 : &p.tm_a1);
-        const CUtensorMap* tb = shared ? (kind == 0 ? &p.tm_ws0 : &p.tm_ws1) : (kind == 0 ? &p.tm_b0 : &p.tm_b1);
+        const CUtensorMap* ta = &p.tm[op.a];
+        const CUtensorMap* tb = &p.tm[op.b];
         const int take_at = min(nk - 1, max(0, nk - CLAIM_AHEAD_KB));
         int a_row = 0, b_row = 0;
         if (lane == 0) {
-            a_row = (shared ? 0 : ti.pkt * p.pEC) + ti.mblk * BLOCK_M;   // (the shared expert's rows are the tokens)
+            a_row = ti.a_row;
             b_row = ti.b_row;
         }
         for (int kb = 0; kb < nk; ++kb) {
@@ -1907,11 +1905,10 @@ __device__ __forceinline__ void with_bias(const __nv_bfloat16* bias, F&& f) {
 __device__ __forceinline__ void epilogue_h(const FmParams& p, uint8_t* smem, const TileInfo* ti, float (&acc)[128], int prev,
                                            Consumer& c) {
     const int n0 = ti->ntile * BLOCK_N, le = ti->le;
-    const bool shared = ti->shared != 0;
+    const GemmOp& op = p.gemm[ti->gemm];
     mainloop_done(p, smem, acc, prev, c);
-    const int nchunks = min(BLOCK_N / 64, ((shared ? p.Ps : p.P) - n0) / 64);
-    const __nv_bfloat16* bias = shared ? (p.s_b_up ? p.s_b_up + n0 : nullptr)
-                                       : (p.b_up ? p.b_up + (size_t)le * p.P + n0 : nullptr);
+    const int nchunks = min(BLOCK_N / 64, (op.n - n0) / 64);
+    const __nv_bfloat16* bias = op.bias ? op.bias + (size_t)le * op.bias_le + n0 : nullptr;
     with_bias(bias, [&](auto has_bias) {
         constexpr bool B = decltype(has_bias)::value;
         if (p.act == 0) stage_h<EPI_G0_RELU, B>(p, smem, acc, bias, nchunks, c.row0, c.lane, c.chunk);
@@ -1929,8 +1926,9 @@ __device__ __forceinline__ void epilogue_out(const FmParams& p, uint8_t* smem, c
     // While the last k-block's MMAs run: the tile's fields from its ring slot and, for the fused epilogue, lane l < 16's
     // routing record of tile row (row0 + l), so that nothing is fetched after the final wait.
     const int ntile = ti->ntile, le = ti->le, pkt = ti->pkt, mblk = ti->mblk, my_rows = ti->rows, src = ti->src;
-    const bool shared = ti->shared != 0;   // the shared expert's s rows: stored into y_s, by token, like EPI_G1_STORE
-    const bool fuse = p.fused != 0 && !shared;
+    const GemmOp& op = p.gemm[ti->gemm];
+    const int dest = op.dest;
+    const bool fuse = dest == DEST_FUSED;
     int my_tok = 0;
     float my_pw = 0.0f, my_mcw = 1.0f;
     if (fuse && p.dense) {
@@ -1943,7 +1941,7 @@ __device__ __forceinline__ void epilogue_out(const FmParams& p, uint8_t* smem, c
     }
     mainloop_done(p, smem, acc, prev, c);
 
-    const int N = p.H, n0 = ntile * BLOCK_N;
+    const int N = op.n, n0 = ntile * BLOCK_N;
     const int e_global = p.rank * p.nLx + le;
     const int nchunks = row0 < my_rows ? min(BLOCK_N / 64, (N - n0) / 64) : 0;
     // this warp's transpose tile is its rows of chunk buffer 0, which the TMA may still be reading for the last
@@ -1954,9 +1952,9 @@ __device__ __forceinline__ void epilogue_out(const FmParams& p, uint8_t* smem, c
         DrainArgs da;
         da.stg = smem + OFF_EPI + row0 * EPI_ROW_BYTES; da.nchunks = nchunks; da.lane = lane; da.row0 = row0;
         da.my_rows = my_rows; da.N = N; da.n0 = n0;
-        da.bias = shared ? p.s_b_down : p.b_down ? p.b_down + (size_t)le * p.H : nullptr;
-        da.out_rows = shared ? p.y_s + (size_t)mblk * BLOCK_M * p.H
-                             : p.peer_ret_y[src] + ((size_t)e_global * p.pEC + (size_t)mblk * BLOCK_M) * p.H;
+        da.bias = op.bias ? op.bias + (size_t)le * op.bias_le : nullptr;
+        da.out_rows = dest == DEST_Y_S ? p.y_s + (size_t)mblk * BLOCK_M * N   // by token
+                                       : p.peer_ret_y[src] + ((size_t)e_global * p.pEC + (size_t)mblk * BLOCK_M) * N;
         da.acc_base = fuse ? p.peer_out_acc[src] : nullptr;
         da.my_tok = my_tok; da.my_pw = my_pw; da.my_mcw = my_mcw;
         with_bias(da.bias, [&](auto has_bias) {
@@ -1993,11 +1991,11 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem) {
         // The tile's ring slot stays ours until its epilogue is set up (mainloop_done arrives on sched_empty): the
         // per-tile fields are read from shared memory after the k-block loop instead of being kept live (spilled) across it.
         const TileInfo* ti = ring + c.q.i;
-        const int kind = ti->kind;
-        if (kind < 0) break;
+        const int gemm = ti->gemm;
+        if (gemm < 0) break;
         float acc[128];
-        const int prev = mainloop(p, smem, acc, tile_kblocks(p, kind, ti->shared), c);
-        if (kind == 0) epilogue_h(p, smem, ti, acc, prev, c);
+        const int prev = mainloop(p, smem, acc, p.gemm[gemm].kblocks, c);
+        if ((gemm & 1) == 0) epilogue_h(p, smem, ti, acc, prev, c);
         else epilogue_out(p, smem, ti, acc, prev, c);
         ++c.ntiles;
     }
@@ -2011,11 +2009,11 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem) {
 // (reference notifyNext's tSA counter, processor.cuh:490-615).  `chunk` counts the chunks stored so far, in the
 // consumers' staging order.
 __device__ __forceinline__ void publish_h(const FmParams& p, uint8_t* smem, const TileInfo& ti, uint32_t& chunk) {
-    // the shared expert's h: its own map and counters, rows = tokens
-    const int n0 = ti.ntile * BLOCK_N, nchunks = min(BLOCK_N / 64, ((ti.shared ? p.Ps : p.P) - n0) / 64);
-    const int row = (ti.shared ? 0 : ti.pkt * p.pEC) + ti.mblk * BLOCK_M;
-    const CUtensorMap* map = ti.shared ? &p.tm_hs : &p.tm_a1;
-    unsigned int* ctr = ti.shared ? p.s0_done + ti.mblk : p.g0_done + (size_t)ti.pkt * p.TCM + ti.mblk;
+    const GemmOp& op = p.gemm[ti.gemm];
+    const int n0 = ti.ntile * BLOCK_N, nchunks = min(BLOCK_N / 64, (op.n - n0) / 64);
+    const int row = ti.a_row;
+    const CUtensorMap* map = &p.tm[p.gemm[ti.gemm + 1].a];   // h is its GEMM1's A
+    unsigned int* ctr = op.done + (size_t)ti.pkt * op.done_pkt + ti.mblk;
     // both buffers' stores in flight: chunk c is issued as soon as it is staged, and only then does the warp wait for
     // the TMA to have read chunk c - 1, whose buffer the consumers refill with chunk c + 1
     for (int c = 0; c < nchunks; ++c, ++chunk) {
@@ -2042,12 +2040,13 @@ __device__ __forceinline__ void publish_out(const FmParams& p, const Launch& L, 
     bar_wait(p, smem, BAR_PUB_FULL + pub.i, pub.phase);
     mbar_arrive(bar(smem, BAR_PUB_EMPTY + pub.i));
     pub.next();
-    if (ti.shared) {   // the shared expert's s rows, read on this GPU by the completion phase
+    const int dest = p.gemm[ti.gemm].dest;
+    if (dest == DEST_Y_S) {   // the shared expert's s rows, read on this GPU by the completion phase
         fence_acq_rel_gpu();
         red_release_gpu_add_u32(p.s1_done + ti.mblk, 1u);
         return;
     }
-    if (p.fused) {
+    if (dest == DEST_FUSED) {
         // local packet, output left in place: nobody waits for a flag (see finish_fused) -- no fence, no counter, no
         // flag; kernel completion covers these adds.  With a shared expert the completion phase adds s to the finished
         // rows, so it waits for the local experts too.
@@ -2078,20 +2077,22 @@ __device__ __forceinline__ void ffn_publisher(const FmParams& p, const Launch& L
     int ntiles = 0;
     uint32_t chunk = 0;   // h chunks stored so far (publish_h)
     for (;;) {
-        int kind = -1;
+        int gemm = -1;
         if (lane == 0) {
             bar_wait(p, smem, BAR_SCHED_FULL + q.i, q.phase);
             const TileInfo ti = ring[q.i];
             mbar_arrive(bar(smem, BAR_SCHED_EMPTY + q.i));
-            kind = ti.kind;
-            if (kind == 0) publish_h(p, smem, ti, chunk);
-            else if (kind == 1) publish_out(p, L, smem, ti, pub);
-            if (kind >= 0) trace_tile(p, TRACE_TILE_PUBLISHED, ntiles);
+            gemm = ti.gemm;
+            if (gemm >= 0) {
+                if ((gemm & 1) == 0) publish_h(p, smem, ti, chunk);
+                else publish_out(p, L, smem, ti, pub);
+                trace_tile(p, TRACE_TILE_PUBLISHED, ntiles);
+            }
         }
-        kind = __shfl_sync(0xffffffffu, kind, 0);
+        gemm = __shfl_sync(0xffffffffu, gemm, 0);
         q.next();
         ++ntiles;
-        if (kind < 0) break;
+        if (gemm < 0) break;
         __syncwarp();
     }
 }
@@ -2108,9 +2109,9 @@ __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
         fence_mbar_init();
     }
     if (warp == 0 && (tid & 31) == 0) {
-        if (!p.dense || p.n_tokens > 0) tma_prefetch_desc(&p.tm_a0);   // (dense, no tokens: no map over x was encoded)
-        tma_prefetch_desc(&p.tm_b0);
-        tma_prefetch_desc(&p.tm_a1); tma_prefetch_desc(&p.tm_b1);
+        if (!p.dense || p.n_tokens > 0) tma_prefetch_desc(&p.tm[TM_A0]);   // (dense, no tokens: no map over x was encoded)
+        tma_prefetch_desc(&p.tm[TM_B0]);
+        tma_prefetch_desc(&p.tm[TM_A1]); tma_prefetch_desc(&p.tm[TM_B1]);
     }
 }
 
@@ -2119,19 +2120,12 @@ __device__ __forceinline__ void ffn_warm_l2(const FmParams& p, const Launch& L) 
         // Warm L2 with the 256-row weight tile this CTA will most likely claim first (item id = CTA index: the first wave is
         // claimed in arrival order), pipeline depth only: HBM is idle during the router and the first tile's loads are
         // then L2 hits.  A wrong guess costs nothing -- the tile is needed by some CTA of the first wave anyway.
-        int id = (int)blockIdx.x;
-        const int sk = p.shared && id < L.total_items ? split_item(L, id) : -1;
-        if (sk >= 0) {   // a shared-expert tile: its weights' column tile
-            const CUtensorMap* tb = sk == 0 ? &p.tm_ws0 : &p.tm_ws1;
-            for (int kb = 0; kb < min(tile_kblocks(p, sk, 1), STAGES); ++kb)
-                tma_prefetch_l2_2d(tb, kb * BLOCK_K, (id / L.s_rb) * BLOCK_N);
-        } else if (id < L.total_items) {
+        const int id = (int)blockIdx.x;
+        if (id < L.total_items) {
             int cursor = 0;
             const WorkItem w = decode_item(p, L, id, cursor);
-            const int kind = w.blk.kind;
-            const CUtensorMap* tb = kind == 0 ? &p.tm_b0 : &p.tm_b1;
-            const int b0 = b_tile_row(p, kind, w.le, w.nt);
-            for (int kb = 0; kb < min(tile_kblocks(p, kind), STAGES); ++kb) tma_prefetch_l2_2d(tb, kb * BLOCK_K, b0);
+            const GemmOp& op = p.gemm[w.blk.gemm];
+            for (int kb = 0; kb < min(op.kblocks, STAGES); ++kb) tma_prefetch_l2_2d(&p.tm[op.b], kb * BLOCK_K, w.b_row);
         }
     }
 }

@@ -24,22 +24,35 @@ def _src(name):
 
 
 # ----------------------------------------------------------------------------- the kernel's tiling and work list
-def test_tiling_matches_the_kernel():
+def test_tiling_and_block_placement_match_the_kernel():
     kern, host = _src("fm_kernel.cuh"), _src("flashmoe_b200.cu")
     assert f"constexpr int BLOCK_M = {es.BLOCK_M};" in kern and f"constexpr int BLOCK_N = {es.BLOCK_N};" in kern
-    for line in ("L->tpc = (n + G - 1) / G;", "L->s_rb = (n + BLOCK_M - 1) / BLOCK_M;", "L->s0_items = L->s_rb * p.TN0s;",
-                 "L->s1_items = L->s_rb * p.TN1;", "const int t0 = blockIdx.x * L.tpc;",
+    # a block's items: column tiles x row blocks, the shared GEMMs' row blocks being s_rb
+    for line in ("L->tpc = (n + G - 1) / G;", "L->s_rb = p.shared ? (n + BLOCK_M - 1) / BLOCK_M : 0;",
+                 "return g < GEMM_S_UP ? L.tcm_items : L.s_rb;",
+                 "for (int g = 0; g < NUM_GEMMS; ++g) start += b.g[g] * p.gemm[g].tn * gemm_row_blocks(L, g);",
+                 "const int local = id - block_start(p, L, w.blk), rbs = gemm_row_blocks(L, w.blk.gemm);",
+                 "w.mb = local % rbs;", "w.nt = local / rbs;", "const int t0 = blockIdx.x * L.tpc;",
                  "const int n_tok = max(0, min(L.tpc, L.S - t0));",
                  "for (int rb = t0 / BLOCK_M + (int)threadIdx.x; rb <= (t0 + n_tok - 1) / BLOCK_M; rb += NUM_THREADS)",
-                 "while (ld_acquire_gpu_u32(p.s1_done + rb) < (unsigned int)p.TN1)"):
+                 "while (ld_acquire_gpu_u32(p.s1_done + rb) < (unsigned int)p.TN1)",
+                 "int n, tn; // output columns and column tiles, ceil(n / BLOCK_N)"):
         assert line in kern, f"fm_kernel.cuh no longer has `{line}`: update exact_shared.regime"
-    for line in ("p.TN0s = ceil_div((int)Ps, fm::BLOCK_N);", "ctx->TN1 = ceil_div(d.H, fm::BLOCK_N);",
+    # the shared GEMMs' column tiles (GemmOp::tn, the eighth field): TN0s = ceil(Ps / BLOCK_N) and TN1; the shared GEMM1
+    # block right after the leading local routed GEMM0 blocks (split_blk), the shared GEMM0 block first
+    for line in ("const int ps = (int)Ps;",
+                 "p.gemm[fm::GEMM_S_UP] = {fm::TM_XS, fm::TM_WS0, 0, 0, 0, d.H / fm::BLOCK_K, ps, "
+                 "ceil_div(ps, fm::BLOCK_N),",
+                 "p.gemm[fm::GEMM_S_DOWN] = {fm::TM_HS, fm::TM_WS1, 0, 0, 0, ps / fm::BLOCK_K, d.H, c->TN1,",
+                 "ctx->TN1 = ceil_div(d.H, fm::BLOCK_N);",
                  "ctx->grid = d.num_sms;", 'const int lag = env_int("FM_G1_LAG", -1);',
                  "if (lag >= 1 && lag < (int)units.size()) { for (size_t i = 0; i < units.size(); ++i) { push(0, units[i]); "
                  "if ((int)i >= lag) push(1, units[i - lag]); }",
                  "for (const Unit& u : units) push(0, u); for (const Unit& u : g1_units) push(1, u);",
-                 "while (ctx->split_blk < ctx->num_blocks && blocks[ctx->split_blk].kind == 0 && "
-                 "blocks[ctx->split_blk].pkt / nLx == rank) ++ctx->split_blk;"):
+                 "while (split < blocks.size() && blocks[split].gemm == fm::GEMM_UP && blocks[split].pkt / nLx == rank) "
+                 "++split;",
+                 "blocks.insert(blocks.begin() + split, {{}, fm::GEMM_S_DOWN, rank * nLx}); "
+                 "blocks.insert(blocks.begin(), {{}, fm::GEMM_S_UP, rank * nLx});"):
         assert line in host, f"flashmoe_b200.cu no longer has `{line}`: update exact_shared.regime"
 
 
