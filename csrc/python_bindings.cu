@@ -128,9 +128,15 @@ py::object moe_forward(py::object input, py::object gate_weights, py::object exp
             "Gate weights must be [H=" + std::to_string(g_dims.H) + ", E=" + std::to_string(g_dims.E) + "]");
     require(es.size() == 4 && es[0] == g_dims.num_local_experts,
             "Expert count mismatch. Expected " + std::to_string(g_dims.num_local_experts) + " local experts");
-    require(es[1] == 2, "Expert weights must have up and down projections [nLx, 2, P, H]");
+    // the context is the compiled configuration's: SwiGLU experts (hidden_act 2) are [nLx, 3, P, H]
+    fm_config_t cfg;
+    check(fm_compiled_config(&cfg), "fm_compiled_config");
+    const int64_t mats = cfg.hidden_act == 2 ? 3 : 2;
+    require(es[1] == mats, mats == 2 ? "Expert weights must have up and down projections [nLx, 2, P, H]"
+                                     : "SwiGLU expert weights must have gate, up and down projections [nLx, 3, P, H]");
     require(es[2] == g_dims.P && es[3] == g_dims.H,
-            "Expert weights must be [*, 2, P=" + std::to_string(g_dims.P) + ", H=" + std::to_string(g_dims.H) + "]");
+            "Expert weights must be [*, " + std::to_string(mats) + ", P=" + std::to_string(g_dims.P) +
+                ", H=" + std::to_string(g_dims.H) + "]");
     py::module_ torch = py::module_::import("torch");
     py::object out = torch.attr("empty_like")(input);   // freshly allocated, caller-owned (reference :131-148)
     const auto stream = torch.attr("cuda").attr("current_stream")().attr("cuda_stream").cast<uintptr_t>();

@@ -29,7 +29,7 @@ ALL_KEYS = (
 REQUIRED_KEYS = tuple(k for k in ALL_KEYS if k != "global_batch")
 
 DTYPE_BF16 = 2  # schema: 0 fp32, 1 tf32, 2 bf16, 3 fp16 (flashmoe_config.schema.json:64-68)
-ACT_RELU, ACT_GELU = 0, 1
+ACT_RELU, ACT_GELU, ACT_SWIGLU = 0, 1, 2
 
 
 class ConfigError(ValueError):
@@ -101,6 +101,11 @@ class MoEConfig:
     @property
     def k(self) -> int:
         return self.expert_top_k
+
+    @property
+    def expert_mats(self) -> int:
+        """Matrices per expert in the expert weights: [W_up, W_down], or SwiGLU's [W_gate, W_up, W_down]."""
+        return 3 if self.hidden_act == ACT_SWIGLU else 2
 
     @property
     def PX(self) -> int:  # padded expert axis of gateOut (types.cuh:480)

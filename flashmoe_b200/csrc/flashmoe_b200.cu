@@ -181,7 +181,8 @@ long long expert_capacity(const fm_config_t& c, long long n) {
 int validate_config(const fm_config_t& c, int world, fm_dims_t* d) {
     if (c.torch_dtype != 2) return fail(FM_EINVAL, "torch_dtype=%d: this build computes in bf16 only (2)", c.torch_dtype);
     if (c.is_training != 0 && c.is_training != 1) return fail(FM_EINVAL, "is_training must be 0 or 1");
-    if (c.hidden_act != 0 && c.hidden_act != 1) return fail(FM_EINVAL, "hidden_act must be 0 (relu) or 1 (gelu)");
+    if (c.hidden_act < 0 || c.hidden_act > 2)
+        return fail(FM_EINVAL, "hidden_act must be 0 (relu), 1 (gelu) or 2 (swiglu)");
     if (c.drop_tokens != 0 && c.drop_tokens != 1) return fail(FM_EINVAL, "drop_tokens must be 0 or 1");
     if (c.capacity_factor < 1) return fail(FM_EINVAL, "capacity_factor must be >= 1");
     if (c.hidden_size <= 0 || c.hidden_size % 64) return fail(FM_EINVAL, "hidden_size must be a positive multiple of 64");
@@ -409,17 +410,22 @@ int launch(fm_ctx* c, const ForwardCall& f) {
     // of 2*P (resp. 2*H) rows is not expressible in 2-D, so rows are addressed as [nLx*2*P, H] / [nLx*2*H, P]:
     // expert i's W_up starts at row i*2*P, its W_down at row (i*2+1)*H of the [.,P] view.  The shared expert's
     // w [2, Ps, H] is one such expert: W_up_s [Ps, H] and W_down_s [H, Ps].
+    // SwiGLU (hidden_act 2): [nLx, 3, P, H] = W_gate, W_up, W_down per expert, so mats = 3 matrices per expert; GEMM0's
+    // maps load 128-row boxes, a gate half and an up half per tile, and W_down is matrix 2.
+    const bool glu = c->cfg.hidden_act == 2;
+    const uint64_t mats = glu ? 3 : 2;
+    const uint32_t box0 = glu ? fm::BLOCK_N / 2 : fm::BLOCK_N;
     struct MapSpec { const void* base; uint64_t rows, cols; uint32_t box_rows; bool needed; };
     const MapSpec maps[fm::NUM_TMAPS] = {
         {a0, a0_rows, (uint64_t)d.H, fm::BLOCK_M, a0_rows > 0},                            // TM_A0
-        {f.expert_w, (uint64_t)nLx * 2 * d.P, (uint64_t)d.H, fm::BLOCK_N, true},           // TM_B0
+        {f.expert_w, nLx * mats * d.P, (uint64_t)d.H, box0, true},                         // TM_B0
         {c->hidden, pkt_rows, (uint64_t)d.P, fm::BLOCK_M, true},                           // TM_A1
-        {f.expert_w, (uint64_t)nLx * 2 * d.H, (uint64_t)d.P, fm::BLOCK_N, true},           // TM_B1
+        {f.expert_w, nLx * mats * d.H, (uint64_t)d.P, fm::BLOCK_N, true},                  // TM_B1
         {f.x, n, (uint64_t)d.H, 32, gate_maps && n > 0},                                   // TM_GX
         {f.gate_w, (uint64_t)d.E, (uint64_t)d.H, std::min(128u, e64), gate_maps},          // TM_GW
         {f.x, n, (uint64_t)d.H, fm::BLOCK_M, sh != nullptr && n > 0},                      // TM_XS
-        {ws, Ps, (uint64_t)d.H, fm::BLOCK_N, sh != nullptr},                               // TM_WS0
-        {ws + Ps * d.H * 2, (uint64_t)d.H, Ps, fm::BLOCK_N, sh != nullptr},                // TM_WS1
+        {ws, glu ? 3 * Ps : Ps, (uint64_t)d.H, box0, sh != nullptr},                       // TM_WS0
+        {ws + (mats - 1) * Ps * d.H * 2, (uint64_t)d.H, Ps, fm::BLOCK_N, sh != nullptr},   // TM_WS1
         {c->h_s, (uint64_t)d.S, Ps, fm::BLOCK_M, sh != nullptr},                           // TM_HS
     };
 
@@ -433,19 +439,23 @@ int launch(fm_ctx* c, const ForwardCall& f) {
     }
     // the GEMMs' operands, fields in fm::GemmOp's order: {A map, B map, A rows per packet, B row of expert 0,
     // B rows per expert, k-blocks, output columns, column tiles, rows from a packet, bias per expert, done counters per
-    // packet, destination, bias, done counters}
-    const int from_packet = c->dense ? 0 : 1;
+    // packet, destination, bias, done counters}.  SwiGLU: the bias is [gate; up] per expert, and a GEMM0 tile is
+    // tile_cols = 128 columns of h from its gate rows and the up rows glu_rows below them (column tiles ceil(n / 128)).
+    const int from_packet = c->dense ? 0 : 1, m = (int)mats;
     using bf16p = const __nv_bfloat16*;
-    p.gemm[fm::GEMM_UP] = {fm::TM_A0, fm::TM_B0, d.pEC, 0, 2 * d.P, d.H / fm::BLOCK_K, d.P, ceil_div(d.P, fm::BLOCK_N),
-                           from_packet, d.P, d.TCM, 0, static_cast<bf16p>(f.bias_up), c->g0_done};
-    p.gemm[fm::GEMM_DOWN] = {fm::TM_A1, fm::TM_B1, d.pEC, d.H, 2 * d.H, d.P / fm::BLOCK_K, d.H, c->TN1, from_packet, d.H,
-                             0, c->fused ? fm::DEST_FUSED : fm::DEST_RETURN, static_cast<bf16p>(f.bias_down), nullptr};
+    p.gemm[fm::GEMM_UP] = {fm::TM_A0, fm::TM_B0, d.pEC, 0, m * d.P, d.H / fm::BLOCK_K, d.P, ceil_div(d.P, fm::BLOCK_N),
+                           from_packet, (m - 1) * d.P, d.TCM, 0, static_cast<bf16p>(f.bias_up), c->g0_done};
+    if (glu) { p.gemm[fm::GEMM_UP].glu_rows = d.P; p.gemm[fm::GEMM_UP].tn = ceil_div(d.P, (int)box0); }
+    p.gemm[fm::GEMM_DOWN] = {fm::TM_A1, fm::TM_B1, d.pEC, (m - 1) * d.H, m * d.H, d.P / fm::BLOCK_K, d.H, c->TN1,
+                             from_packet, d.H, 0, c->fused ? fm::DEST_FUSED : fm::DEST_RETURN,
+                             static_cast<bf16p>(f.bias_down), nullptr};
     if (sh != nullptr) {   // rows are the call's tokens
         p.shared = 1;
         p.y_s = c->y_s; p.s0_done = c->s0_done; p.s1_done = c->s1_done;
         const int ps = (int)Ps;
         p.gemm[fm::GEMM_S_UP] = {fm::TM_XS, fm::TM_WS0, 0, 0, 0, d.H / fm::BLOCK_K, ps, ceil_div(ps, fm::BLOCK_N), 0, 0,
                                  0, 0, static_cast<bf16p>(sh->bias_up), c->s0_done};
+        if (glu) { p.gemm[fm::GEMM_S_UP].glu_rows = ps; p.gemm[fm::GEMM_S_UP].tn = ceil_div(ps, (int)box0); }
         p.gemm[fm::GEMM_S_DOWN] = {fm::TM_HS, fm::TM_WS1, 0, 0, 0, ps / fm::BLOCK_K, d.H, c->TN1, 0, 0, 0, fm::DEST_Y_S,
                                    static_cast<bf16p>(sh->bias_down), nullptr};
     }

@@ -295,13 +295,13 @@ static_assert(sizeof(TileBlock) == 16 && 2 * MAX_EXPERTS + NUM_GEMMS <= 0xffff, 
 // Tensor maps of a launch, FmParams::tm[] ids (encoded by the host from one table in launch()).
 enum : int {
     TM_A0,    // GEMM_UP's A: recv_x as [W*nLx*pEC, H] (dense: x as [n_tokens, H]), box {64, 128}
-    TM_B0,    // expert_weights as [nLx*2*P, H], box {64, 256} (W_up rows)
+    TM_B0,    // expert_weights as [nLx*2*P, H], box {64, 256} (W_up rows); SwiGLU: [nLx*3*P, H], box {64, 128}
     TM_A1,    // hidden as [W*nLx*pEC, P], box {64, 128}: GEMM_DOWN's A loads and GEMM_UP's h stores
-    TM_B1,    // expert_weights as [nLx*2*H, P], box {64, 256} (W_down rows)
+    TM_B1,    // expert_weights as [nLx*2*H, P] (SwiGLU: [nLx*3*H, P]), box {64, 256} (W_down rows)
     TM_GX,    // router on tensor cores: x as [n_tokens, H], box {64, 32}
     TM_GW,    // router on tensor cores: Wg_eff [E, H], box {64, min(128, E rounded up to 64)}
     TM_XS,    // shared expert: x as [n_tokens, H], box {64, 128}: GEMM_S_UP's A
-    TM_WS0,   // W_up_s as [Ps, H], box {64, 256}
+    TM_WS0,   // W_up_s as [Ps, H], box {64, 256}; SwiGLU: the [3, Ps, H] tensor as [3*Ps, H], box {64, 128}
     TM_WS1,   // W_down_s (the same Ps*H block) as [H, Ps], box {64, 256}
     TM_HS,    // h_s as [S, Ps], box {64, 128}: GEMM_S_DOWN's A loads and GEMM_S_UP's h stores
     NUM_TMAPS
@@ -315,7 +315,9 @@ enum : int {
 };
 
 // Everything the FFN's warp roles need about one GEMM's operands, filled by the host per launch.  Tile (mblk, ntile) of
-// packet pkt = src * nLx + le reads A rows pkt * a_pkt_rows + 128 mblk and B rows b_row0 + le * b_le_rows + 256 ntile.
+// packet pkt = src * nLx + le reads A rows pkt * a_pkt_rows + 128 mblk and B rows b_row0 + le * b_le_rows +
+// tile_cols(op) * ntile.  A gated GEMM0 (SwiGLU, glu_rows != 0) reads 128 gate rows there and the 128 up rows glu_rows
+// below them, and writes 128 columns of h = silu(g) * u per tile.
 struct GemmOp {
     int a, b;               // FmParams::tm ids of the A and B operands (a GEMM0 stores h through its GEMM1's A map)
     int a_pkt_rows;         // A rows per packet: pEC, or 0 where the rows are the call's tokens
@@ -328,7 +330,11 @@ struct GemmOp {
     int dest;               // GEMM1: DEST_*
     const __nv_bfloat16* bias;   // [n] per local expert, or nullptr
     unsigned int* done;     // GEMM0: its tiles finished per row block (g0_done, s0_done)
+    int glu_rows;           // SwiGLU GEMM0: B rows from a tile's gate half to its up half (P, Ps); otherwise 0
 };
+
+// Output columns of one column tile: a gated GEMM0's 256-row B tile is two 128-row halves, gate and up.
+__device__ __forceinline__ int tile_cols(const GemmOp& op) { return op.glu_rows ? BLOCK_N / 2 : BLOCK_N; }
 
 // Where phase G takes a launch's routing from.  A caller-routed and a gated launch both store mcw = 1 and take the
 // scaling combine for every k (k = 1 included); only the router launch copies y unscaled at k = 1.
@@ -1559,7 +1565,7 @@ __device__ __forceinline__ WorkItem decode_item(const FmParams& p, const Launch&
     w.nt = local / rbs;
     w.le = w.blk.pkt % p.nLx;
     w.src = w.blk.pkt / p.nLx;
-    w.b_row = op.b_row0 + w.le * op.b_le_rows + w.nt * BLOCK_N;
+    w.b_row = op.b_row0 + w.le * op.b_le_rows + w.nt * tile_cols(op);
     return w;
 }
 
@@ -1681,6 +1687,7 @@ __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem) {
             nk = op.kblocks;
         }
         nk = __shfl_sync(0xffffffffu, nk, 0);
+        const int glu = op.glu_rows;
         const CUtensorMap* ta = &p.tm[op.a];
         const CUtensorMap* tb = &p.tm[op.b];
         const int take_at = min(nk - 1, max(0, nk - CLAIM_AHEAD_KB));
@@ -1700,6 +1707,9 @@ __device__ __forceinline__ void ffn_producer(const FmParams& p, uint8_t* smem) {
                 if (tx) mbar_arrive_expect_tx(full, tx); else mbar_arrive(full);
                 if (ld_a) tma_load_2d(sa, ta, kb * BLOCK_K, a_row, full);
                 if (ld_b) tma_load_2d(sa + A_STAGE_BYTES, tb, kb * BLOCK_K, b_row, full);
+                // SwiGLU: B's map has 128-row boxes; the up rows fill the stage's second 16 KiB.  16 KiB is a whole
+                // number of SWIZZLE_128B periods (1 KiB), so the stage holds exactly what one 256-row box would.
+                if (ld_b && glu) tma_load_2d(sa + A_STAGE_BYTES + B_STAGE_BYTES / 2, tb, kb * BLOCK_K, b_row + glu, full);
                 if (!stamped) { trace_stamp(p, TRACE_FIRST_TMA); stamped = true; }   // first loads of the first tile issued
             }
             stage.next();
@@ -1713,15 +1723,22 @@ __device__ __noinline__ float gelu_erf(float v) {   // GELU, erf form (cutlass::
     return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f));
 }
 
-enum : int { EPI_G0_RELU = 0, EPI_G0_GELU = 1, EPI_G1_STORE = 2, EPI_G1_FUSED_ADD = 3, EPI_G1_FUSED_COPY = 4 };
+// SwiGLU of one element pair: h = fl(fl(g * sigmoid(g)) * u), sigmoid_score's sigmoid (relative error in DESIGN.md).
+__device__ __forceinline__ float silu_mul(float g, float u) { return __fmul_rn(__fmul_rn(g, sigmoid_score(g)), u); }
+
+enum : int {
+    EPI_G0_RELU = 0, EPI_G0_GELU = 1, EPI_G1_STORE = 2, EPI_G1_FUSED_ADD = 3, EPI_G1_FUSED_COPY = 4, EPI_G0_SWIGLU = 5
+};
 
 // registers (wgmma fragment: rows r0 = lane/4 and r0 + 8 of this warp's 16, column pairs 8j + 2*(lane%4)) of the 64
 // accumulator columns [64c, 64c + 64) -> bias / activation / combine scaling in fp32 -> bf16 (RNE) -> 16 rows of 128 B
 // at `stg`, 16-byte piece j of row r at piece j ^ (r & 7) (the TMA's 128-byte swizzle when `stg` is 1 KiB aligned).
-// `bias` points at the chunk's first column (or is unused).
+// `bias` points at the chunk's first column (or is unused).  EPI_G0_SWIGLU: output chunk c in {0, 1} takes the gate
+// from accumulator columns [64c, 64c + 64) and the up projection from the same thread's columns 128 further on; the up
+// bias is `glu` elements past the gate bias.
 template <int MODE, bool HAS_BIAS>
 __device__ __forceinline__ void chunk_to_smem(const float (&acc)[128], int c, uint8_t* stg, const __nv_bfloat16* bias,
-                                              int lane, const float (&pw)[2], const float (&mcw)[2]) {
+                                              int lane, const float (&pw)[2], const float (&mcw)[2], int glu = 0) {
     const int r0 = lane >> 2, cq = (lane & 3) * 2;
     // Rows r0 and r0 + 8 share r & 7 = r0, and `stg` is 128-byte aligned, so piece j of either row is one XOR of bits
     // 4-6 away from piece 0 ^ r0 of row r0: one address register instead of sixteen precomputed ones (which the
@@ -1732,14 +1749,24 @@ __device__ __forceinline__ void chunk_to_smem(const float (&acc)[128], int c, ui
         const uint32_t addr = xor_u32(row_addr, j << 4);
         float2 bv = make_float2(0.0f, 0.0f);
         if (HAS_BIAS) bv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(bias + j * 8 + cq));
+        float2 bu = make_float2(0.0f, 0.0f);
+        if (HAS_BIAS && MODE == EPI_G0_SWIGLU)
+            bu = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(bias + glu + j * 8 + cq));
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             float f[2] = {acc[c * 32 + j * 4 + 2 * h], acc[c * 32 + j * 4 + 2 * h + 1]};
             if (HAS_BIAS) { f[0] += bv.x; f[1] += bv.y; }
+            float u[2] = {0.0f, 0.0f};
+            if (MODE == EPI_G0_SWIGLU) {
+                u[0] = acc[(c + 2) * 32 + j * 4 + 2 * h];
+                u[1] = acc[(c + 2) * 32 + j * 4 + 2 * h + 1];
+                if (HAS_BIAS) { u[0] += bu.x; u[1] += bu.y; }
+            }
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
                 if (MODE == EPI_G0_RELU) f[i] = fmaxf(f[i], 0.0f);                 // ReLU (types.cuh:151-159)
                 else if (MODE == EPI_G0_GELU) f[i] = gelu_erf(f[i]);
+                else if (MODE == EPI_G0_SWIGLU) f[i] = silu_mul(f[i], u[i]);
                 // the reference's combine arithmetic on the bf16-rounded y (processor.cuh:110-169):
                 // term = rne( p~ (x) rne( y / mCw ) ); the bf16 accumulation itself is the REDG in drain_accumulator
                 else if (MODE == EPI_G1_FUSED_ADD) f[i] = pw[h] * rne_bf16(__fdividef(rne_bf16(f[i]), mcw[h]));
@@ -1763,10 +1790,11 @@ __device__ __forceinline__ void chunk_to_smem(const float (&acc)[128], int c, ui
 // fence.proxy.async.global, and then red.release.gpu's g0_done; the scheduler's ld.acquire.gpu of g0_done plus the
 // producer's fence.proxy.async.global before its TMA loads of h complete the chain on the reading side.
 // Rows at or beyond the block's valid rows are staged and stored too: they lie in the packet's pEC padding of h, and
-// GEMM1 multiplies them row-independently and drops their results.
+// GEMM1 multiplies them row-independently and drops their results.  `glu`: EPI_G0_SWIGLU's up-bias offset.
 template <int MODE, bool HAS_BIAS>
 __device__ __forceinline__ void stage_h(const FmParams& p, uint8_t* smem, const float (&acc)[128],
-                                        const __nv_bfloat16* bias, int nchunks, int row0, int lane, uint32_t& chunk) {
+                                        const __nv_bfloat16* bias, int nchunks, int row0, int lane, uint32_t& chunk,
+                                        int glu = 0) {
     const float one[2] = {1.0f, 1.0f};
 #pragma unroll
     for (int c = 0; c < BLOCK_N / 64; ++c) {
@@ -1774,7 +1802,7 @@ __device__ __forceinline__ void stage_h(const FmParams& p, uint8_t* smem, const 
         const int b = chunk & 1;
         bar_wait(p, smem, BAR_STG_FREE + b, ((chunk >> 1) & 1) ^ 1);
         chunk_to_smem<MODE, HAS_BIAS>(acc, c, smem + OFF_EPI + b * EPI_CHUNK_BYTES + row0 * EPI_ROW_BYTES,
-                                      HAS_BIAS ? bias + c * 64 : nullptr, lane, one, one);
+                                      HAS_BIAS ? bias + c * 64 : nullptr, lane, one, one, glu);
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) mbar_arrive(bar(smem, BAR_STG_FULL + b));
@@ -1902,16 +1930,20 @@ __device__ __forceinline__ void with_bias(const __nv_bfloat16* bias, F&& f) {
 
 // GEMM0 epilogue: h.  Every warp stages its 16 rows of each 64-column chunk (N is a multiple of 64, not necessarily of
 // the tile width) and goes straight on to the next tile; the publisher warp stores and publishes them.
+// A SwiGLU tile whose gate half runs past n (P or Ps = 64 mod 128) has read 64 up rows into its gate half's last 64
+// accumulator columns and 64 rows of the flat-viewed W_down into its up half's: both lie inside the weight tensor, and
+// those columns are never stored (nchunks = 1), as with the rows past n of a 256-row box.
 __device__ __forceinline__ void epilogue_h(const FmParams& p, uint8_t* smem, const TileInfo* ti, float (&acc)[128], int prev,
                                            Consumer& c) {
-    const int n0 = ti->ntile * BLOCK_N, le = ti->le;
     const GemmOp& op = p.gemm[ti->gemm];
+    const int cols = tile_cols(op), n0 = ti->ntile * cols, le = ti->le;
     mainloop_done(p, smem, acc, prev, c);
-    const int nchunks = min(BLOCK_N / 64, (op.n - n0) / 64);
+    const int nchunks = min(cols / 64, (op.n - n0) / 64);
     const __nv_bfloat16* bias = op.bias ? op.bias + (size_t)le * op.bias_le + n0 : nullptr;
     with_bias(bias, [&](auto has_bias) {
         constexpr bool B = decltype(has_bias)::value;
-        if (p.act == 0) stage_h<EPI_G0_RELU, B>(p, smem, acc, bias, nchunks, c.row0, c.lane, c.chunk);
+        if (op.glu_rows) stage_h<EPI_G0_SWIGLU, B>(p, smem, acc, bias, nchunks, c.row0, c.lane, c.chunk, op.glu_rows);
+        else if (p.act == 0) stage_h<EPI_G0_RELU, B>(p, smem, acc, bias, nchunks, c.row0, c.lane, c.chunk);
         else stage_h<EPI_G0_GELU, B>(p, smem, acc, bias, nchunks, c.row0, c.lane, c.chunk);
     });
     if (c.stamper) trace_tile(p, TRACE_TILE_STORES, c.ntiles);
@@ -2010,7 +2042,7 @@ __device__ __forceinline__ void ffn_consumer(const FmParams& p, uint8_t* smem) {
 // consumers' staging order.
 __device__ __forceinline__ void publish_h(const FmParams& p, uint8_t* smem, const TileInfo& ti, uint32_t& chunk) {
     const GemmOp& op = p.gemm[ti.gemm];
-    const int n0 = ti.ntile * BLOCK_N, nchunks = min(BLOCK_N / 64, (op.n - n0) / 64);
+    const int cols = tile_cols(op), n0 = ti.ntile * cols, nchunks = min(cols / 64, (op.n - n0) / 64);
     const int row = ti.a_row;
     const CUtensorMap* map = &p.tm[p.gemm[ti.gemm + 1].a];   // h is its GEMM1's A
     unsigned int* ctr = op.done + (size_t)ti.pkt * op.done_pkt + ti.mblk;
@@ -2117,15 +2149,19 @@ __device__ __forceinline__ void ffn_setup(const FmParams& p, uint8_t* smem) {
 
 __device__ __forceinline__ void ffn_warm_l2(const FmParams& p, const Launch& L) {
     if (threadIdx.x == 3 * 32) {
-        // Warm L2 with the 256-row weight tile this CTA will most likely claim first (item id = CTA index: the first wave is
-        // claimed in arrival order), pipeline depth only: HBM is idle during the router and the first tile's loads are
-        // then L2 hits.  A wrong guess costs nothing -- the tile is needed by some CTA of the first wave anyway.
+        // Warm L2 with the 256-row weight tile (SwiGLU: its gate and up halves) this CTA will most likely claim first (item
+        // id = CTA index: the first wave is claimed in arrival order), pipeline depth only: HBM is idle during the router
+        // and the first tile's loads are then L2 hits.  A wrong guess costs nothing -- the tile is needed by some CTA of
+        // the first wave anyway.
         const int id = (int)blockIdx.x;
         if (id < L.total_items) {
             int cursor = 0;
             const WorkItem w = decode_item(p, L, id, cursor);
             const GemmOp& op = p.gemm[w.blk.gemm];
-            for (int kb = 0; kb < min(op.kblocks, STAGES); ++kb) tma_prefetch_l2_2d(&p.tm[op.b], kb * BLOCK_K, w.b_row);
+            for (int kb = 0; kb < min(op.kblocks, STAGES); ++kb) {
+                tma_prefetch_l2_2d(&p.tm[op.b], kb * BLOCK_K, w.b_row);
+                if (op.glu_rows) tma_prefetch_l2_2d(&p.tm[op.b], kb * BLOCK_K, w.b_row + op.glu_rows);
+            }
         }
     }
 }

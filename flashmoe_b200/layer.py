@@ -30,6 +30,12 @@ class FlashMoELayer(torch.nn.Module):
     Parameters are held in the reference's layouts: `gate_weight` [H, E] (consumed flat as [E, H]),
     `expert_weight` [nLx, 2, P, H] (this rank's experts), optional `bias_up` [nLx, P] / `bias_down` [nLx, H].
 
+    With `cfg.hidden_act = 2` (SwiGLU, y = W_down (silu(W_gate x) * (W_up x)), Mixtral / Qwen3-MoE / DeepSeek-V3 experts)
+    `expert_weight` is [nLx, 3, P, H]: [i,0] = W_gate, [i,1] = W_up, [i,2] flat-viewed as W_down [H, P]; from Hugging
+    Face tensors, once at load time, `torch.stack([w_gate, w_up, w_down.reshape(nLx, P, H)], 1)`.  `bias_up` is then
+    [nLx, 2, P] (gate, then up), `shared_weight` [3, Ps, H] and `shared_bias_up` [2, Ps].  h = silu(g) * u is computed
+    in fp32 and rounded to bf16 once (Hugging Face rounds W_gate x, silu and the product separately).
+
     `router`: a `RouterSpec` (sigmoid scores, group-limited top-k, no renormalisation, a route scale, ...) the kernel
     applies to the gate's logits instead of the built-in softmax / top-k / renormalise (`MoEContext.forward_gated`).
     `score_bias` (with a `router` only): hold an fp32 [E] selection bias, `score_bias` (Hugging Face's
@@ -58,10 +64,13 @@ class FlashMoELayer(torch.nn.Module):
         scale = cfg.H ** -0.5
         self.gate_weight = torch.nn.Parameter(torch.randn(cfg.H, cfg.E, device=dev).mul_(scale).bfloat16(),
                                               requires_grad=False)
-        self.expert_weight = torch.nn.Parameter(torch.randn(nlx, 2, cfg.P, cfg.H, device=dev).mul_(scale).bfloat16(),
+        m = cfg.expert_mats
+        up = (2,) if m == 3 else ()   # SwiGLU: a gate and an up bias
+        self.expert_weight = torch.nn.Parameter(torch.randn(nlx, m, cfg.P, cfg.H, device=dev).mul_(scale).bfloat16(),
                                                 requires_grad=False)
         if bias:
-            self.bias_up = torch.nn.Parameter(torch.zeros(nlx, cfg.P, device=dev, dtype=torch.bfloat16), requires_grad=False)
+            self.bias_up = torch.nn.Parameter(torch.zeros(nlx, *up, cfg.P, device=dev, dtype=torch.bfloat16),
+                                              requires_grad=False)
             self.bias_down = torch.nn.Parameter(torch.zeros(nlx, cfg.H, device=dev, dtype=torch.bfloat16), requires_grad=False)
         else:
             self.bias_up = None
@@ -71,10 +80,10 @@ class FlashMoELayer(torch.nn.Module):
         self.shared_inter = shared_inter
         self.shared_weight = self.shared_bias_up = self.shared_bias_down = None
         if shared_inter is not None:
-            self.shared_weight = torch.nn.Parameter(torch.randn(2, shared_inter, cfg.H, device=dev).mul_(scale).bfloat16(),
+            self.shared_weight = torch.nn.Parameter(torch.randn(m, shared_inter, cfg.H, device=dev).mul_(scale).bfloat16(),
                                                     requires_grad=False)
             if bias:
-                self.shared_bias_up = torch.nn.Parameter(torch.zeros(shared_inter, device=dev, dtype=torch.bfloat16),
+                self.shared_bias_up = torch.nn.Parameter(torch.zeros(*up, shared_inter, device=dev, dtype=torch.bfloat16),
                                                          requires_grad=False)
                 self.shared_bias_down = torch.nn.Parameter(torch.zeros(cfg.H, device=dev, dtype=torch.bfloat16),
                                                            requires_grad=False)
@@ -129,6 +138,6 @@ class FlashMoELayer(torch.nn.Module):
 
     def extra_repr(self) -> str:
         c = self.cfg
-        return (f"S={c.S}, H={c.H}, P={c.P}, E={c.E}, k={c.k}, act={'gelu' if c.hidden_act else 'relu'}, "
+        return (f"S={c.S}, H={c.H}, P={c.P}, E={c.E}, k={c.k}, act={('relu', 'gelu', 'swiglu')[c.hidden_act]}, "
                 f"rank={self.ctx.rank}/{self.ctx.world}"
                 + (f", shared_inter={self.shared_inter}" if self.shared_inter is not None else ""))

@@ -87,29 +87,35 @@ def _check_tensor(name: str, t: torch.Tensor, device: torch.device, dtype: torch
 class SharedExpert(NamedTuple):
     """A shared expert (fm_moe_forward_shared): a dense FFN every token passes through, its output added to the routed
     combine.  `w` bf16 [2, Ps, H] is one routed expert's layout ([0] = W_up [Ps, H], [1] flat-viewed as W_down [H, Ps]);
-    `bias_up` bf16 [Ps] and `bias_down` bf16 [H] are optional.  Ps is a multiple of 64.  Several shared experts of size P
+    `bias_up` bf16 [Ps] and `bias_down` bf16 [H] are optional.  Ps is a multiple of 64.  In a SwiGLU context
+    (hidden_act = 2) `w` is [3, Ps, H] (W_gate, W_up, W_down flat-viewed) and `bias_up` [2, Ps] (gate, then up).  Several shared experts of size P
     are one of size n_shared * P: concatenate their W_up rows and their W_down columns."""
     w: torch.Tensor
     bias_up: Optional[torch.Tensor] = None
     bias_down: Optional[torch.Tensor] = None
 
 
-def shared_expert_struct(se: SharedExpert, device: torch.device, H: int, reserved: Optional[int]) -> _lib.FmSharedExpert:
+def shared_expert_struct(se: SharedExpert, device: torch.device, H: int, reserved: Optional[int],
+                         swiglu: bool = False) -> _lib.FmSharedExpert:
     """Check a `SharedExpert` against a context on `device` with hidden size H and reserved intermediate size `reserved`
-    (None: not reserved), and return its fm_shared_expert_t.  The caller keeps the tensors alive."""
+    (None: not reserved), SwiGLU experts when `swiglu`, and return its fm_shared_expert_t.  The caller keeps the tensors
+    alive."""
     if not isinstance(se, SharedExpert):
         raise TypeError(f"shared_expert must be a SharedExpert, got {type(se).__name__}")
     if reserved is None:
         raise RuntimeError("this context has no shared-expert staging: create it with shared_inter=")
+    mats = "[3, Ps, H]" if swiglu else "[2, Ps, H]"
     if not isinstance(se.w, torch.Tensor) or se.w.dim() != 3:
-        raise RuntimeError(f"shared_expert.w must be a 3-D tensor [2, Ps, H], got {getattr(se.w, 'shape', se.w)}")
+        raise RuntimeError(f"shared_expert.w must be a 3-D tensor {mats}, got {getattr(se.w, 'shape', se.w)}")
     ps = int(se.w.shape[1])
-    _check_tensor("shared_expert.w", se.w, device, shape={"up/down": 2, "Ps": ps, "H": H})
+    _check_tensor("shared_expert.w", se.w, device,
+                  shape={"gate/up/down": 3, "Ps": ps, "H": H} if swiglu else {"up/down": 2, "Ps": ps, "H": H})
     if ps <= 0 or ps % 64:
         raise RuntimeError(f"shared_expert.w: Ps = {ps} must be a positive multiple of 64")
     if ps > reserved:
         raise RuntimeError(f"shared_expert.w: Ps = {ps} is above the context's shared_inter = {reserved}")
-    for name, b, dims in (("bias_up", se.bias_up, {"Ps": ps}), ("bias_down", se.bias_down, {"H": H})):
+    up_dims = {"gate/up": 2, "Ps": ps} if swiglu else {"Ps": ps}
+    for name, b, dims in (("bias_up", se.bias_up, up_dims), ("bias_down", se.bias_down, {"H": H})):
         if b is not None:
             _check_tensor(f"shared_expert.{name}", b, device, shape=dims)
     return _lib.FmSharedExpert(se.w.data_ptr(), se.bias_up.data_ptr() if se.bias_up is not None else None,
@@ -216,10 +222,13 @@ class MoEContext:
         s = expert_weights.shape
         if len(s) != 4 or s[0] != nlx:
             raise RuntimeError(f"Expert count mismatch. Expected {nlx} local experts, got {s[0]}")
-        if s[1] != 2:
-            raise RuntimeError("Expert weights must have up and down projections [nLx, 2, P, H]")
+        m = self.cfg.expert_mats
+        if s[1] != m:
+            raise RuntimeError("Expert weights must have up and down projections [nLx, 2, P, H]" if m == 2 else
+                               "SwiGLU expert weights must have gate, up and down projections [nLx, 3, P, H]; got "
+                               f"{s[1]} matrices per expert")
         if s[2] != d["P"] or s[3] != d["H"]:
-            raise RuntimeError(f"Expert weights must be [*, 2, P={d['P']}, H={d['H']}]. Got [*, 2, {s[2]}, {s[3]}]")
+            raise RuntimeError(f"Expert weights must be [*, {m}, P={d['P']}, H={d['H']}]. Got [*, {m}, {s[2]}, {s[3]}]")
 
     def _validate(self, input: torch.Tensor, gate_weights: Optional[torch.Tensor], expert_weights: torch.Tensor,
                   exact_s: bool = True) -> int:
@@ -256,9 +265,10 @@ class MoEContext:
     def _bias_ptrs(self, bias_up, bias_down):
         d = self.dims
         nlx = d["num_local_experts"]
-        for name, b, dim in (("bias_up", bias_up, "P"), ("bias_down", bias_down, "H")):
+        up = {"nLx": nlx, "gate/up": 2, "P": d["P"]} if self.cfg.expert_mats == 3 else {"nLx": nlx, "P": d["P"]}
+        for name, b, dims in (("bias_up", bias_up, up), ("bias_down", bias_down, {"nLx": nlx, "H": d["H"]})):
             if b is not None:
-                _check_tensor(name, b, self.device, shape={"nLx": nlx, dim: d[dim]})
+                _check_tensor(name, b, self.device, shape=dims)
         return (bias_up.data_ptr() if bias_up is not None else None,
                 bias_down.data_ptr() if bias_down is not None else None)
 
@@ -379,7 +389,8 @@ class MoEContext:
         return out
 
     def _shared(self, se: SharedExpert):
-        return ctypes.byref(shared_expert_struct(se, self.device, self.dims["H"], self.shared_inter))
+        return ctypes.byref(shared_expert_struct(se, self.device, self.dims["H"], self.shared_inter,
+                                                 swiglu=self.cfg.expert_mats == 3))
 
     def _launch(self, call, n: int, n_tokens: Optional[torch.Tensor], *rows: torch.Tensor) -> None:
         """The token-count convention of the forward calls: run `call(n_tokens_dev, *row pointers)`, where `rows` are

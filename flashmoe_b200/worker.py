@@ -27,7 +27,7 @@ def make_inputs(cfg: "_config.MoEConfig", nlx: int, rank: int, device, scaled: b
     gw = torch.Generator(device="cpu").manual_seed(0x5EED)
     x = torch.randn(cfg.mini_batch, cfg.sequence_len, cfg.H, generator=g)
     wg = torch.randn(cfg.H, cfg.E, generator=gw)
-    we = torch.randn(nlx, 2, cfg.P, cfg.H, generator=g)
+    we = torch.randn(nlx, cfg.expert_mats, cfg.P, cfg.H, generator=g)   # SwiGLU: [nLx, 3, P, H]
     if scaled:
         wg, we = wg * cfg.H ** -0.5, we * cfg.H ** -0.5
     return x.to(dtype).to(device), wg.to(dtype).to(device), we.to(dtype).to(device)

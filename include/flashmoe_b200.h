@@ -54,7 +54,7 @@ typedef struct fm_config {
     int32_t expert_top_k;
     int32_t global_batch;
     int32_t is_training;
-    int32_t hidden_act; /* 0 relu, 1 gelu */
+    int32_t hidden_act; /* 0 relu, 1 gelu, 2 swiglu (expert_w [nLx, 3, P, H]) */
     int32_t hidden_size;
     int32_t intermediate_size;
     int32_t mini_batch;
@@ -108,6 +108,14 @@ FM_API int fm_symm_use_external(fm_ctx_t* ctx, void* base, size_t bytes);
  *   expert_w     [nLx, 2, P, H]             [i,0] = W_up [P,H]; [i,1] flat-viewed as W_down [H,P] (:104-119)
  *   bias_up      [nLx, P] or NULL (zero)    bias_down [nLx, H] or NULL (zero)        (moe.cuh:117-124)
  *   out          [S, H]                     written in full
+ * With hidden_act = 2 (SwiGLU, y = W_down (silu(W_gate x + b_g) * (W_up x + b_u)) + b_down):
+ *   expert_w     [nLx, 3, P, H]             [i,0] = W_gate [P,H]; [i,1] = W_up [P,H]; [i,2] flat-viewed as W_down [H,P]
+ *                                           (per expert vLLM's w13, gate then up, followed by w2).  From Hugging Face
+ *                                           tensors, once at load time: torch.stack([w_gate, w_up,
+ *                                           w_down.reshape(nLx, P, H)], 1)
+ *   bias_up      [nLx, 2, P] or NULL        [i,0] = gate bias, [i,1] = up bias
+ *   h = rne_bf16(fl(fl(g * sigmoid(g)) * u)), g = fl(W_gate x + b_g), u = fl(W_up x + b_u), all in fp32 with the one
+ *   final rounding (Hugging Face rounds W_gate x, silu and the product to bf16 separately; this does not).
  * Enqueues one fused persistent kernel on `stream` (cudaStream_t); collective across the world: every rank must
  * call it the same number of times.  Does not synchronise. */
 FM_API int fm_moe_forward(fm_ctx_t* ctx, const void* x, const void* gate_w, const void* expert_w,
@@ -202,6 +210,7 @@ FM_API int fm_moe_forward_gated(fm_ctx_t* ctx, const void* x, int n_tokens, cons
  *              same Ps*H block flat-viewed as W_down [H, Ps]
  *   bias_up    bf16 [Ps] or NULL (zero)     bias_down  bf16 [H] or NULL (zero)
  *   inter      Ps, a positive multiple of 64, at most the context's reserved size (fm_shared_reserve)
+ * In a hidden_act = 2 (SwiGLU) context w is [3, Ps, H] (W_gate, W_up, W_down flat-viewed) and bias_up [2, Ps].
  * For every token t < n: s[t] = the bf16 output of that FFN on x[t], with a routed expert's arithmetic (GEMM0 + bias_up ->
  * the context's hidden_act -> bf16 h -> GEMM1 + bias_down -> one bf16 RNE), and
  *   out[t] = rne_bf16(fl32(r[t]) + fl32(s[t]))   (the sum in fp32, then one RNE)
@@ -213,7 +222,7 @@ FM_API int fm_moe_forward_gated(fm_ctx_t* ctx, const void* x, int n_tokens, cons
  * and, with is_training = 1, FM_BUF_AUX_LOSS -- is exactly the call without a shared expert.  The shared tiles run in the
  * same persistent kernel as the routed ones: they need only x, so they fill the time the routed rows take to arrive. */
 typedef struct fm_shared_expert {
-    const void* w;          /* bf16 [2, Ps, H] */
+    const void* w;          /* bf16 [2, Ps, H]; SwiGLU: [3, Ps, H] */
     const void* bias_up;    /* bf16 [Ps] or NULL */
     const void* bias_down;  /* bf16 [H] or NULL */
     int32_t inter;          /* Ps */
@@ -300,7 +309,7 @@ enum fm_buffer {
                             for a -1 pick */
     FM_BUF_COUNTS = 4,   /* int32 [E]     selections per expert on this rank (incl. dropped) */
     FM_BUF_RECV_X = 5,   /* bf16  [W, nLx, pEC, H]  dispatched rows received by this rank */
-    FM_BUF_HIDDEN = 6,   /* bf16  [W, nLx, pEC, P]  h = act(x W_up^T + b) staging */
+    FM_BUF_HIDDEN = 6,   /* bf16  [W, nLx, pEC, P]  h = act(x W_up^T + b) staging; SwiGLU: h = silu(g)*u */
     FM_BUF_RET_Y = 7,    /* bf16  [E, pEC, H]       expert outputs returned to this rank */
     FM_BUF_GATE_OUT = 8, /* bf16  [S, E]  full softmax row (reference gateOut[S,PX] without the padding columns); not
                             written by a routed launch; gated: rne_bf16(s), the full unbiased score row */

@@ -1,0 +1,219 @@
+"""The exact-input reference (tests/exact.py) for SwiGLU experts (hidden_act = 2).
+
+An expert's weights are [3, P, H]: W_gate, W_up and the P*H block flat-viewed as W_down [H, P].  The kernel computes
+g = fl(x W_gate^T + b_g), u = fl(x W_up^T + b_u) (both exact here: the inputs keep every partial sum exact in fp32) and
+h = rne_bf16(fl(fl(g * sigma(g)) * u)) with sigma(g) = rcp_rn(fl(1 + ex2.approx.ftz(fl(-g * fl32(log2 e))))).
+
+Error bound of h against the real g * sigmoid(g) * u, relative, first order (eps_swiglu):
+  fl32(log2 e) is log2 e (1 + d0), |d0| < 2^-26, and the product rounds once (2^-24): the exponent a = -g log2 e is off
+  by at most |a| (2^-24 + 2^-26), which moves 2^a by ln 2 * |a| * 1.25 * 2^-24 = 1.25 * |g| * 2^-24 relative;
+  ex2.approx.ftz: 2^-21 (exact.EPS_EX2); 1 + e rounds once (2^-24) and does not amplify e's relative error (e >= 0);
+  the reciprocal rounds once (2^-24); g * sigma and the product with u round once each (2 * 2^-24).
+  Total 2^-21 + 2^-24 * (1.25 |g| + 4); one more 2^-24 covers the second-order terms: eps = 2^-21 + 2^-24 (1.25|g| + 5).
+The final fp32 -> bf16 RNE is monotone, so h lies in [rne(v (1 - eps)), rne(v (1 + eps))] for the real v.  With
+g >= -64 (the generator's range) every intermediate is a normal fp32 number, so ex2's flush to zero never applies; for
+g <= -100 the power overflows, sigma is +0 and h is a zero, which the interval (of a value far below bf16's smallest
+subnormal) also gives.
+
+GEMM1 is exact given the device's own h (exact.gemm1_reference): the generator keeps |h| in [2^-4, 2^6] and W_down
+sparse, so y's sums stay on one fp32 grid.  No pytest in here.
+"""
+from __future__ import annotations
+
+import dataclasses
+from typing import Optional
+
+import numpy as np
+import torch
+
+from flashmoe_b200.config import MoEConfig
+from tests import exact as ex
+from tests import exact_routed as er
+
+G_MIN = -64.0   # the generator keeps every gate pre-activation at or above this
+
+
+def eps_swiglu(g: np.ndarray) -> np.ndarray:
+    """Relative error bound of the kernel's h = silu(g) * u (module docstring)."""
+    return 2.0 ** -21 + 2.0 ** -24 * (1.25 * np.abs(g) + 5.0)
+
+
+def swiglu_reference(rows: np.ndarray, w_gate: np.ndarray, w_up: np.ndarray, b_gate: Optional[np.ndarray],
+                     b_up: Optional[np.ndarray], what: str = "SwiGLU GEMM0") -> ex.Rounded:
+    """h [M, P] = RNE(silu(rows W_gate^T + b_g) * (rows W_up^T + b_u)) as an interval (float64 rows [M, H], weights
+    [P, H], biases [P] or None).  `exact` is the real value."""
+    ex.assert_exact_sums(rows, w_gate, b_gate, f"{what} (gate)")
+    ex.assert_exact_sums(rows, w_up, b_up, f"{what} (up)")
+    g = rows @ w_gate.T
+    u = rows @ w_up.T
+    if b_gate is not None:
+        g = g + b_gate[None, :]
+    if b_up is not None:
+        u = u + b_up[None, :]
+    with np.errstate(over="ignore"):
+        v = g / (1.0 + np.exp(-g)) * u
+    e = eps_swiglu(g)
+    a, b = ex.f64_to_bf16(v * (1 - e)), ex.f64_to_bf16(v * (1 + e))
+    swap = ex.order_key(a) > ex.order_key(b)
+    return ex.Rounded(np.where(swap, b, a), np.where(swap, a, b), v)
+
+
+# ----------------------------------------------------------------------------- inputs
+@dataclasses.dataclass
+class SwigluInputs:
+    """Exact SwiGLU inputs: the router's x and gate weights from exact.exact_inputs (x in {-1, 0, 1}), expert weights
+    we bf16 [E, 3, P, H], biases bu [E, 2, P] / bd [E, H] or None (CPU tensors)."""
+    base: ex.ExactInputs
+    we: torch.Tensor
+    bu: Optional[torch.Tensor]
+    bd: Optional[torch.Tensor]
+
+    @property
+    def cfg(self) -> MoEConfig:
+        return self.base.cfg
+
+    @property
+    def x64(self) -> np.ndarray:
+        return self.base.x64
+
+    def gate_up64(self, e: int):
+        w = self.we[e].double().numpy()
+        b = None if self.bu is None else self.bu[e].double().numpy()
+        return w[0], w[1], None if b is None else b[0], None if b is None else b[1]
+
+    def w_down64(self, e: int) -> np.ndarray:   # [H, P]: block 2 viewed flat
+        H, P = self.cfg.H, self.cfg.P
+        return self.we[e, 2].reshape(-1).reshape(H, P).double().numpy()
+
+    def bd64(self, e: int) -> Optional[np.ndarray]:
+        return None if self.bd is None else self.bd[e].double().numpy()
+
+    def device(self, dev):
+        return tuple(None if t is None else t.to(dev) for t in (self.base.x, self.base.wg, self.we, self.bu, self.bd))
+
+
+def _bf(a: np.ndarray) -> torch.Tensor:
+    t = torch.from_numpy(np.ascontiguousarray(a)).bfloat16()
+    assert np.array_equal(t.double().numpy(), a), "generator produced a value that is not a bf16 number"
+    return t
+
+
+def swiglu_weights(E: int, P: int, H: int, rng: np.random.Generator, bias: bool, gate_nz: int = 3, up_nz: int = 2,
+                   down_nz: int = 8):
+    """(we [E, 3, P, H], bu [E, 2, P] or None, bd [E, H] or None) as float64 arrays for x in {-1, 0, 1}: W_gate rows
+    with gate_nz entries in {-1, -1/2, 1/2, 1}, b_g in {-1, ..., 1} on 1/2 (so g in [-4, 4] on a grid of 1/2:
+    silu(g) is 0 or at least 0.07 in magnitude); W_up rows with up_nz integers in [-4, 4], b_u integers in [-2, 2]
+    (u an integer, |u| <= 4 up_nz + 2); W_down on 2^-5 with about down_nz nonzeros per output column."""
+    def sparse_rows(nz, vals):
+        w = np.zeros((E, P, H))
+        for e in range(E):
+            for p in range(P):
+                cols = rng.choice(H, size=nz, replace=False)
+                w[e, p, cols] = rng.choice(vals, size=nz)
+        return w
+
+    gate = sparse_rows(gate_nz, np.array([-1.0, -0.5, 0.5, 1.0]))
+    up = sparse_rows(up_nz, np.array([v for v in range(-4, 5) if v]).astype(np.float64))
+    down = (rng.integers(-4, 5, size=(E, H, P)) * (rng.random((E, H, P)) < down_nz / P)) * 2.0 ** ex.WDOWN_GRID
+    we = np.stack([gate, up, down.reshape(E, -1).reshape(E, P, H)], axis=1)
+    bu = bd = None
+    if bias:
+        bu = np.stack([rng.integers(-2, 3, size=(E, P)) * 0.5, rng.integers(-2, 3, size=(E, P)).astype(np.float64)], 1)
+        bd = rng.integers(-64, 65, size=(E, H)) * 2.0 ** -8
+    return we, bu, bd
+
+
+def swiglu_inputs(cfg: MoEConfig, seed: int, bias: bool = False, **router_kw) -> SwigluInputs:
+    """Seeded exact inputs for a hidden_act = 2 context `cfg`; `router_kw` goes to exact.exact_inputs (the x and gate
+    weights)."""
+    assert cfg.hidden_act == 2
+    base = ex.exact_inputs(cfg, seed, x_range=1, **router_kw)
+    we, bu, bd = swiglu_weights(cfg.E, cfg.P, cfg.H, np.random.default_rng(seed + 1), bias)
+    return SwigluInputs(base, _bf(we), None if bu is None else _bf(bu), None if bd is None else _bf(bd))
+
+
+def expert_h(inp: SwigluInputs, e: int, rows64: np.ndarray, what: str) -> ex.Rounded:
+    wg_, wu, bg, bu = inp.gate_up64(e)
+    g = rows64 @ wg_.T + (0 if bg is None else bg[None, :])
+    assert (g >= G_MIN).all(), f"{what}: a gate pre-activation is below {G_MIN}"
+    return swiglu_reference(rows64, wg_, wu, bg, bu, what)
+
+
+# ----------------------------------------------------------------------------- the launch's stages
+def check_experts(inp: SwigluInputs, dev: ex.Device, EC: int, n: int, stats: Optional[ex.Stats] = None,
+                  shared_s: Optional[np.ndarray] = None, unscaled_k1: bool = True) -> ex.Stats:
+    """Every stage after routing of one launch over the first n tokens, given the device's routing (topk_idx, topk_w,
+    mcw; the router itself is exact.check_forward's, and tests/test_gpu_swiglu.py shows it equals a ReLU context's):
+    slot / counts / recv_cnt from topk_idx, recv_x, h inside its interval, ret_y bit for bit from the device's h, and
+    out from the combine of those y (plus s rows when `shared_s`).  `unscaled_k1`: the router route's k = 1 copy;
+    caller and gated routes scale k = 1 by topk_w over mcw = 1."""
+    cfg = inp.cfg
+    E, k, H = cfg.E, cfg.k, cfg.H
+    st = stats if stats is not None else ex.Stats()
+    x = inp.x64[:n]
+    slot, counts, recv_cnt, kept = er.slots_from_routing(dev.topk_idx, E, EC)   # (a caller's -1 picks take no slot)
+    ex.check_equal(dev.slot, slot, "slot", ("token", "pick"))
+    ex.check_equal(dev.counts, counts, "counts", ("expert",))
+    if dev.recv_cnt is not None:
+        ex.check_equal(dev.recv_cnt, recv_cnt, "recv_cnt", ("expert",))
+    toks = ex.packet_tokens(dev.topk_idx, slot, E, EC)
+    xb = ex.f64_to_bf16(x)
+    y_dev_ref = np.zeros((E, max(1, int(recv_cnt.max(initial=0))), H), np.uint16)
+    for e in range(E):
+        c = len(toks[e])
+        if c == 0:
+            continue
+        if dev.recv_x is not None:
+            ex.check_equal(dev.recv_x[e, :c], xb[toks[e]], f"recv_x of expert {e}", ("slot", "column"))
+        h_ref = expert_h(inp, e, x[toks[e]], f"GEMM0 of expert {e}")
+        h_dev = dev.hidden[e, :c]
+        w = ex._interval_check(h_dev, h_ref, f"hidden of expert {e}", ("slot", "column"))
+        st.add("hidden", h_dev.size, ex.rounded_count(h_ref), w)
+        y_ref = ex.gemm1_reference(h_dev, inp.w_down64(e), inp.bd64(e), f"GEMM1 of expert {e}")
+        y_dev_ref[e, :c] = y_ref.lo
+        if dev.ret_y is not None:
+            ex.check_equal(dev.ret_y[e, :c], y_ref.lo, f"ret_y of expert {e}", ("slot", "column"), signed_zero=False)
+            st.add("ret_y", c * H, ex.rounded_count(y_ref))
+    y_of = y_dev_ref[dev.topk_idx, np.where(kept, slot, 0)]
+    kk, pw = kept, dev.topk_w
+    if k == 1 and not unscaled_k1:   # the scaled sum of combine_tokens' k >= 2 path, of one term and one never-kept pad
+        def pad(a):
+            return np.concatenate([a, np.zeros_like(a[:, :1])], 1)
+        y_of, kk, pw = pad(y_of), pad(kept), pad(pw)
+    out_ref = ex.combine_tokens(y_of, kk, pw, dev.mcw)
+    dropped = ~kept.any(axis=1)
+    empty, what = np.zeros((int(dropped.sum()), H), np.uint16), "out"
+    if shared_s is not None:
+        out_ref, what = ex.add_shared(out_ref, shared_s), "out = rne(r + s)"
+        empty = ex.add_shared(ex.Rounded(empty, empty, 0), shared_s[dropped]).lo
+    w = ex._interval_check(dev.out, out_ref, what, ("token", "column"), max_width=None)
+    st.add(what, dev.out.size, ex.rounded_count(out_ref), w)
+    if dropped.any():
+        ex.check_equal(dev.out[dropped], empty, f"{what} rows of tokens whose picks were all dropped",
+                       ("row", "column"), signed_zero=shared_s is None)
+    return st
+
+
+# ----------------------------------------------------------------------------- the shared expert
+@dataclasses.dataclass
+class SharedSwiglu:
+    """A SwiGLU shared expert: w bf16 [3, Ps, H], bu [2, Ps] / bd [H] or None."""
+    w: torch.Tensor
+    bu: Optional[torch.Tensor]
+    bd: Optional[torch.Tensor]
+
+
+def shared_swiglu(H: int, Ps: int, seed: int, bias: bool = False) -> SharedSwiglu:
+    we, bu, bd = swiglu_weights(1, Ps, H, np.random.default_rng(seed), bias)
+    return SharedSwiglu(_bf(we[0]), None if bu is None else _bf(bu[0]), None if bd is None else _bf(bd[0]))
+
+
+def shared_reference(sh: SharedSwiglu, x64: np.ndarray, h_dev: np.ndarray, what: str = "shared expert"):
+    """(h_s interval [n, Ps], y_s from the device's h_s [n, H], exact) for tokens x64 [n, H]."""
+    H, Ps = sh.w.shape[2], sh.w.shape[1]
+    w = sh.w.double().numpy()
+    b = None if sh.bu is None else sh.bu.double().numpy()
+    h = swiglu_reference(x64, w[0], w[1], None if b is None else b[0], None if b is None else b[1], f"{what} GEMM0")
+    y = ex.gemm1_reference(h_dev, w[2].reshape(-1).reshape(H, Ps), None if sh.bd is None else sh.bd.double().numpy(),
+                           f"{what} GEMM1")
+    return h, y
