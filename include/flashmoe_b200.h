@@ -181,7 +181,8 @@ typedef struct fm_router {
  * the router's logits l (the same GEMV / tensor-core product as fm_moe_forward_tokens), then per token t
  *   1. scores s_e: scoring 0 = the router's softmax probability (the bits of gate_out of an fm_moe_forward_tokens
  *      launch); scoring 1 = sigmoid, computed as __frcp_rn(1 + ex2.approx.ftz(fl(-l * log2e))), relative error at most
- *      2^-21 + 2^-24 * (|l| + 2) against 1 / (1 + e^-l);
+ *      2^-21 + 2^-24 * (1.25 |l| + 2) against 1 / (1 + e^-l) while the score is normal; exactly 1.0 for l >= 17.34,
+ *      subnormal for l in about [-88.7, -87.4], +0 from l = -88.73 (the power overflows);
  *   2. choice values c_e = fl(s_e + score_bias[e]) (c = s without a bias); the bias steers selection only;
  *   3. n_group > 1: group score G_g = the largest c of the group (group_top 1) or fl(largest + second largest)
  *      (group_top 2); the topk_group groups with the largest G are kept, the experts of the others cannot be picked

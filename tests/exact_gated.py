@@ -133,11 +133,34 @@ class LayerInputs:
 
 
 # ----------------------------------------------------------------------------- gated routing reference
+SAT_A = -25.0   # power arguments at or below this give a score of exactly 1.0
+
+
 def sigmoid_bounds(logits):
-    """Interval of the kernel's sigmoid (flashmoe_b200.h): relative 2^-21 + 2^-24 (|l| + 2), with a margin."""
-    s = 1.0 / (1.0 + np.exp(-logits))
-    eps = 2.0 ** -21 + 2.0 ** -24 * (np.abs(logits) * 1.01 + 3)
-    return s * (1 - eps), s * (1 + eps), s
+    """Interval (lo, hi, mid) of the kernel's sigmoid_score(l) = rcp_rn(fl(1 + ex2.approx.ftz(a))), a = fl(-l log2e),
+    for exact fp32 logits; lo == hi where the device value is known exactly.
+      a <= SAT_A (l >= 17.33; on the 2^-6 logit grid l >= 17.34): the power is at most 2^-25 (1 + 2^-21) < 2^-24, half
+        an ulp of 1, so 1 + p rounds to 1 and the score is exactly 1.0 -- every such expert ties;
+      a > exact.NORMAL_A (l below about -86.6): the kernel's steps from ex2's ends (exact.sigmoid_f32_ends): a
+        subnormal score for a in (126, 128), exactly +0 once the power overflows (a >= 128, l <= -88.73);
+      elsewhere relative 2^-21 + 2^-24 (1.25 |l| + 3) (flashmoe_b200.h): ex2's 2^-21, the rounded argument (|l| 2^-24),
+        fl32(log2 e)'s own error (under 2^-26, so |l| 2^-26), the sum and the reciprocal, and one 2^-24 for the
+        second-order terms.  (Without the constant's error the bound is exceeded near |l| = 50 when ex2 errs by its
+        full 2^-21; tests/test_exact_tails.py emulates that.)"""
+    logits = np.asarray(logits, dtype=np.float64)
+    with np.errstate(over="ignore"):
+        s = 1.0 / (1.0 + np.exp(-logits))
+    eps = 2.0 ** -21 + 2.0 ** -24 * (1.25 * np.abs(logits) + 3)
+    lo, hi, mid = s * (1 - eps), s * (1 + eps), s.copy()
+    a = (-logits * float(ex.LOG2E_F32)).astype(np.float32).astype(np.float64)
+    sat = a <= SAT_A
+    lo[sat] = hi[sat] = mid[sat] = 1.0
+    tail = a > ex.NORMAL_A
+    if tail.any():
+        t_lo, t_hi = ex.sigmoid_f32_ends(a[tail])
+        lo[tail], hi[tail] = t_lo, t_hi
+        mid[tail] = np.where(t_lo == t_hi, t_lo, s[tail])
+    return lo, hi, mid
 
 
 @dataclasses.dataclass
@@ -158,16 +181,51 @@ def scores(router, k, x, wg_eff) -> Scores:
     return Scores(lo, hi, mid, ex.f64_to_bf16(lo), ex.f64_to_bf16(hi))
 
 
-def _group_scores(c, router):
-    """[n, n_group] group scores of the selection values c [n, E]: the largest, or the sum of the two largest."""
+def _group_scores(c, router, f32=False):
+    """[n, n_group] group scores of the selection values c [n, E]: the largest, or the sum of the two largest (rounded
+    to fp32 as the kernel does with `f32`, for exact c)."""
     n, E = c.shape
     g = -np.sort(-c.reshape(n, router.n_group, E // router.n_group), axis=2)
-    return g[:, :, 0] if router.group_top == 1 else g[:, :, 0] + g[:, :, 1]
+    if router.group_top == 1:
+        return g[:, :, 0]
+    s = g[:, :, 0] + g[:, :, 1]
+    return s.astype(np.float32).astype(np.float64) if f32 else s
 
 
-def kept_groups(c, router):
-    """bool [n, n_group]: the topk_group groups of the largest group score, the lower group on equal scores."""
-    G = _group_scores(np.atleast_2d(c), router)
+@dataclasses.dataclass
+class Selection:
+    """The selection values c = fl(s + b) [n, E] as intervals, and where they are known exactly (an exact score:
+    saturated at 1.0, +0, or a flushed softmax probability; fl(s + b) of exact fp32 operands is then exact too)."""
+    lo: np.ndarray
+    hi: np.ndarray
+    mid: np.ndarray
+    exact: np.ndarray
+
+
+def selection(sc: "Scores", bias, E: int) -> Selection:
+    bv = np.zeros(E) if bias is None else np.asarray(bias, dtype=np.float64)
+    m = 2.0 ** -23 * (np.abs(sc.s_hi) + np.abs(bv)) + 1e-300        # the fp32 rounding of s + b
+    exact = sc.s_lo == sc.s_hi
+    c_ex = (sc.s_lo.astype(np.float32) + bv.astype(np.float32)).astype(np.float32).astype(np.float64)
+    lo = ex.f32_up(np.where(exact, c_ex, sc.s_lo + bv - m)).astype(np.float64)   # (the device's c is an fp32 number)
+    hi = ex.f32_down(np.where(exact, c_ex, sc.s_hi + bv + m)).astype(np.float64)
+    return Selection(lo, hi, np.where(exact, c_ex, sc.s_mid + bv), exact)
+
+
+def group_scores(sel: Selection, router):
+    """(G_lo, G_hi, G_mid, exact) [n, n_group]: bounds of the device's group scores and where they are one value.  The
+    largest c, or the sum of the two largest, is increasing in every c, and the kernel's fp32 sum rounds monotonically,
+    so the kernel's sum of the bounds' two largest bounds it (a float64 sum of two fp32 numbers rounds to fp32 as
+    their exact sum does); equal bounds give the device's value exactly (fl(1 + 1) = 2, or fl(1 + 2^-93) = 1)."""
+    G_lo, G_hi = _group_scores(sel.lo, router, f32=True), _group_scores(sel.hi, router, f32=True)
+    ex_g = G_lo == G_hi
+    return G_lo, G_hi, np.where(ex_g, G_lo, _group_scores(sel.mid, router)), ex_g
+
+
+def kept_groups(c, router, G=None):
+    """bool [n, n_group]: the topk_group groups of the largest group score (of c, or the scores G), the lower group
+    on equal scores."""
+    G = _group_scores(np.atleast_2d(c), router) if G is None else G
     rows = np.arange(G.shape[0])
     kept = np.zeros(G.shape, bool)
     for _ in range(router.topk_group):
@@ -175,12 +233,12 @@ def kept_groups(c, router):
     return kept
 
 
-def route_mid(c, router, k):
+def route_mid(c, router, k, G=None):
     """The reference's picks [n, k] on the selection values c [n, E] (interval midpoints): larger c first, the lower
-    index on equal values, only experts of the kept groups."""
+    index on equal values, only experts of the kept groups (of the group scores G when given)."""
     c = np.atleast_2d(c)
     if router.n_group > 1:
-        allowed = np.repeat(kept_groups(c, router), c.shape[1] // router.n_group, axis=1)
+        allowed = np.repeat(kept_groups(c, router, G), c.shape[1] // router.n_group, axis=1)
         c = np.where(allowed, c, -np.inf)
     return np.argsort(-c, axis=1, kind="stable")[:, :k].astype(np.int32)
 
@@ -199,7 +257,10 @@ def weights_bounds(sc: Scores, picks, router):
 
 def check_gated_routing(logits, bias, router, k, dev_idx, dev_go, dev_w, wg_x):
     """`logits` [n, E] are the exact logits x . Wg_eff^T of wg_x = (x, Wg_eff); they serve only to recognise exact ties
-    (equal logits and equal bias give identical device values), the score intervals come from wg_x.
+    (equal logits and equal bias give identical device values), the score intervals come from wg_x.  Selection values
+    known exactly (a saturated 1.0 or +0 score plus the bias, rounded as the kernel rounds fl(s + b)) that are equal
+    are identical device values too, and so are equal exact group scores: the kernel's strict '>' then decides by the
+    lower index or the lower group, and such a token is decided, not ambiguous.
     gate_out inside its interval; every decided token's picks equal the reference's and its weights lie inside
     their interval; returns the number of ambiguous tokens.  A failure names the stage (gate_out, topk_idx or topk_w),
     the first failing token and pick, and the experts involved."""
@@ -215,23 +276,32 @@ def check_gated_routing(logits, bias, router, k, dev_idx, dev_go, dev_w, wg_x):
                              f"{t}, expert {e}: device {ex._fmt(dev_go[t, e])}, reference "
                              f"[{ex._fmt(sc.go_lo[t, e])}, {ex._fmt(sc.go_hi[t, e])}]")
     bv = np.zeros(E) if bias is None else np.asarray(bias, dtype=np.float64)
-    m = 2.0 ** -23 * (np.abs(sc.s_hi) + np.abs(bv)) + 1e-300        # the fp32 rounding of s + b
-    c_lo, c_hi, c_mid = sc.s_lo + bv - m, sc.s_hi + bv + m, sc.s_mid + bv
-    picks = route_mid(c_mid, router, k)
+    sel = selection(sc, bias, E)
+    c_lo, c_hi, c_mid = sel.lo, sel.hi, sel.mid
+    G = group_scores(sel, router) if router.n_group > 1 else None
+    picks = route_mid(c_mid, router, k, None if G is None else G[2])
     rows = np.arange(n)
     decided = np.ones(n, bool)
     allowed = np.ones((n, E), bool)
-    if router.n_group > 1:   # the kept groups must be certain: every kept group's score above every other group's
-        kept = kept_groups(c_mid, router)
-        G_lo, G_hi = _group_scores(c_lo, router), _group_scores(c_hi, router)
-        G_lo, G_hi = G_lo - 2.0 ** -23 * np.abs(G_lo), G_hi + 2.0 ** -23 * np.abs(G_hi)   # (the sum's rounding)
-        lo_kept = np.where(kept, G_lo, np.inf).min(1)
-        hi_other = np.where(kept, -np.inf, G_hi).max(1)
-        decided &= lo_kept > hi_other
+    if router.n_group > 1:   # the kept groups must be certain: every kept group's score above every other group's, or
+        G_lo, G_hi, G_mid, G_ex = G   # identical to it (known exactly, or of the same inputs) and the lower group
+        kept = kept_groups(c_mid, router, G_mid)
+        gi = np.arange(router.n_group)
+        GS = E // router.n_group   # groups whose (logit, bias) pairs are the same multiset have identical scores
+        order = np.lexsort((np.broadcast_to(bv.reshape(router.n_group, GS), (n, router.n_group, GS)),
+                            logits.reshape(n, router.n_group, GS)), axis=-1)
+        Ls = np.take_along_axis(logits.reshape(n, router.n_group, GS), order, -1)
+        Bs = np.take_along_axis(np.broadcast_to(bv.reshape(router.n_group, GS), Ls.shape), order, -1)
+        same = ((Ls[:, :, None] == Ls[:, None, :]) & (Bs[:, :, None] == Bs[:, None, :])).all(-1)
+        same |= G_ex[:, :, None] & G_ex[:, None, :] & (G_mid[:, :, None] == G_mid[:, None, :])
+        tie = same & (gi[:, None] < gi[None, :])
+        first = (G_lo[:, :, None] > G_hi[:, None, :]) | tie   # [n, g, h]: group g certainly ranks before group h
+        decided &= (first | ~(kept[:, :, None] & ~kept[:, None, :])).all(axis=(1, 2))
         allowed = np.repeat(kept, E // router.n_group, axis=1)
 
     def precedes(r, a, b):   # the device's c[r, a] certainly ranks before c[r, b]: disjoint intervals, or identical
-        same = (logits[r, a] == logits[r, b]) & (bv[a] == bv[b])   # inputs (identical device values) with a < b
+        same = (logits[r, a] == logits[r, b]) & (bv[a] == bv[b])   # inputs (identical device values) or c values
+        same |= sel.exact[r, a] & sel.exact[r, b] & (c_mid[r, a] == c_mid[r, b])   # known exactly, with a < b
         return (c_lo[r, a] > c_hi[r, b]) | (same & (a < b))
 
     for j in range(k - 1):
@@ -306,8 +376,9 @@ def reference_device_gated(inp: ex.ExactInputs, router, bias, EC: int, n: Option
     cfg = inp.cfg
     x = inp.x64[: (cfg.S if n is None else n)]
     sc = scores(router, cfg.k, x, inp.wg_eff64)
-    b = np.zeros(cfg.E) if bias is None else np.asarray(bias, dtype=np.float64)
-    picks = route_mid(sc.s_mid + b, router, cfg.k) if x.shape[0] else np.zeros((0, cfg.k), np.int32)
+    sel = selection(sc, bias, cfg.E)
+    G = group_scores(sel, router)[2] if router.n_group > 1 and x.shape[0] else None
+    picks = route_mid(sel.mid, router, cfg.k, G) if x.shape[0] else np.zeros((0, cfg.k), np.int32)
     w_lo, w_hi = weights_bounds(sc, picks, router)
     dev = routed_device(inp, picks, (0.5 * (w_lo + w_hi)).astype(np.float32), EC, stats)
     dev.gate_out = ex.f64_to_bf16(sc.s_mid)

@@ -10,10 +10,15 @@ Error bound of h against the real g * sigmoid(g) * u, relative, first order (eps
   ex2.approx.ftz: 2^-21 (exact.EPS_EX2); 1 + e rounds once (2^-24) and does not amplify e's relative error (e >= 0);
   the reciprocal rounds once (2^-24); g * sigma and the product with u round once each (2 * 2^-24).
   Total 2^-21 + 2^-24 * (1.25 |g| + 4); one more 2^-24 covers the second-order terms: eps = 2^-21 + 2^-24 (1.25|g| + 5).
-The final fp32 -> bf16 RNE is monotone, so h lies in [rne(v (1 - eps)), rne(v (1 + eps))] for the real v.  With
-g >= -64 (the generator's range) every intermediate is a normal fp32 number, so ex2's flush to zero never applies; for
-g <= -100 the power overflows, sigma is +0 and h is a zero, which the interval (of a value far below bf16's smallest
-subnormal) also gives.
+The final fp32 -> bf16 RNE is monotone, so h lies in [rne(v (1 - eps)), rne(v (1 + eps))] for the real v.  That holds
+while sigma is a normal fp32 number: the power argument a = fl(-g log2e) <= 125 (g >= -86.6).  For large positive g
+the power flushes to +0 and sigma is exactly 1, inside the bound.  Below that the relative bound is false:
+  - a in (126, 128), g in about [-88.7, -87.4]: 1 + 2^a > 2^126 and the correctly rounded reciprocal is subnormal,
+    kept as such (no -ftz), with an absolute 2^-150 error;
+  - a >= 128, g below about -88.72: ex2.approx returns +inf, sigma is +0 and h is exactly +-0, although the real
+    g sigmoid(g) u still rounds to a nonzero bf16 down to g = -99 or so (-7.4e-38 at g = -90, u = 1).
+There (a > 125) the interval follows the kernel's steps from the two ends of ex2's result (silu_mul_f32_ends).
+swiglu_weights keeps g in [-4, 4]; tests/exact_tails.py reaches g in [-136, 136].
 
 GEMM1 is exact given the device's own h (exact.gemm1_reference): the generator keeps |h| in [2^-4, 2^6] and W_down
 sparse, so y's sums stay on one fp32 grid.  No pytest in here.
@@ -50,12 +55,40 @@ def swiglu_reference(rows: np.ndarray, w_gate: np.ndarray, w_up: np.ndarray, b_g
         g = g + b_gate[None, :]
     if b_up is not None:
         u = u + b_up[None, :]
+    return silu_mul_rounded(g, u)
+
+
+def silu_mul_rounded(g: np.ndarray, u: np.ndarray) -> ex.Rounded:
+    """The interval of the kernel's bf16 h = silu_mul(g, u) for exact fp32 pre-activations g, u (float64 arrays):
+    relative eps_swiglu where sigma(g) is a normal number (power argument a = fl(-g log2e) <= ex.NORMAL_A), and
+    beyond it the kernel's steps from ex2's ends (silu_mul_f32_ends): the subnormal sigma band and the +-0 past the
+    overflow cliff (a >= 128).  `exact` is the real g sigmoid(g) u."""
+    g, u = np.broadcast_arrays(np.asarray(g, np.float64), np.asarray(u, np.float64))
     with np.errstate(over="ignore"):
         v = g / (1.0 + np.exp(-g)) * u
     e = eps_swiglu(g)
     a, b = ex.f64_to_bf16(v * (1 - e)), ex.f64_to_bf16(v * (1 + e))
+    tail = power_arg(g) > ex.NORMAL_A
+    if tail.any():
+        lo, hi = silu_mul_f32_ends(g[tail], u[tail])
+        a[tail], b[tail] = ex.f32_to_bf16(lo), ex.f32_to_bf16(hi)
     swap = ex.order_key(a) > ex.order_key(b)
     return ex.Rounded(np.where(swap, b, a), np.where(swap, a, b), v)
+
+
+def power_arg(g: np.ndarray) -> np.ndarray:
+    """a = fl(-g * fl32(log2 e)), the argument of the kernel's ex2 (exact: a product of two fp32 numbers)."""
+    return (-np.asarray(g, np.float64) * float(ex.LOG2E_F32)).astype(np.float32).astype(np.float64)
+
+
+def silu_mul_f32_ends(g: np.ndarray, u: np.ndarray):
+    """Bounds (float32, unordered) of the kernel's fp32 h = fl(fl(g * sigma) * u), sigma = sigmoid_score(g) between
+    exact.sigmoid_f32_ends' ends: both products are monotone in sigma, so its two ends give h's.  At a >= 128 sigma
+    is +0 and h = +-0; for a in (126, 128) sigma is subnormal, still kept by __frcp_rn."""
+    s_lo, s_hi = ex.sigmoid_f32_ends(power_arg(g))
+    g32, u32 = np.asarray(g, np.float32), np.asarray(u, np.float32)
+    return (((g32 * s_lo).astype(np.float32) * u32).astype(np.float32),
+            ((g32 * s_hi).astype(np.float32) * u32).astype(np.float32))
 
 
 # ----------------------------------------------------------------------------- inputs
@@ -134,8 +167,6 @@ def swiglu_inputs(cfg: MoEConfig, seed: int, bias: bool = False, **router_kw) ->
 
 def expert_h(inp: SwigluInputs, e: int, rows64: np.ndarray, what: str) -> ex.Rounded:
     wg_, wu, bg, bu = inp.gate_up64(e)
-    g = rows64 @ wg_.T + (0 if bg is None else bg[None, :])
-    assert (g >= G_MIN).all(), f"{what}: a gate pre-activation is below {G_MIN}"
     return swiglu_reference(rows64, wg_, wu, bg, bu, what)
 
 
