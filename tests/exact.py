@@ -17,13 +17,16 @@ products and the bf16 accumulation of the combine) is checked bit for bit.  Top-
 differ by at least one grid step, ties are exact, and an expert whose probability flushes to zero is picked in index
 order behind the others.
 
-The checkers raise AssertionError naming the stage, the first failing (token, pick) or (packet, row, column), and the
-device and reference bits.  No pytest in here: tests/test_exact_reference.py and tests/test_gpu_exact.py use it.
+One launch of any route, activation (the expert record `Experts`) and shared expert is checked by check_launch, and
+reference_launch builds a correct launch record by the same walk.  The checkers raise AssertionError naming the stage,
+the first failing (token, pick) or (packet, row, column), and the device and reference bits.  `Launcher` runs a route
+on a GPU context and reads the launch back.  No pytest in here.
 """
 from __future__ import annotations
 
 import dataclasses
 import functools
+import os
 from typing import Dict, Optional, Sequence
 
 import numpy as np
@@ -125,15 +128,94 @@ def _fmt(bits) -> str:
     return f"0x{b:04x} ({float(bits_to_f64(np.array([b]))[0]):.9g})"
 
 
+# ----------------------------------------------------------------------------- experts
+class PerExpert:
+    """Expert weights drawn on demand: w[e, i] = fn(e, i), block i of expert e (bf16 [P, H]), of a [E, m, P, H] whole
+    that is never built on the host."""
+
+    def __init__(self, fn, shape):
+        self.fn, self.shape = fn, tuple(shape)
+
+    def __getitem__(self, key):
+        e, i = key
+        return self.fn(int(e), int(i))
+
+
+@dataclasses.dataclass
+class Experts:
+    """E experts of one activation `act` (hidden_act): bf16 weights w [E, m, P, H] -- m = 2, W_up then the P*H block
+    flat-viewed as W_down [H, P]; m = 3 for SwiGLU, W_gate, W_up, W_down -- and biases bu [E, P] ([E, 2, P]: gate, up)
+    and bd [E, H], or None.  `w` may be a PerExpert: the reference reads one expert block at a time, so a model-sized
+    layer is never held in float64 whole.  A shared expert is a record with E = 1."""
+    w: object
+    bu: Optional[torch.Tensor]
+    bd: Optional[torch.Tensor]
+    act: int
+
+    def _block64(self, e: int, i: int) -> np.ndarray:
+        return self.w[e, i].double().numpy()
+
+    def pre(self, e: int, rows: np.ndarray, what: str = "GEMM0"):
+        """The pre-activations of expert e for the rows (float64 [M, H]): [v] or, for SwiGLU, [g, u], each [M, P] and
+        exact (the sums are asserted exact in fp32)."""
+        n_pre = self.w.shape[1] - 1
+        b = None if self.bu is None else self.bu[e].double().numpy().reshape(n_pre, -1)
+        names = ("",) if n_pre == 1 else (" (gate)", " (up)")
+        out = []
+        for i in range(n_pre):
+            w, bi = self._block64(e, i), None if b is None else b[i]
+            assert_exact_sums(rows, w, bi, what + names[i])
+            v = rows @ w.T
+            out.append(v if bi is None else v + bi[None, :])
+        return out
+
+    def h(self, e: int, rows: np.ndarray, what: str = "GEMM0") -> Rounded:
+        """h = RNE(act(pre-activations)) of expert e for the rows: ReLU exact, GELU's interval (gelu_rounded), SwiGLU's
+        (exact_swiglu.silu_mul_rounded)."""
+        pre = self.pre(e, rows, what)
+        if self.act == 0:
+            a = np.maximum(pre[0], 0.0)
+            b = f64_to_bf16(a)
+            return Rounded(b, b, a)
+        if self.act == 1:
+            return gelu_rounded(pre[0])
+        from tests.exact_swiglu import silu_mul_rounded
+
+        return silu_mul_rounded(*pre)
+
+    def down(self, e: int):
+        """(W_down [H, P], b_down [H] or None) of expert e in float64."""
+        _, m, P, H = self.w.shape
+        return (self._block64(e, m - 1).reshape(-1).reshape(H, P),
+                None if self.bd is None else self.bd[e].double().numpy())
+
+    def y(self, e: int, h_bits: np.ndarray, what: str = "GEMM1") -> Rounded:
+        return gemm1_reference(h_bits, *self.down(e), what)
+
+    def device(self, dev):
+        """(w, bu, bd) on `dev`, the weights uploaded one block at a time."""
+        w = torch.empty(self.w.shape, dtype=torch.bfloat16, device=dev)
+        for e in range(w.shape[0]):
+            for i in range(w.shape[1]):
+                w[e, i] = self.w[e, i].to(dev)
+        return (w, *(None if b is None else b.to(dev) for b in (self.bu, self.bd)))
+
+
+def shared_expert(se: Experts, dev):
+    """The runtime.SharedExpert of a one-expert record, on `dev`."""
+    from flashmoe_b200.runtime import SharedExpert
+
+    w, bu, bd = se.device(dev)
+    return SharedExpert(w[0], None if bu is None else bu[0], None if bd is None else bd[0])
+
+
 # ----------------------------------------------------------------------------- inputs
 @dataclasses.dataclass
 class ExactInputs:
     cfg: MoEConfig
     x: torch.Tensor                 # [mini_batch, seq, H] bf16 (CPU)
     wg: torch.Tensor                # [H, E] bf16, flat view = Wg_eff [E, H]
-    we: torch.Tensor                # [E, 2, P, H] bf16; the down block is W_down_eff [H, P] reinterpreted
-    bu: Optional[torch.Tensor]      # [E, P] or None
-    bd: Optional[torch.Tensor]      # [E, H] or None
+    experts: Experts
     underflow_tokens: np.ndarray    # token indices built to flush all but one expert
     zero_tokens: np.ndarray         # token indices with x = 0 (all logits tie)
 
@@ -145,21 +227,9 @@ class ExactInputs:
     def wg_eff64(self) -> np.ndarray:
         return self.wg.reshape(-1).reshape(self.cfg.E, self.cfg.H).double().numpy()
 
-    @functools.cached_property
-    def w_up64(self) -> np.ndarray:
-        return self.we[:, 0].double().numpy()
-
-    @functools.cached_property
-    def w_down64(self) -> np.ndarray:   # [E, H, P]: the [P, H] block viewed flat as [H, P]
-        E, _, P, H = self.we.shape
-        return self.we[:, 1].reshape(E, -1).reshape(E, H, P).double().numpy()
-
-    def bias64(self, which: str) -> Optional[np.ndarray]:
-        b = self.bu if which == "up" else self.bd
-        return None if b is None else b.double().numpy()
-
     def device(self, dev):
-        return tuple(None if t is None else t.to(dev) for t in (self.x, self.wg, self.we, self.bu, self.bd))
+        """(x, gate weights, expert weights, bias_up, bias_down) on `dev`."""
+        return (self.x.to(dev), self.wg.to(dev), *self.experts.device(dev))
 
 
 def exact_inputs(cfg: MoEConfig, seed: int, *, x_range: int = 8, wg_range: int = 4, up_range: int = 8,
@@ -233,8 +303,9 @@ def exact_inputs(cfg: MoEConfig, seed: int, *, x_range: int = 8, wg_range: int =
         return t
 
     we = np.stack([up, down.reshape(E, -1).reshape(E, P, H)], axis=1)
+    experts = Experts(bf(we), None if bu is None else bf(bu), None if bd is None else bf(bd), cfg.hidden_act)
     return ExactInputs(cfg, bf(x).reshape(cfg.mini_batch, cfg.sequence_len, H), bf(wg.reshape(-1).reshape(H, E)),
-                       bf(we), None if bu is None else bf(bu), None if bd is None else bf(bd), under, zeros)
+                       experts, under, zeros)
 
 
 # ----------------------------------------------------------------------------- preconditions
@@ -330,6 +401,58 @@ def slots_from_topk(topk: np.ndarray, E: int, EC: int):
     return slot, counts, np.minimum(counts, EC).astype(np.int32), slot < EC
 
 
+INT32_MAX = 2 ** 31 - 1
+
+
+def slots_from_routing(topk: np.ndarray, E: int, EC: int):
+    """slots_from_topk for routing that may hold -1 (no expert, the caller's routing): slot [n, k] (INT32_MAX for -1),
+    counts [E], recv_cnt [E] = min(counts, EC), kept [n, k] = slot < EC."""
+    topk = np.asarray(topk, dtype=np.int64)
+    valid = topk >= 0
+    assert (topk[valid] < E).all() and (topk[~valid] == -1).all(), "expert index outside [-1, E)"
+    flat, vflat = topk.reshape(-1), valid.reshape(-1)
+    slot = np.full(flat.size, INT32_MAX, dtype=np.int64)
+    sub = flat[vflat]
+    s, counts, recv_cnt, _ = slots_from_topk(sub.reshape(-1, 1), E, EC)   # ascending (token, pick) order kept
+    slot[vflat] = s[:, 0]
+    slot = slot.reshape(topk.shape).astype(np.int32)
+    return slot, counts, recv_cnt, slot < EC
+
+
+def sanitize(topk: np.ndarray, E: int) -> np.ndarray:
+    """The caller's routing the kernel runs: indices outside [0, E) become -1."""
+    t = np.asarray(topk, dtype=np.int32)
+    return np.where((t >= 0) & (t < E), t, -1).astype(np.int32)
+
+
+def routing_case(n: int, E: int, k: int, seed: int, *, skip_frac: float = 0.1, dup_frac: float = 0.1,
+                 hot: int = 0, hot_frac: float = 0.5, empty=(), bad=()):
+    """Seeded caller routing for n tokens: picks drawn from the experts not in `empty`, a `hot_frac` share of them sent
+    to expert `hot` (skew that overflows its capacity), a `dup_frac` share of tokens naming one expert twice, a
+    `skip_frac` share of picks set to -1, and `bad` (token, pick, value) entries written last.  Weights are fp32 in
+    [-1, 2), with some exact zeros.  Returns (topk_idx int32 [n, k], topk_w float32 [n, k])."""
+    g = np.random.default_rng(seed)
+    allowed = np.array([e for e in range(E) if e not in set(empty)])
+    idx = allowed[g.integers(0, len(allowed), size=(n, k))].astype(np.int32)
+    if hot not in set(empty):
+        idx[g.random((n, k)) < hot_frac] = hot
+    if k > 1:
+        dup = g.random(n) < dup_frac
+        idx[dup, 1] = idx[dup, 0]
+    idx[g.random((n, k)) < skip_frac] = -1
+    for t, j, v in bad:
+        if t < n:
+            idx[t, j] = v
+    w = (g.random((n, k)) * 3 - 1).astype(np.float32)
+    w[g.random((n, k)) < 0.05] = 0.0
+    return idx, w
+
+
+def weights_f32(w_bits: np.ndarray) -> np.ndarray:
+    """bf16 bits as the fp32 weights a routed replay takes (the same bits after rne_bf16)."""
+    return (np.asarray(w_bits, dtype=np.uint16).astype(np.uint32) << 16).view(np.float32)
+
+
 def packet_tokens(topk: np.ndarray, slot: np.ndarray, E: int, EC: int):
     """For every expert, the token of each kept slot in slot order (rows of its packet)."""
     out = []
@@ -348,23 +471,9 @@ class Rounded:
     wide_ok: Optional[np.ndarray] = None   # bool: elements whose interval may span several bf16 ulps (GELU below zero)
 
 
-def gemm0_reference(rows: np.ndarray, w_up: np.ndarray, b_up: Optional[np.ndarray], act: int, what: str) -> Rounded:
-    """h = RNE(act(rows . w_up^T + b_up)); ReLU is exact, GELU an interval: EPS_GELU for pre-activations >= 0,
-    gelu_neg_f32 below zero (whose intervals may span several bf16 ulps: `wide_ok`)."""
-    assert_exact_sums(rows, w_up, b_up, what)
-    v = rows @ w_up.T
-    if b_up is not None:
-        v = v + b_up[None, :]
-    if act == 0:
-        a = np.maximum(v, 0.0)
-        b = f64_to_bf16(a)
-        return Rounded(b, b, a)
-    return gelu_rounded(v)
-
-
 def gelu_rounded(v: np.ndarray) -> Rounded:
     """The interval of the kernel's bf16 GELU of the exact pre-activations v (float64, fp32 values), over the whole
-    real line: v >= 0 by EPS_GELU, v < 0 by gelu_neg_f32."""
+    real line: v >= 0 by EPS_GELU, v < 0 by gelu_neg_f32 (whose intervals may span several bf16 ulps: `wide_ok`)."""
     from scipy.special import erf, erfc
 
     v = np.asarray(v, dtype=np.float64)
@@ -512,6 +621,19 @@ def combine_tokens(y_of: np.ndarray, kept: np.ndarray, pw_bits: np.ndarray, mcw:
     return Rounded(f64_to_bf16(acc_lo), f64_to_bf16(acc_hi), real)
 
 
+def combine_routed(y_of: np.ndarray, kept: np.ndarray, w_bits: np.ndarray) -> np.ndarray:
+    """out bf16 bits [n, H] on the caller's (or a gated launch's) routing, mcw = 1: y_of bf16 bits [n, k, H] (ignored
+    where not kept), kept [n, k], w_bits bf16 [n, k].  out[t] is the bf16 accumulation, in pick order from +0, of
+    RNE(w~_j * y_j) over the kept picks, k = 1 included: each term is a single rounding of an exact product, each add
+    rounds to fp32 and then to bf16, so the whole output is exact (no __fdividef interval)."""
+    n, k, H = y_of.shape
+    acc = np.zeros((n, H))
+    for j in range(k):
+        term = bits_to_f64(f64_to_bf16(bits_to_f64(w_bits[:, j])[:, None] * bits_to_f64(y_of[:, j])))
+        acc = np.where(kept[:, j][:, None], bits_to_f64(f64_to_bf16(acc + term)), acc)
+    return f64_to_bf16(acc)
+
+
 def add_shared(r: Rounded, s_bits: np.ndarray) -> Rounded:
     """out = rne_bf16(fl32(r) + fl32(s)): a shared expert's s rows (bf16 bits [n, H]) added to the routed result r after
     r is rounded.  The sum of two bf16 numbers is exact in float64 and rounds once to fp32, then to bf16; the map is
@@ -598,103 +720,192 @@ def check_equal(got: np.ndarray, want: np.ndarray, what: str, labels: Sequence[s
 @dataclasses.dataclass
 class Device:
     """What one launch left behind (host copies); `n` tokens valid."""
-    out: np.ndarray        # bf16 bits [n, H]
-    topk_idx: np.ndarray   # [n, k]
-    topk_w: np.ndarray     # bf16 bits [n, k]
-    mcw: np.ndarray        # fp32 [n]
-    gate_out: np.ndarray   # bf16 bits [n, E]
-    slot: np.ndarray       # [n, k]
-    counts: np.ndarray     # [E]
-    recv_cnt: Optional[np.ndarray]
-    recv_x: Optional[np.ndarray]   # [E, pEC, H] or None (the dense path copies nothing)
-    hidden: np.ndarray     # [E, pEC, P]
-    ret_y: Optional[np.ndarray]    # [E, pEC, H] (gather path) or None
+    out: np.ndarray = None                 # bf16 bits [n, H]
+    topk_idx: np.ndarray = None            # [n, k]
+    topk_w: np.ndarray = None              # bf16 bits [n, k]
+    mcw: np.ndarray = None                 # fp32 [n]
+    gate_out: Optional[np.ndarray] = None  # bf16 bits [n, E] (None on the caller's routing)
+    slot: np.ndarray = None                # [n, k]
+    counts: np.ndarray = None              # [E]
+    recv_cnt: Optional[np.ndarray] = None
+    recv_x: Optional[np.ndarray] = None    # [E, pEC, H] or None (the dense path copies nothing)
+    hidden: np.ndarray = None              # [E, pEC, P]
+    ret_y: Optional[np.ndarray] = None     # [E, pEC, H] (gather path) or None
 
 
-def check_forward(inp: ExactInputs, dev: Device, EC: int, n: Optional[int] = None, stats: Optional[Stats] = None,
-                  shared_s: Optional[np.ndarray] = None):
-    """Every stage of one launch over the first n tokens of `inp` (default all), in pipeline order; GEMM1 and the
-    combine are referenced from the device's own hidden, topk_w and mcw, so a failure names the stage that broke.
-    `shared_s`: a shared expert's s rows (bf16 bits [n, H]); out is then rne(r + s) of the routed result r (add_shared),
-    rows whose picks were all dropped rne(+0 + s)."""
-    cfg = inp.cfg
-    E, k, H = cfg.E, cfg.k, cfg.H
+@dataclasses.dataclass
+class SharedRecord:
+    """What a launch left of the shared expert (bf16 bits, the first n rows)."""
+    h_s: np.ndarray   # [n, Ps]
+    y_s: np.ndarray   # [n, H]
+
+
+def shared_stage(x: np.ndarray, shared: Experts, rec: Optional[SharedRecord] = None,
+                 stats: Optional[Stats] = None) -> SharedRecord:
+    """h_s against the shared expert's GEMM0 of the tokens x (float64 [n, H]), then y_s bit for bit against GEMM1 of
+    the record's own h_s, so a failure names the GEMM that broke.  Without `rec`, the reference's own record (an
+    interval's lower end).  `stats` gets both stages."""
     st = stats if stats is not None else Stats()
-    x = inp.x64[: (cfg.S if n is None else n)]
-    n = x.shape[0]
-    ref = router_reference(x, inp.wg_eff64, k)
-    check_topk(dev.topk_idx, ref)
-    st.add("topk_idx", ref.topk.size)
-    w1 = _interval_check(dev.gate_out, Rounded(ref.go_lo, ref.go_hi, 0.5 * (ref.p_lo + ref.p_hi)), "gate_out",
-                         ("token", "expert"))
-    st.add("gate_out", ref.go_lo.size, int((ref.p_lo != bits_to_f64(ref.go_lo)).sum()), w1)
-    rows = np.arange(n)[:, None]
-    check_equal(dev.topk_w, dev.gate_out[rows, dev.topk_idx], "topk_w vs gate_out[t, topk_idx]", ("token", "pick"))
-    st.add("topk_w", dev.topk_w.size)
-    lo, hi = ref.mcw_bounds()
-    bad = ~((dev.mcw >= lo) & (dev.mcw <= hi))
-    assert not bad.any(), (f"mcw: token {int(np.flatnonzero(bad)[0])}: device {dev.mcw[bad][0]!r} outside "
-                           f"[{lo[bad][0]!r}, {hi[bad][0]!r}]")
-    st.add("mcw", n)
+    h = shared.h(0, x, "GEMM0 of the shared expert")
+    rec = rec if rec is not None else SharedRecord(h.lo, None)
+    assert rec.h_s.shape == h.lo.shape, f"h_s: shape {rec.h_s.shape}, expected {h.lo.shape}"
+    st.add("h_s", h.lo.size, rounded_count(h), _interval_check(rec.h_s, h, "h_s (shared expert)", ("token", "column")))
+    y = shared.y(0, rec.h_s, "GEMM1 of the shared expert")
+    if rec.y_s is None:
+        rec.y_s = y.lo
+    check_equal(rec.y_s, y.lo, "y_s (shared expert)", ("token", "column"), signed_zero=False)
+    st.add("y_s", y.lo.size, rounded_count(y))
+    return rec
 
-    slot, counts, recv_cnt, kept = slots_from_topk(dev.topk_idx, E, EC)
+
+# ----------------------------------------------------------------------------- one launch, reference and checker
+def reference_launch(route: str, inp: ExactInputs, EC: int, n: int, *, routing=None, router=None, score_bias=None,
+                     shared: Optional[Experts] = None, stats: Optional[Stats] = None):
+    """(Device, SharedRecord or None) of one launch over the first n tokens computed by the reference itself (interval
+    midpoints for the routing, lower ends for h): what a correct kernel could have produced.  The planted-fault tests
+    start from it.  Arguments as check_launch's; `stats` gets what checking the record would count."""
+    dev, rec, _ = _launch(route, inp, EC, n, None, None, routing, router, score_bias, shared, stats)
+    return dev, rec
+
+
+def check_launch(route: str, inp: ExactInputs, EC: int, n: int, dev: Device, rec: Optional[SharedRecord] = None, *,
+                 routing=None, router=None, score_bias=None, shared: Optional[Experts] = None,
+                 stats: Optional[Stats] = None) -> int:
+    """Every stage of one launch over the first n tokens of `inp`, in pipeline order, at capacity EC.  `route`:
+      "router"  the built-in softmax router: topk_idx, gate_out, topk_w and mcw against router_reference, the combine
+                of combine_tokens (k = 1 unscaled);
+      "routed"  the caller's `routing` = (topk_idx, topk_w) of at least n tokens: topk_idx sanitized, topk_w =
+                rne_bf16(w), mcw = 1, the combine of combine_routed;
+      "gated"   the rule `router` with `score_bias`: exact_gated.check_gated_routing, then the routed checks on the
+                device's own routing.
+    Then, the same for every route: slot / counts / recv_cnt, recv_x, h of every expert (through inp.experts), y from
+    the device's own h (ret_y on the gather path), out and the rows without a kept pick (+0); with a `shared` expert
+    (record `rec`) h_s, y_s and out = rne(r + s).  GEMM1 and the combine are referenced from the device's own values,
+    so a failure names the stage that broke.  Returns the gated route's ambiguous tokens (0 elsewhere)."""
+    return _launch(route, inp, EC, n, dev, rec, routing, router, score_bias, shared, stats)[2]
+
+
+def _launch(route, inp, EC, n, dev, rec, routing, router, score_bias, shared, stats):
+    """check_launch's walk; with dev = None every stage first takes the reference's value (reference_launch)."""
+    cfg, experts = inp.cfg, inp.experts
+    E, k, H, P = cfg.E, cfg.k, cfg.H, cfg.P
+    st = stats if stats is not None else Stats()
+    build = dev is None
+    x = inp.x64[:n]
+    rows = np.arange(n)[:, None]
+    amb = 0
+    if route == "router":
+        ref = router_reference(x, inp.wg_eff64, k)
+        if build:
+            p_mid = 0.5 * (ref.p_lo + ref.p_hi)
+            mcw = np.zeros(n, np.float32)
+            for j in range(k):
+                mcw = (mcw + p_mid[rows[:, 0], ref.topk[:, j]].astype(np.float32)).astype(np.float32)
+            dev = Device(topk_idx=ref.topk.copy(), topk_w=ref.go_lo[rows, ref.topk], mcw=mcw, gate_out=ref.go_lo.copy())
+        check_topk(dev.topk_idx, ref)
+        st.add("topk_idx", ref.topk.size)
+        w1 = _interval_check(dev.gate_out, Rounded(ref.go_lo, ref.go_hi, 0.5 * (ref.p_lo + ref.p_hi)), "gate_out",
+                             ("token", "expert"))
+        st.add("gate_out", ref.go_lo.size, int((ref.p_lo != bits_to_f64(ref.go_lo)).sum()), w1)
+        check_equal(dev.topk_w, dev.gate_out[rows, dev.topk_idx], "topk_w vs gate_out[t, topk_idx]", ("token", "pick"))
+        st.add("topk_w", dev.topk_w.size)
+        lo, hi = ref.mcw_bounds()
+        bad = ~((dev.mcw >= lo) & (dev.mcw <= hi))
+        assert not bad.any(), (f"mcw: token {int(np.flatnonzero(bad)[0])}: device {dev.mcw[bad][0]!r} outside "
+                               f"[{lo[bad][0]!r}, {hi[bad][0]!r}]")
+        st.add("mcw", n)
+    else:
+        if route == "gated":
+            from tests import exact_gated as eg
+
+            if build:
+                picks, w, gate_out = eg.reference_routing(router, score_bias, k, x, inp.wg_eff64)
+                dev = Device(topk_idx=picks, topk_w=f32_to_bf16(w), mcw=np.ones(n, np.float32), gate_out=gate_out)
+            amb = eg.check_gated_routing(x @ inp.wg_eff64.T, score_bias, router, k, dev.topk_idx, dev.gate_out,
+                                         dev.topk_w, (x, inp.wg_eff64))
+            routing = (dev.topk_idx, weights_f32(dev.topk_w))
+        run = sanitize(routing[0][:n], E)
+        w_bits = f32_to_bf16(np.asarray(routing[1][:n], dtype=np.float32))
+        if build and route == "routed":
+            dev = Device(topk_idx=run, topk_w=w_bits, mcw=np.ones(n, np.float32))
+        check_equal(dev.topk_idx, run, "topk_idx (the caller's, invalid ones -1)", ("token", "pick"))
+        check_equal(dev.topk_w, w_bits, "topk_w = rne_bf16(w)", ("token", "pick"))
+        check_equal(dev.mcw, np.ones(n, np.float32), "mcw = 1", ("token",))
+        st.add("routing tables", 3 * run.size)
+
+    topk = dev.topk_idx
+    slot, counts, recv_cnt, kept = slots_from_routing(topk, E, EC)
+    rmax = max(1, int(recv_cnt.max(initial=0)))
+    if build:
+        dev.slot, dev.counts, dev.recv_cnt = slot, counts, recv_cnt
+        dev.recv_x, dev.ret_y = np.zeros((E, rmax, H), np.uint16), np.zeros((E, rmax, H), np.uint16)
+        dev.hidden = np.zeros((E, rmax, P), np.uint16)
     check_equal(dev.slot, slot, "slot", ("token", "pick"))
     check_equal(dev.counts, counts, "counts", ("expert",))
     if dev.recv_cnt is not None:
         check_equal(dev.recv_cnt, recv_cnt, "recv_cnt", ("expert",))
     st.add("slot/counts/recv_cnt", slot.size + 2 * E)
 
-    toks = packet_tokens(dev.topk_idx, slot, E, EC)
+    toks = packet_tokens(topk, slot, E, EC)
     xb = f64_to_bf16(x)
-    y_dev_ref = np.zeros((E, max(1, int(recv_cnt.max(initial=0))), H), np.uint16)
+    y_ref = np.zeros((E, rmax, H), np.uint16)
     for e in range(E):
         c = len(toks[e])
         if c == 0:
             continue
+        if build:
+            dev.recv_x[e, :c] = xb[toks[e]]
         if dev.recv_x is not None:
             check_equal(dev.recv_x[e, :c], xb[toks[e]], f"recv_x of expert {e}", ("slot", "column"))
             st.add("recv_x", c * H)
-        h_ref = gemm0_reference(x[toks[e]], inp.w_up64[e], None if inp.bu is None else inp.bias64("up")[e],
-                                cfg.hidden_act, f"GEMM0 of expert {e}")
-        h_dev = dev.hidden[e, :c]
-        if cfg.hidden_act == 0:
-            check_equal(h_dev, h_ref.lo, f"hidden of expert {e}", ("slot", "column"), signed_zero=False)
-            st.add("hidden", h_dev.size, rounded_count(h_ref))
-        else:
-            w = _interval_check(h_dev, h_ref, f"hidden of expert {e}", ("slot", "column"))
-            st.add("hidden", h_dev.size, rounded_count(h_ref), w)
-        y_ref = gemm1_reference(h_dev, inp.w_down64[e], None if inp.bd is None else inp.bias64("down")[e],
-                                f"GEMM1 of expert {e}")
-        y_dev_ref[e, :c] = y_ref.lo
+        h = experts.h(e, x[toks[e]], f"GEMM0 of expert {e}")
+        if build:
+            dev.hidden[e, :c] = h.lo
+        w = _interval_check(dev.hidden[e, :c], h, f"hidden of expert {e}", ("slot", "column"))
+        st.add("hidden", c * P, rounded_count(h), w)
+        y = experts.y(e, dev.hidden[e, :c], f"GEMM1 of expert {e}")
+        y_ref[e, :c] = y.lo
+        if build:
+            dev.ret_y[e, :c] = y.lo
         if dev.ret_y is not None:
-            check_equal(dev.ret_y[e, :c], y_ref.lo, f"ret_y of expert {e}", ("slot", "column"), signed_zero=False)
-            st.add("ret_y", c * H, rounded_count(y_ref))
+            check_equal(dev.ret_y[e, :c], y.lo, f"ret_y of expert {e}", ("slot", "column"), signed_zero=False)
+            st.add("ret_y", c * H, rounded_count(y))
         else:
-            st.add("y (in the fused epilogue)", 0, rounded_count(y_ref))
+            st.add("y (in the fused epilogue)", 0, rounded_count(y))
 
-    y_of = y_dev_ref[dev.topk_idx, np.where(kept, slot, 0)]          # [n, k, H]
-    out_ref = combine_tokens(y_of, kept, dev.topk_w, dev.mcw)
-    dropped = ~kept.any(axis=1)
-    empty, what = np.zeros((int(dropped.sum()), H), np.uint16), "out"
-    if shared_s is not None:
-        st.add("out (routed)", 0, rounded_count(out_ref) if k > 1 else 0)
-        out_ref, what = add_shared(out_ref, shared_s), "out = rne(r + s)"
-        empty = add_shared(Rounded(empty, empty, 0), shared_s[dropped]).lo
-    w = _interval_check(dev.out, out_ref, what, ("token", "column"), max_width=None)
-    st.add(what, dev.out.size, rounded_count(out_ref) if k > 1 or shared_s is not None else 0, w)
-    if dropped.any():
-        check_equal(dev.out[dropped], empty, f"{what} rows of tokens whose picks were all dropped (r = +0)",
-                    ("row", "column"), signed_zero=shared_s is None)
-        st.add("all-dropped rows", int(dropped.sum()) * H)
-    return st
+    y_of = y_ref[np.where(kept, topk, 0), np.where(kept, slot, 0)]          # [n, k, H]
+    if route == "router":
+        r = combine_tokens(y_of, kept, dev.topk_w, dev.mcw)
+    else:   # exact; `exact` the combine in real arithmetic, for the rounding statistics
+        out = combine_routed(y_of, kept, dev.topk_w)
+        r = Rounded(out, out, (np.where(kept, bits_to_f64(dev.topk_w), 0.0)[:, :, None] * bits_to_f64(y_of)).sum(1))
+    none = ~kept.any(axis=1)
+    empty, what = np.zeros((int(none.sum()), H), np.uint16), "out"
+    if shared is not None:
+        rec = shared_stage(x, shared, rec, st)
+        r, what = add_shared(r, rec.y_s), "out = rne(r + s)"
+        empty = add_shared(Rounded(empty, empty, 0), rec.y_s[none]).lo
+    if build:
+        dev.out = r.lo
+    w = _interval_check(dev.out, r, what, ("token", "column"), max_width=None)
+    st.add(what, dev.out.size, rounded_count(r), w)
+    if none.any():
+        check_equal(dev.out[none], empty, f"{what} rows of tokens without a kept pick (r = +0)", ("row", "column"),
+                    signed_zero=shared is None)
+        st.add("rows without a kept pick", int(none.sum()) * H)
+    return dev, rec, amb
 
 
 def check_preconditions(inp: ExactInputs, EC: int, min_h_rounded: float, min_out_rounded: float,
                         n: Optional[int] = None, dense: bool = False) -> Stats:
-    """Run the reference alone (the device values replaced by the reference's own) and assert the rounding shares:
+    """Check the reference's own router launch (the dense path without recv_x) and assert the rounding shares:
     inputs that never round do not test RNE.  Returns the statistics."""
-    dev = reference_device(inp, EC, n, dense)
-    st = check_forward(inp, dev, EC, n)
+    n = inp.cfg.S if n is None else n
+    dev, _ = reference_launch("router", inp, EC, n)
+    if dense:
+        dev.recv_x = None
+    st = Stats()
+    check_launch("router", inp, EC, n, dev, stats=st)
     zero = np.zeros(3, np.int64)   # (a call with no tokens has neither)
     hs, os_ = st.d.get("hidden", zero), st.d.get("out", zero)
     if hs[0]:
@@ -704,38 +915,70 @@ def check_preconditions(inp: ExactInputs, EC: int, min_h_rounded: float, min_out
     return st
 
 
-def reference_device(inp: ExactInputs, EC: int, n: Optional[int] = None, dense: bool = False) -> Device:
-    """A Device record computed by the reference itself (midpoints of the intervals): what a correct kernel could
-    have produced.  The planted-fault tests start from it."""
-    cfg = inp.cfg
-    E, k, H, P = cfg.E, cfg.k, cfg.H, cfg.P
-    x = inp.x64[: (cfg.S if n is None else n)]
-    n = x.shape[0]
-    ref = router_reference(x, inp.wg_eff64, k)
-    gate_out = ref.go_lo.copy()
-    rows = np.arange(n)[:, None]
-    p_mid = 0.5 * (ref.p_lo + ref.p_hi)
-    mcw = np.zeros(n, np.float32)
-    for j in range(k):
-        mcw = (mcw + p_mid[rows[:, 0], ref.topk[:, j]].astype(np.float32)).astype(np.float32)
-    slot, counts, recv_cnt, kept = slots_from_topk(ref.topk, E, EC)
-    toks = packet_tokens(ref.topk, slot, E, EC)
-    rmax = max(1, int(recv_cnt.max(initial=0)))
-    recv_x = np.zeros((E, rmax, H), np.uint16)
-    hidden = np.zeros((E, rmax, P), np.uint16)
-    ret_y = np.zeros((E, rmax, H), np.uint16)
-    for e in range(E):
-        c = len(toks[e])
-        if c == 0:
-            continue
-        recv_x[e, :c] = f64_to_bf16(x[toks[e]])
-        h = gemm0_reference(x[toks[e]], inp.w_up64[e], inp.bias64("up")[e] if inp.bu is not None else None,
-                            cfg.hidden_act, "GEMM0")
-        hidden[e, :c] = h.lo
-        ret_y[e, :c] = gemm1_reference(h.lo, inp.w_down64[e], inp.bias64("down")[e] if inp.bd is not None else None,
-                                       "GEMM1").lo
-    topk_w = gate_out[rows, ref.topk]
-    y_of = ret_y[ref.topk, np.where(kept, slot, 0)]
-    out = combine_tokens(y_of, kept, topk_w, mcw).lo
-    return Device(out, ref.topk.copy(), topk_w, mcw, gate_out, slot, counts, recv_cnt, None if dense else recv_x,
-                  hidden, ret_y)
+# ----------------------------------------------------------------------------- launches on the GPU
+MAX_AMBIGUOUS = 0.01   # gated tokens whose picks the intervals cannot decide (their later stages are still checked)
+
+
+def gather_path(cfg: MoEConfig, env=None) -> bool:
+    """The launch writes y rows to ret_y and combines them apart (FM_FUSED_COMBINE=0, or k > 2)."""
+    return (os.environ if env is None else env).get("FM_FUSED_COMBINE") == "0" or cfg.k > 2
+
+
+def dense_path(cfg: MoEConfig, env=None) -> bool:
+    """E = 1 takes the dense path, which reads x in place (no recv_x), unless FM_DENSE_E1=0."""
+    return cfg.E == 1 and (os.environ if env is None else env).get("FM_DENSE_E1", "1") != "0"
+
+
+class Launcher:
+    """The inputs of one route uploaded to one context, which was created under the current environment: `launch`
+    runs the route's forward, `read` reads a launch back as check_launch takes it, `check` checks it."""
+
+    def __init__(self, ctx, route: str, inp: ExactInputs, *, routing=None, router=None, score_bias=None):
+        dev, cfg = ctx.device, inp.cfg
+        self.ctx, self.route, self.inp, self.cfg = ctx, route, inp, cfg
+        self.routing, self.router, self.score_bias = routing, router, score_bias
+        x, self.wg, self.we, self.bu, self.bd = inp.device(dev)
+        self.x = x.reshape(cfg.S, cfg.H)
+        if routing is not None:
+            self.idx, self.w = (torch.from_numpy(a).to(dev) for a in routing)
+        self.sb = None if score_bias is None else torch.from_numpy(score_bias).to(dev)
+        self.gather, self.dense = gather_path(cfg), dense_path(cfg)
+
+    def launch(self, n: Optional[int], shared=None, out=None, n_tokens=None, x=None):
+        """The forward of the first n tokens (of `x` when given), with a runtime.SharedExpert `shared`; n = None:
+        MoEContext.forward of all S (router route)."""
+        ctx, kw = self.ctx, dict(bias_up=self.bu, bias_down=self.bd, out=out)
+        if n is None:
+            return ctx.forward(self.x.reshape(self.inp.x.shape), self.wg, self.we, **kw)
+        x = self.x[:n] if x is None else x
+        m = x.shape[0]
+        kw.update(n_tokens=n_tokens, shared_expert=shared)
+        if self.route == "router":
+            return ctx.forward_tokens(x, self.wg, self.we, **kw)
+        if self.route == "routed":
+            return ctx.forward_routed(x, self.idx[:m], self.w[:m], self.we, **kw)
+        return ctx.forward_gated(x, self.wg, self.we, self.router, score_bias=self.sb, **kw)
+
+    def read(self, out, n: int, shared: bool = False):
+        """(Device, SharedRecord or None) of the first n tokens of the last launch, whose output is `out`."""
+        ctx = self.ctx
+        dev = Device(out=to_bits(out.cpu()).reshape(n, self.cfg.H), topk_idx=ctx.read("topk_idx")[:n],
+                     topk_w=ctx.read("topk_w")[:n], mcw=ctx.read("mcw")[:n],
+                     gate_out=None if self.route == "routed" else ctx.read("gate_out")[:n], slot=ctx.read("slot")[:n],
+                     counts=ctx.read("counts"), recv_cnt=ctx.read("recv_cnt"),
+                     recv_x=None if self.dense else ctx.read("recv_x"), hidden=ctx.read("hidden"),
+                     ret_y=ctx.read("ret_y") if self.gather else None)
+        rec = SharedRecord(ctx.read("shared_hidden")[:n], ctx.read("shared_y")[:n]) if shared else None
+        return dev, rec
+
+    def check(self, dev: Device, rec: Optional[SharedRecord], n: int, shared: Optional[Experts] = None,
+              stats: Optional[Stats] = None) -> int:
+        return check_launch(self.route, self.inp, self.cfg.EC_of(n), n, dev, rec, routing=self.routing,
+                            router=self.router, score_bias=self.score_bias, shared=shared, stats=stats)
+
+    def run(self, n: int, shared: Optional[Experts] = None, stats: Optional[Stats] = None):
+        """launch, read and check one forward of the first n tokens; returns (Device, SharedRecord, ambiguous)."""
+        out = self.launch(n, None if shared is None else shared_expert(shared, self.ctx.device))
+        self.ctx.synchronize()
+        dev, rec = self.read(out, n, shared is not None)
+        return dev, rec, self.check(dev, rec, n, shared, stats)

@@ -8,20 +8,19 @@ row each in the logits scratch (gate_phase in fm_kernel.cuh); the tensor-core ro
 `check_gated_routing` checks a gated launch's gate_out, picks and weights against intervals: the scores are those of the
 softmax reference (exact.router_reference) or of the kernel's sigmoid, the selection value adds the fp32 score bias, the
 kept groups and the picks are decided from the intervals, and a token whose picks the intervals cannot decide is counted
-as ambiguous instead of checked.  The rest of a gated launch is a routed launch on its own routing
-(exact_routed.check_routed_forward).  No pytest in here.
+as ambiguous instead of checked.  The rest of a gated launch is a routed launch on its own routing (exact.check_launch).
+No pytest in here.
 """
 from __future__ import annotations
 
 import dataclasses
 import os
-from typing import List, Optional
+from typing import List
 
 import numpy as np
 import torch
 
 from tests import exact as ex
-from tests import exact_routed as er
 
 # ----------------------------------------------------------------------------- sub-chunk arithmetic (fm_kernel.cuh)
 G_LOGIT_BYTES = 64 * 1024   # the logits scratch
@@ -75,61 +74,27 @@ def regime(E: int, k: int, n: int, grid: int, tc: bool) -> Regime:
 
 
 # ----------------------------------------------------------------------------- inputs at a model's layer size
-class _PerExpert:
-    """w[e] computed on demand: the reference reads one expert's weights at a time."""
-
-    def __init__(self, fn):
-        self.fn = fn
-
-    def __getitem__(self, e):
-        return self.fn(int(e))
-
-
-class LayerInputs:
-    """Exact inputs at a model's layer size (e.g. DeepSeek-V3: H = 7168, P = 2048, E = 256), in the role of
-    exact.ExactInputs: the expert weights are drawn one expert at a time from a seed per (expert, block), uploaded to
-    the device expert by expert and converted to float64 one expert at a time for the reference, so neither side
-    holds all E experts in float64 (60 GB at DeepSeek-V3's size).  x: integers in [-x_range, x_range]; Wg_eff: sparse
-    (density `wg_density`) entries +-2^-6, so the logits of H-term sums stay near unit scale; W_up: integers in
+def layer_inputs(cfg, seed: int, *, x_range: int = 4, wg_density: float = 1 / 16, up_range: int = 2,
+                 down_range: int = 2) -> ex.ExactInputs:
+    """Exact inputs at a model's layer size (e.g. DeepSeek-V3: H = 7168, P = 2048, E = 256): the expert weights are
+    drawn one block at a time from a seed per (expert, block) (exact.PerExpert), so neither the reference nor the upload
+    holds all E experts at once (60 GB in float64 at DeepSeek-V3's size).  x: integers in [-x_range, x_range]; Wg_eff:
+    sparse (density `wg_density`) entries +-2^-6, so the logits of H-term sums stay near unit scale; W_up: integers in
     [-up_range, up_range] * 2^-3; W_down: integers in [-down_range, down_range] * 2^-5.  No biases."""
+    S, H, E, P = cfg.S, cfg.H, cfg.E, cfg.P
+    g = np.random.default_rng(seed)
+    x = g.integers(-x_range, x_range + 1, size=(S, H), dtype=np.int8)
+    wg = (g.integers(0, 2, size=(E, H), dtype=np.int8) * 2 - 1) * (g.random((E, H)) < wg_density)
 
-    bu = bd = None
+    def block(e, i):   # W_up [P, H] (block 0), or W_down_eff [H, P] viewed flat as [P, H] (block 1)
+        r, grid = (up_range, ex.WUP_GRID) if i == 0 else (down_range, ex.WDOWN_GRID)
+        ints = np.random.default_rng((seed, e, i)).integers(-r, r + 1, size=(P, H) if i == 0 else (H, P), dtype=np.int8)
+        return (torch.from_numpy(ints).bfloat16() * 2.0 ** grid).reshape(P, H)
 
-    def __init__(self, cfg, seed: int, *, x_range: int = 4, wg_density: float = 1 / 16, up_range: int = 2,
-                 down_range: int = 2):
-        self.cfg, self.seed, self.up_range, self.down_range = cfg, seed, up_range, down_range
-        S, H, E = cfg.S, cfg.H, cfg.E
-        g = np.random.default_rng(seed)
-        x = g.integers(-x_range, x_range + 1, size=(S, H), dtype=np.int8)
-        wg = (g.integers(0, 2, size=(E, H), dtype=np.int8) * 2 - 1) * (g.random((E, H)) < wg_density)
-        self.x = torch.from_numpy(x).bfloat16().reshape(cfg.mini_batch, cfg.sequence_len, H)
-        self.wg = (torch.from_numpy(wg.astype(np.float32)) * 2.0 ** ex.WG_GRID).bfloat16().reshape(-1).reshape(H, E)
-        self.x64 = x.reshape(S, H).astype(np.float64)
-        self.wg_eff64 = wg.astype(np.float64) * 2.0 ** ex.WG_GRID
-        self.w_up64 = _PerExpert(lambda e: self._ints(e, 0).astype(np.float64) * 2.0 ** ex.WUP_GRID)       # [P, H]
-        self.w_down64 = _PerExpert(lambda e: self._ints(e, 1).astype(np.float64) * 2.0 ** ex.WDOWN_GRID)   # [H, P]
-        self.underflow_tokens = self.zero_tokens = np.zeros(0, np.int64)
-
-    def _ints(self, e: int, block: int) -> np.ndarray:
-        """int8 [P, H] of W_up (block 0) or [H, P] of W_down_eff (block 1) of expert e."""
-        P, H = self.cfg.P, self.cfg.H
-        r = self.up_range if block == 0 else self.down_range
-        g = np.random.default_rng((self.seed, e, block))
-        return g.integers(-r, r + 1, size=(P, H) if block == 0 else (H, P), dtype=np.int8)
-
-    def bias64(self, which):
-        return None
-
-    def device(self, dev):
-        """(x, gate weights, expert weights [E, 2, P, H], None, None) on `dev`; the down block is W_down_eff [H, P]
-        viewed flat as [P, H]."""
-        E, P, H = self.cfg.E, self.cfg.P, self.cfg.H
-        we = torch.empty((E, 2, P, H), dtype=torch.bfloat16, device=dev)
-        for e in range(E):
-            for block, grid in ((0, ex.WUP_GRID), (1, ex.WDOWN_GRID)):
-                w = torch.from_numpy(self._ints(e, block)).to(dev).bfloat16() * 2.0 ** grid
-                we[e, block] = w.reshape(P, H)
-        return self.x.to(dev), self.wg.to(dev), we, None, None
+    none = np.zeros(0, np.int64)
+    return ex.ExactInputs(cfg, torch.from_numpy(x).bfloat16().reshape(cfg.mini_batch, cfg.sequence_len, H),
+                          (torch.from_numpy(wg.astype(np.float32)) * 2.0 ** ex.WG_GRID).bfloat16().reshape(-1).reshape(H, E),
+                          ex.Experts(ex.PerExpert(block, (E, 2, P, H)), None, None, cfg.hidden_act), none, none)
 
 
 # ----------------------------------------------------------------------------- gated routing reference
@@ -329,78 +294,16 @@ def check_gated_routing(logits, bias, router, k, dev_idx, dev_go, dev_w, wg_x):
     return ambiguous
 
 
-# ----------------------------------------------------------------------------- device records from the reference
-def routed_device(inp: ex.ExactInputs, topk: np.ndarray, w: np.ndarray, EC: int, stats: Optional[ex.Stats] = None):
-    """A Device record of a routed launch on (topk, w) computed by the reference (ReLU: exact, GELU: the interval's
-    lower end), with recv_x, hidden and ret_y.  `stats` gets the h and out elements whose exact value needed
-    rounding."""
-    cfg = inp.cfg
-    E, H, P = cfg.E, cfg.H, cfg.P
-    n = topk.shape[0]
-    x = inp.x64[:n]
-    run = er.sanitize(topk, E)
-    w_bits = ex.f32_to_bf16(np.asarray(w, dtype=np.float32))
-    slot, counts, recv_cnt, kept = er.slots_from_routing(run, E, EC)
-    toks = ex.packet_tokens(run, slot, E, EC)
-    rmax = max(1, int(recv_cnt.max(initial=0)))
-    recv_x = np.zeros((E, rmax, H), np.uint16)
-    hidden = np.zeros((E, rmax, P), np.uint16)
-    ret_y = np.zeros((E, rmax, H), np.uint16)
-    for e in range(E):
-        c = len(toks[e])
-        if c == 0:
-            continue
-        recv_x[e, :c] = ex.f64_to_bf16(x[toks[e]])
-        h = ex.gemm0_reference(x[toks[e]], inp.w_up64[e], None if inp.bu is None else inp.bias64("up")[e],
-                               cfg.hidden_act, f"GEMM0 of expert {e}")
-        hidden[e, :c] = h.lo
-        y = ex.gemm1_reference(h.lo, inp.w_down64[e], None if inp.bd is None else inp.bias64("down")[e],
-                               f"GEMM1 of expert {e}")
-        ret_y[e, :c] = y.lo
-        if stats is not None:
-            stats.add("hidden", h.lo.size, ex.rounded_count(h))
-    y_of = ret_y[np.where(kept, run, 0), np.where(kept, slot, 0)]
-    out = er.combine_routed(y_of, kept, w_bits)
-    if stats is not None:   # the combine in real arithmetic against its bf16 result
-        real = (np.where(kept, ex.bits_to_f64(w_bits), 0.0)[:, :, None] * ex.bits_to_f64(y_of)).sum(1)
-        stats.add("out", out.size, int((ex.bits_to_f64(out) != real).sum()))
-    return ex.Device(out, run.copy(), w_bits, np.ones(n, np.float32), None, slot, counts, recv_cnt, recv_x, hidden,
-                     ret_y)
-
-
-def reference_device_gated(inp: ex.ExactInputs, router, bias, EC: int, n: Optional[int] = None,
-                           stats: Optional[ex.Stats] = None) -> ex.Device:
-    """The gated counterpart of exact.reference_device: a Device record computed from the interval midpoints (scores,
-    selection values, picks, weights), what a correct kernel could have produced.  The planted-fault tests start from
-    it."""
-    cfg = inp.cfg
-    x = inp.x64[: (cfg.S if n is None else n)]
-    sc = scores(router, cfg.k, x, inp.wg_eff64)
-    sel = selection(sc, bias, cfg.E)
-    G = group_scores(sel, router)[2] if router.n_group > 1 and x.shape[0] else None
-    picks = route_mid(sel.mid, router, cfg.k, G) if x.shape[0] else np.zeros((0, cfg.k), np.int32)
+def reference_routing(router, bias, k: int, x: np.ndarray, wg_eff: np.ndarray):
+    """A gated launch's routing computed from the interval midpoints (scores, selection values, picks, weights), what
+    a correct kernel could have produced: (picks int32 [n, k], fp32 weights [n, k], gate_out bf16 bits [n, E])."""
+    n, E = x.shape[0], wg_eff.shape[0]
+    sc = scores(router, k, x, wg_eff)
+    sel = selection(sc, bias, E)
+    G = group_scores(sel, router)[2] if router.n_group > 1 and n else None
+    picks = route_mid(sel.mid, router, k, G) if n else np.zeros((0, k), np.int32)
     w_lo, w_hi = weights_bounds(sc, picks, router)
-    dev = routed_device(inp, picks, (0.5 * (w_lo + w_hi)).astype(np.float32), EC, stats)
-    dev.gate_out = ex.f64_to_bf16(sc.s_mid)
-    return dev
-
-
-def weights_f32(w_bits: np.ndarray) -> np.ndarray:
-    """bf16 bits as the fp32 weights a routed replay takes (the same bits after rne_bf16)."""
-    return (np.asarray(w_bits, dtype=np.uint16).astype(np.uint32) << 16).view(np.float32)
-
-
-def check_gated_forward(inp: ex.ExactInputs, dev: ex.Device, router, bias, EC: int,
-                        stats: Optional[ex.Stats] = None, shared_s: Optional[np.ndarray] = None) -> int:
-    """A gated launch over the first n = len(dev.topk_idx) tokens: check_gated_routing, then every later stage as a
-    routed launch on the device's own routing (with a shared expert's s rows `shared_s`, out = rne(r + s)).  Returns
-    the number of ambiguous tokens."""
-    n = dev.topk_idx.shape[0]
-    x = inp.x64[:n]
-    amb = check_gated_routing(x @ inp.wg_eff64.T, bias, router, inp.cfg.k, dev.topk_idx, dev.gate_out, dev.topk_w,
-                              (x, inp.wg_eff64))
-    er.check_routed_forward(inp, dev, dev.topk_idx, weights_f32(dev.topk_w), EC, stats, shared_s)
-    return amb
+    return picks, (0.5 * (w_lo + w_hi)).astype(np.float32), ex.f64_to_bf16(sc.s_mid)
 
 
 # ----------------------------------------------------------------------------- training-mode auxiliary loss

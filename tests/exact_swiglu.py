@@ -1,4 +1,4 @@
-"""The exact-input reference (tests/exact.py) for SwiGLU experts (hidden_act = 2).
+"""The exact-input reference (tests/exact.py) for SwiGLU experts (hidden_act = 2): h's interval and the inputs.
 
 An expert's weights are [3, P, H]: W_gate, W_up and the P*H block flat-viewed as W_down [H, P].  The kernel computes
 g = fl(x W_gate^T + b_g), u = fl(x W_up^T + b_u) (both exact here: the inputs keep every partial sum exact in fp32) and
@@ -25,15 +25,11 @@ sparse, so y's sums stay on one fp32 grid.  No pytest in here.
 """
 from __future__ import annotations
 
-import dataclasses
-from typing import Optional
-
 import numpy as np
 import torch
 
 from flashmoe_b200.config import MoEConfig
 from tests import exact as ex
-from tests import exact_routed as er
 
 G_MIN = -64.0   # the generator keeps every gate pre-activation at or above this
 
@@ -41,21 +37,6 @@ G_MIN = -64.0   # the generator keeps every gate pre-activation at or above this
 def eps_swiglu(g: np.ndarray) -> np.ndarray:
     """Relative error bound of the kernel's h = silu(g) * u (module docstring)."""
     return 2.0 ** -21 + 2.0 ** -24 * (1.25 * np.abs(g) + 5.0)
-
-
-def swiglu_reference(rows: np.ndarray, w_gate: np.ndarray, w_up: np.ndarray, b_gate: Optional[np.ndarray],
-                     b_up: Optional[np.ndarray], what: str = "SwiGLU GEMM0") -> ex.Rounded:
-    """h [M, P] = RNE(silu(rows W_gate^T + b_g) * (rows W_up^T + b_u)) as an interval (float64 rows [M, H], weights
-    [P, H], biases [P] or None).  `exact` is the real value."""
-    ex.assert_exact_sums(rows, w_gate, b_gate, f"{what} (gate)")
-    ex.assert_exact_sums(rows, w_up, b_up, f"{what} (up)")
-    g = rows @ w_gate.T
-    u = rows @ w_up.T
-    if b_gate is not None:
-        g = g + b_gate[None, :]
-    if b_up is not None:
-        u = u + b_up[None, :]
-    return silu_mul_rounded(g, u)
 
 
 def silu_mul_rounded(g: np.ndarray, u: np.ndarray) -> ex.Rounded:
@@ -92,39 +73,6 @@ def silu_mul_f32_ends(g: np.ndarray, u: np.ndarray):
 
 
 # ----------------------------------------------------------------------------- inputs
-@dataclasses.dataclass
-class SwigluInputs:
-    """Exact SwiGLU inputs: the router's x and gate weights from exact.exact_inputs (x in {-1, 0, 1}), expert weights
-    we bf16 [E, 3, P, H], biases bu [E, 2, P] / bd [E, H] or None (CPU tensors)."""
-    base: ex.ExactInputs
-    we: torch.Tensor
-    bu: Optional[torch.Tensor]
-    bd: Optional[torch.Tensor]
-
-    @property
-    def cfg(self) -> MoEConfig:
-        return self.base.cfg
-
-    @property
-    def x64(self) -> np.ndarray:
-        return self.base.x64
-
-    def gate_up64(self, e: int):
-        w = self.we[e].double().numpy()
-        b = None if self.bu is None else self.bu[e].double().numpy()
-        return w[0], w[1], None if b is None else b[0], None if b is None else b[1]
-
-    def w_down64(self, e: int) -> np.ndarray:   # [H, P]: block 2 viewed flat
-        H, P = self.cfg.H, self.cfg.P
-        return self.we[e, 2].reshape(-1).reshape(H, P).double().numpy()
-
-    def bd64(self, e: int) -> Optional[np.ndarray]:
-        return None if self.bd is None else self.bd[e].double().numpy()
-
-    def device(self, dev):
-        return tuple(None if t is None else t.to(dev) for t in (self.base.x, self.base.wg, self.we, self.bu, self.bd))
-
-
 def _bf(a: np.ndarray) -> torch.Tensor:
     t = torch.from_numpy(np.ascontiguousarray(a)).bfloat16()
     assert np.array_equal(t.double().numpy(), a), "generator produced a value that is not a bf16 number"
@@ -156,95 +104,20 @@ def swiglu_weights(E: int, P: int, H: int, rng: np.random.Generator, bias: bool,
     return we, bu, bd
 
 
-def swiglu_inputs(cfg: MoEConfig, seed: int, bias: bool = False, **router_kw) -> SwigluInputs:
-    """Seeded exact inputs for a hidden_act = 2 context `cfg`; `router_kw` goes to exact.exact_inputs (the x and gate
-    weights)."""
+def swiglu_inputs(cfg: MoEConfig, seed: int, bias: bool = False, **router_kw) -> ex.ExactInputs:
+    """Seeded exact inputs for a hidden_act = 2 context `cfg`: the router's x and gate weights from exact.exact_inputs
+    (x in {-1, 0, 1}; `router_kw` goes there), the experts from swiglu_weights."""
     assert cfg.hidden_act == 2
-    base = ex.exact_inputs(cfg, seed, x_range=1, **router_kw)
-    we, bu, bd = swiglu_weights(cfg.E, cfg.P, cfg.H, np.random.default_rng(seed + 1), bias)
-    return SwigluInputs(base, _bf(we), None if bu is None else _bf(bu), None if bd is None else _bf(bd))
+    inp = ex.exact_inputs(cfg, seed, x_range=1, **router_kw)
+    inp.experts = swiglu_experts(cfg.E, cfg.P, cfg.H, np.random.default_rng(seed + 1), bias)
+    return inp
 
 
-def expert_h(inp: SwigluInputs, e: int, rows64: np.ndarray, what: str) -> ex.Rounded:
-    wg_, wu, bg, bu = inp.gate_up64(e)
-    return swiglu_reference(rows64, wg_, wu, bg, bu, what)
+def swiglu_experts(E: int, P: int, H: int, rng: np.random.Generator, bias: bool) -> ex.Experts:
+    we, bu, bd = swiglu_weights(E, P, H, rng, bias)
+    return ex.Experts(_bf(we), None if bu is None else _bf(bu), None if bd is None else _bf(bd), 2)
 
 
-# ----------------------------------------------------------------------------- the launch's stages
-def check_experts(inp: SwigluInputs, dev: ex.Device, EC: int, n: int, stats: Optional[ex.Stats] = None,
-                  shared_s: Optional[np.ndarray] = None, unscaled_k1: bool = True) -> ex.Stats:
-    """Every stage after routing of one launch over the first n tokens, given the device's routing (topk_idx, topk_w,
-    mcw; the router itself is exact.check_forward's, and tests/test_gpu_swiglu.py shows it equals a ReLU context's):
-    slot / counts / recv_cnt from topk_idx, recv_x, h inside its interval, ret_y bit for bit from the device's h, and
-    out from the combine of those y (plus s rows when `shared_s`).  `unscaled_k1`: the router route's k = 1 copy;
-    caller and gated routes scale k = 1 by topk_w over mcw = 1."""
-    cfg = inp.cfg
-    E, k, H = cfg.E, cfg.k, cfg.H
-    st = stats if stats is not None else ex.Stats()
-    x = inp.x64[:n]
-    slot, counts, recv_cnt, kept = er.slots_from_routing(dev.topk_idx, E, EC)   # (a caller's -1 picks take no slot)
-    ex.check_equal(dev.slot, slot, "slot", ("token", "pick"))
-    ex.check_equal(dev.counts, counts, "counts", ("expert",))
-    if dev.recv_cnt is not None:
-        ex.check_equal(dev.recv_cnt, recv_cnt, "recv_cnt", ("expert",))
-    toks = ex.packet_tokens(dev.topk_idx, slot, E, EC)
-    xb = ex.f64_to_bf16(x)
-    y_dev_ref = np.zeros((E, max(1, int(recv_cnt.max(initial=0))), H), np.uint16)
-    for e in range(E):
-        c = len(toks[e])
-        if c == 0:
-            continue
-        if dev.recv_x is not None:
-            ex.check_equal(dev.recv_x[e, :c], xb[toks[e]], f"recv_x of expert {e}", ("slot", "column"))
-        h_ref = expert_h(inp, e, x[toks[e]], f"GEMM0 of expert {e}")
-        h_dev = dev.hidden[e, :c]
-        w = ex._interval_check(h_dev, h_ref, f"hidden of expert {e}", ("slot", "column"))
-        st.add("hidden", h_dev.size, ex.rounded_count(h_ref), w)
-        y_ref = ex.gemm1_reference(h_dev, inp.w_down64(e), inp.bd64(e), f"GEMM1 of expert {e}")
-        y_dev_ref[e, :c] = y_ref.lo
-        if dev.ret_y is not None:
-            ex.check_equal(dev.ret_y[e, :c], y_ref.lo, f"ret_y of expert {e}", ("slot", "column"), signed_zero=False)
-            st.add("ret_y", c * H, ex.rounded_count(y_ref))
-    y_of = y_dev_ref[dev.topk_idx, np.where(kept, slot, 0)]
-    kk, pw = kept, dev.topk_w
-    if k == 1 and not unscaled_k1:   # the scaled sum of combine_tokens' k >= 2 path, of one term and one never-kept pad
-        def pad(a):
-            return np.concatenate([a, np.zeros_like(a[:, :1])], 1)
-        y_of, kk, pw = pad(y_of), pad(kept), pad(pw)
-    out_ref = ex.combine_tokens(y_of, kk, pw, dev.mcw)
-    dropped = ~kept.any(axis=1)
-    empty, what = np.zeros((int(dropped.sum()), H), np.uint16), "out"
-    if shared_s is not None:
-        out_ref, what = ex.add_shared(out_ref, shared_s), "out = rne(r + s)"
-        empty = ex.add_shared(ex.Rounded(empty, empty, 0), shared_s[dropped]).lo
-    w = ex._interval_check(dev.out, out_ref, what, ("token", "column"), max_width=None)
-    st.add(what, dev.out.size, ex.rounded_count(out_ref), w)
-    if dropped.any():
-        ex.check_equal(dev.out[dropped], empty, f"{what} rows of tokens whose picks were all dropped",
-                       ("row", "column"), signed_zero=shared_s is None)
-    return st
-
-
-# ----------------------------------------------------------------------------- the shared expert
-@dataclasses.dataclass
-class SharedSwiglu:
-    """A SwiGLU shared expert: w bf16 [3, Ps, H], bu [2, Ps] / bd [H] or None."""
-    w: torch.Tensor
-    bu: Optional[torch.Tensor]
-    bd: Optional[torch.Tensor]
-
-
-def shared_swiglu(H: int, Ps: int, seed: int, bias: bool = False) -> SharedSwiglu:
-    we, bu, bd = swiglu_weights(1, Ps, H, np.random.default_rng(seed), bias)
-    return SharedSwiglu(_bf(we[0]), None if bu is None else _bf(bu[0]), None if bd is None else _bf(bd[0]))
-
-
-def shared_reference(sh: SharedSwiglu, x64: np.ndarray, h_dev: np.ndarray, what: str = "shared expert"):
-    """(h_s interval [n, Ps], y_s from the device's h_s [n, H], exact) for tokens x64 [n, H]."""
-    H, Ps = sh.w.shape[2], sh.w.shape[1]
-    w = sh.w.double().numpy()
-    b = None if sh.bu is None else sh.bu.double().numpy()
-    h = swiglu_reference(x64, w[0], w[1], None if b is None else b[0], None if b is None else b[1], f"{what} GEMM0")
-    y = ex.gemm1_reference(h_dev, w[2].reshape(-1).reshape(H, Ps), None if sh.bd is None else sh.bd.double().numpy(),
-                           f"{what} GEMM1")
-    return h, y
+def shared_swiglu(H: int, Ps: int, seed: int, bias: bool = False) -> ex.Experts:
+    """A seeded SwiGLU shared expert (E = 1)."""
+    return swiglu_experts(1, Ps, H, np.random.default_rng(seed), bias)

@@ -17,7 +17,7 @@ other columns keep the generators' coarse h.  No pytest in here.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Dict
 
 import numpy as np
 import torch
@@ -105,58 +105,28 @@ def score_bias(E: int) -> np.ndarray:
     return b
 
 
-# ----------------------------------------------------------------------------- GELU
-def gelu_tail_rows(w_up: np.ndarray, w_down: np.ndarray, b_up: Optional[np.ndarray], rng) -> None:
-    """In place, for one expert (w_up [P, H], w_down [H, P], b_up [P] or None): the tail columns get an offset in
+# ----------------------------------------------------------------------------- the tail columns
+def gelu_tail_rows(w, down, b, rng) -> None:
+    """In place, for one GELU expert (w [2, P, H], W_down [H, P], b_up [P] or None): the tail columns get an offset in
     [-7, 3] on 2^-3 at the constant column, two entries +-2^-3 (x in [0, 8]: +-2 more), a signed bias in [-1, 1] on
     2^-3 and a zero W_down column."""
+    w_up = w[0]
     P, H = w_up.shape
     cols = np.flatnonzero(tail_columns(P))
     w_up[cols] = 0
     w_up[cols, H - 1] = rng.integers(-56, 25, size=cols.size) * 2.0 ** ex.WUP_GRID
     for p in cols:
         w_up[p, _free_cols(H, rng, 2)] = rng.choice([-1.0, 1.0], size=2) * 2.0 ** ex.WUP_GRID
-    w_down[:, cols] = 0
-    if b_up is not None:
-        b_up[cols] = rng.integers(-8, 9, size=cols.size) * 2.0 ** ex.WUP_GRID
+    down[:, cols] = 0
+    if b is not None:
+        b[cols] = rng.integers(-8, 9, size=cols.size) * 2.0 ** ex.WUP_GRID
 
 
-def gelu_tail_inputs(cfg, seed: int, bias: bool, saturate: bool = False, **router_kw) -> ex.ExactInputs:
-    """exact.exact_inputs(gelu_friendly) with GELU tail columns in every expert (and saturated router blocks)."""
-    base = ex.exact_inputs(cfg, seed, bias=bias, gelu_friendly=True, **router_kw)
-    E, P, H = cfg.E, cfg.P, cfg.H
-    rng = np.random.default_rng(seed + 7)
-    we = base.we.double().numpy().copy()
-    bu = None if base.bu is None else base.bu.double().numpy().copy()
-    for e in range(E):
-        down = we[e, 1].reshape(-1).reshape(H, P).copy()
-        gelu_tail_rows(we[e, 0], down, None if bu is None else bu[e], rng)
-        we[e, 1] = down.reshape(-1).reshape(P, H)
-    base.we = _bf(we)
-    base.bu = None if bu is None else _bf(bu)
-    base.__dict__.pop("w_up64", None)
-    base.__dict__.pop("w_down64", None)
-    constant_column(base)
-    if saturate:
-        saturating_router(base, seed + 11)
-    return base
-
-
-def gelu_tail_shared(H: int, Ps: int, seed: int, bias: bool) -> es.SharedInputs:
-    se = es.shared_inputs(H, Ps, seed, bias=bias, gelu_friendly=True)
-    w = se.w.double().numpy().copy()
-    down = w[1].reshape(-1).reshape(H, Ps).copy()
-    bu = None if se.bu is None else se.bu.double().numpy().copy()
-    gelu_tail_rows(w[0], down, bu, np.random.default_rng(seed + 5))
-    w[1] = down.reshape(-1).reshape(Ps, H)
-    return es.SharedInputs(_bf(w), None if bu is None else _bf(bu), se.bd)
-
-
-# ----------------------------------------------------------------------------- SwiGLU
-def swiglu_tail_rows(gate, up, down, b_gate, b_up, rng) -> None:
-    """In place, for one expert (gate / up [P, H], down [H, P], biases [P] or None; x in {-1, 0, 1}): the tail columns
-    get a gate offset from SWIGLU_OFFSETS at the constant column plus three entries in [-4, 4] on 1/2 (g within +-12 of
-    it, +-4 more from the bias), an up offset in +-[1, 4] and one entry +-1, and a zero W_down column."""
+def swiglu_tail_rows(w, down, b, rng) -> None:
+    """In place, for one SwiGLU expert (w [3, P, H], W_down [H, P], b_up [2, P] or None; x in {-1, 0, 1}): the tail
+    columns get a gate offset from SWIGLU_OFFSETS at the constant column plus three entries in [-4, 4] on 1/2 (g within
+    +-12 of it, +-4 more from the bias), an up offset in +-[1, 4] and one entry +-1, and a zero W_down column."""
+    gate, up = w[0], w[1]
     P, H = gate.shape
     cols = np.flatnonzero(tail_columns(P))
     gate[cols] = 0
@@ -167,35 +137,50 @@ def swiglu_tail_rows(gate, up, down, b_gate, b_up, rng) -> None:
         gate[p, _free_cols(H, rng, 3)] = rng.choice([v / 2 for v in range(-8, 9) if v], size=3)
         up[p, _free_cols(H, rng, 1)] = rng.choice([-1.0, 1.0])
     down[:, cols] = 0
-    if b_gate is not None:
-        b_gate[cols] = rng.integers(-8, 9, size=cols.size) * 0.5
-        b_up[cols] = rng.integers(-2, 3, size=cols.size)
+    if b is not None:
+        b[0, cols] = rng.integers(-8, 9, size=cols.size) * 0.5
+        b[1, cols] = rng.integers(-2, 3, size=cols.size)
 
 
-def swiglu_tail_inputs(cfg, seed: int, bias: bool, saturate: bool = False, **router_kw) -> sw.SwigluInputs:
-    """exact_swiglu.swiglu_inputs with SwiGLU tail columns in every expert (and saturated router blocks)."""
-    base = ex.exact_inputs(cfg, seed, x_range=1, **router_kw)
-    E, P, H = cfg.E, cfg.P, cfg.H
-    we, bu, bd = sw.swiglu_weights(E, P, H, np.random.default_rng(seed + 1), bias)
-    rng = np.random.default_rng(seed + 7)
+def with_tails(experts: ex.Experts, rng) -> ex.Experts:
+    """The record with the activation's tail columns (gelu_tail_rows, swiglu_tail_rows) in every expert, in order."""
+    tail_rows = gelu_tail_rows if experts.act == 1 else swiglu_tail_rows
+    w = experts.w.double().numpy().copy()
+    bu = None if experts.bu is None else experts.bu.double().numpy().copy()
+    E, m, P, H = w.shape
     for e in range(E):
-        down = we[e, 2].reshape(-1).reshape(H, P).copy()
-        swiglu_tail_rows(we[e, 0], we[e, 1], down, None if bu is None else bu[e, 0], None if bu is None else bu[e, 1],
-                         rng)
-        we[e, 2] = down.reshape(-1).reshape(P, H)
-    constant_column(base)
+        down = w[e, m - 1].reshape(-1).reshape(H, P).copy()
+        tail_rows(w[e], down, None if bu is None else bu[e], rng)
+        w[e, m - 1] = down.reshape(-1).reshape(P, H)
+    return ex.Experts(_bf(w), None if bu is None else _bf(bu), experts.bd, experts.act)
+
+
+def tail_inputs(cfg, seed: int, bias: bool, saturate: bool = False, **router_kw) -> ex.ExactInputs:
+    """Exact inputs with the tail columns of the context's activation (GELU: exact.exact_inputs(gelu_friendly);
+    SwiGLU: exact_swiglu.swiglu_inputs) in every expert, and saturated router blocks with `saturate`."""
+    if cfg.hidden_act == 1:
+        inp = ex.exact_inputs(cfg, seed, bias=bias, gelu_friendly=True, **router_kw)
+    else:
+        inp = sw.swiglu_inputs(cfg, seed, bias, **router_kw)
+    inp.experts = with_tails(inp.experts, np.random.default_rng(seed + 7))
+    constant_column(inp)
     if saturate:
-        saturating_router(base, seed + 11)
-    return sw.SwigluInputs(base, _bf(we), None if bu is None else _bf(bu), None if bd is None else _bf(bd))
+        saturating_router(inp, seed + 11)
+    return inp
 
 
-def swiglu_tail_shared(H: int, Ps: int, seed: int, bias: bool) -> sw.SharedSwiglu:
-    we, bu, bd = sw.swiglu_weights(1, Ps, H, np.random.default_rng(seed), bias)
-    down = we[0, 2].reshape(-1).reshape(H, Ps).copy()
-    swiglu_tail_rows(we[0, 0], we[0, 1], down, None if bu is None else bu[0, 0], None if bu is None else bu[0, 1],
-                     np.random.default_rng(seed + 5))
-    we[0, 2] = down.reshape(-1).reshape(Ps, H)
-    return sw.SharedSwiglu(_bf(we[0]), None if bu is None else _bf(bu[0]), None if bd is None else _bf(bd[0]))
+def tail_shared(H: int, Ps: int, seed: int, act: int, bias: bool) -> ex.Experts:
+    """A shared expert of activation `act` with the tail columns."""
+    if act == 1:
+        se = es.shared_inputs(H, Ps, seed, act=1, bias=bias, gelu_friendly=True)
+    else:
+        se = sw.shared_swiglu(H, Ps, seed, bias)
+    return with_tails(se, np.random.default_rng(seed + 5))
+
+
+def activation_regions(experts: ex.Experts, e: int, rows: np.ndarray) -> Dict[str, int]:
+    """The region counts (gelu_regions, swiglu_regions) of expert e's pre-activations for the rows."""
+    return (gelu_regions if experts.act == 1 else swiglu_regions)(*experts.pre(e, rows))
 
 
 # ----------------------------------------------------------------------------- regions

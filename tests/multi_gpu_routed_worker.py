@@ -15,7 +15,7 @@ import torch.distributed as dist  # noqa: E402
 
 from flashmoe_b200.config import MoEConfig  # noqa: E402
 from flashmoe_b200.runtime import MoEContext, env_rank_world  # noqa: E402
-from tests import exact_routed as er  # noqa: E402
+from tests import exact as ex  # noqa: E402
 
 CASES = [
     dict(num_experts=8, expert_top_k=2, sequence_len=512, hidden_size=256, intermediate_size=512),
@@ -55,7 +55,7 @@ def main():
                 ctx.synchronize()
                 print(f"RANK {rank} case {ci} launch {it} router n={n} OK", flush=True)
                 continue
-            topk, w = er.routing_case(n, cfg.E, cfg.k, seed=1000 * ci + 10 * it + rank, hot=rank % cfg.E)
+            topk, w = ex.routing_case(n, cfg.E, cfg.k, seed=1000 * ci + 10 * it + rank, hot=rank % cfg.E)
             idx_d, w_d = torch.from_numpy(topk).to(dev), torch.from_numpy(w).to(dev)
             out = ctx.forward_routed(x, idx_d, w_d, wed)
             ctx.synchronize()

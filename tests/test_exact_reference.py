@@ -11,12 +11,12 @@ from tests.util import check_output
 
 
 def _oracle(inp, EC, act):
-    cfg = inp.cfg
-    up, down = mo.split_expert_weights(ex.to_bits(inp.we))
+    cfg, xp = inp.cfg, inp.experts
+    up, down = mo.split_expert_weights(ex.to_bits(xp.w))
     return mo.forward(ex.to_bits(inp.x.reshape(cfg.S, cfg.H)),
                       mo.gate_weights_effective(ex.to_bits(inp.wg), cfg.E, cfg.H), up, down, k=cfg.k, EC=EC, act=act,
-                      b_up=None if inp.bu is None else ex.to_bits(inp.bu),
-                      b_down=None if inp.bd is None else ex.to_bits(inp.bd))
+                      b_up=None if xp.bu is None else ex.to_bits(xp.bu),
+                      b_down=None if xp.bd is None else ex.to_bits(xp.bd))
 
 
 @pytest.mark.parametrize("name", ["router_E8_k2_tc0", "router_E64_k4_tc0", "router_E129_k2_tc0", "k3", "fused_k1",
@@ -35,23 +35,22 @@ def test_oracle_agrees_with_exact_reference(name):
     assert ((o.mcw >= lo) & (o.mcw <= hi)).all()
     # h and y: the oracle's expert FFN on every packet against the reference
     xb = ex.to_bits(inp.x.reshape(cfg.S, cfg.H))
-    up, down = mo.split_expert_weights(ex.to_bits(inp.we))
+    xp = inp.experts
+    up, down = mo.split_expert_weights(ex.to_bits(xp.w))
     toks = ex.packet_tokens(ref.topk, slot, cfg.E, cfg.EC)
     y_all = np.zeros((cfg.E, max(1, max(len(t) for t in toks)), cfg.H), np.uint16)
     for e in range(cfg.E):
         if not len(toks[e]):
             continue
         h_o, y_o = mo.expert_ffn(xb[toks[e]], up[e], down[e], act=cfg.hidden_act,
-                                 b_up=None if inp.bu is None else ex.to_bits(inp.bu)[e],
-                                 b_down=None if inp.bd is None else ex.to_bits(inp.bd)[e])
-        h = ex.gemm0_reference(inp.x64[toks[e]], inp.w_up64[e], None if inp.bu is None else inp.bias64("up")[e],
-                               cfg.hidden_act, "GEMM0")
+                                 b_up=None if xp.bu is None else ex.to_bits(xp.bu)[e],
+                                 b_down=None if xp.bd is None else ex.to_bits(xp.bd)[e])
+        h = xp.h(e, inp.x64[toks[e]])
         if cfg.hidden_act == 0:
             ex.check_equal(h_o, h.lo, f"oracle h of expert {e}", ("slot", "column"))
         else:
             ex._interval_check(h_o, h, f"oracle h of expert {e}", ("slot", "column"))
-        y = ex.gemm1_reference(h_o, inp.w_down64[e], None if inp.bd is None else inp.bias64("down")[e], "GEMM1")
-        ex.check_equal(y_o, y.lo, f"oracle y of expert {e}", ("slot", "column"))
+        ex.check_equal(y_o, xp.y(e, h_o).lo, f"oracle y of expert {e}", ("slot", "column"))
         y_all[e, :len(toks[e])] = y_o
     pw = o.gate_out[np.arange(cfg.S)[:, None], o.topk_idx]
     out = ex.combine_tokens(y_all[ref.topk, np.where(kept, slot, 0)], kept, pw, o.mcw)
@@ -62,7 +61,7 @@ def test_oracle_agrees_with_exact_reference(name):
 def test_gpu_cases_are_exact_and_round(name):
     cfg, gen, env = gx.CASES[name]
     inp = ex.exact_inputs(cfg, seed=1000 + sum(map(ord, name)), **gen)   # the GPU test's seed
-    ex.check_preconditions(inp, cfg.EC, gx.MIN_H_ROUNDED, gx.MIN_OUT_ROUNDED, dense=gx._dense(cfg, env))
+    ex.check_preconditions(inp, cfg.EC, gx.MIN_H_ROUNDED, gx.MIN_OUT_ROUNDED, dense=ex.dense_path(cfg, env))
 
 
 def test_multi_launch_cases_are_exact_and_round():
@@ -88,13 +87,17 @@ def test_config_B_inputs_are_exact_and_round(seed):
 def _base(name="router_E8_k2_tc0", seed=11):
     cfg, gen, _ = gx.CASES[name]
     inp = ex.exact_inputs(cfg, seed=seed, **gen)
-    return cfg, inp, ex.reference_device(inp, cfg.EC)
+    return cfg, inp, ex.reference_launch("router", inp, cfg.EC, cfg.S)[0]
+
+
+def _check(inp, dev):
+    ex.check_launch("router", inp, inp.cfg.EC, inp.cfg.S, dev)
 
 
 def test_reference_device_passes_its_own_checks():
     for name in ("router_E8_k2_tc0", "router_E1024_k2", "k3", "bias_gelu"):
         cfg, inp, dev = _base(name)
-        ex.check_forward(inp, dev, cfg.EC)
+        _check(inp, dev)
 
 
 def test_fault_h_one_ulp():
@@ -102,7 +105,7 @@ def test_fault_h_one_ulp():
     e = int(np.argmax(dev.counts))
     dev.hidden[e, 3, 5] += 1
     with pytest.raises(AssertionError, match=f"hidden of expert {e}"):
-        ex.check_forward(inp, dev, cfg.EC)
+        _check(inp, dev)
 
 
 def test_fault_h_truncated_instead_of_rne():
@@ -110,10 +113,10 @@ def test_fault_h_truncated_instead_of_rne():
     slot, _, _, _ = ex.slots_from_topk(dev.topk_idx, cfg.E, cfg.EC)
     toks = ex.packet_tokens(dev.topk_idx, slot, cfg.E, cfg.EC)
     for e in range(cfg.E):
-        v = np.maximum(inp.x64[toks[e]] @ inp.w_up64[e].T, 0)
+        v = np.maximum(inp.experts.pre(e, inp.x64[toks[e]])[0], 0)
         dev.hidden[e, :len(toks[e])] = ex.f64_to_bf16_trunc(v)
     with pytest.raises(AssertionError, match="hidden of expert"):
-        ex.check_forward(inp, dev, cfg.EC)
+        _check(inp, dev)
 
 
 def test_fault_recv_x_rows_swapped():
@@ -122,7 +125,7 @@ def test_fault_recv_x_rows_swapped():
     a, b = 0, next(i for i in range(1, dev.recv_cnt[e]) if not np.array_equal(dev.recv_x[e, 0], dev.recv_x[e, i]))
     dev.recv_x[e, [a, b]] = dev.recv_x[e, [b, a]]
     with pytest.raises(AssertionError, match=f"recv_x of expert {e}"):
-        ex.check_forward(inp, dev, cfg.EC)
+        _check(inp, dev)
 
 
 def test_fault_tie_broken_toward_higher_index():
@@ -132,7 +135,7 @@ def test_fault_tie_broken_toward_higher_index():
     t = int(np.flatnonzero(lg[:, 0] == lg[:, 1])[0])   # a token whose two picks tie
     dev.topk_idx[t] = dev.topk_idx[t][::-1]
     with pytest.raises(AssertionError, match=f"topk_idx: 1 tokens differ; first token {t} "):
-        ex.check_forward(inp, dev, cfg.EC)
+        _check(inp, dev)
 
 
 def test_fault_underflow_tie_broken_by_logit():
@@ -145,28 +148,26 @@ def test_fault_underflow_tie_broken_by_logit():
     dev.topk_idx[t, 1:] = by_logit[: cfg.k - 1]
     assert not np.array_equal(dev.topk_idx[t], ref.topk[t])
     with pytest.raises(AssertionError, match=f"first token {t} "):
-        ex.check_forward(inp, dev, cfg.EC)
+        _check(inp, dev)
 
 
 def test_fault_dropped_pair_contribution_added():
     cfg, inp, dev = _base("packet_cut_at_EC")   # k = 1, experts cut at EC = 64: dropped tokens must be +0
     t = int(np.flatnonzero(dev.slot[:, 0] >= cfg.EC)[0])
     e = int(dev.topk_idx[t, 0])
-    h = ex.gemm0_reference(inp.x64[t:t + 1], inp.w_up64[e], None, 0, "GEMM0")
-    dev.out[t] = ex.gemm1_reference(h.lo, inp.w_down64[e], None, "GEMM1").lo[0]
+    dev.out[t] = inp.experts.y(e, inp.experts.h(e, inp.x64[t:t + 1]).lo).lo[0]
     with pytest.raises(AssertionError, match="out"):
-        ex.check_forward(inp, dev, cfg.EC)
+        _check(inp, dev)
     cfg, inp, dev = _base("router_E8_k2_tc0")   # k = 2: a pair cut at EC still adds its scaled y
     slot, _, _, kept = ex.slots_from_topk(dev.topk_idx, cfg.E, cfg.EC)
     t, j = (int(v) for v in np.argwhere(~kept & kept[:, ::-1])[0])   # one pick kept, the other dropped
     e = int(dev.topk_idx[t, j])
-    h = ex.gemm0_reference(inp.x64[t:t + 1], inp.w_up64[e], None, 0, "GEMM0")
-    y = ex.gemm1_reference(h.lo, inp.w_down64[e], None, "GEMM1").lo
+    y = inp.experts.y(e, inp.experts.h(e, inp.x64[t:t + 1]).lo).lo
     y_of = np.stack([dev.ret_y[dev.topk_idx[t, i], slot[t, i] if kept[t, i] else 0] for i in range(cfg.k)])[None]
     y_of[0, j] = y[0]
     dev.out[t] = ex.combine_tokens(y_of, np.ones((1, cfg.k), bool), dev.topk_w[t:t + 1], dev.mcw[t:t + 1]).lo[0]
     with pytest.raises(AssertionError, match=f"out: .* first at token {t},"):
-        ex.check_forward(inp, dev, cfg.EC)
+        _check(inp, dev)
 
 
 def test_fault_one_fragment_of_out_scaled_passes_check_output_but_not_the_exact_check():

@@ -156,27 +156,26 @@ def _cfg(act, E=16, k=2, S=512, H=320, P=320):
 
 def test_gelu_tail_inputs_reach_every_region_and_keep_gemm1_exact():
     cfg = _cfg(1)
-    inp = et.gelu_tail_inputs(cfg, 5, bias=True)
+    inp = et.tail_inputs(cfg, 5, bias=True)
     st = ex.check_preconditions(inp, cfg.EC, 0.3, 0.3)   # the reference's own launch passes every check
     assert st.d["hidden"][2] > 0
     regions = {}
     for e in range(cfg.E):
-        et.add_regions(regions, et.gelu_regions(inp.x64 @ inp.w_up64[e].T + inp.bias64("up")[e]))
+        et.add_regions(regions, et.activation_regions(inp.experts, e, inp.x64))
     assert regions["GELU v < 0"] > 1000 and regions["GELU -0 tail"] > 100, regions
-    v = inp.x64 @ inp.w_up64[0].T + inp.bias64("up")[0]
+    v = inp.experts.pre(0, inp.x64)[0]
     assert v.min() >= -11 and v.max() < 200 and (v[:, ~et.tail_columns(cfg.P)] >= 0).all()
 
 
 def test_swiglu_tail_inputs_reach_every_region_and_keep_gemm1_exact():
     cfg = _cfg(2)
-    inp = et.swiglu_tail_inputs(cfg, 6, bias=True)
+    inp = et.tail_inputs(cfg, 6, bias=True)
+    xp = inp.experts
     regions = {}
     for e in range(cfg.E):
-        wg_, wu, bg, bu = inp.gate_up64(e)
-        g, u = inp.x64 @ wg_.T + bg, inp.x64 @ wu.T + bu
+        g, u = xp.pre(e, inp.x64)
         et.add_regions(regions, et.swiglu_regions(g, u))
-        h = sw.expert_h(inp, e, inp.x64, "GEMM0")
-        ex.gemm1_reference(h.lo, inp.w_down64(e), inp.bd64(e), "GEMM1")   # asserts exact sums
+        xp.y(e, xp.h(e, inp.x64).lo)   # asserts exact sums
         assert np.abs(g).max() <= 136
     assert all(v > 50 for v in regions.values()), regions
 
@@ -187,18 +186,11 @@ def test_saturating_router_inputs_are_decided(act, router, k):
     """Every token of the saturated-router inputs is decided (ties by the lower index or group, absorbed biases),
     and the regions are populated; the reference's own launch passes check_gated_routing."""
     cfg = _cfg(act, k=k)
-    inp = (et.gelu_tail_inputs if act == 1 else et.swiglu_tail_inputs)(cfg, 7, bias=False, saturate=True)
-    base = inp if act == 1 else inp.base
+    inp = et.tail_inputs(cfg, 7, bias=False, saturate=True)
     bias = et.score_bias(cfg.E) if router.n_group > 1 else None
-    logits = base.x64 @ base.wg_eff64.T
-    sc = eg.scores(router, k, base.x64, base.wg_eff64)
-    sel = eg.selection(sc, bias, cfg.E)
-    G = eg.group_scores(sel, router)[2] if router.n_group > 1 else None
-    picks = eg.route_mid(sel.mid, router, k, G)
-    w_lo, w_hi = eg.weights_bounds(sc, picks, router)
-    w_bits = ex.f32_to_bf16((0.5 * (w_lo + w_hi)).astype(np.float32))
-    amb = eg.check_gated_routing(logits, bias, router, k, picks, ex.f64_to_bf16(sc.s_mid), w_bits,
-                                 (base.x64, base.wg_eff64))
+    logits = inp.x64 @ inp.wg_eff64.T
+    picks, w, gate_out = eg.reference_routing(router, bias, k, inp.x64, inp.wg_eff64)
+    amb = eg.check_gated_routing(logits, bias, router, k, picks, gate_out, ex.f32_to_bf16(w), (inp.x64, inp.wg_eff64))
     assert amb == 0
     reg = et.router_regions(logits, bias, router)
     assert reg["saturated score ties"] > 100 and reg["+0 scores"] > 50, reg

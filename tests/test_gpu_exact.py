@@ -105,35 +105,14 @@ def _ctx(cfg):
     return MoEContext(cfg, timeout_ms=5000)
 
 
-def _read(ctx, cfg, out, n, dense, gather):
-    E, H = cfg.E, cfg.H
-    return ex.Device(out=ex.to_bits(out.cpu()).reshape(n, H), topk_idx=ctx.read("topk_idx")[:n],
-                     topk_w=ctx.read("topk_w")[:n], mcw=ctx.read("mcw")[:n], gate_out=ctx.read("gate_out")[:n],
-                     slot=ctx.read("slot")[:n],
-                     counts=ctx.read("counts")[:E], recv_cnt=ctx.read("recv_cnt")[:E],
-                     recv_x=None if dense else ctx.read("recv_x"), hidden=ctx.read("hidden"),
-                     ret_y=ctx.read("ret_y") if gather else None)
-
-
-def _launch_and_check(ctx, cfg, inp, stats, n=None, dense=False, gather=False):
-    dev = ctx.device
-    x, wg, we, bu, bd = inp.device(dev)
-    if n is None:
-        out = ctx.forward(x, wg, we, bias_up=bu, bias_down=bd)
-        n_tok, EC = cfg.S, cfg.EC
-    else:
-        out = ctx.forward_tokens(x.reshape(cfg.S, cfg.H)[:n], wg, we, bias_up=bu, bias_down=bd)
-        n_tok, EC = n, cfg.EC_of(n)
+def _launch_and_check(ctx, inp, stats, n=None):
+    """One forward on `inp` (n = None: MoEContext.forward of all S tokens, else forward_tokens of n), checked."""
+    run = ex.Launcher(ctx, "router", inp)
+    out = run.launch(n)
     ctx.synchronize()
-    ex.check_forward(inp, _read(ctx, cfg, out, n_tok, dense, gather), EC, n=n_tok, stats=stats)
-
-
-def _gather(cfg, env):
-    return env.get("FM_FUSED_COMBINE") == "0" or cfg.k > 2
-
-
-def _dense(cfg, env):
-    return cfg.E == 1 and env.get("FM_DENSE_E1", "1") != "0"
+    n = inp.cfg.S if n is None else n
+    dev, _ = run.read(out, n)
+    run.check(dev, None, n, stats=stats)
 
 
 TOTAL = ex.Stats()
@@ -148,7 +127,7 @@ def test_every_stage_exact(monkeypatch, name):
     st = ex.Stats()
     ctx = _ctx(cfg)
     try:
-        _launch_and_check(ctx, cfg, inp, st, dense=_dense(cfg, env), gather=_gather(cfg, env))
+        _launch_and_check(ctx, inp, st)
     finally:
         ctx.close()
     TOTAL.merge(st)
@@ -163,7 +142,7 @@ def test_token_counts_on_one_context():
     ctx = _ctx(cfg)
     try:
         for n in TOKEN_COUNTS:
-            _launch_and_check(ctx, cfg, inp, st, n=n)
+            _launch_and_check(ctx, inp, st, n=n)
     finally:
         ctx.close()
     TOTAL.merge(st)
@@ -182,7 +161,7 @@ def test_epilogue_order_shape_five_launches(monkeypatch, fused):
     try:
         for i in range(5):
             inp = ex.exact_inputs(cfg, seed=3000 + 10 * fused + i, ties=tie_groups(cfg.E), zero_tokens=4)
-            _launch_and_check(ctx, cfg, inp, st, gather=not fused)
+            _launch_and_check(ctx, inp, st)
     finally:
         ctx.close()
     TOTAL.merge(st)
@@ -198,13 +177,13 @@ def test_config_B_three_launches_and_gather(monkeypatch):
     ctx = _ctx(cfg)
     try:
         for i in range(3):
-            _launch_and_check(ctx, cfg, ex.exact_inputs(cfg, seed=4000 + i, **CONFIG_B_GEN), st)
+            _launch_and_check(ctx, ex.exact_inputs(cfg, seed=4000 + i, **CONFIG_B_GEN), st)
     finally:
         ctx.close()
     monkeypatch.setenv("FM_FUSED_COMBINE", "0")
     ctx = _ctx(cfg)
     try:
-        _launch_and_check(ctx, cfg, ex.exact_inputs(cfg, seed=4010, **CONFIG_B_GEN), st, gather=True)
+        _launch_and_check(ctx, ex.exact_inputs(cfg, seed=4010, **CONFIG_B_GEN), st)
     finally:
         ctx.close()
     TOTAL.merge(st)

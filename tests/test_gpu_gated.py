@@ -13,8 +13,6 @@ from flashmoe_b200 import _lib
 from flashmoe_b200.config import MoEConfig
 from flashmoe_b200.router import RouterSpec
 from tests import exact as ex
-from tests import exact_routed as er
-from tests.exact_gated import check_gated_routing
 from tests.test_gated_api import gated_routing_f64
 from tests.torch_gated import moe_forward_gated_cpu
 from tests.torch_routed import moe_forward_routed_cpu
@@ -125,28 +123,14 @@ def test_exact_inputs(monkeypatch, name):
     cfg = MoEConfig(num_experts=E, expert_top_k=k, sequence_len=256, hidden_size=128, intermediate_size=192)
     inp = ex.exact_inputs(cfg, seed=9000 + sum(map(ord, name)))
     ctx = _ctx(cfg)
-    dev = ctx.device
-    x, wg, we, bu, bd = inp.device(dev)
-    x = x.reshape(cfg.S, cfg.H)
     bias = (np.random.default_rng(len(name)).permutation(E) * 2.0 ** -9 - 0.05).astype(np.float32) if with_bias \
         else None
-    sb = torch.from_numpy(bias).to(dev) if bias is not None else None
-    gather = env.get("FM_FUSED_COMBINE") == "0" or k > 2
+    run = ex.Launcher(ctx, "gated", inp, router=router, score_bias=bias)
     st = ex.Stats()
     amb_total = tok_total = 0
     for n in (cfg.S, 0, 1, 97):
-        out = ctx.forward_gated(x[:n], wg, we, router, score_bias=sb, bias_up=bu, bias_down=bd)
-        ctx.synchronize()
-        idx, w_bits, go = ctx.read("topk_idx")[:n], ctx.read("topk_w")[:n], ctx.read("gate_out")[:n]
-        logits = inp.x64[:n] @ inp.wg_eff64.T
-        amb_total += check_gated_routing(logits, bias, router, k, idx, go, w_bits, (inp.x64[:n], inp.wg_eff64))
+        amb_total += run.run(n, stats=st)[2]
         tok_total += n
-        w = (w_bits.astype(np.uint32) << 16).view(np.float32)
-        d = ex.Device(out=ex.to_bits(out.cpu()).reshape(n, cfg.H), topk_idx=idx, topk_w=w_bits,
-                      mcw=ctx.read("mcw")[:n], gate_out=None, slot=ctx.read("slot")[:n], counts=ctx.read("counts"),
-                      recv_cnt=ctx.read("recv_cnt"), recv_x=ctx.read("recv_x"), hidden=ctx.read("hidden"),
-                      ret_y=ctx.read("ret_y") if gather else None)
-        er.check_routed_forward(inp, d, idx, w, cfg.EC_of(n), st)
     ctx.close()
     print(f"\n[{name}] ambiguous tokens {amb_total} of {tok_total}; {st.line()}")
     assert amb_total <= max(0, tok_total // 1000), f"{amb_total} ambiguous tokens of {tok_total}"

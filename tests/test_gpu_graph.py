@@ -309,14 +309,13 @@ def test_replayed_device_count_graph_exact_stage_by_stage():
     cfg = MoEConfig(num_experts=8, expert_top_k=2, sequence_len=512, hidden_size=128, intermediate_size=128)
     inp = ex.exact_inputs(cfg, seed=1701, ties=[(0, cfg.E - 1), (2, 3)], zero_tokens=4, underflow_tokens=8)
     ctx = _ctx(cfg)
-    dev = ctx.device
-    x, wg, we, bu, bd = inp.device(dev)
-    xs = x.reshape(cfg.S, cfg.H)
+    run = ex.Launcher(ctx, "router", inp)
+    xs = run.x
     x_full, out_full = torch.empty_like(xs), torch.empty_like(xs)
-    n_dev = torch.zeros(1, dtype=torch.int32, device=dev)
+    n_dev = torch.zeros(1, dtype=torch.int32, device=ctx.device)
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph):
-        ctx.forward_tokens(x_full, wg, we, bias_up=bu, bias_down=bd, out=out_full, n_tokens=n_dev)
+        run.launch(cfg.S, out=out_full, n_tokens=n_dev, x=x_full)
     st = ex.Stats()
     for n in (1, 129, 300, 512):
         x_full.copy_(xs)
@@ -324,11 +323,7 @@ def test_replayed_device_count_graph_exact_stage_by_stage():
         n_dev.fill_(n)
         graph.replay()
         ctx.synchronize()
-        E, H = cfg.E, cfg.H
-        d = ex.Device(out=ex.to_bits(out_full[:n].cpu()), topk_idx=ctx.read("topk_idx")[:n],
-                      topk_w=ctx.read("topk_w")[:n], mcw=ctx.read("mcw")[:n], gate_out=ctx.read("gate_out")[:n],
-                      slot=ctx.read("slot")[:n], counts=ctx.read("counts")[:E], recv_cnt=ctx.read("recv_cnt")[:E],
-                      recv_x=ctx.read("recv_x"), hidden=ctx.read("hidden"), ret_y=None)
-        ex.check_forward(inp, d, cfg.EC_of(n), n=n, stats=st)
+        d, _ = run.read(out_full[:n], n)
+        run.check(d, None, n, stats=st)
     ctx.close()
     print(f"\n[device-count graph, exact] {st.line()}")

@@ -1,6 +1,6 @@
 """Forwards on the caller's routing (MoEContext.forward_routed -> fm_moe_forward_routed) on one H100: the router's own
 routing replayed (bit-identical bookkeeping and rows), every stage exact on inputs whose sums are exact in fp32
-(tests/exact_routed.py), random inputs at config B against tests/torch_routed.py, invalid indices, CUDA graphs with a
+(tests/exact.py), random inputs at config B against tests/torch_routed.py, invalid indices, CUDA graphs with a
 device-side count, rejected contexts, argument checks and the nn.Module wrapper."""
 import numpy as np
 import pytest
@@ -9,7 +9,6 @@ import torch
 from flashmoe_b200 import _lib
 from flashmoe_b200.config import BASELINE_CONFIGS, MoEConfig
 from tests import exact as ex
-from tests import exact_routed as er
 from tests.torch_routed import moe_forward_routed_cpu
 from tests.util import check_output, make_inputs
 
@@ -95,27 +94,20 @@ def test_every_stage_exact(monkeypatch, name):
         monkeypatch.setenv(k, v)
     inp = ex.exact_inputs(cfg, seed=5000 + sum(map(ord, name)), **gen)
     ctx = _ctx(cfg)
-    dev = ctx.device
-    x, _, we, bu, bd = inp.device(dev)
-    x = x.reshape(cfg.S, cfg.H)
-    gather = env.get("FM_FUSED_COMBINE") == "0" or cfg.k > 2
     st = ex.Stats()
     for n in (cfg.S, 0, 1, 97):
-        topk, w = er.routing_case(n, cfg.E, cfg.k, seed=n + 17, hot=2, empty=(5,))
+        topk, w = ex.routing_case(n, cfg.E, cfg.k, seed=n + 17, hot=2, empty=(5,))
         if n > 1:
             topk[1] = -1                                          # a token with no pick at all
-        idx_d, w_d = torch.from_numpy(topk).to(dev), torch.from_numpy(w).to(dev)
-        out = ctx.forward_routed(x[:n], idx_d, w_d, we, bias_up=bu, bias_down=bd)
+        run = ex.Launcher(ctx, "routed", inp, routing=(topk, w))
+        out = run.launch(n)
         ctx.synchronize()
         assert out.shape == (n, cfg.H)
-        d = ex.Device(out=ex.to_bits(out.cpu()).reshape(n, cfg.H), topk_idx=ctx.read("topk_idx")[:n],
-                      topk_w=ctx.read("topk_w")[:n], mcw=ctx.read("mcw")[:n], gate_out=None, slot=ctx.read("slot")[:n],
-                      counts=ctx.read("counts"), recv_cnt=ctx.read("recv_cnt"), recv_x=ctx.read("recv_x"),
-                      hidden=ctx.read("hidden"), ret_y=ctx.read("ret_y") if gather else None)
-        er.check_routed_forward(inp, d, topk, w, cfg.EC_of(n), st)
+        d, _ = run.read(out, n)
+        run.check(d, None, n, stats=st)
         if n == cfg.S:
             slot = d.slot
-            assert (slot == er.INT32_MAX).any() and ((slot >= cfg.EC) & (slot < er.INT32_MAX)).any()
+            assert (slot == ex.INT32_MAX).any() and ((slot >= cfg.EC) & (slot < ex.INT32_MAX)).any()
     ctx.close()
     print(f"\n[{name}] {st.line()}")
 
@@ -141,7 +133,7 @@ def test_invalid_index_is_reported_once_and_treated_as_minus_one():
     ctx = _ctx(cfg)
     dev = ctx.device
     x, wed = inp_x.reshape(cfg.S, cfg.H).to(dev), we.to(dev)
-    topk, w = er.routing_case(cfg.S, cfg.E, cfg.k, seed=3, skip_frac=0.0)
+    topk, w = ex.routing_case(cfg.S, cfg.E, cfg.k, seed=3, skip_frac=0.0)
     clean = topk.copy()
     clean[100, 1] = -1
     clean[400, 0] = -1

@@ -16,7 +16,6 @@ from flashmoe_b200 import _lib
 from flashmoe_b200.config import MoEConfig
 from flashmoe_b200.router import RouterSpec
 from tests import exact as ex
-from tests import exact_routed as er
 from tests.util import make_inputs
 
 pytestmark = pytest.mark.gpu
@@ -64,7 +63,7 @@ class Route:
         self.ctx, self.name = ctx, name
         self.x, self.wg, self.we = x.reshape(cfg.S, cfg.H).to(dev), wg.to(dev), we.to(dev)
         self.bu, self.bd = bu.to(dev), bd.to(dev)
-        idx, w = er.routing_case(cfg.S, cfg.E, cfg.k, seed=seed + 1)
+        idx, w = ex.routing_case(cfg.S, cfg.E, cfg.k, seed=seed + 1)
         self.idx, self.w = torch.from_numpy(idx).to(dev), torch.from_numpy(w).to(dev)
 
     def __call__(self, n, shared=None, out=None, n_tokens=None, x=None):
@@ -171,16 +170,14 @@ def test_shared_y_exact_reference_relu():
     inp = ex.exact_inputs(BASE.replace(num_experts=1, expert_top_k=1, intermediate_size=ps), seed=21, bias=True)
     ctx = _ctx(BASE)
     try:
-        from flashmoe_b200.runtime import SharedExpert
-
         dev = ctx.device
         route = Route(ctx, "router", seed=22)
-        se = SharedExpert(inp.we[0].to(dev), inp.bu[0].to(dev), inp.bd[0].to(dev))
+        xp = inp.experts
+        se = ex.shared_expert(xp, dev)
         x = inp.x.reshape(S, H).to(dev)
         route(S, shared=se, x=x)
         ctx.synchronize()
-        h = ex.gemm0_reference(inp.x64, inp.w_up64[0], inp.bias64("up")[0], 0, "shared h")
-        y = ex.gemm1_reference(h.lo, inp.w_down64[0], inp.bias64("down")[0], "shared y")
+        y = xp.y(0, xp.h(0, inp.x64, "shared h").lo, "shared y")
         ex.check_equal(ctx.read("shared_y"), y.lo, "shared_y", ("token", "column"))
     finally:
         ctx.close()

@@ -19,16 +19,13 @@ from flashmoe_b200.config import MoEConfig
 from flashmoe_b200.router import RouterSpec
 from tests import exact as ex
 from tests import exact_gated as eg
-from tests import exact_routed as er
 from tests import exact_shared as es
 from tests import test_gpu_exact as gx
-from tests import test_gpu_subchunks as gs
 
 pytestmark = pytest.mark.gpu
 
 V3 = RouterSpec("sigmoid", 8, 4, 2, True, 2.5)
 LLAMA4 = RouterSpec("sigmoid", renormalize=False)
-MAX_AMBIGUOUS = 0.01   # gated tokens whose picks the intervals cannot decide (their later stages are still checked)
 TAIL_H, TAIL_PS = (192, 320), (64, 192, 320, 1408)
 N_GRID = -1            # a launch's n: grid * BLOCK_M + 1 on the context's own grid (tpc > BLOCK_M)
 
@@ -56,10 +53,6 @@ class Case:
     @property
     def lag(self):
         return int(dict(self.env).get("FM_G1_LAG", -1))
-
-    @property
-    def gather(self):
-        return dict(self.env).get("FM_FUSED_COMBINE") == "0" or self.cfg.k > 2
 
 
 def _tail(route, H, act):
@@ -108,20 +101,20 @@ def case_inputs(c: Case):
     return ex.exact_inputs(c.cfg, seed=c.seed, **gen)
 
 
-def case_shared(c: Case, Ps: int) -> es.SharedInputs:
+def case_shared(c: Case, Ps: int) -> ex.Experts:
     """The shared expert of a launch with intermediate size Ps: GELU ones gelu_friendly, with W_down_s sparse enough
     that GEMM1's sums stay exact over long Ps."""
     kw = dict(bias=True)
     if c.act:
         kw.update(gelu_friendly=True, up_range=4, down_density=min(1.0, 64 / Ps))
-    return es.shared_inputs(c.cfg.H, Ps, seed=c.seed + Ps, **kw)
+    return es.shared_inputs(c.cfg.H, Ps, seed=c.seed + Ps, act=c.act, **kw)
 
 
 def case_routing(c: Case):
     """(topk_idx, topk_w) for all S tokens of a routed case: skew past EC onto expert 3, duplicates, -1 picks and an
     empty expert (E - 1)."""
     cfg = c.cfg
-    return er.routing_case(cfg.S, cfg.E, cfg.k, c.seed, hot=3, hot_frac=0.3 if cfg.E <= 16 else 0.05, empty=(cfg.E - 1,))
+    return ex.routing_case(cfg.S, cfg.E, cfg.k, c.seed, hot=3, hot_frac=0.3 if cfg.E <= 16 else 0.05, empty=(cfg.E - 1,))
 
 
 def case_score_bias(c: Case) -> Optional[np.ndarray]:
@@ -152,40 +145,9 @@ def _ctx(cfg, shared_inter):
     return MoEContext(cfg, timeout_ms=10000, shared_inter=shared_inter)
 
 
-class Runner:
-    """One context of a case and its device inputs; `launch` runs and reads back one forward with a shared expert."""
-
-    def __init__(self, c: Case, ctx, inp):
-        self.c, self.ctx, self.inp = c, ctx, inp
-        cfg, dev = c.cfg, ctx.device
-        x, self.wg, self.we, self.bu, self.bd = inp.device(dev)
-        self.x = x.reshape(cfg.S, cfg.H)
-        self.routing = case_routing(c) if c.route == "routed" else None
-        if self.routing is not None:
-            self.idx, self.w = (torch.from_numpy(a).to(dev) for a in self.routing)
-        self.sb = case_score_bias(c)
-        self.sb_dev = None if self.sb is None else torch.from_numpy(self.sb).to(dev)
-
-    def call(self, n, se, out=None, n_tokens=None, x=None):
-        ctx, route = self.ctx, self.c.route
-        x = self.x[:n] if x is None else x
-        m = x.shape[0]
-        kw = dict(bias_up=self.bu, bias_down=self.bd, out=out, n_tokens=n_tokens, shared_expert=se)
-        if route == "router":
-            return ctx.forward_tokens(x, self.wg, self.we, **kw)
-        if route == "routed":
-            return ctx.forward_routed(x, self.idx[:m], self.w[:m], self.we, **kw)
-        return ctx.forward_gated(x, self.wg, self.we, V3, score_bias=self.sb_dev, **kw)
-
-    def read(self, out, n):
-        ctx = self.ctx
-        dev = gs._device(ctx, self.c.cfg, out, n, self.c.gather, gate_out=self.c.route != "routed")
-        h_s = ctx.read("shared_hidden")
-        return dev, es.SharedRecord(h_s[:n].copy(), ctx.read("shared_y")[:n].copy())
-
-    def check(self, se, dev, rec, n, st):
-        return es.check_launch(self.c.route, self.inp, se, dev, rec, self.c.cfg.EC_of(n), self.c.act,
-                               routing=self.routing, router=V3, score_bias=self.sb, stats=st)
+def launcher(c: Case, ctx, inp) -> ex.Launcher:
+    return ex.Launcher(ctx, c.route, inp, routing=case_routing(c) if c.route == "routed" else None, router=V3,
+                       score_bias=case_score_bias(c))
 
 
 TOTAL = ex.Stats()
@@ -204,21 +166,17 @@ def test_shared_every_stage_exact(monkeypatch, name):
         grid = ctx.dims["grid"]
         missing = set(c.reach) - reached(c, grid)
         assert not missing, f"the launches do not reach {sorted(missing)} on {grid} CTAs"
-        run = Runner(c, ctx, inp)
+        run = launcher(c, ctx, inp)
         print(f"\n[{name}] grid {grid}")
         for ps, n in launch_ns(c, grid):
-            se = case_shared(c, ps)
-            out = run.call(n, se.device(ctx.device))
-            ctx.synchronize()
-            dev, rec = run.read(out, n)
-            amb += run.check(se, dev, rec, n, st)
+            amb += run.run(n, case_shared(c, ps), st)[2]
             tok += n
             print(f"  Ps={ps} n={n}: {case_regime(c, ps, n, grid).line()}")
     finally:
         ctx.close()
     TOTAL.merge(st)
     print(f"  ambiguous tokens {amb} of {tok}; {time.time() - t0:.1f} s\n  Stats: {st.line()}")
-    assert amb <= MAX_AMBIGUOUS * tok, f"{amb} ambiguous tokens of {tok}"
+    assert amb <= ex.MAX_AMBIGUOUS * tok, f"{amb} ambiguous tokens of {tok}"
 
 
 def test_shared_hidden_readback():
@@ -232,15 +190,11 @@ def test_shared_hidden_readback():
     try:
         with pytest.raises(FlashMoEError, match=r"h_s exists only after a launch with one"):
             ctx.read("shared_hidden")
-        run = Runner(c, ctx, inp)
+        run = launcher(c, ctx, inp)
         for ps in (1408, 192):
-            se = case_shared(c, ps)
-            out = run.call(301, se.device(ctx.device))
-            ctx.synchronize()
-            d, rec = run.read(out, 301)
-            run.check(se, d, rec, 301, ex.Stats())
+            _, rec, _ = run.run(301, case_shared(c, ps))
             assert ctx.read("shared_hidden").shape == (c.cfg.S, ps)
-        run.call(301, None)
+        run.launch(301)
         ctx.synchronize()
         assert np.array_equal(ctx.read("shared_hidden")[:301], rec.h_s)
     finally:
@@ -259,21 +213,21 @@ def test_graph_device_count_replays_exact():
     st = ex.Stats()
     try:
         dev = ctx.device
-        run = Runner(c, ctx, inp)
+        run = launcher(c, ctx, inp)
         S, H = c.cfg.S, c.cfg.H
-        sed = se.device(dev)
+        sed = ex.shared_expert(se, dev)
         x_full = run.x.clone()
         cnt = torch.tensor([S], dtype=torch.int32, device=dev)
         out = torch.full((S, H), 3.0, dtype=torch.bfloat16, device=dev)
         s = torch.cuda.Stream(dev)
         s.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(s):
-            run.call(S, sed, out=out, n_tokens=cnt, x=x_full)   # warm-up
+            run.launch(S, sed, out=out, n_tokens=cnt, x=x_full)   # warm-up
         torch.cuda.current_stream(dev).wait_stream(s)
         ctx.synchronize()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            run.call(S, sed, out=out, n_tokens=cnt, x=x_full)
+            run.launch(S, sed, out=out, n_tokens=cnt, x=x_full)
         for n in (S, 1, 0, 301, 129, S):
             x_full.copy_(run.x)
             x_full[n:] = float("nan")
@@ -283,8 +237,8 @@ def test_graph_device_count_replays_exact():
             ctx.synchronize()
             assert ctx.launch_record()[1] == n
             assert (out[n:] == 3.0).all(), f"replay n={n}: rows past n written"
-            d, rec = run.read(out[:n], n)
-            run.check(se, d, rec, n, st)
+            d, rec = run.read(out[:n], n, shared=True)
+            run.check(d, rec, n, se, st)
     finally:
         ctx.close()
     TOTAL.merge(st)
@@ -301,13 +255,10 @@ def test_training_context_aux_unchanged():
     ctx = _ctx(c.cfg, ps)
     st = ex.Stats()
     try:
-        run = Runner(c, ctx, inp)
+        run = launcher(c, ctx, inp)
         grid = ctx.dims["grid"]
         for n in (512, 301, 1, 0):
-            out = run.call(n, se.device(ctx.device))
-            ctx.synchronize()
-            d, rec = run.read(out, n)
-            run.check(se, d, rec, n, st)
+            d, _, _ = run.run(n, se, st)
             ref = ex.router_reference(inp.x64[:n], inp.wg_eff64, c.cfg.k)
             eg.check_aux(ctx.read("aux_loss").copy(), ref, d.counts, n,
                          eg.regime(c.cfg.E, c.cfg.k, n, grid, eg.tc_router(c.cfg.E)))
@@ -329,14 +280,14 @@ LAYERS = {
 
 def layer_shared(name):
     cfg, _, ps = LAYERS[name]
-    return es.shared_inputs(cfg.H, ps, seed=8000 + len(name), up_range=2, down_range=2)
+    return es.shared_inputs(cfg.H, ps, seed=8000 + len(name), act=cfg.hidden_act, up_range=2, down_range=2)
 
 
 @pytest.mark.parametrize("name", list(LAYERS))
 def test_model_shape_exact(name):
     cfg, router, ps = LAYERS[name]
     t0 = time.time()
-    li = eg.LayerInputs(cfg, seed=8100 + len(name))
+    li = eg.layer_inputs(cfg, seed=8100 + len(name))
     se = layer_shared(name)
     ctx = _ctx(cfg, ps)
     st = ex.Stats()
@@ -346,7 +297,7 @@ def test_model_shape_exact(name):
         wg = li.wg.to(dev)
         g = torch.Generator(device=dev).manual_seed(8200 + len(name))
         we = (torch.randn(cfg.E, 2, cfg.P, cfg.H, device=dev, generator=g) * cfg.H ** -0.5).bfloat16()
-        sed = se.device(dev)
+        sed = ex.shared_expert(se, dev)
         grid = ctx.dims["grid"]
         for n in (cfg.S, 301):
             r = ctx.forward_gated(x[:n], wg, we, router).clone()
@@ -360,7 +311,7 @@ def test_model_shape_exact(name):
                 ex.check_equal(got, want, f"{t} (vs the call without a shared expert)", ("row", "column")[:want.ndim])
             st.add("routing tables", sum(v.size for v in tables.values()))
             h_s, y_s = ctx.read("shared_hidden")[:n].copy(), ctx.read("shared_y")[:n].copy()
-            es.check_shared(li, se, h_s, y_s, n, cfg.hidden_act, st)
+            ex.shared_stage(li.x64[:n], se, ex.SharedRecord(h_s, y_s), st)
             r_bits = ex.to_bits(r.cpu())
             want = ex.add_shared(ex.Rounded(r_bits, r_bits, 0), y_s)
             ex.check_equal(ex.to_bits(out.cpu()), want.lo, "out = rne(r_dev + s)", ("token", "column"),

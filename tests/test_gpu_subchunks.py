@@ -22,7 +22,6 @@ from flashmoe_b200.router import RouterSpec
 from oracle import moe_oracle as mo
 from tests import exact as ex
 from tests import exact_gated as eg
-from tests import exact_routed as er
 from tests import test_gpu_exact as gx
 
 pytestmark = pytest.mark.gpu
@@ -44,7 +43,7 @@ class Case:
     bias_log2: Optional[int] = None    # score bias (permutation(E) - E / 2) * 2^bias_log2; None: no bias
     env: tuple = ()
     gen: tuple = ()                    # exact_inputs keyword arguments
-    layer: bool = False                # exact_gated.LayerInputs (a model-sized layer) instead of exact_inputs
+    layer: bool = False                # exact_gated.layer_inputs (a model-sized layer) instead of exact_inputs
     amb_share: float = 0.001           # ambiguous tokens allowed (their picks are not checked)
 
     @property
@@ -112,7 +111,7 @@ def for_device(c: Case, sms: int) -> Case:
 
 def case_inputs(c: Case):
     if c.layer:
-        return eg.LayerInputs(c.cfg, seed=c.seed)
+        return eg.layer_inputs(c.cfg, seed=c.seed)
     gen = dict(c.gen)
     if c.kind == "router":   # the router cases of tests/test_gpu_exact.py: exact ties, x = 0 tokens, exp underflow
         gen = dict(ties=gx.tie_groups(c.cfg.E), zero_tokens=4, underflow_tokens=8)
@@ -130,19 +129,7 @@ def case_routing(c: Case):
     """(topk_idx, topk_w) of a routed case for all S tokens: skew past EC onto expert 3, duplicates, -1 and an empty
     expert (E - 1); the first n rows are a launch's routing."""
     E, k = c.cfg.E, c.cfg.k
-    return er.routing_case(c.cfg.S, E, k, c.seed, hot=3, hot_frac=0.05, empty=(E - 1,))
-
-
-def _gather(c: Case) -> bool:
-    return dict(c.env).get("FM_FUSED_COMBINE") == "0" or c.cfg.k > 2
-
-
-def _device(ctx, cfg, out, n, gather, gate_out=True):
-    return ex.Device(out=ex.to_bits(out.cpu()).reshape(n, cfg.H), topk_idx=ctx.read("topk_idx")[:n].copy(),
-                     topk_w=ctx.read("topk_w")[:n].copy(), mcw=ctx.read("mcw")[:n].copy(),
-                     gate_out=ctx.read("gate_out")[:n].copy() if gate_out else None, slot=ctx.read("slot")[:n].copy(),
-                     counts=ctx.read("counts").copy(), recv_cnt=ctx.read("recv_cnt").copy(), recv_x=ctx.read("recv_x"),
-                     hidden=ctx.read("hidden"), ret_y=ctx.read("ret_y") if gather else None)
+    return ex.routing_case(c.cfg.S, E, k, c.seed, hot=3, hot_frac=0.05, empty=(E - 1,))
 
 
 def _check_training(ctx, c, inp, dev, n, rg):
@@ -181,34 +168,16 @@ def test_subchunks_every_stage_exact(monkeypatch, name):
             assert len(rg.sub_chunks) >= c.min_sub, f"the fullest CTA takes {len(rg.sub_chunks)} sub-chunks"
         if c.full_scratch:
             assert rg.sel_entries == eg.G_SEL_MAX, f"tpc * k = {rg.sel_entries}, not the full router scratch"
-        dev = ctx.device
-        x, wg, we, bu, bd = inp.device(dev)
-        x = x.reshape(cfg.S, cfg.H)
-        sb = None if bias is None else torch.from_numpy(bias).to(dev)
-        if c.kind == "routed":
-            idx_all, w_all = case_routing(c)
-            idx_d, w_d = torch.from_numpy(idx_all).to(dev), torch.from_numpy(w_all).to(dev)
+        run = ex.Launcher(ctx, c.kind, inp, routing=case_routing(c) if c.kind == "routed" else None,
+                          router=c.router, score_bias=bias)
         st = ex.Stats()
         amb = 0
         for n in token_counts(c, grid):
-            EC = cfg.EC_of(n)
-            if c.kind == "router":
-                out = ctx.forward_tokens(x[:n], wg, we, bias_up=bu, bias_down=bd)
-            elif c.kind == "gated":
-                out = ctx.forward_gated(x[:n], wg, we, c.router, score_bias=sb, bias_up=bu, bias_down=bd)
-            else:
-                out = ctx.forward_routed(x[:n], idx_d[:n], w_d[:n], we, bias_up=bu, bias_down=bd)
-            ctx.synchronize()
-            d = _device(ctx, cfg, out, n, _gather(c), gate_out=c.kind != "routed")
-            if c.kind == "router":
-                ex.check_forward(inp, d, EC, n=n, stats=st)
-                if cfg.is_training:
-                    _check_training(ctx, c, inp, d, n, case_regime(c, n, grid))
-                    st.add("gML/gMeC/loss", 2 * cfg.E + 1)
-            elif c.kind == "gated":
-                amb += eg.check_gated_forward(inp, d, c.router, bias, EC, st)
-            else:
-                er.check_routed_forward(inp, d, idx_all[:n], w_all[:n], EC, st)
+            d, _, a = run.run(n, stats=st)
+            amb += a
+            if cfg.is_training:
+                _check_training(ctx, c, inp, d, n, case_regime(c, n, grid))
+                st.add("gML/gMeC/loss", 2 * cfg.E + 1)
             rn = case_regime(c, n, grid)
             print(f"  n={n}: fullest CTA {len(rn.sub_chunks)} sub-chunk(s) {rn.sub_chunks[:4]}"
                   f"{' ...' if len(rn.sub_chunks) > 4 else ''}")

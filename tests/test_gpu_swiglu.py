@@ -30,9 +30,10 @@ def _cfg(act, E=16, k=2, S=512, H=320, P=320, **kw):
 def test_routing_tables_equal_relu_context(route, k, training):
     from flashmoe_b200.runtime import MoEContext
 
-    inp = sw.swiglu_inputs(_cfg(2, k=k, is_training=training), 31 + k, bias=True, zero_tokens=2,
-                           wg_range=1 if route == "gated" else 4)
-    relu_we = inp.base.we.cuda()
+    router_kw = dict(zero_tokens=2, wg_range=1 if route == "gated" else 4)
+    inp = sw.swiglu_inputs(_cfg(2, k=k, is_training=training), 31 + k, bias=True, **router_kw)
+    # the ReLU weights exact_inputs draws for the same x and gate weights
+    relu_we = ex.exact_inputs(_cfg(0, k=k, is_training=training), 31 + k, x_range=1, **router_kw).experts.w.cuda()
     res = {}
     for act in (0, 2):
         cfg = _cfg(act, k=k, is_training=training)
@@ -65,7 +66,7 @@ def test_routing_tables_equal_relu_context(route, k, training):
 
 
 def test_graph_replays_equal_eager():
-    from flashmoe_b200.runtime import MoEContext, SharedExpert
+    from flashmoe_b200.runtime import MoEContext
 
     cfg = _cfg(2, k=2, P=192)
     inp = sw.swiglu_inputs(cfg, 77, bias=True)
@@ -75,7 +76,7 @@ def test_graph_replays_equal_eager():
         dev = ctx.device
         x, wg, we, bu, bd = inp.device(dev)
         x = x.reshape(cfg.S, cfg.H)
-        se = SharedExpert(sh.w.to(dev), sh.bu.to(dev), sh.bd.to(dev))
+        se = ex.shared_expert(sh, dev)
         S, H = cfg.S, cfg.H
         eager = {}
         for n in (S, 301, 1, 0):

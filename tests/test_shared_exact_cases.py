@@ -1,6 +1,7 @@
 """CPU checks of tests/test_gpu_shared_exact.py: the tiling arithmetic of tests/exact_shared.py is the kernel's, every
 case reaches its regime on a 132-SM H100, its sums are exact in fp32 and enough of h_s and of the r + s step rounds, and
 the checker catches the faults a shared expert can hide, each with a message that names the stage."""
+import dataclasses
 import os
 import re
 
@@ -93,11 +94,14 @@ def test_tile_tails_are_covered():
 
 
 # ----------------------------------------------------------------------------- preconditions and rounding shares
+def _route(c):
+    return dict(routing=gse.case_routing(c) if c.route == "routed" else None, router=gse.V3,
+                score_bias=gse.case_score_bias(c))
+
+
 def _reference(c, inp, ps, n, st=None):
     se = gse.case_shared(c, ps)
-    dev, rec = es.reference_launch(c.route, inp, se, n, c.cfg.EC_of(n), routing=gse.case_routing(c)
-                                   if c.route == "routed" else None, router=gse.V3, score_bias=gse.case_score_bias(c),
-                                   stats=st)
+    dev, rec = ex.reference_launch(c.route, inp, c.cfg.EC_of(n), n, shared=se, stats=st, **_route(c))
     return se, dev, rec
 
 
@@ -111,8 +115,7 @@ def test_case_is_exact_and_rounds(name):
         n = max(n for p, n in gse.launch_ns(c, 132) if p == ps)
         st = ex.Stats()
         se, dev, rec = _reference(c, inp, ps, n, st)
-        es.check_launch(c.route, inp, se, dev, rec, c.cfg.EC_of(n), c.act, routing=gse.case_routing(c)
-                        if c.route == "routed" else None, router=gse.V3, score_bias=gse.case_score_bias(c))
+        ex.check_launch(c.route, inp, c.cfg.EC_of(n), n, dev, rec, shared=se, **_route(c))
         h, o = st.d["h_s"], st.d["out = rne(r + s)"]
         assert h[1] >= gx.MIN_H_ROUNDED * h[0], f"Ps={ps}: only {h[1]} of {h[0]} h_s elements round"
         assert o[1] >= MIN_RS_ROUNDED * o[0], f"Ps={ps}: only {o[1]} of {o[0]} out elements round in r + s"
@@ -123,9 +126,8 @@ def test_model_shape_shared_sums_exact(name):
     """The model-shape shared experts: GEMM0 and GEMM1 sums exact in fp32 on 128 tokens drawn as the layer's (the
     bound is per row; the GPU test checks every row), and h_s on the 2^-3 grid with most of it nonzero."""
     cfg, _, ps = gse.LAYERS[name]
-    li_x = eg.LayerInputs(cfg.replace(sequence_len=128), seed=8100 + len(name)).x64
-    se = gse.layer_shared(name)
-    rec = es.shared_record(li_x, se, cfg.hidden_act)
+    li_x = eg.layer_inputs(cfg.replace(sequence_len=128), seed=8100 + len(name)).x64
+    rec = ex.shared_stage(li_x, gse.layer_shared(name))
     h = ex.bits_to_f64(rec.h_s)
     assert (h != 0).mean() > 0.3 and ex.grid_log2(h) == ex.WUP_GRID
 
@@ -138,11 +140,9 @@ def _base(route="routed", k=2, H=320, ps=320, n=S, act=0):
     c = gse.Case(route, gse._cfg(k=k, H=H, hidden_act=act), ((ps, n),))
     inp = gse.case_inputs(c)
     se, dev, rec = _reference(c, inp, ps, n)
-    routing = gse.case_routing(c) if route == "routed" else None
 
     def check(d=dev, r=rec):
-        es.check_launch(route, inp, se, d, r, c.cfg.EC_of(n), act, routing=routing, router=gse.V3,
-                        score_bias=gse.case_score_bias(c))
+        ex.check_launch(route, inp, c.cfg.EC_of(n), n, d, r, shared=se, **_route(c))
 
     check()   # the reference record itself passes
     return c, inp, se, dev, rec, check
@@ -150,8 +150,7 @@ def _base(route="routed", k=2, H=320, ps=320, n=S, act=0):
 
 def _routed_r(inp, c, n):
     """The routed result r (bf16 bits) of the routed base case, and its per-pick terms (kept, terms [n, k, H])."""
-    idx, w = gse.case_routing(c)
-    dev = eg.routed_device(inp, idx[:n], w[:n], c.cfg.EC_of(n))
+    dev, _ = ex.reference_launch("routed", inp, c.cfg.EC_of(n), n, routing=gse.case_routing(c))
     kept = dev.slot < c.cfg.EC_of(n)
     y_of = dev.ret_y[np.where(kept, dev.topk_idx, 0), np.where(kept, dev.slot, 0)]
     terms = ex.bits_to_f64(ex.f64_to_bf16(ex.bits_to_f64(dev.topk_w)[:, :, None] * ex.bits_to_f64(y_of)))
@@ -174,7 +173,7 @@ def test_fault_s_inside_the_combine(k, at):
     c, inp, se, dev, rec, check = _base(k=k)
     r, kept, terms = _routed_r(inp, c, S)
     dev.out = _accumulate(kept, terms, ex.bits_to_f64(rec.y_s), at)
-    with pytest.raises(AssertionError, match=r"^out = rne\(r \+ s\): \d+ of \d+ differ; first at token"):
+    with pytest.raises(AssertionError, match=r"^out = rne\(r \+ s\): \d+ of \d+ elements outside the reference; first at token"):
         check()
 
 
@@ -182,7 +181,7 @@ def test_fault_s_missing_on_the_last_partial_row_block():
     c, inp, se, dev, rec, check = _base(n=301)
     r, _, _ = _routed_r(inp, c, 301)
     dev.out[256:] = r[256:]
-    with pytest.raises(AssertionError, match=r"^out = rne\(r \+ s\): \d+ of \d+ differ; first at token 2(5[6-9]|[6-9]\d)"):
+    with pytest.raises(AssertionError, match=r"^out = rne\(r \+ s\): \d+ of \d+ elements outside the reference; first at token 2(5[6-9]|[6-9]\d)"):
         check()
 
 
@@ -197,9 +196,10 @@ def test_fault_y_s_rows_of_the_previous_row_block():
 @pytest.mark.parametrize("which", ["dropped", "routed_expert_0"])
 def test_fault_shared_bias_down(which):
     c, inp, se, dev, rec, check = _base()
-    bd = None if which == "dropped" else inp.bias64("down")[0]
-    assert se.bd64 is not None and (bd is None or not np.array_equal(bd, se.bd64))
-    rec.y_s = ex.gemm1_reference(rec.h_s, se.w_down64, bd, "GEMM1").lo
+    w_down, bd_s = se.down(0)
+    bd = None if which == "dropped" else inp.experts.down(0)[1]
+    assert bd_s is not None and (bd is None or not np.array_equal(bd, bd_s))
+    rec.y_s = ex.gemm1_reference(rec.h_s, w_down, bd, "GEMM1").lo
     with pytest.raises(AssertionError, match=r"^y_s \(shared expert\)"):
         check()
 
@@ -208,16 +208,16 @@ def test_fault_partial_ps_tile_of_h_s_from_the_previous_launch():
     """Columns 256..319 of h_s (the last, partial Ps tile at Ps = 320) left from a launch on other tokens; y_s and out
     follow the stale h_s, as a kernel that skipped the tile would produce them."""
     c, inp, se, dev, rec, check = _base()
-    stale = es.shared_record(inp.x64[::-1][:S], se, 0)
+    stale = ex.shared_stage(inp.x64[::-1][:S], se)
     rec.h_s[:, 256:] = stale.h_s[:, 256:]
-    rec.y_s = ex.gemm1_reference(rec.h_s, se.w_down64, se.bd64, "GEMM1").lo
-    with pytest.raises(AssertionError, match=r"^h_s \(shared expert\): \d+ of \d+ differ; first at token \d+, column (2[5-9]\d|3[01]\d)"):
+    rec.y_s = se.y(0, rec.h_s).lo
+    with pytest.raises(AssertionError, match=r"^h_s \(shared expert\): \d+ of \d+ elements outside the reference; first at token \d+, column (2[5-9]\d|3[01]\d)"):
         check()
 
 
 def test_fault_partial_h_tile_of_y_s_from_the_previous_launch():
     c, inp, se, dev, rec, check = _base()
-    stale = es.shared_record(inp.x64[::-1][:S], se, 0)
+    stale = ex.shared_stage(inp.x64[::-1][:S], se)
     rec.y_s[:, 256:] = stale.y_s[:, 256:]
     with pytest.raises(AssertionError, match=r"^y_s \(shared expert\): \d+ of \d+ differ; first at token \d+, column (2[5-9]\d|3[01]\d)"):
         check()
@@ -225,8 +225,8 @@ def test_fault_partial_h_tile_of_y_s_from_the_previous_launch():
 
 def test_fault_gelu_replaced_by_relu_in_h_s():
     c, inp, se, dev, rec, check = _base(route="router", act=1)
-    relu = es.shared_record(inp.x64[:S], se, 0)
-    rec.h_s, rec.y_s = relu.h_s, ex.gemm1_reference(relu.h_s, se.w_down64, se.bd64, "GEMM1").lo
+    relu = ex.shared_stage(inp.x64[:S], dataclasses.replace(se, act=0))
+    rec.h_s, rec.y_s = relu.h_s, relu.y_s
     with pytest.raises(AssertionError, match=r"^h_s \(shared expert\): \d+ of \d+ elements outside the reference"):
         check()
 

@@ -10,7 +10,6 @@ import pytest
 from flashmoe_b200.router import RouterSpec
 from tests import exact as ex
 from tests import exact_gated as eg
-from tests import exact_routed as er
 from tests import test_gpu_exact as gx
 from tests import test_gpu_subchunks as gs
 
@@ -113,15 +112,11 @@ def test_case_is_exact_and_rounds(name):
             ex.check_preconditions(inp, EC, gx.MIN_H_ROUNDED if n > 30 else 0, gx.MIN_OUT_ROUNDED, n=n)
             continue
         st = ex.Stats()
-        if c.kind == "gated":
-            bias = gs.case_bias(c)
-            dev = eg.reference_device_gated(inp, c.router, bias, EC, n, stats=st)
-            if not c.layer:   # (the layer-sized reference is minutes of float64 GEMMs: built once, not re-checked)
-                assert eg.check_gated_forward(inp, dev, c.router, bias, EC) <= gs.max_ambiguous(c, n)
-        else:
-            idx, w = gs.case_routing(c)
-            dev = eg.routed_device(inp, idx[:n], w[:n], EC, stats=st)
-            er.check_routed_forward(inp, dev, idx[:n], w[:n], EC)
+        route = dict(routing=gs.case_routing(c) if c.kind == "routed" else None, router=c.router,
+                     score_bias=gs.case_bias(c))
+        dev, _ = ex.reference_launch(c.kind, inp, EC, n, stats=st, **route)
+        if not c.layer:   # (the layer-sized reference is minutes of float64 GEMMs: built once, not re-checked)
+            assert ex.check_launch(c.kind, inp, EC, n, dev, **route) <= gs.max_ambiguous(c, n)
         if n > 30:
             _shares(st, cfg.k)
 
@@ -170,7 +165,11 @@ def _gated_base(name):
     inp = gs.case_inputs(c)
     bias = gs.case_bias(c)
     rg = gs.case_regime(c, c.cfg.S, env={})
-    return c, inp, bias, rg, eg.reference_device_gated(inp, c.router, bias, c.cfg.EC)
+    return c, inp, bias, rg, ex.reference_launch("gated", inp, c.cfg.EC, c.cfg.S, router=c.router, score_bias=bias)[0]
+
+
+def _check_gated(c, inp, dev, bias):
+    ex.check_launch("gated", inp, c.cfg.EC, c.cfg.S, dev, router=c.router, score_bias=bias)
 
 
 def _reroute(c, inp, dev, rows, router, bias):
@@ -188,7 +187,7 @@ def test_fault_bias_missing_after_the_first_subchunk():
     later = np.flatnonzero(rg.position(c.cfg.S) > 0)
     _reroute(c, inp, dev, later, c.router, None)
     with pytest.raises(AssertionError, match=r"topk_idx \(gated\): \d+ decided tokens differ; first token (\d+)") as ei:
-        eg.check_gated_forward(inp, dev, c.router, bias, c.cfg.EC)
+        _check_gated(c, inp, dev, bias)
     assert int(re.search(r"first token (\d+)", str(ei.value)).group(1)) in set(later)
 
 
@@ -197,7 +196,7 @@ def test_fault_group_limit_ignored_after_the_first_subchunk():
     later = np.flatnonzero(rg.position(c.cfg.S) > 0)
     _reroute(c, inp, dev, later, _ungrouped(c.router), bias)
     with pytest.raises(AssertionError, match=r"topk_idx \(gated\)"):
-        eg.check_gated_forward(inp, dev, c.router, bias, c.cfg.EC)
+        _check_gated(c, inp, dev, bias)
 
 
 def _second_subchunk_over_first(topk, rg, n):
@@ -217,16 +216,12 @@ def test_fault_second_subchunk_sel_e_over_the_first(name):
     inp = gs.case_inputs(c)
     rg = gs.case_regime(c, cfg.S, env={})
     bias = gs.case_bias(c)
-    dev = ex.reference_device(inp, cfg.EC) if c.kind == "router" else \
-        eg.reference_device_gated(inp, c.router, bias, cfg.EC)
+    dev, _ = ex.reference_launch(c.kind, inp, cfg.EC, cfg.S, router=c.router, score_bias=bias)
     seen = _second_subchunk_over_first(dev.topk_idx, rg, cfg.S)
     assert not np.array_equal(seen, dev.topk_idx)
     dev.slot, dev.counts, dev.recv_cnt, _ = ex.slots_from_topk(seen, cfg.E, cfg.EC)
     with pytest.raises(AssertionError, match=r"^slot: \d+ of \d+ differ; first at token"):
-        if c.kind == "router":
-            ex.check_forward(inp, dev, cfg.EC)
-        else:
-            eg.check_gated_forward(inp, dev, c.router, bias, cfg.EC)
+        ex.check_launch(c.kind, inp, cfg.EC, cfg.S, dev, router=c.router, score_bias=bias)
 
 
 def test_fault_weight_renormalised_by_the_previous_tokens_sum():
@@ -239,7 +234,7 @@ def test_fault_weight_renormalised_by_the_previous_tokens_sum():
     W_prev, picks = W[t - 1], dev.topk_idx[t - 1:t + 1]
     dev.topk_w[t, 0] = ex.f64_to_bf16(np.array([sc.s_mid[t, picks[1, 0]] / W_prev * c.router.scale]))[0]
     with pytest.raises(AssertionError, match=rf"topk_w \(gated\): 1 tokens .*; first token {t} pick 0 "):
-        eg.check_gated_forward(inp, dev, c.router, bias, c.cfg.EC)
+        _check_gated(c, inp, dev, bias)
 
 
 def _aux_from(p, counts, n, rows):

@@ -3,8 +3,6 @@ float64 SwiGLU and with the torch restatement of the whole forward (tests/torch_
 restatement against oracle/torch_moe on a layout-equivalent input, the generator's conditions (g >= -64, exact GEMM
 sums), the kernel's partial-tile argument replayed in float64, and the stage checker accepting a correct launch record
 and rejecting a planted fault.  CPU only."""
-import dataclasses
-
 import numpy as np
 import pytest
 import torch
@@ -16,10 +14,8 @@ from tests import exact_swiglu as sw
 
 
 def _ref(g, u):
-    """swiglu_reference on one row whose gate and up pre-activations are exactly g and u (rows = identity)."""
-    g, u = np.atleast_1d(np.asarray(g, np.float64)), np.atleast_1d(np.asarray(u, np.float64))
-    r = sw.swiglu_reference(np.eye(len(g)), np.diag(g), np.diag(u), None, None)
-    return ex.Rounded(np.diagonal(r.lo).copy(), np.diagonal(r.hi).copy(), np.diagonal(r.exact).copy())
+    """h's interval for gate and up pre-activations g and u."""
+    return sw.silu_mul_rounded(np.atleast_1d(np.asarray(g, np.float64)), np.atleast_1d(np.asarray(u, np.float64)))
 
 
 def test_corner_g0_is_zero():
@@ -66,13 +62,12 @@ def _cfg(E=4, k=2, S=256, H=128, P=192):
 def test_generator_keeps_g_above_minus_64_and_sums_exact():
     cfg = _cfg()
     inp = sw.swiglu_inputs(cfg, 11, bias=True)
-    assert tuple(inp.we.shape) == (4, 3, 192, 128) and tuple(inp.bu.shape) == (4, 2, 192)
+    xp = inp.experts
+    assert tuple(xp.w.shape) == (4, 3, 192, 128) and tuple(xp.bu.shape) == (4, 2, 192)
     for e in range(cfg.E):
-        wg_, wu, bg, bu = inp.gate_up64(e)
-        g = inp.x64 @ wg_.T + bg
+        g, _ = xp.pre(e, inp.x64)
         assert g.min() >= sw.G_MIN
-        h = sw.expert_h(inp, e, inp.x64, "GEMM0")
-        ex.gemm1_reference(h.lo, inp.w_down64(e), inp.bd64(e), "GEMM1")   # asserts exact sums
+        xp.y(e, xp.h(e, inp.x64).lo)   # asserts exact sums
 
 
 def test_partial_last_tile_reads_stay_in_the_tensor_and_are_not_stored():
@@ -82,12 +77,13 @@ def test_partial_last_tile_reads_stay_in_the_tensor_and_are_not_stored():
     cfg = _cfg()
     E, P, H = cfg.E, cfg.P, cfg.H
     inp = sw.swiglu_inputs(cfg, 12, bias=True)
-    flat = inp.we.double().numpy().reshape(E * 3 * P, H)
+    xp = inp.experts
+    flat = xp.w.double().numpy().reshape(E * 3 * P, H)
     x = inp.x64[:128]
     tn = -(-P // 128)
     for e in range(E):
-        ref = sw.expert_h(inp, e, x, "GEMM0")
-        bias = inp.bu[e].double().numpy().reshape(-1)   # [gate; up], glu_rows = P apart
+        ref = xp.h(e, x)
+        bias = xp.bu[e].double().numpy().reshape(-1)   # [gate; up], glu_rows = P apart
         for nt in range(tn):
             b_row, n0 = e * 3 * P + nt * 128, nt * 128
             assert b_row + P + 128 <= flat.shape[0]
@@ -99,40 +95,19 @@ def test_partial_last_tile_reads_stay_in_the_tensor_and_are_not_stored():
                 np.testing.assert_array_equal(g / (1 + np.exp(-g)) * u, ref.exact[:, n0 + 64 * c:n0 + 64 * c + 64])
 
 
-def _reference_device(inp, EC):
-    """A launch record built from the reference itself (interval midpoints rounded), with the router's routing."""
-    cfg = inp.cfg
-    # (the routing part of exact.reference_device; its ReLU experts are replaced below)
-    base = ex.reference_device(dataclasses.replace(inp.base, cfg=cfg.replace(hidden_act=0)), EC)
-    E, H = cfg.E, cfg.H
-    slot, counts, recv_cnt, kept = ex.slots_from_topk(base.topk_idx, E, EC)
-    toks = ex.packet_tokens(base.topk_idx, slot, E, EC)
-    rmax = max(1, int(recv_cnt.max()))
-    hidden = np.zeros((E, rmax, cfg.P), np.uint16)
-    ret_y = np.zeros((E, rmax, H), np.uint16)
-    for e in range(E):
-        c = len(toks[e])
-        if c:
-            hidden[e, :c] = sw.expert_h(inp, e, inp.x64[toks[e]], "GEMM0").lo
-            ret_y[e, :c] = ex.gemm1_reference(hidden[e, :c], inp.w_down64(e), inp.bd64(e), "GEMM1").lo
-    y_of = ret_y[base.topk_idx, np.where(kept, slot, 0)]
-    out = ex.combine_tokens(y_of, kept, base.topk_w, base.mcw).lo
-    return ex.Device(out, base.topk_idx, base.topk_w, base.mcw, base.gate_out, base.slot, base.counts, base.recv_cnt,
-                     base.recv_x, hidden, ret_y)
-
-
 def test_checker_accepts_the_reference_and_rejects_a_planted_fault():
     cfg = _cfg()
     inp = sw.swiglu_inputs(cfg, 13, bias=True, zero_tokens=2)
-    dev = _reference_device(inp, cfg.EC)
-    st = sw.check_experts(inp, dev, cfg.EC, cfg.S)
+    dev, _ = ex.reference_launch("router", inp, cfg.EC, cfg.S)
+    st = ex.Stats()
+    ex.check_launch("router", inp, cfg.EC, cfg.S, dev, stats=st)
     h = st.d["hidden"]
     assert h[1] > 0.5 * h[0], "the inputs must make h round"
     e = int(np.flatnonzero(dev.recv_cnt)[0])
     j = int(np.flatnonzero(dev.hidden[e, 0])[0])
     dev.hidden[e, 0, j] += 2   # two bf16 ulps off
     with pytest.raises(AssertionError, match=f"hidden of expert {e}"):
-        sw.check_experts(inp, dev, cfg.EC, cfg.S)
+        ex.check_launch("router", inp, cfg.EC, cfg.S, dev)
 
 
 def _torch_device(res, E, EC):
@@ -153,27 +128,29 @@ def test_reference_agrees_with_torch_swiglu_router(k, bias):
 
     cfg = _cfg(k=k)
     inp = sw.swiglu_inputs(cfg, 20 + k, bias=bias, zero_tokens=2)
-    res = moe_forward_swiglu_cpu(inp.base.x.reshape(cfg.S, cfg.H), inp.base.wg, inp.we, k=k, EC=cfg.EC,
-                                 bias_up=inp.bu, bias_down=inp.bd)
+    res = moe_forward_swiglu_cpu(inp.x.reshape(cfg.S, cfg.H), inp.wg, inp.experts.w, k=k, EC=cfg.EC,
+                                 bias_up=inp.experts.bu, bias_down=inp.experts.bd)
     dev = _torch_device(res, cfg.E, cfg.EC)
-    ex.check_topk(dev.topk_idx, ex.router_reference(inp.x64, inp.base.wg_eff64, k))
-    st = sw.check_experts(inp, dev, cfg.EC, cfg.S)
+    # gate_out: the reference's own, with the torch forward's weights at its picks (they must lie in the interval)
+    dev.gate_out = ex.reference_launch("router", inp, cfg.EC, cfg.S)[0].gate_out
+    dev.gate_out[np.arange(cfg.S)[:, None], dev.topk_idx] = dev.topk_w
+    st = ex.Stats()
+    ex.check_launch("router", inp, cfg.EC, cfg.S, dev, stats=st)
     assert st.d["hidden"][0] > 0 and st.d["ret_y"][0] > 0
 
 
 @pytest.mark.parametrize("k", [1, 2])
 def test_reference_agrees_with_torch_swiglu_routed(k):
-    from tests import exact_routed as er
     from tests.torch_swiglu import moe_forward_swiglu_routed_cpu
 
     cfg = _cfg(k=k)
     inp = sw.swiglu_inputs(cfg, 30 + k, bias=True)
-    idx, w = er.routing_case(cfg.S, cfg.E, k, 30 + k, hot=1, hot_frac=0.4, empty=(3,))
-    res = moe_forward_swiglu_routed_cpu(inp.base.x.reshape(cfg.S, cfg.H), torch.from_numpy(idx), torch.from_numpy(w),
-                                        inp.we, EC=cfg.EC, bias_up=inp.bu, bias_down=inp.bd)
+    xp = inp.experts
+    idx, w = ex.routing_case(cfg.S, cfg.E, k, 30 + k, hot=1, hot_frac=0.4, empty=(3,))
+    res = moe_forward_swiglu_routed_cpu(inp.x.reshape(cfg.S, cfg.H), torch.from_numpy(idx), torch.from_numpy(w),
+                                        xp.w, EC=cfg.EC, bias_up=xp.bu, bias_down=xp.bd)
     dev = _torch_device(res, cfg.E, cfg.EC)
-    ex.check_equal(dev.topk_idx, idx, "topk_idx", ("token", "pick"))
-    sw.check_experts(inp, dev, cfg.EC, cfg.S, unscaled_k1=False)
+    ex.check_launch("routed", inp, cfg.EC, cfg.S, dev, routing=(idx, w))
 
 
 def test_torch_swiglu_relu_equivalent_layout():
