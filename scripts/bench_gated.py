@@ -8,7 +8,7 @@ For every config and n three arms run alternating, `rounds` times `steps` forwar
   ms_gated           forward_gated(n) with DeepSeek-V3's rule (sigmoid, score bias, n_group 8, topk_group 4, top-2
                      group scores, renormalise, scale 2.5);
   ms_torch_router    DeepSeek's router formula (its Gate.forward) in torch on the device, then forward_routed(n).
-Configs: bench.py's (E128: 128 experts, top-2, d_model 2048, ffn 2048) and DSV3, defined here: DeepSeek-V3's layer
+Configs: bench.py's (E128: 128 experts, top-2, d_model 2048, ffn 2048) and DSV3 (bench_common.py): DeepSeek-V3's layer
 shape on one GPU (E = 256, k = 8, H = 7168, P = 2048, S = 4096; 15 GB of expert weights, generated on the device from a
 seeded generator).  The gated arm's picks are compared with the torch arm's (fraction of tokens with the same top-k
 set).  One GPU; prints one JSON line with the card's name and power limit next to the figures; writes no files.
@@ -16,9 +16,9 @@ set).  One GPU; prints one JSON line with the card's name and power limit next t
 from __future__ import annotations
 
 import argparse
+import functools
 import json
 import os
-import statistics
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -27,12 +27,8 @@ sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
 import bench  # noqa: E402   (seeded inputs; bench.py itself is not changed by this script)
-from flashmoe_b200.config import MoEConfig  # noqa: E402
-from flashmoe_b200.router import RouterSpec  # noqa: E402
-from scripts.bench_varlen import card, parse_tokens  # noqa: E402
-
-RULE = RouterSpec("sigmoid", 8, 4, 2, True, 2.5)
-DSV3 = MoEConfig(num_experts=256, expert_top_k=8, sequence_len=4096, hidden_size=7168, intermediate_size=2048)
+from scripts import bench_common as common  # noqa: E402
+from scripts.bench_common import DSV3, RULE  # noqa: E402
 
 
 def deepseek_router(x, wg_eff, bias, rule, k):
@@ -52,36 +48,16 @@ def deepseek_router(x, wg_eff, bias, rule, k):
     return idx.to(torch.int32), w.float()
 
 
-def inputs(name, cfg, dev):
-    if name in bench.BASELINE_CONFIGS:
-        x, wg, we = bench.make_inputs(cfg, cfg.E, 0)
-        return x.to(dev).view(cfg.S, cfg.H), wg.to(dev), we.to(dev)
-    g = torch.Generator(device=dev).manual_seed(0x5EED)
-    x = torch.randn(cfg.S, cfg.H, generator=g, device=dev).bfloat16()
-    wg = (torch.randn(cfg.H, cfg.E, generator=g, device=dev) * cfg.H ** -0.5).bfloat16()
-    we = torch.empty(cfg.E, 2, cfg.P, cfg.H, dtype=torch.bfloat16, device=dev)
-    for e in range(cfg.E):   # (one expert at a time: no fp32 copy of the 15 GB)
-        we[e] = (torch.randn(2, cfg.P, cfg.H, generator=g, device=dev) * cfg.H ** -0.5).bfloat16()
-    return x, wg, we
-
-
 def run_config(name, tokens, steps, warmup, rounds, dev):
     from flashmoe_b200.runtime import MoEContext
 
     cfg = bench.BASELINE_CONFIGS[name] if name in bench.BASELINE_CONFIGS else DSV3
     ctx = MoEContext(cfg, device=dev.index, timeout_ms=30000)
-    xd, wgd, wed = inputs(name, cfg, dev)
+    xd, wgd, wed = common.inputs(name, cfg, dev)
     wg_eff = wgd.view(-1).view(cfg.E, cfg.H)
     bias = (torch.randn(cfg.E, generator=torch.Generator(device=dev).manual_seed(7), device=dev) * 0.05).float()
 
-    def device_ms(fn):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        torch.cuda.synchronize(dev)
-        return e0.elapsed_time(e1) / steps
+    sync = functools.partial(torch.cuda.synchronize, dev)
 
     entries = []
     for n in tokens:
@@ -101,19 +77,10 @@ def run_config(name, tokens, steps, warmup, rounds, dev):
         arms = {"ms_router": lambda: ctx.forward_tokens(xn, wgd, wed, out=out_n),
                 "ms_gated": lambda: ctx.forward_gated(xn, wgd, wed, RULE, score_bias=bias, out=out_n),
                 "ms_torch_router": torch_arm}
-        for fn in arms.values():
-            for _ in range(warmup):
-                fn()
-        torch.cuda.synchronize(dev)
-        times = {k: [] for k in arms}
-        for _ in range(rounds):
-            for k, fn in arms.items():
-                times[k].append(device_ms(fn))
+        times = common.alternate(arms, warmup, rounds, sync, lambda fn: common.device_ms(fn, steps, sync))
         ctx.check()
         e = {"tokens": n, "ec": cfg.EC_of(n), "same_picks_as_torch": same}
-        for k, v in times.items():
-            e[k] = statistics.median(v)
-            e[k + "_runs"] = v
+        e.update(common.medians(times))
         e["gated_minus_router_us"] = (e["ms_gated"] - e["ms_router"]) * 1e3
         e["torch_minus_gated_us"] = (e["ms_torch_router"] - e["ms_gated"]) * 1e3
         entries.append(e)
@@ -127,26 +94,18 @@ def run_config(name, tokens, steps, warmup, rounds, dev):
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--configs", default="E128,DSV3")
-    ap.add_argument("--tokens", default="1,128,4096", metavar="N1,N2,..")
-    ap.add_argument("--steps", type=int, default=200)
-    ap.add_argument("--warmup", type=int, default=32)
-    ap.add_argument("--rounds", type=int, default=3)
+    common.add_run_args(ap, tokens="1,128,4096", steps=200, warmup=32, rounds=3)
     args = ap.parse_args()
-    names = [c for c in args.configs.split(",") if c]
     known = {**bench.BASELINE_CONFIGS, "DSV3": DSV3}
-    bad = [c for c in names if c not in known]
-    if not names or bad:
-        ap.error(f"--configs: unknown {bad}; choose from {sorted(known)}")
-    tokens = {c: parse_tokens(ap, args.tokens, known[c].S) for c in names}
-    if args.steps < 1 or args.rounds < 1:
-        ap.error("--steps and --rounds must be >= 1")
+    names = common.parse_names(ap, "--configs", args.configs, known)
+    tokens = {c: common.parse_tokens(ap, args.tokens, known[c].S) for c in names}
+    common.check_counts(ap, args)
     if not torch.cuda.is_available():
-        print("bench_gated.py: no CUDA device; the MoE forward path has no CPU fallback", file=sys.stderr)
-        return 3
+        return common.no_cuda("bench_gated.py")
     dev = torch.device("cuda", torch.cuda.current_device())
     runs = [run_config(c, tokens[c], args.steps, args.warmup, args.rounds, dev) for c in names]
     print(json.dumps({"metric": "moe_layer_fwd_gated_ms", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
-                      "rounds": args.rounds, "card": card(dev), "runs": runs}), flush=True)
+                      "rounds": args.rounds, "card": common.card(dev), "runs": runs}), flush=True)
     return 0
 
 

@@ -27,12 +27,11 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
 
 import torch  # noqa: E402
 
 import bench  # noqa: E402   (configs and their description; bench.py itself is not changed by this script)
-from bench_varlen import card, parse_tokens  # noqa: E402
+from scripts import bench_common as common  # noqa: E402
 
 
 def run_graph(name, layers, tokens, steps, warmup, rounds, dev):
@@ -70,37 +69,29 @@ def run_graph(name, layers, tokens, steps, warmup, rounds, dev):
     graph_dev = capture(S, True)
 
     def window(fn):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        """(wall, device) ms per step; the wall clock runs from a synchronised start to the synchronise that ends the
+        event window."""
         torch.cuda.synchronize(dev)
-        t0 = time.perf_counter()
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        torch.cuda.synchronize(dev)
-        wall = (time.perf_counter() - t0) * 1e3 / steps
-        return wall, e0.elapsed_time(e1) / steps
+        t = [time.perf_counter()]
+
+        def settle():
+            torch.cuda.synchronize(dev)
+            t.append(time.perf_counter())
+
+        device = common.device_ms(fn, steps, settle)
+        return (t[1] - t[0]) * 1e3 / steps, device
 
     entries = []
     for n in tokens:
         graph_n = capture(n, False)
         arms = {"eager": lambda: stack(n, False), "graph_per_n": graph_n.replay, "graph_dev_n": graph_dev.replay}
         n_dev.fill_(n)
-        for fn in arms.values():
-            for _ in range(warmup):
-                fn()
-        ctx.synchronize()
-        runs = {k: {"wall": [], "device": []} for k in arms}
-        for _ in range(rounds):
-            for k, fn in arms.items():
-                wall, device = window(fn)
-                runs[k]["wall"].append(wall)
-                runs[k]["device"].append(device)
+        runs = common.alternate(arms, warmup, rounds, ctx.synchronize, window)
         ctx.synchronize()   # raises if a launch reported a problem
         e = {"tokens": n}
         for k, r in runs.items():
-            for what in ("wall", "device"):
-                v = r[what]
+            for i, what in enumerate(("wall", "device")):
+                v = [w[i] for w in r]
                 e[f"{k}_{what}_ms_per_step"] = statistics.median(v)
                 e[f"{k}_{what}_ms_per_step_range"] = [min(v), max(v)]
                 e[f"{k}_{what}_ms_per_layer"] = statistics.median(v) / layers
@@ -114,24 +105,20 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--config", default="B", choices=sorted(bench.BASELINE_CONFIGS))
     ap.add_argument("--layers", type=int, default=8)
-    ap.add_argument("--tokens", default="1,8,128,4096", metavar="N1,N2,..")
-    ap.add_argument("--steps", type=int, default=50)
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--rounds", type=int, default=5)
+    common.add_run_args(ap, tokens="1,8,128,4096", steps=50, warmup=5, rounds=5)
     args = ap.parse_args()
-    tokens = parse_tokens(ap, args.tokens, bench.BASELINE_CONFIGS[args.config].S)
+    tokens = common.parse_tokens(ap, args.tokens, bench.BASELINE_CONFIGS[args.config].S)
     if args.layers < 1:
         ap.error("--layers must be >= 1")
-    if args.steps < 1 or args.rounds < 1 or args.warmup < 0:
-        ap.error("--steps and --rounds must be >= 1, --warmup >= 0")
+    common.check_counts(ap, args, warmup=True)
     if not torch.cuda.is_available():
-        print("bench_graph.py: no CUDA device; the MoE forward path has no CPU fallback", file=sys.stderr)
-        return 3
+        return common.no_cuda("bench_graph.py")
     dev = torch.device("cuda", torch.cuda.current_device())
     entries = run_graph(args.config, args.layers, tokens, args.steps, args.warmup, args.rounds, dev)
     cfg = bench.BASELINE_CONFIGS[args.config]
     line = {"metric": "moe_layer_stack_graph_ms", "config": bench.config_dict(args.config, cfg, 1), "layers": args.layers,
-            "steps": args.steps, "warmup": args.warmup, "rounds": args.rounds, "card": card(dev), "graph": entries}
+            "steps": args.steps, "warmup": args.warmup, "rounds": args.rounds, "card": common.card(dev),
+            "graph": entries}
     print(json.dumps(line), flush=True)
     return 0
 

@@ -15,9 +15,9 @@ the figures; writes no files.
 from __future__ import annotations
 
 import argparse
+import functools
 import json
 import os
-import statistics
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -27,7 +27,7 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 import bench  # noqa: E402   (seeded inputs; bench.py itself is not changed by this script)
-from scripts.bench_varlen import card, parse_tokens  # noqa: E402
+from scripts import bench_common as common  # noqa: E402
 
 
 def torch_router(x, wg, k):
@@ -40,20 +40,10 @@ def run_config(name, tokens, steps, warmup, rounds, dev):
     from flashmoe_b200.runtime import MoEContext
 
     cfg = bench.BASELINE_CONFIGS[name]
-    S, H = cfg.S, cfg.H
     ctx = MoEContext(cfg, device=dev.index, timeout_ms=30000)
-    x, wg, we = bench.make_inputs(cfg, cfg.E, 0)
-    xd, wgd, wed = x.to(dev).view(S, H), wg.to(dev), we.to(dev)
-    del we
+    xd, wgd, wed = common.inputs(name, cfg, dev)
 
-    def device_ms(fn):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        torch.cuda.synchronize(dev)
-        return e0.elapsed_time(e1) / steps
+    sync = functools.partial(torch.cuda.synchronize, dev)
 
     entries = []
     for n in tokens:
@@ -76,19 +66,10 @@ def run_config(name, tokens, steps, warmup, rounds, dev):
         arms = {"ms_router": lambda: ctx.forward_tokens(xn, wgd, wed, out=out_n),
                 "ms_routed": lambda: ctx.forward_routed(xn, idx, w, wed, out=out_n),
                 "ms_torch_router": torch_arm}
-        for fn in arms.values():
-            for _ in range(warmup):
-                fn()
-        torch.cuda.synchronize(dev)
-        times = {k: [] for k in arms}
-        for _ in range(rounds):
-            for k, fn in arms.items():
-                times[k].append(device_ms(fn))
+        times = common.alternate(arms, warmup, rounds, sync, lambda fn: common.device_ms(fn, steps, sync))
         ctx.check()
         e = {"tokens": n, "ec": cfg.EC_of(n), "parity_slot_counts_recv_cnt": parity}
-        for k, v in times.items():
-            e[k] = statistics.median(v)
-            e[k + "_runs"] = v
+        e.update(common.medians(times))
         e["routed_minus_router_us"] = (e["ms_routed"] - e["ms_router"]) * 1e3
         entries.append(e)
     ctx.close()
@@ -99,25 +80,17 @@ def run_config(name, tokens, steps, warmup, rounds, dev):
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--configs", default="B,E128")
-    ap.add_argument("--tokens", default="1,128,4096", metavar="N1,N2,..")
-    ap.add_argument("--steps", type=int, default=200)
-    ap.add_argument("--warmup", type=int, default=32)
-    ap.add_argument("--rounds", type=int, default=3)
+    common.add_run_args(ap, tokens="1,128,4096", steps=200, warmup=32, rounds=3)
     args = ap.parse_args()
-    names = [c for c in args.configs.split(",") if c]
-    bad = [c for c in names if c not in bench.BASELINE_CONFIGS]
-    if not names or bad:
-        ap.error(f"--configs: unknown {bad}; choose from {sorted(bench.BASELINE_CONFIGS)}")
-    tokens = {c: parse_tokens(ap, args.tokens, bench.BASELINE_CONFIGS[c].S) for c in names}
-    if args.steps < 1 or args.rounds < 1:
-        ap.error("--steps and --rounds must be >= 1")
+    names = common.parse_names(ap, "--configs", args.configs, bench.BASELINE_CONFIGS)
+    tokens = {c: common.parse_tokens(ap, args.tokens, bench.BASELINE_CONFIGS[c].S) for c in names}
+    common.check_counts(ap, args)
     if not torch.cuda.is_available():
-        print("bench_routed.py: no CUDA device; the MoE forward path has no CPU fallback", file=sys.stderr)
-        return 3
+        return common.no_cuda("bench_routed.py")
     dev = torch.device("cuda", torch.cuda.current_device())
     runs = [run_config(c, tokens[c], args.steps, args.warmup, args.rounds, dev) for c in names]
     print(json.dumps({"metric": "moe_layer_fwd_routed_ms", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
-                      "rounds": args.rounds, "card": card(dev), "runs": runs}), flush=True)
+                      "rounds": args.rounds, "card": common.card(dev), "runs": runs}), flush=True)
     return 0
 
 

@@ -9,7 +9,7 @@ For every config and n three arms run alternating, `rounds` times `steps` forwar
   ms_torch       the same forward without one, then F.linear -> act -> F.linear (bf16 out) and out + s in bf16, in torch
                  on the same stream;
   ms_plain       the forward without a shared expert (the floor).
-Configs: B (bench.py's, built-in router, Ps = P) and DSV3 (bench_gated.py's DeepSeek-V3 layer shape, gated with the V3
+Configs: B (bench.py's, built-in router, Ps = P) and DSV3 (bench_common.py's DeepSeek-V3 layer shape, gated with the V3
 rule, Ps = 2048).  The torch arm is also a reference: the fraction of output elements bit-identical to the fused arm's,
 and the fraction within one bf16 ulp of s, are reported.  One GPU; prints one JSON line with the card's name and power
 limit next to the figures; writes no files.
@@ -17,9 +17,9 @@ limit next to the figures; writes no files.
 from __future__ import annotations
 
 import argparse
+import functools
 import json
 import os
-import statistics
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -29,8 +29,8 @@ import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
 
 import bench  # noqa: E402   (seeded inputs; bench.py itself is not changed by this script)
-from scripts.bench_gated import DSV3, RULE, inputs  # noqa: E402
-from scripts.bench_varlen import card, parse_tokens  # noqa: E402
+from scripts import bench_common as common  # noqa: E402
+from scripts.bench_common import DSV3, RULE  # noqa: E402
 
 
 def run_config(name, tokens, steps, warmup, rounds, dev):
@@ -39,7 +39,7 @@ def run_config(name, tokens, steps, warmup, rounds, dev):
     cfg = bench.BASELINE_CONFIGS[name] if name in bench.BASELINE_CONFIGS else DSV3
     ps = cfg.P if name in bench.BASELINE_CONFIGS else 2048
     ctx = MoEContext(cfg, device=dev.index, timeout_ms=30000, shared_inter=ps)
-    xd, wgd, wed = inputs(name, cfg, dev)
+    xd, wgd, wed = common.inputs(name, cfg, dev)
     g = torch.Generator(device=dev).manual_seed(0x5AED)
     se = SharedExpert((torch.randn(2, ps, cfg.H, generator=g, device=dev) * cfg.H ** -0.5).bfloat16())
     w_up, w_down = se.w[0], se.w[1].reshape(-1).view(cfg.H, ps)   # [1] flat-viewed as W_down [H, Ps]
@@ -47,14 +47,7 @@ def run_config(name, tokens, steps, warmup, rounds, dev):
     bias = (torch.randn(cfg.E, generator=torch.Generator(device=dev).manual_seed(7), device=dev) * 0.05).float()
     gated = name not in bench.BASELINE_CONFIGS
 
-    def device_ms(fn):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        torch.cuda.synchronize(dev)
-        return e0.elapsed_time(e1) / steps
+    sync = functools.partial(torch.cuda.synchronize, dev)
 
     entries = []
     for n in tokens:
@@ -82,19 +75,10 @@ def run_config(name, tokens, steps, warmup, rounds, dev):
         within = ((fused.float() - ref.float()).abs() <= ulp).float().mean().item() if n else 1.0
 
         arms = {"ms_fused": lambda: forward(out_f, se), "ms_torch": torch_arm, "ms_plain": lambda: forward(out_n)}
-        for fn in arms.values():
-            for _ in range(warmup):
-                fn()
-        torch.cuda.synchronize(dev)
-        times = {k: [] for k in arms}
-        for _ in range(rounds):
-            for k, fn in arms.items():
-                times[k].append(device_ms(fn))
+        times = common.alternate(arms, warmup, rounds, sync, lambda fn: common.device_ms(fn, steps, sync))
         ctx.check()
         e = {"tokens": n, "bitwise_equal_to_torch": same, "within_one_ulp_of_s": within}
-        for k, v in times.items():
-            e[k] = statistics.median(v)
-            e[k + "_runs"] = v
+        e.update(common.medians(times))
         e["torch_minus_fused_us"] = (e["ms_torch"] - e["ms_fused"]) * 1e3
         e["fused_minus_plain_us"] = (e["ms_fused"] - e["ms_plain"]) * 1e3
         entries.append(e)
@@ -109,26 +93,18 @@ def run_config(name, tokens, steps, warmup, rounds, dev):
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--configs", default="B,DSV3")
-    ap.add_argument("--tokens", default="1,128,4096", metavar="N1,N2,..")
-    ap.add_argument("--steps", type=int, default=200)
-    ap.add_argument("--warmup", type=int, default=32)
-    ap.add_argument("--rounds", type=int, default=3)
+    common.add_run_args(ap, tokens="1,128,4096", steps=200, warmup=32, rounds=3)
     args = ap.parse_args()
-    names = [c for c in args.configs.split(",") if c]
     known = {**bench.BASELINE_CONFIGS, "DSV3": DSV3}
-    bad = [c for c in names if c not in known]
-    if not names or bad:
-        ap.error(f"--configs: unknown {bad}; choose from {sorted(known)}")
-    tokens = {c: parse_tokens(ap, args.tokens, known[c].S) for c in names}
-    if args.steps < 1 or args.rounds < 1:
-        ap.error("--steps and --rounds must be >= 1")
+    names = common.parse_names(ap, "--configs", args.configs, known)
+    tokens = {c: common.parse_tokens(ap, args.tokens, known[c].S) for c in names}
+    common.check_counts(ap, args)
     if not torch.cuda.is_available():
-        print("bench_shared.py: no CUDA device; the MoE forward path has no CPU fallback", file=sys.stderr)
-        return 3
+        return common.no_cuda("bench_shared.py")
     dev = torch.device("cuda", torch.cuda.current_device())
     runs = [run_config(c, tokens[c], args.steps, args.warmup, args.rounds, dev) for c in names]
     print(json.dumps({"metric": "moe_layer_fwd_shared_ms", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
-                      "rounds": args.rounds, "card": card(dev), "runs": runs}), flush=True)
+                      "rounds": args.rounds, "card": common.card(dev), "runs": runs}), flush=True)
     return 0
 
 

@@ -17,6 +17,7 @@ one JSON line with the card's name and power limit next to the figures; writes n
 from __future__ import annotations
 
 import argparse
+import functools
 import json
 import os
 import statistics
@@ -29,14 +30,13 @@ import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
 
 from flashmoe_b200.config import MoEConfig  # noqa: E402
-from scripts.bench_gated import RULE  # noqa: E402
-from scripts.bench_varlen import card, parse_tokens  # noqa: E402
+from scripts import bench_common as common  # noqa: E402
+from scripts.bench_common import DSV3, RULE  # noqa: E402
 
 SHAPES = {
     "mixtral": (MoEConfig(num_experts=8, expert_top_k=2, sequence_len=4096, hidden_size=4096, intermediate_size=14336),
                 None),
-    "dsv3": (MoEConfig(num_experts=256, expert_top_k=8, sequence_len=4096, hidden_size=7168, intermediate_size=2048),
-             2048),
+    "dsv3": (DSV3, 2048),
 }
 
 
@@ -66,14 +66,7 @@ def run_shape(name, tokens, steps, warmup, rounds, dev):
             return ctx.forward_gated(x[:n], wg, we, RULE, shared_expert=se)
         return ctx.forward_tokens(x[:n], wg, we, shared_expert=se)
 
-    def device_ms(fn):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        torch.cuda.synchronize(dev)
-        return e0.elapsed_time(e1) / steps
+    sync = functools.partial(torch.cuda.synchronize, dev)
 
     entries = []
     for n in tokens:
@@ -105,14 +98,7 @@ def run_shape(name, tokens, steps, warmup, rounds, dev):
             return out
 
         fns = {"swiglu": lambda: fused(2, n), "gelu": lambda: fused(1, n), "torch": torch_arm}
-        for fn in fns.values():
-            for _ in range(warmup):
-                fn()
-        torch.cuda.synchronize(dev)
-        ms = {a: [] for a in fns}
-        for _ in range(rounds):
-            for a, fn in fns.items():
-                ms[a].append(device_ms(fn))
+        ms = common.alternate(fns, warmup, rounds, sync, lambda fn: common.device_ms(fn, steps, sync))
         med = {a: statistics.median(v) for a, v in ms.items()}
         shared_flops = 0 if ps is None else 2 * n * ps * H
         f_glu = 6.0 * P * H * picks + 3 * shared_flops
@@ -133,25 +119,21 @@ def run_shape(name, tokens, steps, warmup, rounds, dev):
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--shapes", default="mixtral,dsv3")
-    ap.add_argument("--tokens", default="1,128,4096")
-    ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3)
+    common.add_run_args(ap, tokens="1,128,4096", steps=20, warmup=3, rounds=3)
     a = ap.parse_args(argv)
-    shapes = [s for s in a.shapes.split(",") if s]
-    bad = [s for s in shapes if s not in SHAPES]
-    if bad:
-        ap.error(f"--shapes: unknown {bad}; choose from {sorted(SHAPES)}")
-    tokens = parse_tokens(ap, a.tokens, 4096)
+    shapes = common.parse_names(ap, "--shapes", a.shapes, SHAPES)
+    tokens = common.parse_tokens(ap, a.tokens, 4096)
+    common.check_counts(ap, a)
     if not torch.cuda.is_available():
-        sys.exit("bench_swiglu.py measures the GPU path and needs a CUDA device")
+        return common.no_cuda("bench_swiglu.py")
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    res = {"card": card(dev), "results": []}
+    res = {"card": common.card(dev), "results": []}
     for s in shapes:
         res["results"] += run_shape(s, tokens, a.steps, a.warmup, a.rounds, dev)
     print(json.dumps(res))
+    return 0
 
 
 if __name__ == "__main__":
-    main()
+    sys.exit(main())

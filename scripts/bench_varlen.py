@@ -18,7 +18,6 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import statistics
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -27,32 +26,9 @@ sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
 import bench  # noqa: E402   (seeded inputs, rank helpers; bench.py itself is not changed by this script)
+from scripts import bench_common as common  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12   # H100 SXM data sheet HBM3 bandwidth: the floor is stated against it, not a measured rate
-
-
-def parse_tokens(ap, text, S):
-    try:
-        tokens = [int(t) for t in text.split(",") if t.strip()]
-    except ValueError:
-        ap.error(f"--tokens takes a comma-separated list of integers, got {text!r}")
-    if not tokens or any(n < 0 or n > S for n in tokens):
-        ap.error(f"--tokens: every count must be in [0, S = {S}]")
-    return tokens
-
-
-def card(dev):
-    info = {"name": torch.cuda.get_device_name(dev), "power_limit_w": None, "sm_max_mhz": None}
-    try:
-        import pynvml
-
-        pynvml.nvmlInit()
-        h = pynvml.nvmlDeviceGetHandleByIndex(dev.index)
-        info["power_limit_w"] = pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
-        info["sm_max_mhz"] = pynvml.nvmlDeviceGetMaxClockInfo(h, pynvml.NVML_CLOCK_SM)
-    except Exception:
-        pass
-    return info
 
 
 def run_varlen(env, name, tokens, steps, warmup, rounds):
@@ -66,15 +42,6 @@ def run_varlen(env, name, tokens, steps, warmup, rounds):
     x, wg, we = bench.make_inputs(cfg, nlx, rank)
     xd, wgd, wed = x.to(dev).view(S, H), wg.to(dev), we.to(dev)
     del we
-
-    def device_ms(fn):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        env.barrier()
-        return env.max_over_ranks(e0.elapsed_time(e1) / steps)
 
     entries = []
     for n in tokens:
@@ -91,14 +58,8 @@ def run_varlen(env, name, tokens, steps, warmup, rounds):
                                timeout_ms=30000)
             xn3, out_n3 = xn.view(1, n, H), torch.empty(1, n, H, dtype=torch.bfloat16, device=dev)
             arms["ms_context_of_n"] = lambda: ctx_n.forward(xn3, wgd, wed, out=out_n3)
-        for fn in arms.values():
-            for _ in range(warmup):
-                fn()
-        env.barrier()
-        times = {k: [] for k in arms}
-        for _ in range(rounds):
-            for k, fn in arms.items():
-                times[k].append(device_ms(fn))
+        times = common.alternate(arms, warmup, rounds, env.barrier,
+                                 lambda fn: env.max_over_ranks(common.device_ms(fn, steps, env.barrier)))
         # work of the forward_tokens call: executed token-expert pairs and the experts that received rows
         ctx.forward_tokens(xn, wgd, wed, out=out_n)
         ctx.synchronize()
@@ -107,10 +68,7 @@ def run_varlen(env, name, tokens, steps, warmup, rounds):
         used_local = int((recv.sum(axis=0) > 0).sum())
         floor_bytes = used_local * 2 * P * H * 2 + cfg.E * H * 2 + 2 * n * H * 2
         floor_ms = env.max_over_ranks(floor_bytes / HBM_BYTES_PER_S * 1e3)
-        e = {"tokens": n, "ec": cfg.EC_of(n)}
-        for k, v in times.items():
-            e[k] = statistics.median(v)
-            e[k + "_runs"] = v
+        e = {"tokens": n, "ec": cfg.EC_of(n), **common.medians(times)}
         ms = e["ms"]
         e.update({"tokens_per_s": world * n / (ms * 1e-3), "token_expert_pairs_executed": pairs,
                   "experts_with_rows_per_rank": used_local, "hbm_floor_bytes_per_rank": floor_bytes,
@@ -132,17 +90,12 @@ def run_varlen(env, name, tokens, steps, warmup, rounds):
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--config", default="B", choices=sorted(bench.BASELINE_CONFIGS))
-    ap.add_argument("--tokens", required=True, metavar="N1,N2,..")
-    ap.add_argument("--steps", type=int, default=200)
-    ap.add_argument("--warmup", type=int, default=32)
-    ap.add_argument("--rounds", type=int, default=3)
+    common.add_run_args(ap, tokens=None, steps=200, warmup=32, rounds=3)
     args = ap.parse_args()
-    tokens = parse_tokens(ap, args.tokens, bench.BASELINE_CONFIGS[args.config].S)
-    if args.steps < 1 or args.rounds < 1:
-        ap.error("--steps and --rounds must be >= 1")
+    tokens = common.parse_tokens(ap, args.tokens, bench.BASELINE_CONFIGS[args.config].S)
+    common.check_counts(ap, args)
     if not torch.cuda.is_available():
-        print("bench_varlen.py: no CUDA device; the MoE forward path has no CPU fallback", file=sys.stderr)
-        return 3
+        return common.no_cuda("bench_varlen.py")
     rank, world, local = bench.env_int("RANK", 0), bench.env_int("WORLD_SIZE", 1), bench.env_int("LOCAL_RANK", 0)
     torch.cuda.set_device(local % torch.cuda.device_count())
     dev = torch.device("cuda", torch.cuda.current_device())
@@ -154,8 +107,8 @@ def main():
     entries = run_varlen(env, args.config, tokens, args.steps, args.warmup, args.rounds)
     line = {"metric": "moe_layer_fwd_varlen_ms", "config": bench.config_dict(args.config, bench.BASELINE_CONFIGS[args.config],
                                                                              world),
-            "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "rounds": args.rounds, "card": card(dev),
-            "hbm_floor_rate_bytes_per_s": HBM_BYTES_PER_S, "varlen": entries}
+            "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "rounds": args.rounds,
+            "card": common.card(dev), "hbm_floor_rate_bytes_per_s": HBM_BYTES_PER_S, "varlen": entries}
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
