@@ -24,7 +24,7 @@ BUF_SHARED_HIDDEN = 13
 EXPORTED_SYMBOLS = (
     "fm_compiled_config", "fm_create", "fm_destroy", "fm_get_dims", "fm_num_local_experts", "fm_symm_size",
     "fm_symm_local_ptr", "fm_symm_export", "fm_symm_attach_ipc", "fm_symm_attach_ptrs", "fm_symm_use_external",
-    "fm_moe_forward", "fm_moe_forward_tokens", "fm_moe_forward_tokens_dev", "fm_moe_forward_routed", "fm_moe_forward_gated", "fm_shared_reserve", "fm_moe_forward_shared", "fm_last_launch", "fm_output_buffer", "fm_moe_forward_host", "fm_host_submit", "fm_host_wait", "fm_check", "fm_set_timeout_ms", "fm_set_trace", "fm_launch_count",
+    "fm_moe_forward", "fm_moe_forward_tokens", "fm_moe_forward_tokens_dev", "fm_moe_forward_routed", "fm_moe_forward_gated", "fm_shared_reserve", "fm_moe_forward_shared", "fm_last_launch", "fm_output_buffer", "fm_moe_forward_host", "fm_host_submit", "fm_host_wait", "fm_check", "fm_set_timeout_ms", "fm_set_trace", "fm_set_weight_on_input", "fm_launch_count",
     "fm_buffer_bytes",
     "fm_read_buffer", "fm_last_error", "fm_version",
 )
@@ -103,6 +103,7 @@ def load() -> ctypes.CDLL:
     L.fm_check.argtypes = [vp]
     L.fm_set_timeout_ms.argtypes = [vp, ctypes.c_uint32]
     L.fm_set_trace.argtypes = [vp, ctypes.c_int]
+    L.fm_set_weight_on_input.argtypes = [vp, ctypes.c_int]
     L.fm_launch_count.argtypes = [vp]
     L.fm_launch_count.restype = ctypes.c_uint64
     L.fm_buffer_bytes.argtypes = [vp, ctypes.c_int, ctypes.POINTER(ctypes.c_size_t)]

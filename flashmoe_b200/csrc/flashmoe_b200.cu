@@ -161,6 +161,7 @@ struct fm_ctx {
     fm::DebugRecord* dbg_dev = nullptr;
     unsigned long long* trace = nullptr;
     bool trace_on = false;
+    bool weight_on_input = false;   // fm_set_weight_on_input (caller and gated routes)
     TmapCache tm[fm::NUM_TMAPS];   // FmParams::tm (fm_symm_use_external moves recv_x's base)
     // shared expert (fm_shared_reserve): staging h_s [S, shared_max] and y_s [S, H], row-block counters [S / 128]
     int shared_max = 0;
@@ -505,6 +506,7 @@ int launch(fm_ctx* c, const ForwardCall& f) {
     }
     p.dbg = c->dbg_dev;
     p.trace = c->trace_on ? c->trace : nullptr;
+    p.weight_on_input = c->weight_on_input && f.route != fm::ROUTE_ROUTER ? 1 : 0;   // (the router route copies y unscaled)
 
     cudaLaunchConfig_t lc = {};
     lc.gridDim = dim3(c->grid);
@@ -1056,6 +1058,17 @@ FM_API int fm_set_timeout_ms(fm_ctx_t* ctx, uint32_t ms) {
 FM_API int fm_set_trace(fm_ctx_t* ctx, int enable) {
     if (ctx == nullptr) return fail(FM_EINVAL, "null context");
     ctx->trace_on = enable != 0;
+    return FM_OK;
+}
+
+FM_API int fm_set_weight_on_input(fm_ctx_t* ctx, int enable) {
+    if (ctx == nullptr) return fail(FM_EINVAL, "null context");
+    if (enable != 0 && enable != 1) return fail(FM_EINVAL, "enable must be 0 or 1, got %d", enable);
+    if (enable && ctx->d.k != 1)
+        return fail(FM_EINVAL, "the router weight on the input needs k = 1 (each pick would need its own copy of the "
+                               "row); this context has k = %d", ctx->d.k);
+    if (enable && ctx->d.E == 1) return fail(FM_EINVAL, "the router weight on the input needs E > 1 (no routing at E = 1)");
+    ctx->weight_on_input = enable == 1;
     return FM_OK;
 }
 

@@ -422,6 +422,9 @@ struct FmParams {
     int shared;
     __nv_bfloat16* y_s;
     unsigned int *s0_done, *s1_done;
+    // fm_set_weight_on_input on a caller or gated launch (k = 1): every dispatched row is rne_bf16(x[t] * w~) and the
+    // combine takes weight 1 (recv_meta's p~ and the gather path's c_w); 0 on the router route
+    int weight_on_input;
     DebugRecord* dbg;
     unsigned long long* trace;  // optional [grid][TRACE_SLOTS] %globaltimer stamps (nullptr = off)
 };
@@ -1314,6 +1317,30 @@ __device__ __forceinline__ void ack_rows(const FmParams& p, unsigned int par, in
 constexpr int RMAX = 8;
 constexpr int RANGES_IN_REGS = 32 * RMAX;
 
+// The router weight on the input (FmParams::weight_on_input, k = 1): staged row r (`nb` bytes at s + r * stride, a whole
+// token row or a piece of one) of token t_first + r becomes rne_bf16(fl32(x) * fl32(w~)), w~ = topk_w[t, 0]; the product
+// of two bf16 numbers is exact in fp32, so this is torch's bf16 x * w.  Warp `w` of `nw` takes rows w, w + nw, ...  The
+// caller fences (async proxy) and synchronises before the bulk stores read the rows.  Out of line on purpose, like
+// gate_phase_routed: inlined into the kernel it raised the spill loads from 552 to 560 B.
+__device__ __noinline__ void scale_staged_rows(const FmParams& p, uint8_t* s, int t_first, int rows, int stride, int nb,
+                                                  int w, int nw) {
+    const int lane = threadIdx.x & 31;
+    for (int r = w; r < rows; r += nw) {
+        const float wt = __bfloat162float(p.topk_w[t_first + r]);
+        for (int c = lane * 16; c < nb; c += 32 * 16) {
+            uint4* q = reinterpret_cast<uint4*>(s + (size_t)r * stride + c);
+            float f[8];
+            unpack8(*q, f);
+            uint4 o;
+            o.x = pack_bf16x2(__fmul_rn(f[0], wt), __fmul_rn(f[1], wt));
+            o.y = pack_bf16x2(__fmul_rn(f[2], wt), __fmul_rn(f[3], wt));
+            o.z = pack_bf16x2(__fmul_rn(f[4], wt), __fmul_rn(f[5], wt));
+            o.w = pack_bf16x2(__fmul_rn(f[6], wt), __fmul_rn(f[7], wt));
+            *q = o;
+        }
+    }
+}
+
 // Warps 4-11: every (token, pick) pair's slot and routing record, and the rows for experts on this rank.
 __device__ __forceinline__ void dispatch_local_rows(const FmParams& p, const Launch& L, uint8_t* smem, int t0, int n_tok,
                                                     const int* base_s, const int* own_s) {
@@ -1336,6 +1363,11 @@ __device__ __forceinline__ void dispatch_local_rows(const FmParams& p, const Lau
         }
         bar_wait(p, smem, BAR_XROWS, xphase);
         xphase ^= 1;
+        if (p.weight_on_input) {   // (k = 1: a staged row has at most one destination, so it is scaled in place)
+            scale_staged_rows(p, x_s, t0 + g0, rows, row_bytes, row_bytes, ltid >> 5, EPI_THREADS / 32);
+            fence_proxy_async_smem();   // these generic writes -> the bulk stores' reads and the next group's load
+            named_sync<NAMED_BAR_LOCAL, EPI_THREADS>();
+        }
         for (int i = ltid; i < rows * k; i += EPI_THREADS) {   // one thread per (token, pick)
             const int tl = i / k, j = i - tl * k;
             const int ti = g0 + tl, t = t0 + ti;
@@ -1349,7 +1381,8 @@ __device__ __forceinline__ void dispatch_local_rows(const FmParams& p, const Lau
                 if (p.fused) {   // what the expert's GEMM1 epilogue needs to combine this row
                     uint4 m;
                     m.x = (unsigned int)t;
-                    m.y = __float_as_uint(__bfloat162float(p.topk_w[(size_t)t * k + j]));
+                    // (the weight already scaled the row: the owner combines it with weight 1, whatever its own setting)
+                    m.y = __float_as_uint(p.weight_on_input ? 1.0f : __bfloat162float(p.topk_w[(size_t)t * k + j]));
                     m.z = __float_as_uint(p.mcw[t]);
                     m.w = 0u;
                     st_global_v4(p.peer_recv_meta[owner] + row, m);
@@ -1438,6 +1471,11 @@ __device__ __forceinline__ void dispatch_remote_rows(const FmParams& p, const La
                 }
                 bar_wait(p, smem, BAR_REMOTE, rphase);
                 rphase ^= 1;
+                if (p.weight_on_input) {
+                    scale_staged_rows(p, win, t0 + tw, rows, row_bytes, row_bytes, 0, 1);
+                    fence_proxy_async_smem();
+                    __syncwarp();
+                }
                 for (int i = lane; i < rows * k; i += 32) {
                     const size_t gi = (size_t)(t0 + tw) * k + i;
                     const int e = p.topk_idx[gi];
@@ -1461,6 +1499,11 @@ __device__ __forceinline__ void dispatch_remote_rows(const FmParams& p, const La
                     }
                     bar_wait(p, smem, BAR_REMOTE, rphase);
                     rphase ^= 1;
+                    if (p.weight_on_input) {
+                        scale_staged_rows(p, win, t0 + tw, 1, nb, nb, 0, 1);
+                        fence_proxy_async_smem();
+                        __syncwarp();
+                    }
                     for (int i = lane; i < k; i += 32) {
                         const size_t gi = (size_t)(t0 + tw) * k + i;
                         const int e = p.topk_idx[gi];
@@ -2354,7 +2397,7 @@ __device__ __forceinline__ void combine_phase(const FmParams& p, const Launch& L
         const int s = p.slot[gi];
         c_e[i] = e;
         c_s[i] = s;
-        c_w[i] = __bfloat162float(p.topk_w[gi]);
+        c_w[i] = p.weight_on_input ? 1.0f : __bfloat162float(p.topk_w[gi]);   // (the weight scaled the dispatched row)
         if (s < EC) {
             const unsigned long long* fl = p.ret_flag + (size_t)e * p.TCM + (s / BLOCK_M);
             SpinGuard g;

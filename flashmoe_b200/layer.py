@@ -43,11 +43,24 @@ class FlashMoELayer(torch.nn.Module):
     `shared_inter`: hold a shared expert of that intermediate size Ps, `shared_weight` [2, Ps, H] (one routed expert's
     layout; plus `shared_bias_up` [Ps] / `shared_bias_down` [H] with `bias`), which every token passes through on every
     route: out[t] = rne_bf16(routed[t] + s[t]) (`MoEContext.forward_tokens`'s `shared_expert`).
+
+    `weight_on_input` (k = 1, E > 1): the router weight scales each routed token's input row, rne_bf16(x[t] * w~), and
+    the combine takes weight 1 -- Hugging Face's `Llama4TextMoe` (`MoEContext`'s `weight_on_input`).  On the gated
+    and the caller route only.  Llama 4 Scout / Maverick are `hidden_act = 2`, k = 1, `drop_tokens = 0`,
+    `router=RouterSpec("sigmoid", renormalize=False)`, `shared_inter = P` and `weight_on_input=True`; their Hugging
+    Face tensors convert once at load time (E experts, P = intermediate_size, Ps = the shared MLP's):
+
+        gu, dp = experts.gate_up_proj, experts.down_proj           # [E, H, 2P], [E, P, H]
+        expert_weight = torch.stack([gu[:, :, :P].transpose(1, 2), gu[:, :, P:].transpose(1, 2),
+                                     dp.transpose(1, 2).reshape(E, P, H)], 1)
+        shared_weight = torch.stack([shared_expert.gate_proj.weight, shared_expert.up_proj.weight,
+                                     shared_expert.down_proj.weight.reshape(Ps, H)])
+        gate_weight = router.weight.view(H, E)                     # [E, H] read flat, not transposed
     """
 
     def __init__(self, cfg: MoEConfig, rank: int = 0, world: int = 1, device: Optional[int] = None, group=None,
                  bias: bool = False, router: Optional[RouterSpec] = None, score_bias: bool = False,
-                 shared_inter: Optional[int] = None):
+                 shared_inter: Optional[int] = None, weight_on_input: bool = False):
         super().__init__()
         cfg.check_hot_path()
         if router is not None:
@@ -58,7 +71,8 @@ class FlashMoELayer(torch.nn.Module):
             raise ValueError("score_bias needs a router rule (router=RouterSpec(...))")
         self.cfg = cfg
         self.router = router
-        self.ctx = MoEContext(cfg, rank=rank, world=world, device=device, group=group, shared_inter=shared_inter)
+        self.ctx = MoEContext(cfg, rank=rank, world=world, device=device, group=group, shared_inter=shared_inter,
+                              weight_on_input=weight_on_input)
         dev = self.ctx.device
         nlx = self.ctx.num_local_experts
         scale = cfg.H ** -0.5
@@ -140,4 +154,5 @@ class FlashMoELayer(torch.nn.Module):
         c = self.cfg
         return (f"S={c.S}, H={c.H}, P={c.P}, E={c.E}, k={c.k}, act={('relu', 'gelu', 'swiglu')[c.hidden_act]}, "
                 f"rank={self.ctx.rank}/{self.ctx.world}"
-                + (f", shared_inter={self.shared_inter}" if self.shared_inter is not None else ""))
+                + (f", shared_inter={self.shared_inter}" if self.shared_inter is not None else "")
+                + (", weight_on_input=True" if getattr(self.ctx, "weight_on_input", False) else ""))

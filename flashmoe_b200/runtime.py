@@ -122,12 +122,22 @@ def shared_expert_struct(se: SharedExpert, device: torch.device, H: int, reserve
                                se.bias_down.data_ptr() if se.bias_down is not None else None, ps)
 
 
+def _check_weight_on_input(enable, cfg: MoEConfig) -> None:
+    """The conditions of fm_set_weight_on_input, checked before any native call."""
+    if enable not in (True, False):
+        raise ValueError(f"weight_on_input must be a bool, got {enable!r}")
+    if enable and cfg.k != 1:
+        raise ValueError(f"weight_on_input needs k = 1 (each pick would need its own copy of the row); got k = {cfg.k}")
+    if enable and cfg.E == 1:
+        raise ValueError("weight_on_input needs E > 1 (an E = 1 context has no routing)")
+
+
 class MoEContext:
     """Owns the native context (workspaces, symmetric slab, peer mappings) for one rank."""
 
     def __init__(self, cfg: Optional[MoEConfig] = None, rank: int = 0, world: int = 1,
                  device: Optional[int] = None, group=None, timeout_ms: Optional[int] = None,
-                 symmetric: Optional[str] = None, shared_inter: Optional[int] = None):
+                 symmetric: Optional[str] = None, shared_inter: Optional[int] = None, weight_on_input: bool = False):
         """`symmetric` selects how the peers' slabs are mapped when world > 1: "ipc" (default; cudaMalloc + CUDA IPC
         handles over torch.distributed) or "torch" (the slab is allocated with torch.distributed._symmetric_memory --
         the allocator PyTorch backs with CUDA VMM / NVSHMEM -- and the peer pointers come from its rendezvous; this is
@@ -135,7 +145,15 @@ class MoEContext:
         override: FM_SYMM=ipc|torch.
 
         `shared_inter`: reserve the staging of a shared expert of intermediate size up to this (a multiple of 64;
-        fm_shared_reserve), so that the forward calls accept `shared_expert=`."""
+        fm_shared_reserve), so that the forward calls accept `shared_expert=`.
+
+        `weight_on_input`: scale each routed token's input row by its router weight instead of the expert's output
+        (fm_set_weight_on_input; Llama 4): on `forward_routed` and `forward_gated` a kept pick dispatches
+        rne_bf16(x[t] * rne_bf16(w)) and the combine takes weight 1, so out equals a plain context's
+        `forward_routed(x', topk_idx, ones)` on the scaled rows x' bit for bit; a shared expert still sees the unscaled x.
+        The router route (`forward`, `forward_tokens`) is unchanged.  Needs k = 1 and E > 1 (ValueError otherwise)."""
+        if weight_on_input:
+            _check_weight_on_input(weight_on_input, cfg if cfg is not None else _lib.compiled_config())
         self._L = _lib.load()
         self._ctx = ctypes.c_void_p()
         if device is None:
@@ -155,6 +173,9 @@ class MoEContext:
         if shared_inter is not None:
             _lib.check(self._L.fm_shared_reserve(self._ctx, int(shared_inter)))
             self.shared_inter = int(shared_inter)
+        self.weight_on_input = False
+        if weight_on_input:
+            self.set_weight_on_input(True)
         # tokens of the last forward (valid rows of the routing tables `read` returns); None after a call with a
         # device-side count (launch_record() has it)
         self.last_tokens: Optional[int] = 0
@@ -490,6 +511,13 @@ class MoEContext:
 
     def set_trace(self, enable: bool) -> None:
         _lib.check(self._L.fm_set_trace(self._ctx, 1 if enable else 0))
+
+    def set_weight_on_input(self, enable: bool) -> None:
+        """Turn the router weight on the input (the constructor's `weight_on_input`) on or off for the next launches; a
+        captured graph keeps the setting it was captured with."""
+        _check_weight_on_input(enable, self.cfg)
+        _lib.check(self._L.fm_set_weight_on_input(self._ctx, 1 if enable else 0))
+        self.weight_on_input = bool(enable)
 
     def check(self) -> None:
         """Raise if the last kernel reported a protocol timeout (call after a synchronise)."""

@@ -167,7 +167,8 @@ FM_API int fm_moe_forward_routed(fm_ctx_t* ctx, const void* x, int n_tokens, con
                                  const int32_t* topk_idx, const float* topk_w, const void* expert_w,
                                  const void* bias_up, const void* bias_down, void* out, void* stream);
 
-/* A router rule for fm_moe_forward_gated (DeepSeek-V2/V3, Kimi K2, GLM-4.5, Qwen-MoE, OLMoE and Llama 4 style routers). */
+/* A router rule for fm_moe_forward_gated (DeepSeek-V2/V3, Kimi K2, GLM-4.5, Qwen-MoE, OLMoE and Llama 4 style routers;
+ * Llama 4 also needs fm_set_weight_on_input, since it scales the expert's input row by the weight, not its output). */
 typedef struct fm_router {
     int32_t scoring;      /* 0 softmax (the router's own recurrence), 1 sigmoid */
     int32_t n_group;      /* experts split into n_group contiguous groups of E / n_group; 1 = no group limit */
@@ -204,8 +205,8 @@ FM_API int fm_moe_forward_gated(fm_ctx_t* ctx, const void* x, int n_tokens, cons
                                 const void* expert_w, const void* bias_up, const void* bias_down, void* out,
                                 void* stream);
 
-/* ---- shared expert (DeepSeek-V2/V3 and Kimi K2 n_shared_experts, Qwen-MoE shared_expert_intermediate_size, Llama 4,
- * GLM-4.5, DeepSpeed Residual-MoE) ----
+/* ---- shared expert (DeepSeek-V2/V3 and Kimi K2 n_shared_experts, Qwen-MoE shared_expert_intermediate_size, Llama 4
+ * with fm_set_weight_on_input, GLM-4.5, DeepSpeed Residual-MoE) ----
  * A dense FFN every token passes through, its output added to the routed combine:
  *   w          bf16 [2, Ps, H], contiguous: exactly one routed expert's slice of expert_w -- [0] is W_up [Ps, H], [1] is the
  *              same Ps*H block flat-viewed as W_down [H, Ps]
@@ -259,7 +260,7 @@ FM_API int fm_moe_forward_shared(fm_ctx_t* ctx, const void* x, int n_tokens, con
  * context.  A launch keeps no per-launch state in its parameters: the kernel takes its epoch, grid-barrier target and
  * token-dependent sizes from the context's device-side launch counter (and the device-side count) when it starts.
  * What is fixed at capture: the pointers (x, out, weights, biases, score_bias, n_tokens_dev), a host-side n_tokens, a
- * gated call's fm_router_t values, and the fm_set_trace and fm_set_timeout_ms settings (the contents of score_bias are
+ * gated call's fm_router_t values, and the fm_set_trace, fm_set_weight_on_input and fm_set_timeout_ms settings (the contents of score_bias are
  * read at every replay, so a graph follows in-place bias updates).  Replays of launches on one context must run in stream order, one at a
  * time, like eager calls.  With world > 1 every rank issues the same number of launches, eager calls and replays
  * together, in the same order.  The host-buffer entry points (fm_moe_forward_host, fm_host_submit) cannot be captured.
@@ -298,6 +299,22 @@ FM_API int fm_set_timeout_ms(fm_ctx_t* ctx, uint32_t ms);
 FM_API uint64_t fm_launch_count(const fm_ctx_t* ctx);
 /* Per-CTA phase / tile time stamps into FM_BUF_TRACE (profiling aid; off by default). */
 FM_API int fm_set_trace(fm_ctx_t* ctx, int enable);
+/* Apply the router weight to each routed token's INPUT row instead of its expert output (Llama 4's Llama4TextMoe, vLLM's
+ * apply_router_weight_on_input); enable 0 / 1, default 0.  With it on, the caller route (fm_moe_forward_routed) and the
+ * gated route (fm_moe_forward_gated), directly or through fm_moe_forward_shared, change as follows:
+ *   - a kept pick of token t dispatches rne_bf16(fl32(x[t]) * fl32(w~)) instead of x[t], w~ = the stored topk_w entry
+ *     (rne_bf16 of the caller's weight or of the rule's w); the fp32 product of two bf16 numbers is exact, so this is
+ *     bit for bit torch's bf16 x * w;
+ *   - the combine takes weight 1: out[t] is the expert's output row y (bias included); with a shared expert
+ *     out[t] = rne_bf16(fl32(y) + fl32(s)), s computed from the unscaled x[t].
+ * So out is bit for bit what a context with the setting off returns from fm_moe_forward_routed(x', topk_idx, ones), x'
+ * the scaled rows, on the fused and the gather combine.  topk_idx, topk_w = rne_bf16(w), mcw = 1, slot, counts and
+ * gate_out are those of the same call with the setting off; FM_BUF_RECV_X holds the scaled rows.  The router route
+ * (fm_moe_forward, _tokens[_dev], the host entry points) is unchanged: its k = 1 combine copies y unscaled.  FM_EINVAL
+ * for a null context, enable not 0 / 1, and enable = 1 on a context with k != 1 (each pick would need its own copy of the
+ * row) or E = 1.  Fixed at capture, like fm_set_trace.  With world > 1 each rank's own setting governs the rows it
+ * sends (the sender picks the combine weight), so ranks may differ. */
+FM_API int fm_set_weight_on_input(fm_ctx_t* ctx, int enable);
 
 /* ---- inspection (tests / debugging): copy an internal device buffer to host memory after synchronising ---- */
 enum fm_buffer {
