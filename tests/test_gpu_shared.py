@@ -1,12 +1,8 @@
 """Shared experts (fm_moe_forward_shared, `shared_expert=` on the forward calls) on one H100: the definition
 out[t] = rne_bf16(r[t] + s[t]) bit for bit against the same context's call without one, on every route, k, combine,
 activation, bias, Ps and token count; s itself against the dense E = 1 path and the exact-input references; graphs with
-a device-side count; the argument checks; the layer; and two ranks (skipped with fewer than two GPUs)."""
+a device-side count; the argument checks; and the layer.  Two ranks: tests/test_gpu_multi.py's "shared" scenario."""
 import ctypes
-import os
-import socket
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -19,7 +15,6 @@ from tests import exact as ex
 from tests.util import make_inputs
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 # E = 16, P = 256: Ps = 64, 320 (a partial 256-column tile), P and 2P; DeepSeek-V3's rule at 8 groups of 2
 BASE = MoEConfig(num_experts=16, expert_top_k=2, sequence_len=512, hidden_size=256, intermediate_size=256)
@@ -343,21 +338,3 @@ def test_rejected_contexts_and_reservations():
     assert c.call(c.args()) == -1 and b"num_experts > 1" in dense._L.fm_last_error()
     assert dense.launch_count == 0
     dense.close()
-
-
-# ------------------------------------------------------------------ two ranks
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def test_two_ranks():
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs")
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr",
-           "127.0.0.1", "--master-port", str(_free_port()), os.path.join(ROOT, "tests", "multi_gpu_shared_worker.py")]
-    res = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=ROOT)
-    assert res.returncode == 0, res.stdout[-4000:] + "\n" + res.stderr[-4000:]
-    for r in range(2):
-        assert f"RANK {r} SHARED ALL OK" in res.stdout
